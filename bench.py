@@ -42,10 +42,15 @@ def parse():
     ap.add_argument("--ddp-backend", default=None)
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--ref-ext", action="store_true",
-                    help="reference arm only: make the reference's OWN CUDA extensions importable (rebuilt with an sm_100 "
+                    help="reference arm only: make the reference's OWN CUDA extensions importable (built for sm_90 "
                          "gencode into baseline/_ref_ext by baseline/build_ref_ext.sh) = BASELINE.md B2; the default "
                          "reference arm is its stock install without extensions (B1)")
     ap.add_argument("--report-losses", action="store_true", help="add the losses read back in the end-to-end region")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy: its loss, "
+                         "the norm of every updated parameter, and a fixed sample of the updated parameters.  Inputs and "
+                         "initial weights are seeded; two runs agree up to the fp32 summation order of the attention dQ "
+                         "and embedding-gradient accumulations (DESIGN.md, Reproducibility)")
     ap.add_argument("--sync-overflow-check", action="store_true",
                     help="ours: read the grad norm on the host every step (reference behaviour) instead of the "
                          "deferred, device-side overflow skip")
@@ -145,6 +150,25 @@ def make_batches(n, bsz, seq_len, vocab, pad_idx, mask_idx, special, seed):
             "target": torch.from_numpy(target),
         })
     return out
+
+
+def dump_outputs(out_dir, trainer, log):
+    """What a caller of ``Trainer.train_step`` receives from one step: the logged loss and the updated model.
+    Parameters are sampled at fixed, seeded positions (4 Mi values of the flattened model, 16 MB) so that two builds
+    can be compared element for element."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    v = log.get("loss", None) if log is not None else None   # None: the update was skipped (fp16 overflow)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float("nan") if v is None else float(v)], dtype=np.float64))
+    params = [p.detach() for p in trainer.model.parameters()]
+    np.save(os.path.join(out_dir, "param_norms.npy"),
+            np.array([p.float().norm().item() for p in params], dtype=np.float64))
+    flat = torch.cat([p.float().reshape(-1) for p in params])
+    idx = np.random.RandomState(0).randint(0, flat.numel(), size=min(flat.numel(), 4 << 20))
+    sample = flat[torch.from_numpy(idx).to(flat.device)].cpu().numpy().astype(np.float32)
+    np.save(os.path.join(out_dir, "param_sample.npy"), sample)
 
 
 def train_flags(a, world):
@@ -249,6 +273,7 @@ def build_trainer(a, impl, world, rank, local_rank):
     args = options.parse_args_and_arch(parser, input_args=flags)
     args.distributed_rank = rank
     args.device_id = local_rank
+    torch.manual_seed(args.seed)   # identical initial weights and dropout streams from run to run
     task = tasks.setup_task(args)
     model = task.build_model(args)
     loss = task.build_loss(args)
@@ -336,11 +361,13 @@ def main():
         torch.cuda.synchronize()
 
     seen_losses = []
+    last_log = [None]
 
     def run_steps(batches, n, read_loss):
         last = None
         for i in range(n):
             out = trainer.train_step(split_micro(batches[i % len(batches)]))
+            last_log[0] = out
             if read_loss and out is not None:
                 v = out.get("loss", None)
                 last = float(v) if v is not None else None  # device -> host read of the step result
@@ -369,6 +396,8 @@ def main():
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     elapsed_ms = float(t.item())
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, trainer, last_log[0])
 
     # ---- timed region 2: end to end (pinned host batch -> H2D each step, loss read back each step) ----
     e2e = None
@@ -430,7 +459,7 @@ def main():
                 if getattr(getattr(trainer, "optimizer", None), "uses_fused_tail", False) else "replicated",
                 "ema_decay": a.ema_decay if a.ema_decay > 0 else None,
                 "l2": "no explicit flush: each step streams >1.7 GB of weights/optimizer state/activations, "
-                      "far above the 126 MB L2, and 8 distinct input batches rotate",
+                      "far above the 50 MB L2, and 8 distinct input batches rotate",
             },
             "clocks": clocks,
             "e2e": e2e,

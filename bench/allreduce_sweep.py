@@ -7,7 +7,7 @@ Launch:  python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-
 For every size (1 KB .. --max-mb, x4 steps) and dtype it verifies the result against
 ``torch.distributed.all_reduce`` (NCCL) on identical inputs, then times both with CUDA events
 (max over ranks) and reports bus bandwidth ``bytes * 2(N-1)/N / t`` (BASELINE.md B3 / config 5) next to the NVLink
-roofline (900 GB/s per direction nominal, 770 GB/s measured peer copy, /opt/skills/guides/B200_PROFILING.md).  Every line
+roofline (H100 SXM NVLink 4: 450 GB/s per direction nominal).  Every line
 carries the SM clock / throttle record sampled while it was measured.  Rank 0 prints one JSON object per line.
 """
 import argparse
@@ -17,6 +17,8 @@ import sys
 
 import torch
 import torch.distributed as dist
+
+NVLINK_GBS = 450.0   # H100 SXM, NVLink 4: 18 links, 450 GB/s per direction (data sheet)
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
@@ -112,8 +114,7 @@ def main():
             row["nccl_us"] = round(ms * 1e3, 2)
             row["nccl_busbw_GBs"] = round(nbytes * 2 * (world - 1) / world / (ms * 1e-3) / 1e9, 2)
             best = max(row.get(k + "_busbw_GBs", 0.0) for k in algos)
-            row["best_frac_of_900"] = round(best / 900.0, 3)
-            row["best_frac_of_measured_770"] = round(best / 770.0, 3)
+            row["best_frac_of_nvlink"] = round(best / NVLINK_GBS, 3)
             if clocks is not None:
                 row["clocks"] = clocks.since(mark)
             if rank == 0:

@@ -2,9 +2,9 @@
 """Achieved HBM bandwidth of the memory-bound kernels at the flagship (BERT-base, 32x512 tokens) shapes.
 
 Each op is timed with CUDA events over ``--iters`` launches after warm-up; the operands of
-consecutive launches rotate over enough distinct buffers to exceed the 126 MB L2.  Prints one JSON
+consecutive launches rotate over enough distinct buffers to exceed the 50 MB L2.  Prints one JSON
 line per op: microseconds, the minimum bytes the op must move, and the resulting GB/s (compare with
-the measured copy peak in MEASURED_PEAKS.json).
+the 3.35 TB/s of HBM3 in the H100 SXM data sheet).
 """
 import argparse
 import json

@@ -14,7 +14,7 @@ ranks, "local gradients are ready" -> "new 16-bit parameters on every rank, grad
           reduce-scatter, norm exchange, clip, Adam on the 1/N shard, parameter all-gather by multimem.st)  (b200 default)
 
 and checks that the three leave the same 16-bit parameters behind.  Each line carries the roofline
-max(36 B/param / measured HBM copy rate, gradient bytes / 900 GB/s) and the SM clock record.  Rank 0 prints one JSON
+max(36 B/param / HBM peak, gradient bytes / 450 GB/s per direction of H100 NVLink 4) and the SM clock record.  Rank 0 prints one JSON
 object per size.
 """
 import argparse
@@ -140,7 +140,7 @@ def main():
         d = torch.tensor([diff], device="cuda")
         dist.all_reduce(d, op=dist.ReduceOp.MAX)
         if rank == 0:
-            roof_ms = max(n * 36 / (hbm * 1e9), (mb << 20) / 900e9) * 1e3
+            roof_ms = max(n * 36 / (hbm * 1e9), (mb << 20) / 450e9) * 1e3
             net = {k: max(v - copy_ms, 1e-6) for k, v in results.items()}
             print(json.dumps({
                 "grad_mb": mb, "params": n, "world": world, "dtype": args.dtype, "buckets": len(buckets),

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Per-op comparison (BASELINE.md B4): our sm_100a kernels vs the reference's own CUDA extensions rebuilt for
-sm_100 (``baseline/_ref_ext``, see ``baseline/build_ref_ext.sh``) vs PyTorch natives - same shapes, same script.
+"""Per-op comparison (BASELINE.md B4): our sm_90a kernels vs the reference's own CUDA extensions built for
+sm_90 (``baseline/_ref_ext``, see ``baseline/build_ref_ext.sh``) vs PyTorch natives - same shapes, same script.
 
     python bench/op_compare.py --impl ours      >  gpurun_out/op_ours.jsonl
     python bench/op_compare.py --impl reference >  gpurun_out/op_ref.jsonl     # imports baseline/_ref + _ref_ext ONLY
@@ -9,10 +9,10 @@ sm_100 (``baseline/_ref_ext``, see ``baseline/build_ref_ext.sh``) vs PyTorch nat
 
 Both frameworks expose the same public API (``unicore.modules.LayerNorm`` / ``RMSNorm`` / ``softmax_dropout``,
 ``unicore.optim.fused_adam``, ``unicore.utils.multi_tensor_total_norm`` / ``fp32_to_bf16_sr``), so each arm is the same
-code with a different ``sys.path``.  Every measurement: the op on rotating operands (working set > the 126 MB L2)
+code with a different ``sys.path``.  Every measurement: the op on rotating operands (working set > the 50 MB L2)
 captured ONCE in a CUDA graph (so neither arm pays Python / allocator time), replayed after warm-up, timed with CUDA
 events.  forward is timed under ``no_grad``; backward = (forward + backward) - forward.  One JSON line per op with the
-minimum bytes the op has to move, GB/s, the fraction of the measured copy peak (MEASURED_PEAKS.json) and the SM clock /
+minimum bytes the op has to move, GB/s, the fraction of the HBM peak (MEASURED_PEAKS.json if present, else the H100 data sheet) and the SM clock /
 throttle record sampled while it ran.
 """
 import argparse
@@ -31,7 +31,7 @@ def peaks():
         with open(os.path.join(REPO, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"])
     except Exception:  # noqa: BLE001
-        return 6650.0  # profiling recipe fallback
+        return 3350.0  # H100 SXM data sheet: 3.35 TB/s of HBM3
 
 
 class Clocks:
@@ -159,7 +159,7 @@ def main():
 
     def report(name, us, nbytes, graph, mark, note=None):
         rec = {"op": name, "impl": a.impl, "us": round(us, 2), "MB": round(nbytes / 1e6, 2),
-               "GBps": round(nbytes / us / 1e3, 1), "frac_of_measured_hbm": round(nbytes / us / 1e3 / hbm, 3),
+               "GBps": round(nbytes / us / 1e3, 1), "frac_of_hbm_peak": round(nbytes / us / 1e3 / hbm, 3),
                "graph": graph, "clocks": clocks.since(mark), "native_so": loaded}
         if note:
             rec["note"] = note
@@ -377,12 +377,12 @@ def merge(paths):
                 continue
             r = json.loads(line)
             rows.setdefault(r["op"], {})[r["impl"]] = r
-    print("| op | ours us (GB/s, % of copy peak) | reference ext (sm_100 rebuild) us | torch native us | ours / reference |")
+    print("| op | ours us (GB/s, % of copy peak) | reference ext (sm_90 build) us | torch native us | ours / reference |")
     print("|---|---|---|---|---|")
     for op, by in rows.items():
         def cell(k):
             r = by.get(k)
-            return "-" if r is None else "%.1f (%.0f, %.0f %%)" % (r["us"], r["GBps"], 100 * r["frac_of_measured_hbm"])
+            return "-" if r is None else "%.1f (%.0f, %.0f %%)" % (r["us"], r["GBps"], 100 * r["frac_of_hbm_peak"])
         ratio = "-"
         if "ours" in by and "reference" in by:
             ratio = "%.2fx" % (by["reference"]["us"] / by["ours"]["us"])

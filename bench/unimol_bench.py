@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Uni-Mol (SE(3)-invariant molecular transformer) pre-training step benchmark — BASELINE.json config
-"Uni-Mol SE(3) Transformer bf16 on 8xB200 (softmax_dropout + LayerNorm hot path)".
+"Uni-Mol SE(3) Transformer bf16 on 8 GPUs (softmax_dropout + LayerNorm hot path)".
 
 Drives ``examples/unimol`` (arch ``unimol_base``: 15 layers, 512 dim, 64 heads, pair-bias attention, masked
 atom-type / coordinate / distance heads) through the public ``Trainer.train_step`` on synthetic molecules
@@ -28,7 +28,7 @@ def main():
     ap.add_argument("--ddp-backend", default=None)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"],
                     help="reference: the unmodified reference framework from baseline/_ref (BASELINE.md B6)")
-    ap.add_argument("--ref-ext", action="store_true", help="reference arm: with its own CUDA extensions (sm_100 rebuild)")
+    ap.add_argument("--ref-ext", action="store_true", help="reference arm: with its own CUDA extensions (sm_90 build)")
     ap.add_argument("--portable", action="store_true",
                     help="use examples/unimol_portable (public Uni-Core API only; the plug-in both frameworks can load) "
                          "instead of this framework's optimised examples/unimol; implied by --impl reference")

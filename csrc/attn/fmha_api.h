@@ -1,10 +1,14 @@
-// Host launchers of the tcgen05 fused attention kernels (csrc/attn/fmha_*_sm100.cu).
+// Host launchers of the wgmma fused attention kernels (csrc/attn/fmha_*_sm90.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 namespace ub {
+
+// rows of the TMA boxes of q / k / v (and dO): the forward walks 128-key tiles with 64 query rows per CTA, the
+// backward walks 64-row query tiles with 64 keys per CTA
+constexpr int kFwdQBoxRows = 64, kFwdKVBoxRows = 128, kBwdBoxRows = 64;
 
 struct FmhaFwdParams {
   const void* q;   // [B, Lq, H, 64] via strides (elements)
@@ -14,42 +18,35 @@ struct FmhaFwdParams {
   float* lse;      // [B, H, Lq]
   const void* bias;        // [bias_batch (1 or B), H, Lq, Lk] contiguous, same 16-bit type as q; may be null
   const uint8_t* kpm;      // [B, Lk] bool, nonzero = masked; may be null
-  uint32_t* drop_bits;     // [B, H, Lq, ceil(Lk/32)] dropout keep bits (written by fwd, read by bwd); null if p == 0
+  // [B, H, Lq, ceil(Lk/32)] dropout keep bits (written by fwd, read by bwd); null if p == 0.  Word w of a row holds
+  // keys 32w .. 32w + 31: key 32w + 2i in bit i, key 32w + 2i + 1 in bit 16 + i.
+  uint32_t* drop_bits;
   long long q_sb, q_sl, q_sh, k_sb, k_sl, k_sh, v_sb, v_sl, v_sh;
   int B, H, Lq, Lk;
   int bias_batch, bias_is_f32, is_bf16;
   float scale, p_drop;
   unsigned long long seed, offset;
-  long long* trace;        // profiling only: per-phase clock64() stamps of CTA (0,0,0), thread 0; usually null
-  // TMA descriptors (csrc/attn/tma_map.h), 128-byte swizzle: 128 x 64 tiles of q / k / v, 128 x 64 half tiles of the bias
+  // TMA descriptors (csrc/attn/tma_map.h), 128-byte swizzle: row tiles of q / k / v, 64 x 64 tiles of the bias
   CUtensorMap sw_q, sw_k, sw_v, sw_bias;
 };
-// One-role kernel (fmha_fwd_sm100.cu, two CTAs per SM) by default; UNICORE_B200_FMHA_FWD=ws selects the warp-specialised
-// kernel (fmha_fwd_ws_sm100.cu: TMA warp + MMA warp + two softmax groups on two query tiles).
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
-bool fmha_fwd_ws_supported(const FmhaFwdParams& p);
-void launch_fmha_fwd_ws(const FmhaFwdParams& p, cudaStream_t stream);
 
 struct FmhaBwdParams {
   FmhaFwdParams f;   // same inputs as forward (out/lse hold the forward results)
   const void* dout;  // [B, Lq, H, 64] contiguous
   float* delta;      // [B, H, Lq] scratch: rowsum(dO * O)
-  void* dq_part;     // [ceil(Lk / 128), B, Lq, H, 64] 16-bit: per-key-tile partial dQ (plain stores; fp32 atomics on one
-                     // accumulator cost ~4000 cycles per tile), summed by the finishing kernel
+  float* dq_acc;     // [B, H, ceil(Lq / 64) * 64, 64] fp32, zeroed: every key tile adds its dQ share with bulk reductions
   void* dq;          // [B, Lq, H, 64] 16-bit results, addressed through (batch, seq, head) element strides so
   void* dk;          // that they can be slices of one packed [B, L, 3, H, 64] gradient tensor
   void* dv;
   long long dq_sb, dq_sl, dq_sh, dk_sb, dk_sl, dk_sh, dv_sb, dv_sl, dv_sh;
-  // Bias gradient: every CTA stores its 16-bit dS tile (already in shared memory for the MMAs) with ONE TMA
+  // Bias gradient: every CTA stores its 16-bit dS tile (already in shared memory for the dQ product) with one TMA
   // store into ds_buf [B, H, Lq, Lk]; a follow-up kernel sums it over the batch into dbias (fp32 accumulate)
-  // when the bias is shared by the batch.  (fp32 atomics on a shared dbias tensor were the bottleneck of the
-  // kernel: 4096 red.v4 per tile.)  Both null when the bias needs no gradient.
+  // when the bias is shared by the batch.  Both null when the bias needs no gradient.
   void* ds_buf;      // [B, H, Lq, Lk] 16-bit
   void* dbias;       // [bias_batch, H, Lq, Lk] 16-bit; == ds_buf when bias_batch == B
-  CUtensorMap sw_ds;   // 128-byte-swizzled map of ds_buf (two 64-column boxes per tile)
-  int debug_flags;   // profiling only: 1 = skip dBias reductions, 2 = skip dQ reductions, 4 = skip exp/dS math
-  long long* trace;  // profiling only: clock64() stamps of one CTA (see UB_BTRACE); usually null
-  CUtensorMap sw_do;  // 128 x 64 tiles of dO (128-byte swizzle)
+  CUtensorMap sw_ds;   // 128-byte-swizzled map of ds_buf (64 x 64 boxes)
+  CUtensorMap sw_do;   // 64 x 64 tiles of dO (128-byte swizzle)
 };
 void launch_fmha_bwd(const FmhaBwdParams& p, cudaStream_t stream);
 

@@ -26,7 +26,7 @@ std::pair<uint64_t, uint64_t> reserve_philox(uint64_t increment) {
 }
 
 void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const Tensor& v, const OptTensor& bias,
-                 const OptTensor& kpm, double p_drop, double scale) {
+                 const OptTensor& kpm, double p_drop, double scale, int q_box_rows, int kv_box_rows) {
   TORCH_CHECK(q.is_cuda() && k.is_cuda() && v.is_cuda());
   TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, "q/k/v must be [B, L, H, D]");
   TORCH_CHECK(q.size(3) == 64 && k.size(3) == 64 && v.size(3) == 64, "head_dim must be 64");
@@ -79,9 +79,9 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   // TMA descriptors: heads must be contiguous (stride 64) so that (head, 16-byte chunk) is one dimension
   TORCH_CHECK(q.stride(2) == 64 && k.stride(2) == 64 && v.stride(2) == 64, "q/k/v head stride must be 64");
   const bool bf16 = p.is_bf16 != 0;
-  bool ok = ub::make_head_tile_map_sw128(&p.sw_q, p.q, bf16, p.B, p.Lq, p.H, p.q_sb, p.q_sl, p.q_sh, 128);
-  ok = ok && ub::make_head_tile_map_sw128(&p.sw_k, p.k, bf16, p.B, p.Lk, p.H, p.k_sb, p.k_sl, p.k_sh, 128);
-  ok = ok && ub::make_head_tile_map_sw128(&p.sw_v, p.v, bf16, p.B, p.Lk, p.H, p.v_sb, p.v_sl, p.v_sh, 128);
+  bool ok = ub::make_head_tile_map_sw128(&p.sw_q, p.q, bf16, p.B, p.Lq, p.H, p.q_sb, p.q_sl, p.q_sh, q_box_rows);
+  ok = ok && ub::make_head_tile_map_sw128(&p.sw_k, p.k, bf16, p.B, p.Lk, p.H, p.k_sb, p.k_sl, p.k_sh, kv_box_rows);
+  ok = ok && ub::make_head_tile_map_sw128(&p.sw_v, p.v, bf16, p.B, p.Lk, p.H, p.v_sb, p.v_sl, p.v_sh, kv_box_rows);
   if (p.bias != nullptr) ok = ok && ub::make_bias_tile_map_sw128(&p.sw_bias, p.bias, bf16, p.bias_batch * p.H, p.Lq, p.Lk);
   TORCH_CHECK(ok, "cuTensorMapEncodeTiled failed for the attention operands");
 }
@@ -91,7 +91,7 @@ std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k,
                                                       double scale) {
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaFwdParams p{};
-  fill_common(p, q, k, v, bias, kpm, p_drop, scale);
+  fill_common(p, q, k, v, bias, kpm, p_drop, scale, ub::kFwdQBoxRows, ub::kFwdKVBoxRows);
   Tensor out = torch::empty({p.B, p.Lq, p.H, 64}, q.options());
   Tensor lse = torch::empty({p.B, p.H, p.Lq}, q.options().dtype(at::kFloat));
   p.out = out.data_ptr();
@@ -106,26 +106,7 @@ std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k,
     bits = torch::empty({p.B, p.H, p.Lq, (p.Lk + 31) / 32}, q.options().dtype(at::kInt));
     p.drop_bits = reinterpret_cast<uint32_t*>(bits->data_ptr());
   }
-  Tensor trace;
-  p.trace = nullptr;
-  if (std::getenv("UNICORE_FMHA_TRACE") != nullptr) {
-    trace = torch::zeros({64, 12}, q.options().dtype(at::kLong));
-    p.trace = reinterpret_cast<long long*>(trace.data_ptr<int64_t>());
-  }
   ub::launch_fmha_fwd(p, at::cuda::getCurrentCUDAStream().stream());
-  if (p.trace != nullptr) {
-    Tensor host = trace.cpu();
-    auto acc = host.accessor<int64_t, 2>();
-    const int tiles = (p.Lk + 127) / 128;
-    for (int j = 0; j < tiles && j < 64; ++j) {
-      printf("fmha_fwd trace tile %d:", j);
-      for (int sidx = 1; sidx < 12; ++sidx) printf(" %lld", (long long)(acc[j][sidx] - acc[j][sidx - 1]));
-      if (j > 0) printf("  | since prev tile start %lld", (long long)(acc[j][0] - acc[j - 1][0]));
-      printf("\n   abs:");
-      for (int sidx = 0; sidx < 12; ++sidx) printf(" %lld", (long long)(acc[j][sidx] - acc[0][0]));
-      printf("\n");
-    }
-  }
   cudaError_t err = cudaGetLastError();
   TORCH_CHECK(err == cudaSuccess, "fmha_fwd launch failed: ", cudaGetErrorString(err));
   return {out, lse, bits};
@@ -141,7 +122,7 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   // spares autograd three zero-filled select-backward tensors and two full-size adds per layer.
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaBwdParams p{};
-  fill_common(p.f, q, k, v, bias, kpm, p_drop, scale);
+  fill_common(p.f, q, k, v, bias, kpm, p_drop, scale, ub::kBwdBoxRows, ub::kBwdBoxRows);
   TORCH_CHECK(dout.is_contiguous() && out.is_contiguous() && lse.is_contiguous());
   p.f.out = out.data_ptr();
   p.f.lse = lse.data_ptr<float>();
@@ -151,14 +132,11 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   }
   p.dout = dout.data_ptr();
   TORCH_CHECK(ub::make_head_tile_map_sw128(&p.sw_do, p.dout, p.f.is_bf16 != 0, p.f.B, p.f.Lq, p.f.H,
-                                           (long long)p.f.Lq * p.f.H * 64, (long long)p.f.H * 64, 64, 128),
+                                           (long long)p.f.Lq * p.f.H * 64, (long long)p.f.H * 64, 64, ub::kBwdBoxRows),
               "cuTensorMapEncodeTiled failed for dO");
-  {
-    const char* dbg = std::getenv("UNICORE_FMHA_DEBUG");
-    p.debug_flags = dbg ? std::atoi(dbg) : 0;
-  }
   Tensor delta = torch::empty({p.f.B, p.f.H, p.f.Lq}, q.options().dtype(at::kFloat));
-  Tensor dq_part = torch::empty({(p.f.Lk + 127) / 128, p.f.B, p.f.H, (p.f.Lq + 127) / 128 * 128, 64}, q.options());
+  // zeroed by the launcher; padded to whole 64-row query tiles
+  Tensor dq_acc = torch::empty({p.f.B, p.f.H, (p.f.Lq + 63) / 64 * 64, 64}, q.options().dtype(at::kFloat));
   Tensor dq, dk, dv;
   if (packed_grad) {
     TORCH_CHECK(p.f.Lq == p.f.Lk, "packed gradients need self-attention shapes");
@@ -187,31 +165,11 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
                 "cuTensorMapEncodeTiled failed for the dS scratch tensor");
   }
   p.delta = delta.data_ptr<float>();
-  p.dq_part = dq_part.data_ptr();
+  p.dq_acc = dq_acc.data_ptr<float>();
   p.dq = dq.data_ptr();
   p.dk = dk.data_ptr();
   p.dv = dv.data_ptr();
-  TORCH_CHECK((reinterpret_cast<uintptr_t>(p.dk) & 31) == 0 && (reinterpret_cast<uintptr_t>(p.dv) & 31) == 0 &&
-                  (reinterpret_cast<uintptr_t>(p.dq_part) & 31) == 0,
-              "fmha_bwd outputs must be 32-byte aligned (256-bit stores)");
-  Tensor btrace;
-  p.trace = nullptr;
-  if (std::getenv("UNICORE_FMHA_TRACE") != nullptr) {
-    btrace = torch::zeros({64, 12}, q.options().dtype(at::kLong));
-    p.trace = reinterpret_cast<long long*>(btrace.data_ptr<int64_t>());
-  }
   ub::launch_fmha_bwd(p, at::cuda::getCurrentCUDAStream().stream());
-  if (p.trace != nullptr) {
-    Tensor host = btrace.cpu();
-    auto acc = host.accessor<int64_t, 2>();
-    const int tiles = (p.f.Lq + 127) / 128;
-    for (int j = 0; j < tiles && j < 64; ++j) {
-      printf("fmha_bwd trace tile %d:", j);
-      for (int sidx = 1; sidx < 10; ++sidx) printf(" %lld", (long long)(acc[j][sidx] - acc[j][sidx - 1]));
-      if (j > 0) printf("  | since prev tile start %lld", (long long)(acc[j][0] - acc[j - 1][0]));
-      printf("\n");
-    }
-  }
   cudaError_t err = cudaGetLastError();
   TORCH_CHECK(err == cudaSuccess, "fmha_bwd launch failed: ", cudaGetErrorString(err));
   return {dq, dk, dv, dbias};

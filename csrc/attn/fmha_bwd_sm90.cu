@@ -1,0 +1,392 @@
+// Fused multi-head attention backward for sm_90a (head_dim 64, fp16/bf16), flash-attention style
+// (reference: autograd through unicore/modules/multihead_attention.py:47-113 + softmax_fast.h:513-666):
+// probabilities are recomputed from the saved log-sum-exp; the dropout keep bits come from the
+// forward pass (1 bit / element).
+//
+//   grid = (64-key tiles, H, B); one CTA = one warpgroup owns K_j, V_j and walks the 64-row query tiles i.  The
+//   products are computed transposed (keys are the M dimension), so that P^T and dS^T are accumulator tiles whose
+//   16-bit conversions are directly the register A operands of the dV / dK products:
+//     S^T  = K_j Q_i^T                      wgmma m64n64, both operands K-major from shared memory
+//     dP^T = V_j dO_i^T                     wgmma m64n64
+//     P = exp2((S*scale + bias + kmask) * log2e - LSE_i * log2e) ;  dS = P o (drop(dP) - delta_i)
+//     dV_j += drop(P)^T dO_i                wgmma, A from registers, dO MN-major
+//     dK_j += dS^T Q_i                      wgmma, A from registers, Q MN-major
+//     dQ_i += dS K_j                        wgmma, dS from shared memory (stmatrix.trans of the registers, written in
+//                                           place over the consumed bias tile), K MN-major; the fp32 tile is added to
+//                                           a global fp32 accumulator with ONE bulk reduction (cp.reduce.async.bulk)
+//     dS tile (16-bit, in shared memory for the dQ product) -> TMA store; a follow-up kernel sums it over the batch
+//     into dBias.
+//   Q_i, dO_i and the bias tile are fetched one query tile ahead (two stages), one thread issues every copy.
+// Pre-pass: delta = rowsum(dO o O).   Post-pass: dq = scale * the fp32 accumulator (and dbias = batch sum of dS).
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <math_constants.h>
+
+#include <algorithm>
+
+#include "../common.cuh"
+#include "fmha_api.h"
+#include "wgmma.cuh"
+
+namespace ub {
+namespace {
+
+using namespace tc;
+
+constexpr int kBM = 64, kBN = 64, kD = 64;   // query rows per step, keys per CTA, head dim
+constexpr int kBwdThreads = 128;
+
+// shared memory map (bytes); every operand tile is 64 rows x 128 B, 128-byte swizzled
+constexpr uint32_t kOffK = 0;
+constexpr uint32_t kOffV = 8192;
+constexpr uint32_t kOffQ = 16384;      // 2 stages x 8 KB
+constexpr uint32_t kOffDO = 32768;     // 2 stages x 8 KB
+constexpr uint32_t kOffDS = 49152;     // 2 stages x 8 KB: bias tile [q][key], then dS in place
+constexpr uint32_t kOffDQ = 65536;     // fp32 [64][64] dQ tile, row-major (the layout of the global accumulator)
+constexpr uint32_t kOffStats = 81920;  // 2 stages x {float lse2[64], float delta[64], uint32 bits[64][2]}
+constexpr uint32_t kOffBar = kOffStats + 2048;
+constexpr uint32_t kBwdSmemBytes = kOffBar + 32 + 1024;   // + alignment slack of the 1024-byte-aligned base
+
+template <typename T>
+UB_DEVICE uint32_t bwd_pack2(float a, float b);
+template <>
+UB_DEVICE uint32_t bwd_pack2<__half>(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+template <>
+UB_DEVICE uint32_t bwd_pack2<__nv_bfloat16>(float a, float b) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+template <typename T>
+UB_DEVICE float2 bwd_unpack2(uint32_t w) {
+  if constexpr (std::is_same<T, __half>::value) {
+    return __half22float2(*reinterpret_cast<const __half2*>(&w));
+  } else {
+    return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
+  }
+}
+
+// ---- pre-pass: delta[b,h,q] = sum_d dO * O -----------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(256) fmha_delta_kernel(const T* __restrict__ dout, const T* __restrict__ out,
+                                                           float* __restrict__ delta, int B, int H, int Lq) {
+  // 8 threads per (b, q, h) row of 64 elements
+  const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long long rowi = gid >> 3;
+  const int part = (int)(gid & 7);
+  const long long nrows = (long long)B * Lq * H;
+  float acc = 0.f;
+  if (rowi < nrows) {
+    float a[8], o[8];
+    unpack<T>(ld_global_nc_v4(dout + rowi * 64 + part * 8), a);
+    unpack<T>(ld_global_nc_v4(out + rowi * 64 + part * 8), o);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) acc += a[e] * o[e];
+  }
+  acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+  acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+  acc += __shfl_xor_sync(0xffffffffu, acc, 4);
+  if (rowi < nrows && part == 0) {
+    const long long hq = rowi % ((long long)Lq * H);
+    const long long b = rowi / ((long long)Lq * H);
+    const int q = (int)(hq / H), h = (int)(hq % H);
+    delta[(b * H + h) * Lq + q] = acc;
+  }
+}
+
+// ---- post-pass: dq = scale * fp32 accumulator, written through (batch, seq, head) strides -------------------------
+template <typename T>
+__global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __restrict__ acc, T* __restrict__ out, int H,
+                                                                int Lq, int Lq_pad, long long nvec, float scale, long long sb,
+                                                                long long sl, long long sh) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
+    // v enumerates [b][h][q][8 groups of 8 columns]
+    const int part = (int)(v & 7);
+    const long long row = v >> 3;
+    const int q = (int)(row % Lq);
+    const long long bh = row / Lq;
+    const int h = (int)(bh % H);
+    const long long b = bh / H;
+    const float4* src = reinterpret_cast<const float4*>(acc + ((bh * Lq_pad + q) * 64 + part * 8));
+    const float4 x0 = src[0], x1 = src[1];
+    const float x[8] = {x0.x * scale, x0.y * scale, x0.z * scale, x0.w * scale,
+                        x1.x * scale, x1.y * scale, x1.z * scale, x1.w * scale};
+    st_global_v4(out + b * sb + (long long)q * sl + (long long)h * sh + part * 8, pack<T>(x));
+  }
+}
+
+// ---- main kernel ----------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(kBwdThreads, 2) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_base = smem_u32(smem_raw);
+  const uint32_t smem_base = (raw_base + 1023u) & ~1023u;   // 128-byte swizzle: tiles must be 1024-byte aligned
+  uint8_t* smem = smem_raw + (smem_base - raw_base);
+  const FmhaFwdParams& p = bp.f;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, c = lane & 3;
+  const int key0 = blockIdx.x * kBN, h = blockIdx.y, b = blockIdx.z;
+  const uint32_t bar_kv = smem_base + kOffBar, bar_in0 = smem_base + kOffBar + 8;   // + 8 * stage
+  const bool has_bias = p.bias != nullptr;
+  const bool drop = p.p_drop > 0.f && p.drop_bits != nullptr;
+  const int n_qtiles = (p.Lq + kBM - 1) / kBM;
+  const int Lq_pad = n_qtiles * kBM;
+  const long long bh = (long long)b * p.H + h;
+  const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
+  const int words_per_row = (p.Lk + 31) / 32;
+  constexpr uint32_t kTileBytes = kBM * kD * 2;
+
+  auto load_tile = [&](int i) {   // one thread: Q_i, dO_i (and the bias tile) -> stage i & 1
+    const uint32_t st = (uint32_t)(i & 1), bar = bar_in0 + 8u * st;
+    mbar_expect_tx(bar, 2 * kTileBytes + (has_bias ? kTileBytes : 0u));
+    tma_load_4d(smem_base + kOffQ + st * 8192, &p.sw_q, 0, h, i * kBM, b, bar);
+    tma_load_4d(smem_base + kOffDO + st * 8192, &bp.sw_do, 0, h, i * kBM, b, bar);
+    if (has_bias) tma_load_3d(smem_base + kOffDS + st * 8192, &p.sw_bias, key0, i * kBM, bias_nb, bar);
+  };
+  auto load_stats = [&](int i) {  // all threads: LSE (log2 units, +inf = row contributes nothing), delta, keep bits
+    uint8_t* s = smem + kOffStats + (i & 1) * 1024;
+    const int q = i * kBM + (tid & 63);
+    const bool ok = q < p.Lq;
+    if (tid < 64) {
+      const float lse = ok ? p.lse[bh * p.Lq + q] : -CUDART_INF_F;
+      reinterpret_cast<float*>(s)[tid] = lse == -CUDART_INF_F ? CUDART_INF_F : lse * 1.4426950408889634f;
+    } else {
+      reinterpret_cast<float*>(s + 256)[tid - 64] = ok ? bp.delta[bh * p.Lq + q] : 0.f;
+    }
+    if (drop) {
+      const int qb = i * kBM + (tid >> 1), wi = (key0 >> 5) + (tid & 1);
+      reinterpret_cast<uint32_t*>(s + 512)[tid] =
+          (qb < p.Lq && wi < words_per_row) ? p.drop_bits[(bh * p.Lq + qb) * words_per_row + wi] : 0xffffffffu;
+    }
+  };
+
+  if (tid == 0) {
+    mbar_init(bar_kv, 1);
+    mbar_init(bar_in0, 1);
+    mbar_init(bar_in0 + 8, 1);
+    fence_mbarrier_init();
+    mbar_expect_tx(bar_kv, 2 * kTileBytes);
+    tma_load_4d(smem_base + kOffK, &p.sw_k, 0, h, key0, b, bar_kv);
+    tma_load_4d(smem_base + kOffV, &p.sw_v, 0, h, key0, b, bar_kv);
+    load_tile(0);
+  }
+  load_stats(0);
+
+  // my two keys (accumulator rows) and their additive masks
+  const int kl0 = warp * 16 + g, kl1 = kl0 + 8;
+  const int kr0 = key0 + kl0, kr1 = key0 + kl1;
+  const float kadd0 = (kr0 >= p.Lk || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr0] != 0)) ? -CUDART_INF_F : 0.f;
+  const float kadd1 = (kr1 >= p.Lk || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr1] != 0)) ? -CUDART_INF_F : 0.f;
+  // keep-bit positions of my keys inside their 32-key word (word (warp >> 1) of the tile's two)
+  const int kk0 = 16 * (warp & 1) + g, kk1 = kk0 + 8;
+  const int bit0 = (kk0 & 1) * 16 + (kk0 >> 1), bit1 = (kk1 & 1) * 16 + (kk1 >> 1);
+  const int kword = warp >> 1;
+
+  const float keep_scale = p.p_drop > 0.f ? dropout_keep_scale14(dropout_thresh14(p.p_drop)) : 1.f;
+  constexpr float kLog2e = 1.4426950408889634f;
+  // lane -> address of its row for ldmatrix / stmatrix (.trans) of a 16-query x 16-key block of the [q][key] tile
+  const int lm = lane >> 3, lj = lane & 7;
+  const int ld_q = (lm >> 1) * 8 + lj, ld_chunk = 2 * warp + (lm & 1);
+
+  float dv[32], dk[32];
+#pragma unroll
+  for (int e = 0; e < 32; ++e) {
+    dv[e] = 0.f;
+    dk[e] = 0.f;
+  }
+  __syncthreads();   // barriers initialised, stats of tile 0 in shared memory
+  mbar_wait(bar_kv, 0);
+
+  for (int i = 0; i < n_qtiles; ++i) {
+    const uint32_t st = (uint32_t)(i & 1);
+    __syncthreads();   // (A) tile i-1 is finished by every thread: its stage, stats and dQ staging may be reused
+    if (tid == 0) {
+      bulk_wait_read();   // the dS store and the dQ reduction of tile i-1 have read shared memory
+      if (i + 1 < n_qtiles) load_tile(i + 1);
+    }
+    if (i + 1 < n_qtiles) load_stats(i + 1);
+    mbar_wait(bar_in0 + 8u * st, (uint32_t)((i >> 1) & 1));
+
+    const uint32_t sQ = smem_base + kOffQ + st * 8192, sDO = smem_base + kOffDO + st * 8192;
+    const uint32_t sDS = smem_base + kOffDS + st * 8192;
+    float s[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kD / 16; ++kk)
+      wgmma_m64n64_ss<T, 0>(s, make_desc_sw128(smem_base + kOffK + kk * 32), make_desc_sw128(sQ + kk * 32), kk > 0 ? 1u : 0u);
+#pragma unroll
+    for (int kk = 0; kk < kD / 16; ++kk)
+      wgmma_m64n64_ss<T, 0>(dp, make_desc_sw128(smem_base + kOffV + kk * 32), make_desc_sw128(sDO + kk * 32), kk > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_operands(s);
+    fence_operands(dp);
+
+    // ---- P^T, dS^T in registers ---------------------------------------------------------------------------------
+    const uint8_t* stats = smem + kOffStats + st * 1024;
+    const float* lse2_s = reinterpret_cast<const float*>(stats);
+    const float* delta_s = reinterpret_cast<const float*>(stats + 256);
+    const uint32_t* bits_s = reinterpret_cast<const uint32_t*>(stats + 512);
+    uint32_t pa[4][4], da[4][4];   // [16-query block][A-operand register] of drop(P)^T and dS^T
+#pragma unroll
+    for (int sb = 0; sb < 4; ++sb) {
+      uint32_t bias_r[4] = {0u, 0u, 0u, 0u};
+      const uint32_t addr = sDS + sw128_off(16 * sb + ld_q, ld_chunk);
+      if (has_bias) ldmatrix_x4_trans(addr, bias_r);
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {   // r: rows (key kl0 or kl1) x query half (16sb + 2c or 16sb + 8 + 2c)
+        const int e = 8 * sb + 2 * r;
+        const bool hi_key = (r & 1) != 0;
+        const int ql = 16 * sb + 8 * (r >> 1) + 2 * c;
+        const float2 bb = has_bias ? bwd_unpack2<T>(bias_r[r]) : make_float2(0.f, 0.f);
+        const float ka = hi_key ? kadd1 : kadd0;
+        const float2 l2 = *reinterpret_cast<const float2*>(lse2_s + ql);
+        const float2 dl = *reinterpret_cast<const float2*>(delta_s + ql);
+        const float x0 = fmaf(s[e], p.scale, bb.x + ka), x1 = fmaf(s[e + 1], p.scale, bb.y + ka);
+        const float p0 = ex2_approx(fmaf(x0, kLog2e, -l2.x)), p1 = ex2_approx(fmaf(x1, kLog2e, -l2.y));
+        bool k0 = true, k1 = true;
+        if (drop) {
+          const int bit = hi_key ? bit1 : bit0;
+          k0 = (bits_s[ql * 2 + kword] >> bit) & 1u;
+          k1 = (bits_s[(ql + 1) * 2 + kword] >> bit) & 1u;
+        }
+        const float ds0 = p0 * (dp[e] * (k0 ? keep_scale : 0.f) - dl.x);
+        const float ds1 = p1 * (dp[e + 1] * (k1 ? keep_scale : 0.f) - dl.y);
+        pa[sb][r] = bwd_pack2<T>(k0 ? p0 : 0.f, k1 ? p1 : 0.f);   // keep_scale is applied to dV in the epilogue
+        da[sb][r] = bwd_pack2<T>(ds0, ds1);                         // the softmax scale to dQ / dK at read-out
+      }
+    }
+
+    // ---- dS -> shared memory as [q][key] (in place over the bias tile: each warp rewrites exactly what it read);
+    //      before the products below, which read the same registers asynchronously ---------------------------------
+#pragma unroll
+    for (int sb = 0; sb < 4; ++sb) stmatrix_x4_trans(sDS + sw128_off(16 * sb + ld_q, ld_chunk), da[sb]);
+    fence_proxy_async_smem();
+
+    // ---- dV += drop(P)^T dO, dK += dS^T Q ---------------------------------------------------------------------
+    wgmma_fence();
+#pragma unroll
+    for (int sb = 0; sb < 4; ++sb) wgmma_m64n64_rs<T, 1>(dv, pa[sb], make_desc_sw128(sDO + sb * 2048), 1u);
+#pragma unroll
+    for (int sb = 0; sb < 4; ++sb) wgmma_m64n64_rs<T, 1>(dk, da[sb], make_desc_sw128(sQ + sb * 2048), 1u);
+    wgmma_commit();
+    __syncthreads();   // (B) the whole dS tile is in shared memory
+
+    // ---- dQ = dS K ------------------------------------------------------------------------------------------
+    float dq[32];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kBN / 16; ++kk)
+      wgmma_m64n64_ss<T, 1>(dq, make_desc_sw128(sDS + kk * 32), make_desc_sw128(smem_base + kOffK + kk * 2048), kk > 0 ? 1u : 0u);
+    wgmma_commit();
+    if (tid == 0 && bp.ds_buf != nullptr) {   // bias gradient: the dS tile leaves through one TMA store
+      tma_store_3d(&bp.sw_ds, key0, i * kBM, (int)bh, sDS);
+      bulk_commit();
+    }
+    wgmma_wait<0>();
+    fence_operands(dv);
+    fence_operands(dk);
+    fence_operands(dq);
+    float* dq_s = reinterpret_cast<float*>(smem + kOffDQ);
+#pragma unroll
+    for (int n = 0; n < 8; ++n) {
+      *reinterpret_cast<float2*>(dq_s + kl0 * 64 + 8 * n + 2 * c) = make_float2(dq[4 * n], dq[4 * n + 1]);
+      *reinterpret_cast<float2*>(dq_s + kl1 * 64 + 8 * n + 2 * c) = make_float2(dq[4 * n + 2], dq[4 * n + 3]);
+    }
+    fence_proxy_async_smem();
+    __syncthreads();   // (C) the dQ tile is in shared memory
+    if (tid == 0) {
+      bulk_reduce_add_f32(bp.dq_acc + (bh * Lq_pad + (long long)i * kBM) * kD, smem_base + kOffDQ, kBM * kD * 4);
+      bulk_commit();
+    }
+  }
+  if (tid == 0) bulk_wait_all();   // shared memory must outlive the last store's and reduction's reads
+
+  // ---- epilogue: dK_j, dV_j (rows = my two keys) ------------------------------------------------------------------
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int key = half ? kr1 : kr0;
+    if (key >= p.Lk) continue;
+    T* dvg = reinterpret_cast<T*>(bp.dv) + (long long)b * bp.dv_sb + (long long)key * bp.dv_sl + (long long)h * bp.dv_sh;
+    T* dkg = reinterpret_cast<T*>(bp.dk) + (long long)b * bp.dk_sb + (long long)key * bp.dk_sl + (long long)h * bp.dk_sh;
+#pragma unroll
+    for (int n = 0; n < 8; ++n) {
+      const int e = 4 * n + 2 * half;
+      *reinterpret_cast<uint32_t*>(dvg + 8 * n + 2 * c) = bwd_pack2<T>(dv[e] * keep_scale, dv[e + 1] * keep_scale);
+      *reinterpret_cast<uint32_t*>(dkg + 8 * n + 2 * c) = bwd_pack2<T>(dk[e] * p.scale, dk[e + 1] * p.scale);
+    }
+  }
+}
+
+// dbias[n] = sum_b ds[b, n] (fp32 accumulate), n over H * Lq * Lk in 16-byte vectors
+template <typename T>
+__global__ void __launch_bounds__(256) fmha_dbias_reduce_kernel(const T* __restrict__ ds, T* __restrict__ dbias, int B,
+                                                                  long long nvec) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int b0 = 0; b0 < B; b0 += 4) {
+      Vec16 in[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+        if (b0 + u < B) in[u] = ld_global_nc_v4(ds + ((long long)(b0 + u) * nvec + v) * 8);
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        if (b0 + u < B) {
+          float x[8];
+          unpack<T>(in[u], x);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) acc[e] += x[e];
+        }
+      }
+    }
+    st_global_v4(dbias + v * 8, pack<T>(acc));
+  }
+}
+
+int device_sms() {
+  static int sms = [] {
+    int dev = 0, n = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    return n > 0 ? n : 132;
+  }();
+  return sms;
+}
+
+template <typename T>
+void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
+  const FmhaFwdParams& p = bp.f;
+  const long long nrows = (long long)p.B * p.Lq * p.H;
+  const int n_qt = (p.Lq + kBM - 1) / kBM;
+  cudaMemsetAsync(bp.dq_acc, 0, (size_t)p.B * p.H * n_qt * kBM * kD * sizeof(float), stream);
+  fmha_delta_kernel<T><<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
+      reinterpret_cast<const T*>(bp.dout), reinterpret_cast<const T*>(p.out), bp.delta, p.B, p.H, p.Lq);
+  dim3 grid((p.Lk + kBN - 1) / kBN, p.H, p.B);
+  auto kern = fmha_bwd_kernel<T>;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmemBytes);
+  kern<<<grid, kBwdThreads, kBwdSmemBytes, stream>>>(bp);
+  const long long cap = (long long)device_sms() * 16;
+  if (bp.ds_buf != nullptr && bp.dbias != bp.ds_buf) {
+    const long long nv = (long long)p.H * p.Lq * p.Lk / 8;
+    const long long rb = std::min((nv + 255) / 256, cap);
+    fmha_dbias_reduce_kernel<T><<<(unsigned)rb, 256, 0, stream>>>(reinterpret_cast<const T*>(bp.ds_buf),
+                                                                 reinterpret_cast<T*>(bp.dbias), p.B, nv);
+  }
+  const long long nvec = nrows * 8;
+  const long long blocks = std::min((nvec + 255) / 256, cap);
+  fmha_dq_convert_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>(bp.dq_acc, reinterpret_cast<T*>(bp.dq), p.H, p.Lq,
+                                                                  n_qt * kBM, nvec, p.scale, bp.dq_sb, bp.dq_sl, bp.dq_sh);
+}
+
+}  // namespace
+
+void launch_fmha_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
+  if (bp.f.is_bf16) run_bwd<__nv_bfloat16>(bp, stream);
+  else run_bwd<__half>(bp, stream);
+}
+
+}  // namespace ub

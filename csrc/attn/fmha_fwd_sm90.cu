@@ -1,0 +1,274 @@
+// Fused multi-head attention forward for sm_90a (head_dim 64, fp16/bf16):
+//   O = dropout(softmax(scale * Q K^T + bias + key_padding)) V        LSE = logsumexp of the logits
+// One kernel for what the reference runs as bmm -> masked_fill -> softmax_dropout -> bmm plus four transposes
+// (unicore/modules/multihead_attention.py:47-113, csrc/softmax_dropout/softmax_fast.h:207-434).
+//
+// One CTA = one warpgroup (128 threads) = one 64-row query tile of one (batch, head); it walks the 128-key tiles:
+//   1. TMA (128-byte-swizzled boxes, csrc/attn/tma_map.h): K, V and the bias tile of key tile j+1 are requested into
+//      the other of two stages while tile j is computed; one thread issues every copy, completion on an mbarrier.
+//   2. S = Q K_j^T           4 x wgmma m64n128k16, both operands K-major from shared memory, fp32 in registers
+//   3. softmax in registers: logits = S*scale + bias + key mask, row max across the 4 threads of a quad, online
+//      rescaling of O and of the row sum, Philox dropout on packed 16-bit pairs (the keep bits are stored for the
+//      backward pass), P converted in place into the register A operand of the next product
+//   4. O += P V_j            8 x wgmma m64n64k16, A (P) from registers, V presented MN-major from its row-major bytes
+//   q/k/v are read through strides straight out of the packed in_proj output; O is written as [B, Lq, H, 64] so
+//   that out_proj consumes it without a transpose.
+// 104 KB of shared memory and <= 255 registers per thread: two CTAs (8 warps) per SM, so one CTA's softmax overlaps
+// the other's tensor-core work and copies.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <math_constants.h>
+
+#include "../common.cuh"
+#include "fmha_api.h"
+#include "wgmma.cuh"
+
+namespace ub {
+namespace {
+
+using namespace tc;
+
+constexpr int kBlockM = 64;    // query rows per CTA
+constexpr int kBlockN = 128;   // keys per tile
+constexpr int kHeadDim = 64;
+constexpr int kFwdThreads = 128;
+
+constexpr uint32_t kSmemQ = 0;                       // 64 x 64 x 2   = 8 KB
+constexpr uint32_t kSmemK = 8192;                    // 2 stages x 16 KB
+constexpr uint32_t kSmemV = kSmemK + 2 * 16384;      // 2 stages x 16 KB
+constexpr uint32_t kSmemBias = kSmemV + 2 * 16384;   // 2 stages x (two 64-key boxes of 64 rows = 16 KB)
+constexpr uint32_t kSmemKAdd = kSmemBias + 2 * 16384;  // 2 stages x float[128]: 0 or -inf per key
+constexpr uint32_t kSmemBar = kSmemKAdd + 1024;
+constexpr uint32_t kFwdSmemBytes = kSmemBar + 64 + 1024;   // + alignment slack of the 1024-byte-aligned base
+
+template <typename T>
+UB_DEVICE uint32_t pack2(float a, float b);
+template <>
+UB_DEVICE uint32_t pack2<__half>(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+template <>
+UB_DEVICE uint32_t pack2<__nv_bfloat16>(float a, float b) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+template <typename T>
+UB_DEVICE float2 unpack2(uint32_t w) {
+  if constexpr (std::is_same<T, __half>::value) {
+    return __half22float2(*reinterpret_cast<const __half2*>(&w));
+  } else {
+    return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
+  }
+}
+
+UB_DEVICE uint32_t select4(const Philox4& r, int i) { return i == 0 ? r.x : (i == 1 ? r.y : (i == 2 ? r.z : r.w)); }
+
+template <typename T>
+__global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_base = smem_u32(smem_raw);
+  const uint32_t smem_base = (raw_base + 1023u) & ~1023u;   // 128-byte swizzle: tiles must be 1024-byte aligned
+  uint8_t* smem = smem_raw + (smem_base - raw_base);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, c = lane & 3;
+  const int q0 = blockIdx.x * kBlockM, h = blockIdx.y, b = blockIdx.z;
+  const uint32_t bar0 = smem_base + kSmemBar;   // bar0 + 8 * stage: K / V / bias of a key tile (+ Q on the first)
+  float* kadd = reinterpret_cast<float*>(smem + kSmemKAdd);
+
+  const bool has_bias = p.bias != nullptr;
+  const int n_tiles = (p.Lk + kBlockN - 1) / kBlockN;
+  const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
+  constexpr uint32_t kKVBytes = kBlockN * kHeadDim * 2, kBiasBytes = kBlockM * kBlockN * 2, kQBytes = kBlockM * kHeadDim * 2;
+  auto load_tile = [&](int j) {   // one thread; the first tile's phase also covers Q (one arrival per phase)
+    const uint32_t st = (uint32_t)(j & 1), bar = bar0 + 8u * st;
+    mbar_expect_tx(bar, 2 * kKVBytes + (has_bias ? kBiasBytes : 0u) + (j == 0 ? kQBytes : 0u));
+    if (j == 0) tma_load_4d(smem_base + kSmemQ, &p.sw_q, 0, h, q0, b, bar);
+    tma_load_4d(smem_base + kSmemK + st * 16384, &p.sw_k, 0, h, j * kBlockN, b, bar);
+    tma_load_4d(smem_base + kSmemV + st * 16384, &p.sw_v, 0, h, j * kBlockN, b, bar);
+    if (has_bias) {   // 64 rows x 128 keys = two 64-key boxes
+      tma_load_3d(smem_base + kSmemBias + st * 16384, &p.sw_bias, j * kBlockN, q0, bias_nb, bar);
+      tma_load_3d(smem_base + kSmemBias + st * 16384 + 8192, &p.sw_bias, j * kBlockN + 64, q0, bias_nb, bar);
+    }
+  };
+  if (tid == 0) {
+    mbar_init(bar0, 1);
+    mbar_init(bar0 + 8, 1);
+    fence_mbarrier_init();
+    load_tile(0);
+  }
+
+  const int rl0 = warp * 16 + g, rl1 = rl0 + 8;   // my two rows of the tile
+  const int row0 = q0 + rl0, row1 = q0 + rl1;
+  const uint8_t* kpm_row = p.kpm != nullptr ? p.kpm + (long long)b * p.Lk : nullptr;
+  const bool drop = p.p_drop > 0.f;
+  const uint32_t t14 = dropout_thresh14(p.p_drop);
+  const uint32_t t14x2 = t14 | (t14 << 16);
+  // the 1/(1-p) of the kept probabilities is applied once, to the normalised output row
+  const float keep_scale = drop ? dropout_keep_scale14(t14) : 1.f;
+  const unsigned long long bh = (unsigned long long)b * p.H + h;
+  const unsigned long long lin0 = bh * p.Lq + (row0 < p.Lq ? row0 : 0), lin1 = bh * p.Lq + (row1 < p.Lq ? row1 : 0);
+  const int words_per_row = (p.Lk + 31) / 32;
+
+  constexpr float kLog2e = 1.4426950408889634f;
+  float m0 = -CUDART_INF_F, m1 = -CUDART_INF_F, l0 = 0.f, l1 = 0.f;   // running max (in use) and partial row sums
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+
+  for (int j = 0; j < n_tiles; ++j) {
+    const uint32_t st = (uint32_t)(j & 1);
+    const int key0 = j * kBlockN;
+    bool masked = false;
+    {
+      const int key = key0 + tid;
+      masked = key >= p.Lk || (kpm_row != nullptr && kpm_row[key] != 0);
+      kadd[st * 128 + tid] = masked ? -CUDART_INF_F : 0.f;
+    }
+    // barrier: every thread is done with tile j-1, so its stage may be refilled with tile j+1
+    const bool tile_masked = __syncthreads_or(masked) != 0;
+    if (tid == 0 && j + 1 < n_tiles) load_tile(j + 1);
+    mbar_wait(bar0 + 8u * st, (uint32_t)((j >> 1) & 1));
+
+    // ---- S = Q K^T --------------------------------------------------------------------------------------
+    float s[64];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kHeadDim / 16; ++kk)
+      wgmma_m64n128_ss<T, 0>(s, make_desc_sw128(smem_base + kSmemQ + kk * 32),
+                             make_desc_sw128(smem_base + kSmemK + st * 16384 + kk * 32), kk > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_operands(s);
+
+    // ---- logits, row max ----------------------------------------------------------------------------------
+    float mx0 = -CUDART_INF_F, mx1 = -CUDART_INF_F;
+    const uint8_t* bias_tile = smem + kSmemBias + st * 16384;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const int col = 8 * i + 2 * c;
+      float2 b0 = make_float2(0.f, 0.f), b1 = make_float2(0.f, 0.f);
+      if (has_bias) {
+        const uint8_t* box = bias_tile + (i >> 3) * 8192 + c * 4;
+        b0 = unpack2<T>(*reinterpret_cast<const uint32_t*>(box + sw128_off(rl0, i & 7)));
+        b1 = unpack2<T>(*reinterpret_cast<const uint32_t*>(box + sw128_off(rl1, i & 7)));
+      }
+      if (tile_masked) {
+        const float2 ka = *reinterpret_cast<const float2*>(kadd + st * 128 + col);
+        b0.x += ka.x; b0.y += ka.y; b1.x += ka.x; b1.y += ka.y;
+      }
+      s[4 * i + 0] = fmaf(s[4 * i + 0], p.scale, b0.x);
+      s[4 * i + 1] = fmaf(s[4 * i + 1], p.scale, b0.y);
+      s[4 * i + 2] = fmaf(s[4 * i + 2], p.scale, b1.x);
+      s[4 * i + 3] = fmaf(s[4 * i + 3], p.scale, b1.y);
+      mx0 = fmaxf(mx0, fmaxf(s[4 * i + 0], s[4 * i + 1]));
+      mx1 = fmaxf(mx1, fmaxf(s[4 * i + 2], s[4 * i + 3]));
+    }
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+    mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+    mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+    const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);
+    // exponent offset: the running max, or 0 while every key seen so far is masked (the max itself stays -inf, so the
+    // first tile with a finite logit rescales from it and the offset follows that row's real maximum)
+    const float mu0 = mn0 == -CUDART_INF_F ? 0.f : mn0, mu1 = mn1 == -CUDART_INF_F ? 0.f : mn1;
+    const float alpha0 = ex2_approx((m0 - mu0) * kLog2e), alpha1 = ex2_approx((m1 - mu1) * kLog2e);   // m = -inf -> 0
+    m0 = mn0;
+    m1 = mn1;
+    l0 *= alpha0;
+    l1 *= alpha1;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o[4 * i + 0] *= alpha0;
+      o[4 * i + 1] *= alpha0;
+      o[4 * i + 2] *= alpha1;
+      o[4 * i + 3] *= alpha1;
+    }
+
+    // ---- probabilities, dropout, P -> register A operand ---------------------------------------------------------
+    const float nm0 = -mu0 * kLog2e, nm1 = -mu1 * kLog2e;
+    uint32_t pa[32];                 // pa[2i] = row rl0, keys 8i + 2c, +1; pa[2i + 1] = row rl1
+    uint32_t kw0[4] = {0u, 0u, 0u, 0u}, kw1[4] = {0u, 0u, 0u, 0u};   // keep bits, one word per 32 keys
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const float p00 = ex2_approx(fmaf(s[4 * i + 0], kLog2e, nm0)), p01 = ex2_approx(fmaf(s[4 * i + 1], kLog2e, nm0));
+      const float p10 = ex2_approx(fmaf(s[4 * i + 2], kLog2e, nm1)), p11 = ex2_approx(fmaf(s[4 * i + 3], kLog2e, nm1));
+      l0 += p00 + p01;
+      l1 += p10 + p11;
+      uint32_t km0 = 0xffffffffu, km1 = 0xffffffffu;
+      if (drop) {
+        // one Philox call per (row, 8 keys): word c decides the pair of keys 8i + 2c, +1 (bit layout of fmha_api.h)
+        const unsigned long long k8 = (unsigned long long)(key0 + 8 * i);
+        km0 = keep_mask2(select4(philox4x32<7>(p.seed, p.offset, (lin0 * p.Lk + k8) >> 3), c), t14x2);
+        km1 = keep_mask2(select4(philox4x32<7>(p.seed, p.offset, (lin1 * p.Lk + k8) >> 3), c), t14x2);
+        const uint32_t bit = 0x00010001u << (4 * (i & 3) + c);
+        kw0[i >> 2] |= km0 & bit;
+        kw1[i >> 2] |= km1 & bit;
+      }
+      pa[2 * i] = pack2<T>(p00, p01) & km0;
+      pa[2 * i + 1] = pack2<T>(p10, p11) & km1;
+    }
+    if (drop && p.drop_bits != nullptr) {
+#pragma unroll
+      for (int w = 0; w < 4; ++w) {
+        kw0[w] |= __shfl_xor_sync(0xffffffffu, kw0[w], 1);
+        kw0[w] |= __shfl_xor_sync(0xffffffffu, kw0[w], 2);
+        kw1[w] |= __shfl_xor_sync(0xffffffffu, kw1[w], 1);
+        kw1[w] |= __shfl_xor_sync(0xffffffffu, kw1[w], 2);
+      }
+      // thread c of the quad stores word c of both rows
+      const uint32_t w0 = c == 0 ? kw0[0] : (c == 1 ? kw0[1] : (c == 2 ? kw0[2] : kw0[3]));
+      const uint32_t w1 = c == 0 ? kw1[0] : (c == 1 ? kw1[1] : (c == 2 ? kw1[2] : kw1[3]));
+      if (key0 + 32 * c < p.Lk) {
+        const int wi = (key0 >> 5) + c;
+        if (row0 < p.Lq) p.drop_bits[lin0 * words_per_row + wi] = w0;
+        if (row1 < p.Lq) p.drop_bits[lin1 * words_per_row + wi] = w1;
+      }
+    }
+
+    // ---- O += P V ---------------------------------------------------------------------------------------
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kBlockN / 16; ++kk) {
+      const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
+      wgmma_m64n64_rs<T, 1>(o, a, make_desc_sw128(smem_base + kSmemV + st * 16384 + kk * 2048), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_operands(o);
+  }
+
+  // ---- epilogue ---------------------------------------------------------------------------------------
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float inv0 = l0 > 0.f ? keep_scale / l0 : 0.f, inv1 = l1 > 0.f ? keep_scale / l1 : 0.f;
+  T* out = reinterpret_cast<T*>(p.out);
+  if (row0 < p.Lq) {
+    uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row0) * p.H + h) * kHeadDim + 2 * c);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) og[4 * i] = pack2<T>(o[4 * i + 0] * inv0, o[4 * i + 1] * inv0);
+    if (c == 0) p.lse[lin0] = l0 > 0.f ? m0 + __logf(l0) : -CUDART_INF_F;   // natural-log LSE of the logits
+  }
+  if (row1 < p.Lq) {
+    uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row1) * p.H + h) * kHeadDim + 2 * c);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) og[4 * i] = pack2<T>(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
+    if (c == 0) p.lse[lin1] = l1 > 0.f ? m1 + __logf(l1) : -CUDART_INF_F;
+  }
+}
+
+}  // namespace
+
+void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream) {
+  dim3 grid((p.Lq + kBlockM - 1) / kBlockM, p.H, p.B);
+  auto run = [&](auto kern) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFwdSmemBytes);
+    kern<<<grid, kFwdThreads, kFwdSmemBytes, stream>>>(p);
+  };
+  if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16>);
+  else run(fmha_fwd_kernel<__half>);
+}
+
+}  // namespace ub

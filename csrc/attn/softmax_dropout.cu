@@ -1,8 +1,8 @@
-// softmax(x + mask + bias) followed by dropout, forward and backward, for sm_100a.
+// softmax(x + mask + bias) followed by dropout, forward and backward, for sm_90a.
 //
 // Stand-alone counterpart of reference csrc/softmax_dropout/* (used when attention probabilities
 // must be materialised, e.g. return_attn=True / head_dim 8 models; the BERT path uses the fused
-// tcgen05 attention kernel instead).  Differences from the reference kernels:
+// wgmma attention kernel instead).  Differences from the reference kernels:
 //   * a row is owned by a group of 1..256 threads that keeps it in registers; 128-bit accesses;
 //   * any row length that is a multiple of the vector width up to 8192 takes the fast path WITH
 //     dropout (reference: dropout only for K <= 1024, block kernel on the default stream above);
@@ -336,7 +336,7 @@ static int sm_count2() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }

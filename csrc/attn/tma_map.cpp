@@ -48,7 +48,7 @@ bool make_head_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int
 bool make_bias_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int NB, int Lq, int Lk) {
   const cuuint64_t dims[3] = {(cuuint64_t)Lk, (cuuint64_t)Lq, (cuuint64_t)NB};
   const cuuint64_t strides[2] = {(cuuint64_t)Lk * 2, (cuuint64_t)Lq * Lk * 2};
-  const cuuint32_t box[3] = {64, 128, 1};
+  const cuuint32_t box[3] = {64, 64, 1};
   return encode_sw128(map, base, bf16, 3, dims, strides, box);
 }
 

@@ -1,9 +1,7 @@
 // Tensor maps (TMA descriptors) of the attention kernels: 128-byte-swizzled boxes (CU_TENSOR_MAP_SWIZZLE_128B).
-// A box row is one whole 128-byte line (64 16-bit elements): one TMA request per row.  (The first version described
-// the tiles as 5-D tensors whose boxes wrote the SWIZZLE_NONE 8x8 core-matrix layout; those boxes have 16-byte rows
-// and cost ~1.7 cycles per row - 3500 cycles for a K + V tile pair - which bounded both attention kernels.)
-// Shared-memory layout of a box: row r at r * 128, its 16-byte chunk c at ((c ^ (r & 7)) * 16) - the canonical UMMA
-// SWIZZLE_128B layout (K-major operands, and MN-major operands whose MN extent is 64; tcgen05.cuh make_smem_desc_sw128).
+// A box row is one whole 128-byte line (64 16-bit elements).
+// Shared-memory layout of a box: row r at r * 128, its 16-byte chunk c at ((c ^ (r & 7)) * 16) - the canonical wgmma
+// SWIZZLE_128B layout (K-major operands, and MN-major operands whose MN extent is 64; wgmma.cuh make_desc_sw128).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -14,7 +12,7 @@ namespace ub {
 // [B, L, H, 64] tensor, box = box_rows x 64 of one (batch, head); coordinates {0, head, row0, batch}.
 bool make_head_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int B, int L, int H, long long sb,
                               long long sl, long long sh, int box_rows);
-// bias [NB, Lq, Lk]: box = 128 rows x 64 columns (a 128 x 128 tile is two boxes); coordinates {key0, q0, nb}.
+// bias [NB, Lq, Lk]: box = 64 rows x 64 columns (a 64 x 128 tile is two boxes); coordinates {key0, q0, nb}.
 bool make_bias_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int NB, int Lq, int Lk);
 
 }  // namespace ub

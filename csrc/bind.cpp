@@ -1,4 +1,4 @@
-// PyTorch bindings of the unicore_b200 sm_100a kernels (module ``unicore_b200._C``).
+// PyTorch bindings of the unicore_b200 sm_90a kernels (module ``unicore_b200._C``).
 // Only this translation unit sees the PyTorch headers; kernels are declared in csrc/api.h.
 #include <ATen/cuda/CUDAContext.h>
 #include <ATen/cuda/CUDAGeneratorImpl.h>
@@ -746,7 +746,7 @@ void register_comm(pybind11::module_& m);
 void register_symm_mem(pybind11::module_& m);
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "unicore_b200 sm_100a kernels";
+  m.doc() = "unicore_b200 sm_90a kernels";
   m.def("multi_tensor_l2norm", &multi_tensor_l2norm);
   m.def("multi_tensor_scale", &multi_tensor_scale);
   m.def("multi_tensor_adam", &multi_tensor_adam);

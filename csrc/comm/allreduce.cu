@@ -1,4 +1,4 @@
-// Gradient all-reduce over NVLink 5 / NVSwitch peer memory (sm_100a), replacing the NCCL all-reduce
+// Gradient all-reduce over NVLink 4 / NVSwitch peer memory (sm_90a), replacing the NCCL all-reduce
 // issued by DDP in the reference (unicore/models/distributed_unicore_model.py:37-46) on the
 // gradient path.  The flat 16-bit gradient arena lives in symmetric memory (every rank maps every
 // peer's buffer + an NVLS multicast alias), so the kernels below read/write peers with plain

@@ -5,7 +5,7 @@
 
 namespace ub {
 
-constexpr int kMaxPeers = 8;         // one NVSwitch domain (HGX B200: 8 GPUs)
+constexpr int kMaxPeers = 8;         // one NVSwitch domain (HGX H100: 8 GPUs)
 constexpr int kMaxCommBlocks = 64;   // flag slots: [kMaxCommBlocks][kMaxPeers] uint32 per rank (last 3 reserved)
 
 enum CommAlgo : int { kAlgoAuto = 0, kAlgoOneShot = 1, kAlgoTwoShot = 2, kAlgoNvls = 3 };

@@ -1,4 +1,4 @@
-// The fused optimizer tail of --ddp-backend b200: ONE kernel after backward (sm_100a, NVLink 5 / NVSwitch peer memory).
+// The fused optimizer tail of --ddp-backend b200: ONE kernel after backward (sm_90a, NVLink 4 / NVSwitch peer memory).
 //
 // What the reference does between the end of backward and the next forward (unicore/trainer.py:700-760):
 //   NCCL all-reduce of every gradient bucket (models/distributed_unicore_model.py:37-46)  ->  NCCL all-reduce of the
@@ -93,7 +93,7 @@ UB_DEVICE float tail_reduce_slice(const TailGroup& G, int rank, int world, long 
       }
     }
   } else {
-    // peer loads: one vector per thread and trip, `world` independent 16-byte loads in flight (148 x 512 threads keep
+    // peer loads: one vector per thread and trip, `world` independent 16-byte loads in flight (132 x 512 threads keep
     // ~2 MB on the wire at 2 GPUs, the bandwidth-delay product of a link)
     for (long long v = lo_vec + (long long)blockIdx.x * kCommThreads + threadIdx.x; v < hi_vec; v += stride) {
       Vec16 in[kMaxPeers];
@@ -354,7 +354,7 @@ int fused_tail_max_blocks() {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fused_tail_kernel, kCommThreads, 0);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
     if (per_sm < 1) per_sm = 1;
     blocks = sms;  // one CTA per SM: enough to saturate HBM and the links, always co-resident
     (void)per_sm;

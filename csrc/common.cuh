@@ -1,4 +1,4 @@
-// Shared device helpers for the unicore_b200 sm_100a kernels.
+// Shared device helpers for the unicore_b200 sm_90a kernels.
 //   * 128-bit vector load/store wrappers and 16-bit <-> fp32 pack/unpack
 //   * warp / block reductions
 //   * counter-based Philox4x32-10 (no per-thread state, no curand_init)
@@ -147,8 +147,8 @@ UB_DEVICE uint32_t keep_mask2(uint32_t rnd, uint32_t t14x2) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// packed fp32x2 arithmetic (sm_100: FFMA2 / FMUL2 / FADD2 - two fp32 lanes per issued instruction);
-// used where a kernel is issue-bound rather than bandwidth-bound (GELU, softmax statistics).
+// fp32 pairs: the kernels keep their math on element pairs (two adjacent columns); sm_90 has no packed fp32x2
+// instructions, so every operation is two scalar FFMA / FMUL / FADD.
 // ------------------------------------------------------------------------------------------------
 struct alignas(8) F2 {
   float x, y;
@@ -156,21 +156,9 @@ struct alignas(8) F2 {
 UB_DEVICE unsigned long long f2_bits(F2 a) { return *reinterpret_cast<unsigned long long*>(&a); }
 UB_DEVICE F2 f2_from_bits(unsigned long long b) { return *reinterpret_cast<F2*>(&b); }
 UB_DEVICE F2 f2(float a) { return F2{a, a}; }
-UB_DEVICE F2 fma2(F2 a, F2 b, F2 c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(f2_bits(a)), "l"(f2_bits(b)), "l"(f2_bits(c)));
-  return f2_from_bits(d);
-}
-UB_DEVICE F2 mul2(F2 a, F2 b) {
-  unsigned long long d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(f2_bits(a)), "l"(f2_bits(b)));
-  return f2_from_bits(d);
-}
-UB_DEVICE F2 add2(F2 a, F2 b) {
-  unsigned long long d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(f2_bits(a)), "l"(f2_bits(b)));
-  return f2_from_bits(d);
-}
+UB_DEVICE F2 fma2(F2 a, F2 b, F2 c) { return F2{fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)}; }
+UB_DEVICE F2 mul2(F2 a, F2 b) { return F2{a.x * b.x, a.y * b.y}; }
+UB_DEVICE F2 add2(F2 a, F2 b) { return F2{a.x + b.x, a.y + b.y}; }
 UB_DEVICE float rcp_approx(float x) {
   float y;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

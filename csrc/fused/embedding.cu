@@ -1,5 +1,5 @@
 // Gradient of an embedding lookup  y[r, :] = W[token[r], :]  (unicore/modules of the reference use nn.Embedding; its
-// backward in ATen is a radix sort of the indices + segmented reduction: ~30 launches and 0.45 ms per BERT-base step).
+// backward in ATen is a radix sort of the indices + segmented reduction: ~30 launches per BERT-base step).
 //
 // Two kernels, no sort:
 //   scatter : a warp per row adds dy[r, :] (as fp32) into scratch[token[r], :] with red.global.add.v4.f32 and marks
@@ -88,9 +88,9 @@ void launch_embedding_bwd(const void* dy, const long long* tokens, float* scratc
                           cudaStream_t stream) {
   const int warps_per_block = kEmbThreads / 32;
   long long b1 = (rows + warps_per_block - 1) / warps_per_block;
-  if (b1 > 148 * 16) b1 = 148 * 16;
+  if (b1 > 132 * 16) b1 = 132 * 16;
   long long b2 = (vocab + warps_per_block - 1) / warps_per_block;
-  if (b2 > 148 * 16) b2 = 148 * 16;
+  if (b2 > 132 * 16) b2 = 132 * 16;
   if (rows == 0) b1 = 0;
   if (dtype == kBF16) {
     if (b1 > 0)

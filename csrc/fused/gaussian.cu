@@ -2,7 +2,7 @@
 //   t = mul[edge] * d + bias[edge]                       (one scalar per atom pair, per-edge-type affine map)
 //   y[n, k] = exp(-0.5 ((t - mean_k) / std_k)^2) / (sqrt(2 * 3.14159) * std_k),   std_k = |stds_k| + 1e-5
 // The PyTorch formulation is two embedding look-ups over B*L*L indices, a broadcast and a TorchScript-fused
-// expression: its backward sorts the 2 M indices for the (deterministic) embedding gradient, 8 ms per step, and
+// expression: its backward sorts the 2 M indices for the (deterministic) embedding gradient on every step, and
 // TorchScript re-specialises on every new padded length.  Here: one forward kernel that writes the [N, K] features
 // once, and one backward kernel that recomputes y, reduces d mean / d std per column and scatters d mul / d bias
 // through a per-CTA shared-memory histogram (the edge-type table is small: < 1024 entries).
@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(kGbfThreads) gbf_bwd_kernel(const T* __restric
 }
 
 static int gbf_grid(long long n, int K) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int rows_per_cta = kGbfThreads / (K / 8);

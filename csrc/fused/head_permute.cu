@@ -1,4 +1,4 @@
-// Token-major <-> head-major relayout of packed projections, for sm_100a.
+// Token-major <-> head-major relayout of packed projections, for sm_90a.
 //
 //   token-major  [B, L, T, H, D]   what `in_proj` writes (T = 3: q | k | v) and what `out_proj` reads (T = 1)
 //   head-major   T x [B, H, L, D]  what the batched attention GEMMs need (one matrix per (b, h))
@@ -67,7 +67,7 @@ template <typename T>
 static void run_head_permute(void* token_major, const HeadPtrs& heads, int B, int L, int NT, int H, int DV, float scale0,
                              bool to_heads, cudaStream_t stream) {
   const long long total = (long long)B * NT * ((L + 1) / 2) * H * 2 * DV;
-  int sms = 148;
+  int sms = 132;
   int dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);

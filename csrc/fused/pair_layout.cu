@@ -1,4 +1,4 @@
-// Pair-representation relayout for sm_100a:  head-major [B, H, M] <-> pair-major [B, M, H]  (M = Lq * Lk).
+// Pair-representation relayout for sm_90a:  head-major [B, H, M] <-> pair-major [B, M, H]  (M = Lq * Lk).
 //
 // Pair-bias models (Uni-Mol; reference usage in SURVEY App. E) keep the pair representation head-major while
 // it is the attention bias ([B*H, L, L]) and pair-major ([B, L, L, H]) for the heads that consume it.  In
@@ -230,7 +230,7 @@ static PairGeom make_pair_geom(int B, int H, int L, long long M) {
 
 static int pair_grid(const PairGeom& g) {
   const long long total = (long long)g.B * g.HV * g.MV;
-  int sms = 148, dev = 0;
+  int sms = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   long long blocks = (total + 255) / 256;

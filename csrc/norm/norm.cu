@@ -1,5 +1,5 @@
 // LayerNorm / RMSNorm forward + single-pass backward, and the fused
-// "bias + dropout + residual + LayerNorm" block epilogue, for sm_100a.
+// "bias + dropout + residual + LayerNorm" block epilogue, for sm_90a.
 //
 // Replaces reference csrc/layernorm/layernorm.cu:25-148, layernorm_backward.cu:130-247, csrc/rmsnorm/rmsnorm.cu:25-125,
 // rmsnorm_backward.cu:108-196:
@@ -688,7 +688,7 @@ __global__ void __launch_bounds__(1024) colsum_finalize_kernel(const float* __re
 // v3 kernels: ONE WARP PER ROW (or 32/LPR short rows per warp), no block-level synchronisation in the row loop.
 //
 // The v2 kernels spend their time in barriers: six __syncthreads per 8-row tile (stage hand-over plus the cross-warp
-// row reductions of a 96-thread row group) at 35 % of the HBM copy rate (profiles/elementwise_bench_r1.jsonl).  Here a
+// row reductions of a 96-thread row group).  Here a
 // row of up to 32 * VPL 16-byte vectors is held by one warp - lane l owns vectors l, l + 32, ... - so the row
 // reductions are five shuffles, every load is a fully coalesced 512-byte warp request and nothing in the loop waits
 // for another warp.  A warp works on R rows at a time and already has the NEXT R rows in flight (register double
@@ -719,8 +719,7 @@ UB_DEVICE float row_sum(float v) {
 // in flight as packed 16-bit vectors (kPF), gamma / beta / bias are NOT held in registers: they are re-read at their
 // single use per row from L1 (a 1.5 KB working set that never leaves it), which is two issue slots per eight elements
 // and frees 24-36 registers for occupancy.  kFull: the row is exactly 32 * VPL vectors - no per-vector predicates.
-// ncu of the first v3 (profiles/ncu_norm_v3.txt): 18 instructions per element, 64 % issue-slot utilisation at 53 % of
-// the copy rate - instruction-bound (re-conversion passes, predicate selects, register-copy double buffer, spills).
+// (A first version that re-converted the packed row in every pass was instruction-bound.)
 template <typename T, int VPL, int LPR, int R, bool kPF, bool kRMS, bool kFused, bool kFull>
 __global__ void __launch_bounds__(kNormV3Threads, (VPL <= 3 ? 3 : (VPL == 4 ? 2 : 1))) norm_fwd_v3_kernel(
     const T* __restrict__ x, const T* __restrict__ gamma, const T* __restrict__ beta, T* __restrict__ y,
@@ -1047,7 +1046,7 @@ static int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }

@@ -1,4 +1,4 @@
-// Multi-tensor optimizer kernels for sm_100a: L2 norm, scale, Adam (+16-bit write-back,
+// Multi-tensor optimizer kernels for sm_90a: L2 norm, scale, Adam (+16-bit write-back,
 // stochastic rounding, EMA, grad zeroing), fp32->bf16 stochastic rounding, EMA.
 //
 // Replaces reference csrc/adam/adam_kernel.cu:16-152 (scalar accesses, one launch per tensor),
@@ -84,7 +84,7 @@ static int persistent_grid(long long chunks) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   const long long cap = (long long)sms * 8;  // 8 CTAs of 256 threads per SM = full occupancy
   return (int)(chunks < cap ? chunks : cap);
@@ -149,7 +149,7 @@ __global__ void __launch_bounds__(kThreads) l2norm_kernel(NormTensors t, long lo
   }
 }
 
-int l2norm_max_ctas() { return 148 * 8 * 2; }
+int l2norm_max_ctas() { return 132 * 8 * 2; }
 
 void launch_l2norm(const NormTensors& t, float* acc, float* partials, unsigned* counter, float* out, int finalize,
                    cudaStream_t stream) {

@@ -1,4 +1,4 @@
-"""Registers the Blackwell-native BERT (``unicore_b200/models/bert.py``) under the names the
+"""Registers the Hopper-native BERT (``unicore_b200/models/bert.py``) under the names the
 reference example uses (``examples/bert/model.py:18,223-260``)."""
 from unicore.models import register_model, register_model_architecture
 from unicore_b200.models.bert import BertModel as _BertImpl

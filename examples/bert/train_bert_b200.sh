@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Single node, one process per B200, gradient all-reduce on the NVLink peer-memory kernels.
+# Single node, one process per H100, gradient all-reduce on the NVLink peer-memory kernels.
 # usage: bash examples/bert/train_bert_b200.sh <data-dir> [save-dir]
 set -euo pipefail
 DATA=${1:?data directory with dict.txt, train.lmdb, valid.lmdb}

@@ -1,11 +1,11 @@
 """Packaging for unicore-b200.
 
 ``pip install -e .`` installs the pure-Python framework (``unicore``, ``unicore_cli``,
-``unicore_b200``) and the ``unicore-train`` console script.  The sm_100a extension
+``unicore_b200``) and the ``unicore-train`` console script.  The sm_90a extension
 ``unicore_b200._C`` is built in-tree with ``python setup.py build_ext --inplace`` (needs nvcc;
 skipped automatically when nvcc is absent or ``UNICORE_NO_CUDA_EXT=1``).  Unlike the reference
 (eight opt-in extensions targeting sm_70/80/90, ``setup.py:141-387``) there is ONE extension and it
-targets ``-gencode arch=compute_100a,code=sm_100a`` only.
+targets ``-gencode arch=compute_90a,code=sm_90a`` only.
 """
 import os
 import shutil
@@ -26,7 +26,7 @@ if shutil.which("nvcc") and os.environ.get("UNICORE_NO_CUDA_EXT", "0") != "1":
 setup(
     name="unicore-b200",
     version="0.1.0",
-    description="Blackwell-native distributed training framework with the Uni-Core API",
+    description="Hopper-native (H100) distributed training framework with the Uni-Core API",
     packages=find_packages(exclude=["tests", "tests.*", "baseline", "bench", "profiles"]),
     include_package_data=True,
     python_requires=">=3.9",

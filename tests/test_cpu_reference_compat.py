@@ -1,9 +1,11 @@
-"""Compatibility proofs against the reference implementation (SURVEY.md section 7.1-2 and 7.1-4): its example plug-in
-runs unmodified through this framework's ``--user-dir``, and checkpoints travel in both directions.  The reference is
-used as installed in ``baseline/_ref`` (or ``/root/reference``); the tests skip when neither is present."""
+"""Compatibility proofs against the reference implementation (SURVEY.md section 7.1-4): checkpoints travel in both
+directions, and a plug-in written against the public API trains to the same losses.  What the unmodified reference
+computed for these runs is stored in ``tests/golden/reference_records.json``, and the checkpoint it wrote in
+``tests/golden/checkpoint_interop_reference.pt``; both implementations build their initial weights from the same seed,
+which the recorded checksum of those weights pins down."""
+import hashlib
 import json
 import os
-import random
 import subprocess
 import sys
 
@@ -11,50 +13,19 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PY = sys.executable
+with open(os.path.join(ROOT, "tests", "golden", "reference_records.json")) as _f:
+    GOLDEN = json.load(_f)
 
 
-def reference_example_dir():
-    for base in ("/root/reference/examples", os.path.join(ROOT, "baseline", "_ref", "examples")):
-        if os.path.isfile(os.path.join(base, "bert", "task.py")):
-            return os.path.join(base, "bert")
-    return None
+def init_sha256(path):
+    import torch
 
-
-def test_reference_bert_example_runs_unmodified_through_user_dir(tmp_path):
-    """``--user-dir <reference>/examples/bert``: the reference's own task.py / model.py (its imports, its registry
-    decorators, its dataset pipeline, its BERT built from ``unicore.modules``) train, validate and checkpoint here."""
-    pytest.importorskip("tokenizers")
-    example = reference_example_dir()
-    if example is None:
-        pytest.skip("reference examples not available")
-    rng = random.Random(0)
-    words = ["alpha", "beta", "gamma", "delta", "epsilon", "zeta", "eta", "theta", "iota", "kappa", "lambda", "mu"]
-    for split, n in (("train", 96), ("valid", 24)):
-        with open(tmp_path / (split + ".txt"), "w") as f:
-            for _ in range(n):
-                f.write(" ".join(rng.choice(words) for _ in range(rng.randint(6, 14))) + " .\n")
-    data = tmp_path / "data"
-    prep = os.path.join(ROOT, "examples", "bert", "example_data", "prepare_data.py")
-    out = subprocess.run([PY, prep, "--train", str(tmp_path / "train.txt"), "--valid", str(tmp_path / "valid.txt"),
-                          "--out", str(data), "--build-dict", "--min-count", "1", "--format", "records"],
-                         stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert out.returncode == 0, out.stdout
-    save = str(tmp_path / "ck")
-    env = dict(os.environ, PYTHONPATH=ROOT, OMP_NUM_THREADS="1")
-    cmd = [PY, os.path.join(ROOT, "unicore_cli", "train.py"), str(data), "--user-dir", example,
-           "--task", "bert", "--loss", "masked_lm", "--arch", "bert_base", "--encoder-layers", "2",
-           "--encoder-embed-dim", "32", "--encoder-ffn-embed-dim", "64", "--encoder-attention-heads", "4",
-           "--max-seq-len", "32", "--optimizer", "adam", "--lr", "1e-3", "--lr-scheduler", "fixed", "--batch-size", "8",
-           "--max-update", "6", "--log-format", "simple", "--log-interval", "1", "--num-workers", "0", "--cpu",
-           "--valid-subset", "valid", "--validate-interval-updates", "3", "--save-interval-updates", "3",
-           "--save-dir", save, "--distributed-world-size", "1", "--seed", "1"]
-    run = subprocess.run(cmd, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
-    assert run.returncode == 0, run.stdout[-4000:]
-    losses = [float(l.split("loss=")[1].split(",")[0]) for l in run.stdout.splitlines() if "train_inner" in l and "loss=" in l]
-    assert len(losses) >= 5 and all(v == v for v in losses) and "valid" in run.stdout
-    assert os.path.isfile(os.path.join(save, "checkpoint_last.pt"))
-    # it really was the reference's plug-in: its modules come from the reference tree, the framework from this repo
-    assert example.startswith(("/root/reference", os.path.join(ROOT, "baseline", "_ref")))
+    sd = torch.load(path, map_location="cpu")
+    h = hashlib.sha256()
+    for k in sorted(sd):
+        h.update(k.encode())
+        h.update(sd[k].detach().contiguous().numpy().tobytes())
+    return h.hexdigest()
 
 
 def _interop(impl, init, *extra):
@@ -66,43 +37,53 @@ def _interop(impl, init, *extra):
 
 
 def test_checkpoints_travel_between_the_reference_and_this_framework(tmp_path):
-    """bf16 + weight decay (two flat optimizer groups) + clipping + EMA on the CPU: each side trains 3 updates, saves,
-    and trains 2 more; the OTHER side loads that file through its own ``Trainer.load_checkpoint`` and must reproduce
-    the 2 losses, the update count, the learning rate and the EMA (flat layout, reference
-    ``unicore/optim/fp16_optimizer.py:54-121``; schema ``unicore/trainer.py:224-284``)."""
-    if not os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "unicore")):
-        pytest.skip("reference not installed under baseline/_ref")
+    """bf16 + weight decay (two flat optimizer groups) + clipping + EMA on the CPU, in both directions (flat layout,
+    reference ``unicore/optim/fp16_optimizer.py:54-121``; schema ``unicore/trainer.py:224-284``):
+    * this framework loads the checkpoint the reference wrote (``tests/golden/checkpoint_interop_reference.pt``) and
+      continues with the reference's own next losses, learning rate and EMA;
+    * this framework trains 3 updates from the same initial weights and saves: the file has the reference's schema, the
+      losses are the reference's, and the reference continued from exactly this file to the recorded losses and EMA,
+      which loading it here reproduces."""
+    gold = GOLDEN["checkpoint_interop"]
+    ref, ref_loads_ref, ref_loads_ours = gold["reference"], gold["reference_loads_reference"], gold["reference_loads_ours"]
+    width = ["--embed-dim", str(gold["embed_dim"])]
     init = str(tmp_path / "init.pt")
-    sides = {}
-    for impl in ("reference", "ours"):
-        rec = _interop(impl, init, "--steps", "3", "--save", str(tmp_path / (impl + ".pt")), "--more", "2")
-        if "unavailable" in rec:
-            pytest.skip(rec["unavailable"])
-        sides[impl] = rec
-    a, b = sides["reference"], sides["ours"]
-    assert a["saved_keys"] == b["saved_keys"] and a["saved_opt_state_numel"] == b["saved_opt_state_numel"]
-    assert a["losses_before"] == pytest.approx(b["losses_before"], abs=2e-3)
-    for loader, writer in (("ours", "reference"), ("reference", "ours")):
-        got = _interop(loader, init, "--load", str(tmp_path / (writer + ".pt")), "--more", "2")
-        assert got["loaded_updates"] == 3 and got["loaded_epoch"] == 1
-        assert got["losses_after"] == pytest.approx(sides[writer]["losses_after"], abs=3e-3), (loader, writer)
-        assert got["ema_checksum"] == pytest.approx(sides[writer]["ema_checksum"], rel=1e-5)
+
+    # reference -> this framework
+    ref_ck = os.path.join(ROOT, "tests", "golden", "checkpoint_interop_reference.pt")
+    got = _interop("ours", init, "--load", ref_ck, "--more", "2", *width)
+    assert init_sha256(init) == gold["init_sha256"]
+    assert got["loaded_updates"] == ref_loads_ref["loaded_updates"] == 3
+    assert got["loaded_epoch"] == ref_loads_ref["loaded_epoch"] == 1
+    assert got["lr_after_load"] == pytest.approx(ref_loads_ref["lr_after_load"], rel=1e-9)
+    assert got["losses_after"] == pytest.approx(ref_loads_ref["losses_after"], abs=3e-3)
+    assert got["ema_checksum"] == pytest.approx(ref_loads_ref["ema_checksum"], rel=1e-5)
+
+    # this framework -> reference
+    ours = _interop("ours", init, "--steps", "3", "--save", str(tmp_path / "ours.pt"), "--more", "2", *width)
+    assert ours["saved_keys"] == ref["saved_keys"] and ours["saved_opt_state_numel"] == ref["saved_opt_state_numel"]
+    assert ours["losses_before"] == pytest.approx(ref["losses_before"], abs=2e-3)
+    assert ours["losses_after"] == pytest.approx(ref["losses_after"], abs=3e-3)
+    assert ours["losses_after"] == pytest.approx(ref_loads_ours["losses_after"], abs=3e-3)
+    assert ours["ema_checksum"] == pytest.approx(ref_loads_ours["ema_checksum"], rel=1e-5)
+    got = _interop("ours", init, "--load", str(tmp_path / "ours.pt"), "--more", "2", *width)
+    assert got["loaded_updates"] == ref_loads_ours["loaded_updates"] == 3
+    assert got["loaded_epoch"] == ref_loads_ours["loaded_epoch"] == 1
+    assert got["lr_after_load"] == pytest.approx(ref_loads_ours["lr_after_load"], rel=1e-9)
+    assert got["losses_after"] == pytest.approx(ref_loads_ours["losses_after"], abs=3e-3)
+    assert got["ema_checksum"] == pytest.approx(ref_loads_ours["ema_checksum"], rel=1e-5)
 
 
 def test_portable_unimol_plugin_gives_the_same_losses_under_both_frameworks(tmp_path):
-    """``examples/unimol_portable`` only uses the public Uni-Core API: the identical plug-in code trains under the
-    reference and under this framework, from the same weights, to the same losses (BASELINE.md B6)."""
-    if not os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "unicore")):
-        pytest.skip("reference not installed under baseline/_ref")
+    """``examples/unimol_portable`` only uses the public Uni-Core API: the identical plug-in code trains under this
+    framework, from the reference's initial weights, to the losses it reached under the reference (BASELINE.md B6)."""
+    gold = GOLDEN["unimol_portable"]
     tool = os.path.join(ROOT, "tools", "unimol_portable_check.py")
     init = str(tmp_path / "u.pt")
-    runs = {}
-    for impl in ("ours", "reference"):
-        out = subprocess.run([PY, tool, "--impl", impl, "--init", init, "--steps", "3"], env=dict(os.environ, OMP_NUM_THREADS="1"),
-                             stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
-        assert out.returncode == 0, out.stdout[-3000:]
-        runs[impl] = json.loads([l for l in out.stdout.splitlines() if l.startswith("{")][-1])
-        if "unavailable" in runs[impl]:
-            pytest.skip(runs[impl]["unavailable"])
-    assert len(runs["ours"]["losses"]) == 3 and runs["ours"]["losses"][-1] < runs["ours"]["losses"][0]
-    assert runs["ours"]["losses"] == pytest.approx(runs["reference"]["losses"], abs=2e-3)
+    out = subprocess.run([PY, tool, "--impl", "ours", "--init", init, "--steps", "3"], env=dict(os.environ, OMP_NUM_THREADS="1"),
+                         stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
+    assert out.returncode == 0, out.stdout[-3000:]
+    ours = json.loads([l for l in out.stdout.splitlines() if l.startswith("{")][-1])["losses"]
+    assert init_sha256(init) == gold["init_sha256"]
+    assert len(ours) == 3 and ours[-1] < ours[0]
+    assert ours == pytest.approx(gold["losses"], abs=2e-3)

@@ -1,4 +1,4 @@
-"""tcgen05 fused attention (forward + backward) against an fp32 PyTorch reference."""
+"""wgmma fused attention (forward + backward) against an fp32 PyTorch reference."""
 
 import pytest
 import torch
@@ -111,6 +111,77 @@ def test_fmha_qkvpacked_backward(dtype):
     assert (bias.grad.float() - bias_r.grad).abs().max().item() < tol * max(1.0, bias_r.grad.abs().max().item())
 
 
+def _keep_mask_by_probes(q, k, p, scale, seed, bias=None, kpm=None):
+    """The forward kernel's dropout keep mask [B, H, Lq, Lk], read back through value probes: with v = e_d at key
+    blk * 64 + d, output column d is P_drop of that key (same seed -> same Philox stream)."""
+    from unicore import ops
+
+    B, Lk, H, _ = k.shape
+    masks = []
+    for blk in range((Lk + 63) // 64):
+        eye = torch.zeros(B, Lk, H, 64, device="cuda", dtype=q.dtype)
+        n = min(64, Lk - blk * 64)
+        for d in range(n):
+            eye[:, blk * 64 + d, :, d] = 1
+        torch.manual_seed(seed)
+        pd = ops.fused_attention(q.detach(), k.detach(), eye, bias=None if bias is None else bias.detach(),
+                                 key_padding_mask=kpm, dropout_p=p, training=True, scale=scale)
+        masks.append(pd.permute(0, 2, 1, 3)[..., :n])
+    return (torch.cat(masks, dim=-1) != 0).float()
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("shape", [(2, 3, 200, 136), (1, 2, 72, 328)])
+@pytest.mark.parametrize("p", [0.0, 0.25])
+def test_fmha_backward_ragged(dtype, shape, p):
+    """Backward with Lq != Lk and lengths that are not multiples of the 64-row / 64-key tiles: query rows past Lq,
+    keys past Lk, the last (partial) keep-bit word of a row and clipped dS stores, with a per-batch bias gradient,
+    key padding and dropout."""
+    ops = _ops()
+    B, H, Lq, Lk = shape
+    _, q, k, v = _make(B, H, Lq, Lk, dtype, packed=False, seed=5)
+    bias = torch.randn(B, H, Lq, Lk, device="cuda").to(dtype).requires_grad_(True)
+    kpm = torch.zeros(B, Lk, dtype=torch.bool, device="cuda")
+    kpm[0, Lk - 40:] = True
+    scale = 0.125
+    keep = _keep_mask_by_probes(q, k, p, scale, 11, bias, kpm) if p > 0 else None
+    torch.manual_seed(11)
+    out = ops.fused_attention(q, k, v, bias=bias, key_padding_mask=kpm, dropout_p=p, training=True, scale=scale)
+    dout = torch.randn_like(out)
+    out.backward(dout)
+    qr, kr, vr, br = (t.detach().float().requires_grad_(True) for t in (q, k, v, bias))
+    ref, _ = _ref(qr, kr, vr, br, kpm, scale, keep=keep, p=p)
+    ref.backward(dout.float())
+    tol = 1e-2 if dtype == torch.float16 else 6e-2
+    assert (out.float() - ref).abs().max().item() < tol
+    for g, gr in ((q.grad, qr.grad), (k.grad, kr.grad), (v.grad, vr.grad), (bias.grad, br.grad)):
+        assert (g.float() - gr).abs().max().item() < tol * max(1.0, gr.abs().max().item())
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+def test_fmha_leading_masked_tile_with_very_negative_logits(dtype):
+    """The first 128-key tile is entirely padding and every real logit is far below -87 (exp underflows in fp32
+    without a proper offset): the softmax must still be the fp32 reference's, forward and backward."""
+    ops = _ops()
+    B, H, Lq, Lk = 2, 2, 64, 320
+    _, q, k, v = _make(B, H, Lq, Lk, dtype, packed=False, seed=6)
+    bias = (torch.randn(1, H, Lq, Lk, device="cuda") - 200.0).to(dtype)
+    kpm = torch.zeros(B, Lk, dtype=torch.bool, device="cuda")
+    kpm[:, :130] = True
+    scale = 0.125
+    out = ops.fused_attention(q, k, v, bias=bias, key_padding_mask=kpm, dropout_p=0.0, training=True, scale=scale)
+    dout = torch.randn_like(out)
+    out.backward(dout)
+    qr, kr, vr = (t.detach().float().requires_grad_(True) for t in (q, k, v))
+    ref, _ = _ref(qr, kr, vr, bias, kpm, scale)
+    ref.backward(dout.float())
+    tol = 1e-2 if dtype == torch.float16 else 6e-2
+    assert ref.abs().max().item() > 0.1
+    assert (out.float() - ref).abs().max().item() < tol
+    for g, gr in ((q.grad, qr.grad), (k.grad, kr.grad), (v.grad, vr.grad)):
+        assert (g.float() - gr).abs().max().item() < tol * max(1.0, gr.abs().max().item())
+
+
 def test_fmha_dropout_consistency():
     """Dropout: keep-rate, and backward uses exactly the forward's mask (checked via a linear probe)."""
     ops = _ops()
@@ -164,7 +235,7 @@ def test_self_attention_module_matches_materialised_path():
 
 @pytest.mark.parametrize("post_ln", [False])
 def test_encoder_layer_matches_fp32_formulation(post_ln):
-    """Whole pre-LN layer (tcgen05 attention, bias-GELU, column-sum bias gradients) against the plain fp32
+    """Whole pre-LN layer (wgmma attention, bias-GELU, column-sum bias gradients) against the plain fp32
     formulation of the same layer, forward and all gradients (dropout off)."""
     import copy
 

@@ -1,4 +1,4 @@
-"""Numerics of every hand-written sm_100a kernel against plain PyTorch fp32 references."""
+"""Numerics of every hand-written sm_90a kernel against plain PyTorch fp32 references."""
 import math
 
 import pytest

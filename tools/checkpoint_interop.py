@@ -82,6 +82,7 @@ def main():
     ap.add_argument("--load", default="")
     ap.add_argument("--more", type=int, default=2, help="updates after the save / load whose losses are reported")
     ap.add_argument("--precision", default="bf16", choices=["bf16", "fp32"])
+    ap.add_argument("--embed-dim", type=int, default=64, help="encoder width (the FFN is twice as wide)")
     a = ap.parse_args()
     why = bench.setup_paths(a.impl)
     if why is not None:
@@ -102,7 +103,8 @@ def main():
     register_task(a.impl)
     flags = [
         "--task", "interop_mlm", "--loss", "masked_lm", "--arch", "bert_base", "--encoder-layers", "2",
-        "--encoder-embed-dim", "64", "--encoder-ffn-embed-dim", "128", "--encoder-attention-heads", "4",
+        "--encoder-embed-dim", str(a.embed_dim), "--encoder-ffn-embed-dim", str(2 * a.embed_dim),
+        "--encoder-attention-heads", "4",
         "--max-seq-len", "32", "--dropout", "0.0", "--emb-dropout", "0.0", "--attention-dropout", "0.0",
         "--activation-dropout", "0.0", "--pooler-dropout", "0.0", "--optimizer", "adam", "--adam-betas", "(0.9, 0.98)",
         "--adam-eps", "1e-6", "--weight-decay", "0.01", "--clip-norm", "1.0", "--lr-scheduler", "polynomial_decay",

@@ -43,7 +43,7 @@ def zipf_batches(n, bsz, seq_len, vocab, pad_idx, mask_idx, special, seed):
 
 
 def gpu_main(a):
-    """100-step style loss curve of the flagship configuration on one B200 (VERDICT r1 item 8c)."""
+    """Loss curve of the flagship configuration on one GPU."""
     why = bench.setup_paths(a.impl)
     if why is not None:
         print(json.dumps({"impl": a.impl, "unavailable": why}))

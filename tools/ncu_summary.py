@@ -1,8 +1,8 @@
 #!/usr/bin/env python3
-"""Condense an Nsight Compute report into the handful of lines kept under ``profiles/``.
+"""Condense an Nsight Compute report into a handful of lines.
 
-    ncu --set full --clock-control none --import-source on -k regex:fmha -c 6 -o gpurun_out/x  python bench/attn_bench.py ...
-    python tools/ncu_summary.py gpurun_out/x.ncu-rep [kernel-name-substring] > profiles/ncu_x.txt
+    ncu --set full --clock-control none --import-source on -k regex:fmha -c 6 -o out/x  python bench/attn_bench.py ...
+    python tools/ncu_summary.py out/x.ncu-rep [kernel-name-substring] > ncu_x.txt
 
 Reads the report with ``ncu -i ... --page raw --csv`` (works without a GPU) and prints, per selected kernel launch,
 the metrics the profiling recipe asks for: duration, issue / tensor-pipe / memory utilisation, DRAM traffic, occupancy

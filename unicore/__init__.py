@@ -1,4 +1,4 @@
-"""unicore: Uni-Core compatible training framework, Blackwell-native underneath.
+"""unicore: Uni-Core compatible training framework, Hopper-native underneath.
 
 Importing the package populates the registries (optimizers, LR schedulers, losses, built-in tasks)
 and installs the historical module aliases ``unicore.distributed_utils / meters / metrics /

@@ -4,7 +4,7 @@ Parity: reference ``unicore/data/iterators.py`` (``CountingIterator:28``,
 ``EpochBatchIterator:151`` incl. ``state_dict:311`` / ``load_state_dict:326`` with position
 re-scaling, ``GroupedIterator:406``, ``ShardedIterator:438``, ``BufferedIterator:496``).
 
-B200 design difference: the reference's "GPU-CPU overlapping" loader only overlaps *collation*
+Design difference: the reference's "GPU-CPU overlapping" loader only overlaps *collation*
 (SURVEY D19 - batches stay pageable so the H2D copy is synchronous).  ``BufferedIterator`` here
 can page-lock each prefetched batch in its producer thread (``pin_memory=True``) so that the
 trainer's ``non_blocking`` copy is a real async DMA, and ``DevicePrefetcher`` stages the next

@@ -2,7 +2,7 @@
 the model projects only those positions (``masked_tokens``); ``sample_size`` - what the gradients are normalised by - is
 the device-resident number of masked tokens.
 
-B200 path: log-softmax + NLL over the ``[n_masked, vocab]`` logits is one fused kernel
+GPU path: log-softmax + NLL over the ``[n_masked, vocab]`` logits is one fused kernel
 (``unicore.ops.softmax_cross_entropy``) that never materialises fp32 log-probabilities, and the masked positions are
 resolved without a host stall (``utils.request_mask_index``).
 """

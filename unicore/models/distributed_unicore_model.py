@@ -4,7 +4,7 @@
   CPU modules (the reference passes ``device_ids`` unconditionally and fails there).
 * ``apex``   - apex DDP when installed.
 * ``no_c10d`` / ``legacy_ddp`` - explicit flat-buffer all-reduce after backward.
-* ``b200``   - symmetric-memory engine: gradients are reduced by hand-written sm_100a kernels over
+* ``b200``   - symmetric-memory engine: gradients are reduced by hand-written sm_90a kernels over
   NVLink peer memory and fused with the optimizer (``unicore_b200.parallel``); needs CUDA + NCCL
   and falls back to ``c10d`` otherwise.
 All engines are wrapped in ``ModuleProxyWrapper``.  Parity: reference

@@ -5,8 +5,8 @@ Parity: reference ``unicore/modules/multihead_attention.py`` - ``SelfMultiheadAt
 boolean ``key_padding_mask``, ``return_attn`` yielding ``(out, pre-softmax logits incl. bias,
 probabilities)``) and ``CrossMultiheadAttention:121``.
 
-B200 path: unless ``return_attn`` is requested, the whole ``QK^T -> +bias/mask -> softmax ->
-dropout -> @V`` chain runs in the tcgen05 kernel behind ``ops.fused_attention``; q/k/v are strided
+GPU path: unless ``return_attn`` is requested, the whole ``QK^T -> +bias/mask -> softmax ->
+dropout -> @V`` chain runs in the wgmma kernel behind ``ops.fused_attention``; q/k/v are strided
 views of the projection output (no transpose/contiguous copies) and the bias is *not* expanded over
 the batch.  With ``return_attn`` the materialised path (bmm + ``softmax_dropout`` kernel) is used.
 """
@@ -39,7 +39,7 @@ def _materialised_attention(qh, kh, vh, key_padding_mask, attn_bias4, dropout, t
     """qh, kh, vh: head-major ``[B, H, L, D]`` (contiguous, query already scaled).
 
     Returns ``(out [B, Lq, H*D], logits?, probs?)``; scores are materialised (``return_attn`` / head dims the
-    tcgen05 kernel does not cover).  Parity: reference ``multihead_attention.py:78-118``.
+    wgmma kernel does not cover).  Parity: reference ``multihead_attention.py:78-118``.
     """
     bsz, heads, tgt_len, dim = qh.shape
     src_len = kh.shape[2]

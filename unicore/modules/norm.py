@@ -1,4 +1,4 @@
-"""LayerNorm / RMSNorm modules backed by the sm_100a kernels in ``unicore.ops``.
+"""LayerNorm / RMSNorm modules backed by the sm_90a kernels in ``unicore.ops``.
 
 Parity: reference ``unicore/modules/layer_norm.py:50-82`` and ``rms_norm.py:82-135`` (always
 affine, eps 1e-5, fp32 statistics).  Unlike the reference there is no hidden-size whitelist: the

@@ -6,8 +6,8 @@ Parity: reference ``unicore/modules/transformer_encoder_layer.py:15``,
 Same constructor arguments, parameter names (=> identical ``state_dict`` keys) and forward
 signatures, including ``return_attn`` on the encoder layer.
 
-B200 execution plan for one layer (post-LN shown; pre-LN analogous):
-  in_proj GEMM -> fused tcgen05 attention (bias tile + key padding + dropout inside) ->
+GPU execution plan for one layer (post-LN shown; pre-LN analogous):
+  in_proj GEMM -> fused wgmma attention (bias tile + key padding + dropout inside) ->
   out_proj GEMM -> ONE kernel: bias + dropout + residual + LayerNorm ->
   fc1 GEMM -> ONE kernel: bias + GELU -> fc2 GEMM -> ONE kernel: bias + dropout + residual + LN.
 The relative-position bias stays ``[1, H, L, L]`` (never repeated over the batch) and the key
@@ -263,7 +263,7 @@ class _StackMixin:
             # The bucket table is a constant: with its one-hot matrix E [bins, L*L] (cached) the lookup is the GEMM
             # W^T E - it lands directly in [H, L, L] order (no permute copy), and autograd's backward is the GEMM
             # dBias E^T with fp32 accumulation instead of ATen's embedding backward (a radix sort of L*L indices plus
-            # a segmented reduction: ~0.2 ms and 12 launches per BERT-base step).  Same values: each output element is
+            # a segmented reduction: 12 launches per BERT-base step).  Same values: each output element is
             # one table entry times 1.
             return (weight.t() @ self._bucket_one_hot(seq_len, weight)).view(-1, seq_len, seq_len)
         values = F.embedding(self.rp_bucket[:seq_len, :seq_len], weight)

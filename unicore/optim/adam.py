@@ -1,6 +1,6 @@
 """Adam (decoupled weight decay, i.e. AdamW-style) and its CLI wrapper.
 
-``UnicoreAdam`` uses ``FusedAdam`` (one multi-tensor sm_100a launch per step) when the CUDA
+``UnicoreAdam`` uses ``FusedAdam`` (one multi-tensor sm_90a launch per step) when the CUDA
 extension is loaded and the params are on a GPU, else the pure-PyTorch ``Adam`` below.
 Parity: reference ``unicore/optim/adam.py:22-204`` (flags ``--adam-betas``, ``--adam-eps``,
 ``--weight-decay``; python Adam decays with ``lr * wd``; amsgrad supported).
@@ -37,7 +37,7 @@ class UnicoreAdam(UnicoreOptimizer):
 
             fused_cls, use_fused = FusedAdam, True  # (its kernel call has a PyTorch fallback)
         if use_fused:
-            logger.info("using FusedAdam (sm_100a multi-tensor kernel)")
+            logger.info("using FusedAdam (sm_90a multi-tensor kernel)")
             self._optimizer = fused_cls(params, **self.optimizer_config)
         else:
             self._optimizer = Adam(params, **self.optimizer_config)

@@ -11,7 +11,7 @@ Step semantics follow ``_FP16OptimizerMixin`` (reference ``:139-308``): loss is 
 loss scale, every later gradient scaling (1/loss_scale, world/sample_size, clipping) is folded
 into the scalar ``_multiply_factor`` and applied *inside* the optimizer kernel.
 
-B200 fused tail (CUDA + FusedAdam): the reference runs
+Fused tail (CUDA + FusedAdam): the reference runs
 ``grad16->grad32 copy, L2 norm, Adam, param32->param16 copy, zero_grad(2 memsets)`` as separate
 passes (~86 B/param incl. EMA).  Here the norm (+ non-finite detection) is computed directly from
 the 16-bit flat gradient (2 B/param) and ONE kernel then does unscale/clip + Adam on the fp32

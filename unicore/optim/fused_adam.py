@@ -5,7 +5,7 @@ Math (reference kernel ``csrc/adam/adam_kernel.cu:38-78`` / wrapper ``optim/fuse
 ``m = b1 m + (1-b1) g``, ``v = b2 v + (1-b2) g^2``, ``p = p (1 - step_size*wd) - step_size m/(sqrt(v)+eps)``.
 Note the decay is scaled by the *bias-corrected* step size (differs from the python ``Adam``).
 
-B200 design: all parameters of all groups go to ``unicore.ops.fused_adam`` as tensor lists with
+GPU design: all parameters of all groups go to ``unicore.ops.fused_adam`` as tensor lists with
 per-tensor hyper-parameters, i.e. one launch per step irrespective of the number of tensors; the
 kernel uses 128-bit accesses, accepts fp32 or half/bf16 params+grads with fp32 moments, and can
 emit a 16-bit copy of the updated parameter (optionally stochastically rounded) and zero the
@@ -15,7 +15,7 @@ import torch
 
 
 def get_fused_adam_class():
-    """Return ``FusedAdam`` when the sm_100a extension is importable, else ``None``."""
+    """Return ``FusedAdam`` when the sm_90a extension is importable, else ``None``."""
     from unicore import ops
 
     return FusedAdam if ops.HAS_CUDA_EXT else None

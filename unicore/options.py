@@ -6,7 +6,7 @@ defaults and semantics follow the reference CLI (``unicore/options.py:24-428``; 
 SURVEY.md Appendix A) so existing launch scripts work unchanged. The flag tables below are
 declarative: ``(names, kwargs)`` rows consumed by ``_add_rows``.
 
-B200 additions (all optional, defaults preserve reference behaviour):
+Additions (all optional, defaults preserve reference behaviour):
 ``--ddp-backend b200`` (gradient all-reduce kernels over NVLink symmetric memory, bucketed and overlapped with
 backward, gradient norm accumulated in the same pass; falls back to c10d when peer memory is unavailable),
 ``--pin-memory`` (pinned batches + non-blocking H2D) and ``--deferred-overflow-check`` (fp16: the overflow
@@ -104,7 +104,7 @@ def _dataset_rows():
               help="maximum number of sentences in a validation batch (defaults to --max-sentences)"),
         _flag("--max-valid-steps", type=int, metavar="N", help="How many batches to evaluate"),
         _flag("--curriculum", default=0, type=int, metavar="N", help="don't shuffle batches for first N epochs"),
-        # B200 addition: page-locked host staging so the H2D copy overlaps compute
+        # addition: page-locked host staging so the H2D copy overlaps compute
         _flag("--pin-memory", action="store_true",
               help="page-lock prefetched batches so host-to-device copies are asynchronous"),
     ]

@@ -7,8 +7,8 @@ Parity map (reference ``unicore/utils.py``): ``apply_to_sample:43``, ``move_to_c
 ``eval_str_list/dict/bool:278-303``, ``checkpoint_sequential:306``, tensor-tree helpers
 ``:336-411``, ``fp32_to_bf16_sr:414``, ``set_jit_fusion_options:426``, ``validate_with_ema:437``.
 
-B200 differences: the grad-norm and stochastic-rounding helpers dispatch to the hand-written
-sm_100a kernels in ``unicore.ops`` (single-launch multi-tensor L2 norm, counter-based Philox SR)
+Differences: the grad-norm and stochastic-rounding helpers dispatch to the hand-written
+sm_90a kernels in ``unicore.ops`` (single-launch multi-tensor L2 norm, counter-based Philox SR)
 and fall back to plain PyTorch on CPU.
 """
 import contextlib
@@ -72,7 +72,7 @@ def move_to_cpu(sample):
 
 
 def pin_sample(sample):
-    """Page-lock every tensor of a sample (B200 addition: makes ``move_to_cuda`` truly async)."""
+    """Page-lock every tensor of a sample (addition: makes ``move_to_cuda`` truly async)."""
     if not torch.cuda.is_available():
         return sample
     return apply_to_sample(lambda t: t.pin_memory() if not t.is_pinned() else t, sample)
@@ -84,10 +84,9 @@ def pin_sample(sample):
 class _HostReader:
     """Device scalar(s) -> host without parking the thread in a blocking stream synchronize.
 
-    ``tensor.item()`` sleeps in ``cudaStreamSynchronize``; waking up costs 0.3-0.8 ms on virtualised
-    hosts (measured on the B200 boxes: the GPU sat idle that long after each of the two per-step
-    host reads).  Here the value is copied asynchronously into a cached pinned buffer and the
-    thread polls the completion event instead.
+    ``tensor.item()`` sleeps in ``cudaStreamSynchronize``; waking up is slow on virtualised
+    hosts, and the GPU sits idle that long after each such host read.  Here the value is copied
+    asynchronously into a cached pinned buffer and the thread polls the completion event instead.
     """
 
     def __init__(self):
@@ -283,7 +282,7 @@ def request_mask_index(mask: torch.Tensor) -> None:
     """Start resolving ``mask_to_index(mask)`` without waiting: the number of True entries is summed on the device and
     copied to pinned host memory asynchronously.  A masked-LM loss calls this BEFORE the model runs; by the time the LM
     head asks for the indices the copy - queued ahead of the whole encoder - has long completed, so the host neither
-    stalls nor lets the launch queue run dry (a blocking read at this point cost ~0.25 ms of idle GPU per step)."""
+    stalls nor lets the launch queue run dry (a blocking read at this point idles the GPU every step)."""
     global _mask_index_cache
     ref = _mask_index_cache[0]
     if ref is not None and ref() is mask:
@@ -464,8 +463,8 @@ def torch_seed(seed, *addl_seeds):
     Used for per-(update, micro-batch, rank) dropout reproducibility and the rank-invariant
     optimizer-step stream that stochastic rounding relies on (reference ``trainer.py:602-607,712``).
     The generators are driven directly: ``torch.manual_seed`` walks every device backend (and queues
-    a formatted stack trace per call for uninitialised ones), ~0.5 ms per use, which sat on the
-    critical path twice per training step.
+    a formatted stack trace per call for uninitialised ones), which sat on the critical path twice
+    per training step.
     """
     if seed is None:
         yield
@@ -679,7 +678,7 @@ def fp32_to_bf16_sr(t: torch.Tensor, o: torch.Tensor) -> None:
 
 
 def set_jit_fusion_options() -> None:
-    """Kept for CLI parity. The B200 build does not rely on TorchScript fusers: hot element-wise
+    """Kept for CLI parity. This build does not rely on TorchScript fusers: hot element-wise
     chains are explicit CUDA kernels, so we only make sure legacy fusers are off."""
     try:
         torch._C._jit_set_profiling_executor(True)

@@ -1,4 +1,4 @@
-"""unicore_b200: the Blackwell (sm_100a) core under the Uni-Core compatible ``unicore`` API.
+"""unicore_b200: the Hopper (sm_90a) core under the Uni-Core compatible ``unicore`` API.
 
 ``ops``      hand-written CUDA kernels + autograd wrappers (``csrc/`` -> ``unicore_b200._C``)
 ``parallel`` symmetric-memory data parallel engine (peer-memory all-reduce fused with Adam)

@@ -1,4 +1,4 @@
-"""BERT (masked-LM encoder) on the fused Blackwell op set.
+"""BERT (masked-LM encoder) on the fused Hopper op set.
 
 Architecture = the reference example (``examples/bert/model.py:19-260``): token embedding + learned
 absolute positions, ``TransformerEncoder`` with T5-style relative-position bias (32 buckets, max
@@ -6,7 +6,7 @@ distance 128), post-LN by default, LM head (dense -> act -> LayerNorm -> tied pr
 evaluated only at masked positions; parameter names are identical, so checkpoints interchange.
 Architectures: bert/bert_base 12L-768-3072-12H, bert_large 24L-1024-4096-16H, xlm 16L-1280-5120-16H.
 
-B200 notes: the padding mask is handed to the fused attention kernel as ``[B, L]`` (no host sync to
+GPU notes: the padding mask is handed to the fused attention kernel as ``[B, L]`` (no host sync to
 test whether the batch has padding when the fused path is active, no ``[B*H, L, L]`` ``-inf``
 tensor); the LM-head activation uses the fused bias+GELU kernel.
 """

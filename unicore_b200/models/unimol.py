@@ -12,7 +12,7 @@ full ``[B*H, N, N]`` bias.  This file implements the publicly described architec
   logits, which become the next layer's bias (pair update);
 * heads: masked-atom LM, pair-distance regression, SE(3)-equivariant coordinate update.
 
-Hot ops on B200: ``ops.softmax_dropout`` (materialised, head_dim 8 is not an MMA shape), LayerNorm(512)
+Hot ops on the GPU: ``ops.softmax_dropout`` (materialised, head_dim 8 is not an MMA shape), LayerNorm(512)
 and LayerNorm(64) kernels, bias+GELU; the GEMMs go to cuBLAS.
 """
 import math

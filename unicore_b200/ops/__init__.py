@@ -1,4 +1,4 @@
-"""Python surface of the hand-written sm_100a kernels (+ PyTorch fallbacks for CPU runs)."""
+"""Python surface of the hand-written sm_90a kernels (+ PyTorch fallbacks for CPU runs)."""
 from ._native import HAS_CUDA_EXT, USE_NATIVE, native, use_native  # noqa: F401
 from .attention_ops import (  # noqa: F401
     attention_reference,

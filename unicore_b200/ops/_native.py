@@ -1,10 +1,10 @@
-"""Loader for the in-tree sm_100a extension ``unicore_b200._C``.
+"""Loader for the in-tree sm_90a extension ``unicore_b200._C``.
 
 The extension is built in-tree (``python setup.py build_ext --inplace`` or
 ``__graft_entry__.build()``) so the ``.so`` travels with the source snapshot.  Policy:
 
 * CPU-only process (no CUDA device): the extension is optional, ops use PyTorch fallbacks.
-* CUDA device present: a missing/unloadable extension is a hard error unless
+* Hopper device (compute capability 9.x): a missing/unloadable extension is a hard error unless
   ``UNICORE_ALLOW_FALLBACK=1`` - silent eager fallbacks on a GPU box would hide that the native
   path is not running.
 """
@@ -26,30 +26,27 @@ except Exception as exc:  # noqa: BLE001 - ImportError, OSError (missing libs), 
 HAS_CUDA_EXT = _C is not None
 
 
-def _is_blackwell() -> bool:
+def _is_hopper() -> bool:
     try:
-        return torch.cuda.is_available() and torch.cuda.get_device_capability()[0] >= 10
+        return torch.cuda.is_available() and torch.cuda.get_device_capability()[0] == 9
     except Exception:  # noqa: BLE001
         return False
 
 
-if _is_blackwell() and _C is None and os.environ.get("UNICORE_ALLOW_FALLBACK", "0") != "1":
-    # fail loudly where the kernels are the product; on other GPUs (A100 / H100 development boxes, CI) the PyTorch
-    # fallbacks are what runs anyway
+if _is_hopper() and _C is None and os.environ.get("UNICORE_ALLOW_FALLBACK", "0") != "1":
+    # fail loudly where the kernels are the product
     raise ImportError(
-        "unicore_b200._C (sm_100a kernels) failed to load on a CUDA machine: {!r}. Build it with "
+        "unicore_b200._C (sm_90a kernels) failed to load on a CUDA machine: {!r}. Build it with "
         "`python setup.py build_ext --inplace` (or __graft_entry__.build()), or set "
         "UNICORE_ALLOW_FALLBACK=1 to run on PyTorch fallbacks.".format(_ERR)
     )
 
-# kernels are compiled for sm_100a only; on other GPUs use the fallbacks
-USE_NATIVE = HAS_CUDA_EXT and _is_blackwell() and os.environ.get("UNICORE_DISABLE_NATIVE", "0") != "1"
+# kernels are compiled for sm_90a only (arch-specific code loads on no other GPU); elsewhere use the fallbacks
+USE_NATIVE = HAS_CUDA_EXT and _is_hopper() and os.environ.get("UNICORE_DISABLE_NATIVE", "0") != "1"
 if torch.cuda.is_available() and not USE_NATIVE:
-    import logging
-
-    logging.getLogger(__name__).warning(
-        "unicore_b200: the sm_100a kernels are not in use on this machine (%s); PyTorch fallbacks run instead",
-        "extension not built: {!r}".format(_ERR) if _C is None else "not a Blackwell GPU or UNICORE_DISABLE_NATIVE=1")
+    logger.warning(
+        "unicore_b200: the sm_90a kernels are not in use on this machine (%s); PyTorch fallbacks run instead",
+        "extension not built: {!r}".format(_ERR) if _C is None else "not a Hopper GPU or UNICORE_DISABLE_NATIVE=1")
 
 
 # kernels launched per binding call (used for the benchmark's ``gpu_launches`` figure)

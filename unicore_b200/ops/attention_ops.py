@@ -2,13 +2,12 @@
 
 The reference materialises the ``[B*H, L, L]`` score tensor three times per layer
 (``unicore/modules/multihead_attention.py:47-114``: bmm -> softmax_dropout -> bmm, plus four
-transpose+contiguous copies).  The sm_100a kernel (``csrc/attn/fmha_sm100.cu``) keeps scores in
-tensor memory: ``tcgen05.mma`` computes S = QK^T into TMEM, softmax warps read it with
-``tcgen05.ld``, add the bias tile / padding mask, apply Philox dropout, write P (16-bit) to shared
-memory and a second ``tcgen05.mma`` accumulates O += PV in TMEM.  q/k/v are consumed directly from
-the packed ``in_proj`` output through strides (no transposes) and O is written as ``[B, L, H*D]``.
-Backward recomputes P from the saved log-sum-exp (flash-attention style) and regenerates the
-dropout mask from the same Philox counters.
+transpose+contiguous copies).  The sm_90a kernels (``csrc/attn/fmha_{fwd,bwd}_sm90.cu``) keep scores in
+registers: ``wgmma`` computes S = QK^T, the softmax adds the bias tile / padding mask and applies Philox
+dropout in registers, and P is the register operand of a second ``wgmma`` that accumulates O += PV.
+q/k/v are consumed directly from the packed ``in_proj`` output through strides (no transposes) and O is
+written as ``[B, L, H*D]``.  Backward recomputes P from the saved log-sum-exp (flash-attention style) and
+reads the dropout keep bits the forward kernel stored.
 """
 import math
 
@@ -115,7 +114,7 @@ def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool
 
 
 def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None):
-    """Dispatch to the tcgen05 kernel when shapes/dtypes allow, else to the PyTorch reference."""
+    """Dispatch to the wgmma kernel when shapes/dtypes allow, else to the PyTorch reference."""
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
     if fused_attention_supported(q, k, v, bias, key_padding_mask):

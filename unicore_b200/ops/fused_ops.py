@@ -2,7 +2,7 @@
 
 These fusions do not exist in the reference (it runs GELU, three dropouts, residual adds,
 LayerNorm and the fp32 log-softmax as separate ATen kernels,
-``unicore/modules/transformer_encoder_layer.py:79-94``, ``losses/masked_lm.py:31-36``); on B200
+``unicore/modules/transformer_encoder_layer.py:79-94``, ``losses/masked_lm.py:31-36``); on the GPU
 every one of them is HBM-bound, so they are merged into the minimum number of passes:
 
 * ``bias_gelu(x, bias)``                      - GEMM-output bias add + exact GELU (erf), fwd/bwd;
@@ -79,7 +79,7 @@ class _LinearFn(torch.autograd.Function):
             if ctx.w_sink is not None:
                 if weight.numel() * 64 < dy2.shape[0] * dy2.shape[1]:
                     # tiny weight, very long reduction (pair-tensor heads: 64 x 128 outputs over millions of rows): the
-                    # beta = 1 GEMM falls onto a slow non-split-K kernel (measured 485 us); plain mm + a small add
+                    # beta = 1 GEMM falls onto a slow non-split-K kernel; plain mm + a small add
                     ctx.w_sink.grad.add_(dy2.t().mm(x2))
                 else:
                     ctx.w_sink.grad.addmm_(dy2.t(), x2)
@@ -290,8 +290,7 @@ def vocab_projection(x, weight, bias=None, multiple=64):
     """``F.linear(x, weight, bias)`` for an output dimension (vocabulary) that is not a multiple of 8.
 
     With V = 30522 the logits' rows are only 4-byte aligned, which sends all three GEMMs of the
-    projection (fwd, dgrad, wgrad) down cuBLAS' slow element-aligned path (measured 3x slower on
-    B200).  The weight/bias are zero-padded to a multiple of ``multiple`` rows on the fly (47 MB
+    projection (fwd, dgrad, wgrad) down cuBLAS' slow element-aligned path.  The weight/bias are zero-padded to a multiple of ``multiple`` rows on the fly (47 MB
     copy for BERT-base, ~15 us) and the result is returned as the ``[:, :V]`` view of the padded
     logits; ``softmax_cross_entropy`` recognises such views and reads/writes the padded buffer in
     place, so no compaction copy is ever made.
@@ -356,7 +355,7 @@ class _EmbeddingFn(torch.autograd.Function):
 
 def embedding(tokens: torch.Tensor, weight: torch.Tensor, padding_idx: Optional[int] = None) -> torch.Tensor:
     """``F.embedding`` whose backward is two kernels (fp32 ``red`` scatter + finalize, ``csrc/fused/embedding.cu``)
-    instead of ATen's radix sort + segmented reduction (~30 launches, 0.45 ms per BERT-base step), writing into the
+    instead of ATen's radix sort + segmented reduction (~30 launches per BERT-base step), writing into the
     gradient arena when the weight is claimed."""
     if (
         use_native(weight) and torch.is_grad_enabled() and weight.requires_grad

@@ -3,7 +3,7 @@
 With flat arenas (``unicore/optim/fp16_optimizer.py``) every parameter's ``.grad`` is a view of one 16-bit buffer.
 Plain autograd still computes each parameter gradient into a temporary and then ADDS it to that view with one more
 kernel per parameter (``AccumulateGrad``): for BERT-base that is ~155 extra launches and three passes over the gradient
-bytes per step (0.7 ms of device time + launch gaps on a B200, ``profiles/step_profile_1gpu.txt``: 186 ``add`` kernels).
+bytes per step.
 
 The backward kernels of this framework can accumulate in place instead: the weight-gradient GEMM runs with beta = 1 on
 the arena view (``addmm_``), the bias / LayerNorm column-sum finalisers add to the view.  A custom autograd Function

@@ -1,4 +1,4 @@
-"""LayerNorm / RMSNorm with hand-written sm_100a forward and single-pass backward kernels.
+"""LayerNorm / RMSNorm with hand-written sm_90a forward and single-pass backward kernels.
 
 Replaces reference extensions N4-N7 (``csrc/layernorm/layernorm.cu:25-148``, ``layernorm_backward.cu:130-247``,
 ``csrc/rmsnorm/rmsnorm.cu:25-125``, ``rmsnorm_backward.cu:108-196``; Python callers ``unicore/modules/layer_norm.py:22-48``,

@@ -1,6 +1,6 @@
 """Optimizer-side ops: multi-tensor L2 norm / scale, fused Adam, stochastic rounding, EMA.
 
-Native kernels: ``csrc/optim/*.cu`` (sm_100a, 128-bit vector accesses, any number of tensors per
+Native kernels: ``csrc/optim/*.cu`` (sm_90a, 128-bit vector accesses, any number of tensors per
 launch through a device-side descriptor table).  Replaces reference extensions N1-N3
 (``csrc/adam``, ``csrc/multi_tensor``, ``csrc/rounding``).  PyTorch fallbacks keep identical
 math for CPU runs.

@@ -8,7 +8,7 @@ Contract (reference ``unicore/modules/softmax_dropout.py:100-144`` + ``csrc/soft
   row ``r % bias_rows``); anything else is pre-added in PyTorch;
 * gradient flows to ``input`` and ``bias``.
 
-B200 kernel (``csrc/attn/softmax_dropout.cu``): one warp per row with 128-bit loads, rows of any
+sm_90a kernel (``csrc/attn/softmax_dropout.cu``): one warp per row with 128-bit loads, rows of any
 length (dropout included for K > 1024, which the reference cannot fuse), current-stream launch,
 and **no stored dropout mask**: keep/drop decisions are a pure function of
 ``(philox seed, offset, element index)`` and are regenerated in backward.

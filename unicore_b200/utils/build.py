@@ -1,8 +1,8 @@
-"""In-tree build of ``unicore_b200._C`` (one extension, sm_100a only).
+"""In-tree build of ``unicore_b200._C`` (one extension, sm_90a only).
 
 Two entry points share the same source list and flags:
 * ``build_inplace()`` - used by ``__graft_entry__.build()``: compiles every ``.cu`` with
-  ``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` (no PyTorch headers needed there, a few
+  ``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` (no PyTorch headers needed there, a few
   seconds each, in parallel), the binding ``.cpp`` files with the host compiler against the PyTorch
   headers, and links ``unicore_b200/_C<abi-suffix>.so`` next to the Python sources so that the
   artefact travels with the repository snapshot.  Objects are cached by source mtime.
@@ -22,7 +22,7 @@ CSRC = os.path.join(ROOT, "csrc")
 OBJ_DIR = os.path.join(ROOT, "build", "obj")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17", "--use_fast_math",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -79,6 +79,11 @@ def build_inplace(verbose=False, force=False):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     cxx = os.environ.get("CXX", "g++")
     os.makedirs(OBJ_DIR, exist_ok=True)
+    # objects built with other flags (another architecture, another compiler) are never reused
+    stamp = os.path.join(OBJ_DIR, "flags.txt")
+    flags = "\n".join([nvcc, cxx] + NVCC_FLAGS + CXX_FLAGS)
+    if not os.path.exists(stamp) or open(stamp).read() != flags:
+        force = True
     cu, cpp = sources()
     hdr_mtime = _headers_mtime()
     includes, libdirs, abi = _torch_paths()
@@ -107,7 +112,9 @@ def build_inplace(verbose=False, force=False):
                     print(out)
     target = so_path()
     objs = [_obj_for(s) for s in cu + cpp]
-    if force or jobs or not os.path.exists(target):
+    # relink whenever the library is missing or older than an object (e.g. an earlier link failed)
+    stale_so = not os.path.exists(target) or any(os.path.getmtime(o) > os.path.getmtime(target) for o in objs)
+    if force or jobs or stale_so:
         link = [cxx, "-shared", "-o", target] + objs
         for d in libdirs:
             link += ["-L", d, "-Wl,-rpath," + d]
@@ -115,6 +122,9 @@ def build_inplace(verbose=False, force=False):
         link += ["-L", cuda_lib, "-Wl,-rpath," + cuda_lib]
         link += ["-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch_cuda", "-ltorch", "-ltorch_python", "-lcudart", "-lcuda"]
         _run(link)
+    # only a complete build (compiled and linked with these flags) is recorded
+    with open(stamp, "w") as f:
+        f.write(flags)
     return target
 
 
