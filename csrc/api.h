@@ -65,6 +65,22 @@ void launch_fp32_to_bf16_sr(const float* in, void* out, long long n, unsigned lo
 void launch_ema(float* ema, const float* p, long long n, float decay, cudaStream_t stream);
 
 // ---- LayerNorm / RMSNorm -----------------------------------------------------------------------------------
+// Launch plan of the norm kernels for a [rows, cols] input: which kernel generation and template case runs, on what
+// grid, and how the rows are dealt out.  The launchers run exactly this plan.  Every kernel loops over tiles of
+// `tile_rows` consecutive rows; tile t goes to unit t % units (a unit is a warp for v3, a CTA for v2 and v1), so a
+// unit runs tiles_min or tiles_max tiles.
+enum NormKind : int { kNormFwd = 0, kNormBwd = 1, kNormFusedFwd = 2 };  // the fused op's backward runs kNormBwd
+struct NormPlan {
+  int gen;          // 3: one warp per row, 2: bulk-copy input ring, 1: rows in registers; 0: no kernel for this width
+  int nvec;         // 16-byte vectors per row
+  int vpl, lpr, r;  // v3: vectors per lane, lanes per row; v3 and v2: rows per warp (v3) or row group (v2) and tile
+  int tpr, groups;  // v2 and v1: threads per row, row groups per CTA
+  int vpt;          // v1: vectors per thread
+  int full;         // the row has no partial vector slot (v3: nvec == vpl * lpr, v2 / v1: every thread has all slots)
+  int grid, threads, tile_rows;
+  long long units, rows_per_sweep, tiles_min, tiles_max;
+};
+NormPlan norm_plan(int rows, int cols, int dtype, int kind);
 void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd,
                           int rows, int cols, float eps, int dtype, cudaStream_t stream);
 // part: float[3 * norm_bwd_parts(...) * cols] scratch (per-CTA partial column sums); dgamma/dbeta in `dtype`
@@ -80,6 +96,14 @@ void launch_rmsnorm_bwd(const void* dy, const void* x, const float* rstd, const 
                         float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate = 0);
 
 // ---- softmax + dropout ---------------------------------------------------------------------------------------
+// Launch plan of the softmax-dropout kernels (the launchers run exactly this plan).  `aligned`: every buffer of the
+// call is 16-byte aligned.  Vector path: a row is owned by `tpr` threads holding `vpt` 16-byte vectors each; scalar
+// path (vec == 0): one warp per row.  Both are grid-stride loops over rows, `sweeps` passes of the whole grid.
+struct SoftmaxPlan {
+  int vec, vpt, tpr, grid, threads;
+  long long rows_per_sweep, sweeps;
+};
+SoftmaxPlan softmax_plan(long long rows, int K, int dtype, bool aligned, bool bwd);
 // x: [rows, K] overwritten with softmax probabilities; out: dropout result (may alias x when p == 0)
 // mask row = row / mask_div (mask_rows = rows / mask_div), bias row = row % bias_rows
 void launch_softmax_dropout_fwd(void* x, void* out, const void* mask, const void* bias, long long rows, int K,

@@ -22,6 +22,8 @@
 // gradient that arrived for the logits output (`addend`) before its single store.
 #include <math_constants.h>
 
+#include <initializer_list>
+
 #include "../api.h"
 #include "../common.cuh"
 
@@ -379,6 +381,52 @@ static int resident_blocks(Kernel kernel) {
   return per_sm * sm_count2();
 }
 
+template <typename T, int VPT>
+static int resident_fwd() {
+  static const int n = resident_blocks(softmax_dropout_fwd_kernel<T, VPT>);
+  return n;
+}
+
+template <typename T, int VPT>
+static int resident_bwd() {
+  static const int n = resident_blocks(softmax_dropout_bwd_kernel<T, VPT>);
+  return n;
+}
+
+template <typename T>
+static SoftmaxPlan plan_sm(long long rows, int K, bool aligned, bool bwd, SmGeom& g) {
+  SoftmaxPlan pl{};
+  int vpt = 0;
+  if (make_sm_geom(g, rows, K, VecTraits<T>::kElems, vpt) && aligned) {
+    const int rows_per_cta = kSmThreads / g.tpr;
+    const long long need = (rows + rows_per_cta - 1) / rows_per_cta;
+    int resident = 0;
+    UB_SM_VPT(vpt, resident = bwd ? resident_bwd<T, VPT>() : resident_fwd<T, VPT>());
+    pl.vec = 1;
+    pl.vpt = vpt;
+    pl.tpr = g.tpr;
+    pl.grid = (int)(need < resident ? need : resident);
+    pl.threads = kSmThreads;
+    pl.rows_per_sweep = (long long)pl.grid * rows_per_cta;
+  } else {  // scalar kernels: 8 warps per CTA, one row per warp
+    const long long need = (rows + 7) / 8;
+    const long long cap = (long long)sm_count2() * 8;
+    pl.tpr = 32;
+    pl.grid = (int)(need < cap ? need : cap);
+    pl.threads = 256;
+    pl.rows_per_sweep = (long long)pl.grid * 8;
+  }
+  pl.sweeps = pl.rows_per_sweep > 0 ? (rows + pl.rows_per_sweep - 1) / pl.rows_per_sweep : 0;
+  return pl;
+}
+
+SoftmaxPlan softmax_plan(long long rows, int K, int dtype, bool aligned, bool bwd) {
+  SmGeom g;
+  if (dtype == kF32) return plan_sm<float>(rows, K, aligned, bwd, g);
+  if (dtype == kF16) return plan_sm<__half>(rows, K, aligned, bwd, g);
+  return plan_sm<__nv_bfloat16>(rows, K, aligned, bwd, g);
+}
+
 // 1 / P(keep) for the 14-bit threshold the kernels compare against (mirrors dropout_thresh14)
 static float keep_scale_for(float p) {
   if (!(p > 0.f)) return 1.f;
@@ -387,35 +435,31 @@ static float keep_scale_for(float p) {
   return 16384.f / (16384.f - t14);
 }
 
+static bool aligned16(std::initializer_list<const void*> ptrs) {
+  uintptr_t bits = 0;
+  for (const void* q : ptrs) bits |= reinterpret_cast<uintptr_t>(q);
+  return (bits & 15) == 0;
+}
+
 template <typename T>
 static void run_sm_fwd(void* x, void* out, const void* mask, const void* bias, long long rows, int K,
                        long long mask_div, long long bias_rows, float p, unsigned long long seed,
                        unsigned long long offset, void* logits, float* lse, cudaStream_t stream, void* probs) {
   SmGeom g;
-  int vpt = 0;
   if (probs == nullptr) probs = x;
-  const bool vec = make_sm_geom(g, rows, K, VecTraits<T>::kElems, vpt) &&
-                   ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(probs) |
-                     reinterpret_cast<uintptr_t>(mask) | reinterpret_cast<uintptr_t>(bias) |
-                     reinterpret_cast<uintptr_t>(logits)) & 15) == 0;
+  const SoftmaxPlan pl = plan_sm<T>(rows, K, aligned16({x, out, probs, mask, bias, logits}), false, g);
   g.mask_div = mask_div > 0 ? mask_div : 1;
   g.bias_rows = bias_rows > 0 ? bias_rows : 1;
   const float keep_scale = keep_scale_for(p);
-  if (vec) {
-    const int rows_per_cta = kSmThreads / g.tpr;
-    const long long need = (rows + rows_per_cta - 1) / rows_per_cta;
-    UB_SM_VPT(vpt, {
-      static const int resident = resident_blocks(softmax_dropout_fwd_kernel<T, VPT>);
-      const int grid = (int)(need < resident ? need : resident);
-      softmax_dropout_fwd_kernel<T, VPT><<<grid, kSmThreads, 0, stream>>>(
+  if (pl.vec) {
+    UB_SM_VPT(pl.vpt, {
+      softmax_dropout_fwd_kernel<T, VPT><<<pl.grid, kSmThreads, 0, stream>>>(
           (const T*)x, (T*)probs, (T*)out, (const T*)mask, (const T*)bias, g, p, keep_scale, seed, offset, (T*)logits, lse);
     });
   } else {
-    long long need = (rows + 7) / 8;
-    const long long cap = (long long)sm_count2() * 8;
-    const int grid = (int)(need < cap ? need : cap);
-    softmax_dropout_fwd_scalar<T><<<grid, 256, 0, stream>>>((const T*)x, (T*)probs, (T*)out, (const T*)mask, (const T*)bias,
-                                                            g, p, keep_scale, seed, offset, (T*)logits, lse);
+    softmax_dropout_fwd_scalar<T><<<pl.grid, pl.threads, 0, stream>>>((const T*)x, (T*)probs, (T*)out, (const T*)mask,
+                                                                      (const T*)bias, g, p, keep_scale, seed, offset,
+                                                                      (T*)logits, lse);
   }
 }
 
@@ -423,28 +467,18 @@ template <typename T>
 static void run_sm_bwd(const void* dy, void* dx, const void* probs, long long rows, int K, float p, unsigned long long seed,
                        unsigned long long offset, const float* lse, const void* addend, cudaStream_t stream) {
   SmGeom g;
-  int vpt = 0;
-  const bool vec = make_sm_geom(g, rows, K, VecTraits<T>::kElems, vpt) &&
-                   ((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(dx) | reinterpret_cast<uintptr_t>(probs) |
-                     reinterpret_cast<uintptr_t>(addend)) & 15) == 0;
+  const SoftmaxPlan pl = plan_sm<T>(rows, K, aligned16({dy, dx, probs, addend}), true, g);
   g.mask_div = 1;
   g.bias_rows = 1;
   const float keep_scale = keep_scale_for(p);
-  if (vec) {
-    const int rows_per_cta = kSmThreads / g.tpr;
-    const long long need = (rows + rows_per_cta - 1) / rows_per_cta;
-    UB_SM_VPT(vpt, {
-      static const int resident = resident_blocks(softmax_dropout_bwd_kernel<T, VPT>);
-      const int grid = (int)(need < resident ? need : resident);
-      softmax_dropout_bwd_kernel<T, VPT><<<grid, kSmThreads, 0, stream>>>(
+  if (pl.vec) {
+    UB_SM_VPT(pl.vpt, {
+      softmax_dropout_bwd_kernel<T, VPT><<<pl.grid, kSmThreads, 0, stream>>>(
           (const T*)dy, (T*)dx, (const T*)probs, g, p, keep_scale, seed, offset, lse, (const T*)addend);
     });
   } else {
-    long long need = (rows + 7) / 8;
-    const long long cap = (long long)sm_count2() * 8;
-    const int grid = (int)(need < cap ? need : cap);
-    softmax_dropout_bwd_scalar<T><<<grid, 256, 0, stream>>>((const T*)dy, (T*)dx, (const T*)probs, g, p, keep_scale, seed,
-                                                            offset, lse, (const T*)addend);
+    softmax_dropout_bwd_scalar<T><<<pl.grid, pl.threads, 0, stream>>>((const T*)dy, (T*)dx, (const T*)probs, g, p,
+                                                                      keep_scale, seed, offset, lse, (const T*)addend);
   }
 }
 

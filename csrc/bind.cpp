@@ -209,11 +209,24 @@ void ema_update(Tensor ema, const Tensor& p, double decay) {
 // ---------------------------------------------------------------------------------------------------
 // norms
 // ---------------------------------------------------------------------------------------------------
+// The norm kernels read rows, gamma, beta and bias with 16-byte vector loads and bulk copies from the first element on.
+void check_norm_operand(const Tensor& t, const char* name) {
+  check_cuda_contig(t, name);
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) == 0, name, " must be 16-byte aligned");
+}
+
+void check_norm_width(const Tensor& x) {
+  TORCH_CHECK(x.dim() == 2, "norm input must be 2-D [rows, cols]");
+  TORCH_CHECK(ub::norm_plan((int)x.size(0), (int)x.size(1), dtype_tag(x), ub::kNormFwd).gen != 0,
+              "no norm kernel for this row width and dtype");
+}
+
 std::tuple<Tensor, Tensor, Tensor> layernorm_fwd(const Tensor& x, const Tensor& gamma, const Tensor& beta, double eps) {
-  check_cuda_contig(x, "x");
-  check_cuda_contig(gamma, "gamma");
-  check_cuda_contig(beta, "beta");
-  TORCH_CHECK(x.dim() == 2 && gamma.numel() == x.size(1) && beta.numel() == x.size(1));
+  check_norm_operand(x, "x");
+  check_norm_operand(gamma, "gamma");
+  check_norm_operand(beta, "beta");
+  check_norm_width(x);
+  TORCH_CHECK(gamma.numel() == x.size(1) && beta.numel() == x.size(1));
   TORCH_CHECK(gamma.scalar_type() == x.scalar_type() && beta.scalar_type() == x.scalar_type());
   const c10::cuda::CUDAGuard guard(x.device());
   const int rows = (int)x.size(0), cols = (int)x.size(1);
@@ -242,8 +255,11 @@ static Tensor grad_out(const OptTensor& sink, const Tensor& like, int bit, int& 
 std::tuple<Tensor, Tensor, Tensor> layernorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& mean,
                                                  const Tensor& rstd, const Tensor& gamma, const OptTensor& dgamma_sink,
                                                  const OptTensor& dbeta_sink) {
-  check_cuda_contig(dy, "dy");
-  check_cuda_contig(x, "x");
+  check_norm_operand(dy, "dy");
+  check_norm_operand(x, "x");
+  check_norm_operand(gamma, "gamma");
+  check_norm_width(x);
+  TORCH_CHECK(dy.sizes() == x.sizes() && dy.scalar_type() == x.scalar_type() && gamma.numel() == x.size(1));
   const c10::cuda::CUDAGuard guard(x.device());
   const int rows = (int)x.size(0), cols = (int)x.size(1);
   Tensor dx = torch::empty_like(x);
@@ -259,9 +275,10 @@ std::tuple<Tensor, Tensor, Tensor> layernorm_bwd(const Tensor& dy, const Tensor&
 }
 
 std::tuple<Tensor, Tensor> rmsnorm_fwd(const Tensor& x, const Tensor& gamma, double eps) {
-  check_cuda_contig(x, "x");
-  check_cuda_contig(gamma, "gamma");
-  TORCH_CHECK(x.dim() == 2 && gamma.numel() == x.size(1) && gamma.scalar_type() == x.scalar_type());
+  check_norm_operand(x, "x");
+  check_norm_operand(gamma, "gamma");
+  check_norm_width(x);
+  TORCH_CHECK(gamma.numel() == x.size(1) && gamma.scalar_type() == x.scalar_type());
   const c10::cuda::CUDAGuard guard(x.device());
   const int rows = (int)x.size(0), cols = (int)x.size(1);
   Tensor y = torch::empty_like(x);
@@ -274,8 +291,11 @@ std::tuple<Tensor, Tensor> rmsnorm_fwd(const Tensor& x, const Tensor& gamma, dou
 
 std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& x, const Tensor& rstd, const Tensor& gamma,
                                        const OptTensor& dgamma_sink) {
-  check_cuda_contig(dy, "dy");
-  check_cuda_contig(x, "x");
+  check_norm_operand(dy, "dy");
+  check_norm_operand(x, "x");
+  check_norm_operand(gamma, "gamma");
+  check_norm_width(x);
+  TORCH_CHECK(dy.sizes() == x.sizes() && dy.scalar_type() == x.scalar_type() && gamma.numel() == x.size(1));
   const c10::cuda::CUDAGuard guard(x.device());
   const int rows = (int)x.size(0), cols = (int)x.size(1);
   Tensor dx = torch::empty_like(x);
@@ -287,6 +307,49 @@ std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& x, const 
                          dgamma.data_ptr(), part.data_ptr<float>(), rows, cols, dtype_tag(x), cur_stream(), acc);
   check_launch("rmsnorm_bwd");
   return {dx, dgamma};
+}
+
+// Launch plans (no kernel runs): what the launchers do for a shape, so tests can check which path a shape reaches.
+pybind11::dict norm_plan(int64_t rows, int64_t cols, at::ScalarType dtype, const std::string& kind) {
+  TORCH_CHECK(kind == "fwd" || kind == "bwd" || kind == "fused", "kind must be fwd, bwd or fused (the fused forward)");
+  TORCH_CHECK(dtype == at::kFloat || dtype == at::kHalf || dtype == at::kBFloat16, "unsupported dtype ", dtype);
+  const int tag = dtype == at::kFloat ? ub::kF32 : (dtype == at::kHalf ? ub::kF16 : ub::kBF16);
+  const ub::NormPlan p = ub::norm_plan((int)rows, (int)cols, tag,
+                                       kind == "fwd" ? ub::kNormFwd : (kind == "bwd" ? ub::kNormBwd : ub::kNormFusedFwd));
+  pybind11::dict d;
+  d["gen"] = p.gen;
+  d["nvec"] = p.nvec;
+  d["vpl"] = p.vpl;
+  d["lpr"] = p.lpr;
+  d["r"] = p.r;
+  d["tpr"] = p.tpr;
+  d["groups"] = p.groups;
+  d["vpt"] = p.vpt;
+  d["full"] = (bool)p.full;
+  d["grid"] = p.grid;
+  d["threads"] = p.threads;
+  d["tile_rows"] = p.tile_rows;
+  d["units"] = p.units;
+  d["rows_per_sweep"] = p.rows_per_sweep;
+  d["tiles_min"] = p.tiles_min;
+  d["tiles_max"] = p.tiles_max;
+  return d;
+}
+
+pybind11::dict softmax_plan(int64_t rows, int64_t K, at::ScalarType dtype, bool aligned, const std::string& kind) {
+  TORCH_CHECK(kind == "fwd" || kind == "bwd", "kind must be fwd or bwd");
+  TORCH_CHECK(dtype == at::kFloat || dtype == at::kHalf || dtype == at::kBFloat16, "unsupported dtype ", dtype);
+  const int tag = dtype == at::kFloat ? ub::kF32 : (dtype == at::kHalf ? ub::kF16 : ub::kBF16);
+  const ub::SoftmaxPlan p = ub::softmax_plan(rows, (int)K, tag, aligned, kind == "bwd");
+  pybind11::dict d;
+  d["vec"] = (bool)p.vec;
+  d["vpt"] = p.vpt;
+  d["tpr"] = p.tpr;
+  d["grid"] = p.grid;
+  d["threads"] = p.threads;
+  d["rows_per_sweep"] = p.rows_per_sweep;
+  d["sweeps"] = p.sweeps;
+  return d;
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -482,9 +545,14 @@ void embedding_bwd(const Tensor& dy, const Tensor& tokens, int64_t padding_idx, 
 std::tuple<Tensor, Tensor, Tensor, Tensor, int64_t, int64_t> bias_dropout_add_ln_fwd(
     const Tensor& x, const OptTensor& bias, const Tensor& residual, const Tensor& gamma, const Tensor& beta, double p,
     double eps) {
-  check_cuda_contig(x, "x");
-  check_cuda_contig(residual, "residual");
-  TORCH_CHECK(x.dim() == 2 && residual.sizes() == x.sizes() && residual.scalar_type() == x.scalar_type());
+  check_norm_operand(x, "x");
+  check_norm_operand(residual, "residual");
+  check_norm_operand(gamma, "gamma");
+  check_norm_operand(beta, "beta");
+  if (bias.has_value() && bias->defined()) check_norm_operand(*bias, "bias");
+  check_norm_width(x);
+  TORCH_CHECK(x.scalar_type() == at::kHalf || x.scalar_type() == at::kBFloat16, "bias_dropout_add_ln supports fp16 / bf16");
+  TORCH_CHECK(residual.sizes() == x.sizes() && residual.scalar_type() == x.scalar_type());
   TORCH_CHECK(gamma.scalar_type() == x.scalar_type() && beta.scalar_type() == x.scalar_type());
   const c10::cuda::CUDAGuard guard(x.device());
   const int rows = (int)x.size(0), cols = (int)x.size(1);
@@ -515,8 +583,13 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, OptTensor> bias_dropout_add_ln_bwd(co
                                                                               const OptTensor& dgamma_sink,
                                                                               const OptTensor& dbeta_sink,
                                                                               const OptTensor& dbias_sink) {
-  check_cuda_contig(dy, "dy");
-  check_cuda_contig(summed, "summed");
+  check_norm_operand(dy, "dy");
+  check_norm_operand(summed, "summed");
+  check_norm_operand(gamma, "gamma");
+  check_norm_width(summed);
+  TORCH_CHECK(summed.scalar_type() == at::kHalf || summed.scalar_type() == at::kBFloat16,
+              "bias_dropout_add_ln supports fp16 / bf16");
+  TORCH_CHECK(dy.sizes() == summed.sizes() && dy.scalar_type() == summed.scalar_type() && gamma.numel() == summed.size(1));
   const c10::cuda::CUDAGuard guard(dy.device());
   const int rows = (int)summed.size(0), cols = (int)summed.size(1);
   Tensor dsum = torch::empty_like(summed);
@@ -758,6 +831,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("rmsnorm_fwd", &rmsnorm_fwd);
   m.def("rmsnorm_bwd", &rmsnorm_bwd, pybind11::arg("dy"), pybind11::arg("x"), pybind11::arg("rstd"), pybind11::arg("gamma"),
         pybind11::arg("dgamma_sink") = pybind11::none());
+  m.def("norm_plan", &norm_plan, pybind11::arg("rows"), pybind11::arg("cols"), pybind11::arg("dtype"), pybind11::arg("kind"));
+  m.def("softmax_plan", &softmax_plan, pybind11::arg("rows"), pybind11::arg("K"), pybind11::arg("dtype"),
+        pybind11::arg("aligned") = true, pybind11::arg("kind") = "fwd");
   m.def("softmax_dropout_fwd", &softmax_dropout_fwd);
   m.def("softmax_dropout_bwd", &softmax_dropout_bwd);
   m.def("softmax_dropout_logits_fwd", &softmax_dropout_logits_fwd);

@@ -10,6 +10,7 @@
 //   * backward reads x and dy ONCE and emits dx plus per-CTA partial dgamma/dbeta (fp32), which a
 //     small second kernel reduces deterministically (reference: x, dy read twice + 2 extra kernels);
 //   * fp32 statistics, biased variance, rstd = rsqrt(var + eps).
+#include <algorithm>
 #include <type_traits>
 
 #include "../api.h"
@@ -946,10 +947,11 @@ __global__ void __launch_bounds__(kNormV3BwdThreads, (VPL <= 1 ? 2 : 1)) norm_bw
           float xf[EPV], df[EPV];
           unpack<T>(xv[i][k], xf);
           unpack<T>(dv[i][k], df);
-          const float nmr = -mu[i] * rs[i];
 #pragma unroll
           for (int e = 0; e < EPV; ++e) {
-            xh[i][k][e] = fmaf(xf[e], rs[i], nmr);
+            // subtract first: x * rstd - mean * rstd cancels two large products when |mean| >> std (loses ~|mean| / std
+            // ulp of x_hat), x - mean is exact there
+            xh[i][k][e] = (xf[e] - mu[i]) * rs[i];
             gy[i][k][e] = df[e] * gf[e];
             s0[i] += gy[i][k][e];
             s1[i] = fmaf(gy[i][k][e], xh[i][k][e], s1[i]);
@@ -1057,96 +1059,13 @@ static int pow2ceil(int v) {
   return p;
 }
 
-static NormGeom make_geom(int rows, int cols, int epv, int& vpt) {
-  NormGeom g;
-  g.rows = rows;
-  g.cols = cols;
-  g.nvec = cols / epv;
-  if (g.nvec <= 128) {
-    g.tpr = pow2ceil(g.nvec) < 32 ? pow2ceil(g.nvec) : 32;
-  } else {
-    g.tpr = pow2ceil((g.nvec + 3) / 4);
-  }
-  if (g.tpr > 256) g.tpr = 256;
-  vpt = (g.nvec + g.tpr - 1) / g.tpr;
-  return g;
-}
-
-static int fwd_grid(const NormGeom& g) {
-  const int rows_per_cta = kNormThreads / g.tpr;
-  const long long need = ((long long)g.rows + rows_per_cta - 1) / rows_per_cta;
-  const long long cap = (long long)sm_count() * 8;
-  return (int)(need < cap ? need : cap);
-}
-
 constexpr int kFwdR = 2, kBwdR = 2;
-
-static bool make_geom2(int rows, int cols, int epv, NormGeom2& g) {
-  g.rows = rows;
-  g.cols = cols;
-  g.nvec = cols / epv;
-  if (g.nvec < 1 || g.nvec > kNormV2Threads) return false;
-  g.tpr = g.nvec < 32 ? pow2ceil(g.nvec) : ((g.nvec + 31) / 32) * 32;
-  g.groups = kNormV2Threads / g.tpr;
-  return true;
-}
-
-static int v2_grid(const NormGeom2& g, int R) {
-  const long long need = ((long long)g.rows + (long long)g.groups * R - 1) / ((long long)g.groups * R);
-  const long long cap = (long long)sm_count() * 2;
-  const long long n = need < cap ? need : cap;
-  return (int)(n < 1 ? 1 : n);
-}
 
 static int dtype_epv(int dtype) { return dtype == kF32 ? 4 : 8; }
 
-// ---- v3 geometry -----------------------------------------------------------------------------------------------------
-static bool make_geom3(int rows, int cols, int epv, NormGeom3& g, int& vpl, int& lpr) {
-  g.rows = rows;
-  g.cols = cols;
-  g.nvec = cols / epv;
-  if (g.nvec < 1 || cols % epv != 0) return false;
-  if (g.nvec <= 32) {
-    lpr = pow2ceil(g.nvec);
-    vpl = 1;
-  } else {
-    lpr = 32;
-    vpl = (g.nvec + 31) / 32;
-  }
-  return vpl <= kNormV3MaxVPL;
-}
-
-static int v3_rows_per_iter(int vpl, int lpr) { return (lpr == 32 && vpl == 1) ? 2 : 1; }
-
-// persistent grid: `per_sm` CTAs of 8 warps per SM, fewer when the rows do not fill them
-static int v3_grid(int rows, int lpr, int r, int warps, int per_sm) {
-  const int rows_per_cta = warps * (32 / lpr) * r;
-  const long long need = ((long long)rows + rows_per_cta - 1) / rows_per_cta;
-  const long long cap = (long long)sm_count() * per_sm;
-  const long long n = need < cap ? need : cap;
-  return (int)(n < 1 ? 1 : n);
-}
-static int v3_fwd_per_sm(int vpl) { return vpl <= 3 ? 3 : (vpl == 4 ? 2 : 1); }  // bwd: as many CTAs as fit (1 or 2 per SM); each emits one fp32 partial row per array
-static int v3_bwd_per_sm(int vpl) { return vpl <= 1 ? 2 : 1; }
-
-bool norm_v2_supported(int cols, int dtype) {
-  NormGeom2 g;
-  NormGeom3 g3;
-  int vpl, lpr;
-  return make_geom3(1, cols, dtype_epv(dtype), g3, vpl, lpr) || make_geom2(1, cols, dtype_epv(dtype), g);
-}
-
-int norm_bwd_parts(int rows, int cols, int dtype) {
-  // one fp32 partial row per CTA (x3 arrays); few CTAs per SM keep the finalize pass short
-  NormGeom3 g3;
-  int vpl, lpr;
-  if (make_geom3(rows, cols, dtype_epv(dtype), g3, vpl, lpr)) return v3_grid(rows, lpr, v3_rows_per_iter(vpl, lpr), kNormV3BwdWarps, v3_bwd_per_sm(vpl));
-  NormGeom2 g;
-  if (make_geom2(rows, cols, dtype_epv(dtype), g)) return v2_grid(g, kBwdR);
-  const long long cap = (long long)sm_count() * 2;
-  const long long need = ((long long)rows + 7) / 8;
-  long long n = need < cap ? need : cap;
-  return (int)(n < 1 ? 1 : n);
+template <typename T>
+constexpr int dtype_of() {
+  return std::is_same<T, float>::value ? kF32 : (std::is_same<T, __half>::value ? kF16 : kBF16);
 }
 
 // (vectors per lane, lanes per row) -> rows per warp iteration R and whether the next R rows are prefetched: about four
@@ -1154,6 +1073,7 @@ int norm_bwd_parts(int rows, int cols, int dtype) {
 #define UB_V3_CASE(V, L, RR, PF, ...)                                                                     \
   if (vpl == V && lpr == L) {                                                                             \
     constexpr int VPL = V; constexpr int LPR = L; constexpr int R = RR; constexpr bool kPF = PF;          \
+    (void)VPL; (void)LPR; (void)R; (void)kPF;                                                             \
     __VA_ARGS__;                                                                                          \
     return true;                                                                                          \
   }
@@ -1164,18 +1084,80 @@ int norm_bwd_parts(int rows, int cols, int dtype) {
   UB_V3_CASE(2, 32, 1, true, __VA_ARGS__) UB_V3_CASE(3, 32, 1, true, __VA_ARGS__)                         \
   UB_V3_CASE(4, 32, 1, true, __VA_ARGS__)
 
+// true if UB_DISPATCH_V3 has a kernel for (vpl, lpr); r = its rows per warp iteration
+static bool v3_case(int vpl, int lpr, int& r) {
+  UB_DISPATCH_V3(r = R);
+  return false;
+}
+
+// Persistent grids: v3 runs `per_sm` CTAs per SM (forward 8 warps, backward 12 warps; the backward emits one fp32
+// partial row per CTA and array, so few CTAs keep the finalize pass short), v2 two CTAs per SM, v1 eight (forward)
+// or two (backward) - fewer when the rows do not fill them.
+NormPlan norm_plan(int rows, int cols, int dtype, int kind) {
+  NormPlan p{};
+  const int epv = dtype_epv(dtype);
+  if (rows < 0 || cols < epv || cols % epv != 0) return p;
+  const bool bwd = kind == kNormBwd;
+  p.nvec = cols / epv;
+  long long cap;
+  if (p.nvec <= 32 * kNormV3MaxVPL && v3_case(p.nvec <= 32 ? 1 : (p.nvec + 31) / 32, p.nvec <= 32 ? pow2ceil(p.nvec) : 32, p.r)) {
+    p.gen = 3;
+    p.lpr = p.nvec <= 32 ? pow2ceil(p.nvec) : 32;
+    p.vpl = (p.nvec + p.lpr - 1) / p.lpr;
+    if (kind == kNormFusedFwd) p.r = 1;  // the fused forward works on one row group at a time
+    p.full = p.nvec == p.vpl * p.lpr;
+    const int warps = bwd ? kNormV3BwdWarps : kNormV3Warps;
+    p.threads = warps * 32;
+    p.tile_rows = (32 / p.lpr) * p.r;
+    cap = (long long)sm_count() * (bwd ? (p.vpl <= 1 ? 2 : 1) : (p.vpl <= 3 ? 3 : (p.vpl == 4 ? 2 : 1)));
+    const long long need = ((long long)rows + warps * p.tile_rows - 1) / (warps * p.tile_rows);
+    p.grid = (int)std::max(1ll, std::min(need, cap));
+    p.units = (long long)p.grid * warps;
+  } else if (p.nvec <= kNormV2Threads) {
+    p.gen = 2;
+    p.tpr = p.nvec < 32 ? pow2ceil(p.nvec) : ((p.nvec + 31) / 32) * 32;
+    p.groups = kNormV2Threads / p.tpr;
+    p.r = bwd ? kBwdR : kFwdR;
+    p.full = p.nvec == p.tpr;
+    p.threads = p.tpr * p.groups;
+    p.tile_rows = p.groups * p.r;
+    const long long need = ((long long)rows + p.tile_rows - 1) / p.tile_rows;
+    p.grid = (int)std::max(1ll, std::min(need, (long long)sm_count() * 2));
+    p.units = p.grid;
+  } else {
+    p.tpr = p.nvec <= 128 ? std::min(pow2ceil(p.nvec), 32) : std::min(pow2ceil((p.nvec + 3) / 4), kNormThreads);
+    p.vpt = (p.nvec + p.tpr - 1) / p.tpr;
+    if (p.vpt > 4) return NormPlan{};
+    p.gen = 1;
+    p.groups = kNormThreads / p.tpr;
+    p.full = p.nvec == p.vpt * p.tpr;
+    p.threads = kNormThreads;
+    p.tile_rows = p.groups;
+    const long long need = bwd ? ((long long)rows + 7) / 8 : ((long long)rows + p.tile_rows - 1) / p.tile_rows;
+    p.grid = (int)std::max(1ll, std::min(need, (long long)sm_count() * (bwd ? 2 : 8)));
+    p.units = p.grid;
+  }
+  const long long tiles = ((long long)rows + p.tile_rows - 1) / p.tile_rows;
+  p.rows_per_sweep = p.units * p.tile_rows;
+  p.tiles_min = tiles / p.units;
+  p.tiles_max = (tiles + p.units - 1) / p.units;
+  return p;
+}
+
+bool norm_v2_supported(int cols, int dtype) { return norm_plan(1, cols, dtype, kNormBwd).gen >= 2; }
+
+int norm_bwd_parts(int rows, int cols, int dtype) { return norm_plan(rows, cols, dtype, kNormBwd).grid; }
+
 template <typename T, bool kRMS, bool kFused>
-static bool run_fwd_v3(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd, int rows,
-                       int cols, float eps, const void* bias, const void* residual, void* summed, float p,
-                       float keep_scale, unsigned long long seed, unsigned long long offset, cudaStream_t stream) {
-  NormGeom3 g;
-  int vpl, lpr;
-  if (!make_geom3(rows, cols, VecTraits<T>::kElems, g, vpl, lpr)) return false;
-  const int grid = v3_grid(rows, lpr, kFused ? 1 : v3_rows_per_iter(vpl, lpr), kNormV3Warps, v3_fwd_per_sm(vpl));
-  const bool full = g.nvec == vpl * lpr;
+static bool run_fwd_v3(const NormPlan& pl, const void* x, const void* gamma, const void* beta, void* y, float* mean,
+                       float* rstd, int rows, int cols, float eps, const void* bias, const void* residual, void* summed,
+                       float p, float keep_scale, unsigned long long seed, unsigned long long offset,
+                       cudaStream_t stream) {
+  const NormGeom3 g{rows, cols, pl.nvec};
+  const int vpl = pl.vpl, lpr = pl.lpr, grid = pl.grid;
   UB_DISPATCH_V3({
     constexpr int RF = kFused ? 1 : R;
-    if (full)
+    if (pl.full)
       norm_fwd_v3_kernel<T, VPL, LPR, RF, kPF, kRMS, kFused, true><<<grid, kNormV3Threads, 0, stream>>>(
           (const T*)x, (const T*)gamma, (const T*)beta, (T*)y, mean, rstd, g, eps, (const T*)bias, (const T*)residual,
           (T*)summed, p, keep_scale, seed, offset);
@@ -1188,22 +1170,20 @@ static bool run_fwd_v3(const void* x, const void* gamma, const void* beta, void*
 }
 
 template <typename T, bool kRMS, bool kFused>
-static bool run_bwd_v3(const void* dy, const void* x, const float* mean, const float* rstd, const void* gamma, void* dx,
-                       void* dgamma, void* dbeta, void* dbias, float* part, int rows, int cols, void* dx_drop, float p,
-                       float keep_scale, unsigned long long seed, unsigned long long offset, cudaStream_t stream) {
-  NormGeom3 g;
-  int vpl, lpr;
-  if (!make_geom3(rows, cols, VecTraits<T>::kElems, g, vpl, lpr)) return false;
-  const int grid = v3_grid(rows, lpr, v3_rows_per_iter(vpl, lpr), kNormV3BwdWarps, v3_bwd_per_sm(vpl));
+static bool run_bwd_v3(const NormPlan& pl, const void* dy, const void* x, const float* mean, const float* rstd,
+                       const void* gamma, void* dx, void* dgamma, void* dbeta, void* dbias, float* part, int rows,
+                       int cols, void* dx_drop, float p, float keep_scale, unsigned long long seed,
+                       unsigned long long offset, cudaStream_t stream) {
+  const NormGeom3 g{rows, cols, pl.nvec};
+  const int vpl = pl.vpl, lpr = pl.lpr, grid = pl.grid;
   const size_t smem = (size_t)kNormV3BwdWarps * cols * sizeof(float);
   auto finish = [&]() {
     colsum_finalize_kernel<T><<<dim3((cols + 31) / 32, 3), 1024, 0, stream>>>(part, grid, cols, (T*)dgamma, (T*)dbeta,
                                                                               (T*)dbias, g_acc_mask);
   };
-  const bool full = g.nvec == vpl * lpr;
   UB_DISPATCH_V3({
-    auto kern = full ? norm_bwd_v3_kernel<T, VPL, LPR, R, (kPF && VPL <= 3), kRMS, kFused, true>
-                     : norm_bwd_v3_kernel<T, VPL, LPR, R, (kPF && VPL <= 3), kRMS, kFused, false>;
+    auto kern = pl.full ? norm_bwd_v3_kernel<T, VPL, LPR, R, (kPF && VPL <= 3), kRMS, kFused, true>
+                        : norm_bwd_v3_kernel<T, VPL, LPR, R, (kPF && VPL <= 3), kRMS, kFused, false>;
     if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, kNormV3BwdThreads, smem, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx, part, g,
                                                  (T*)dx_drop, dbias != nullptr ? 1 : 0, p, keep_scale, seed, offset);
@@ -1234,25 +1214,24 @@ static void run_fwd(const void* x, const void* gamma, const void* beta, void* y,
                     int cols, float eps, const void* bias, const void* residual, void* summed, float p,
                     unsigned long long seed, unsigned long long offset, cudaStream_t stream) {
   const float keep_scale = p > 0.f ? 1.f / (1.f - p) : 1.f;
-  if (run_fwd_v3<T, kRMS, kFused>(x, gamma, beta, y, mean, rstd, rows, cols, eps, bias, residual, summed, p, keep_scale,
-                                  seed, offset, stream))
-    return;
-  NormGeom2 g2;
-  if (make_geom2(rows, cols, VecTraits<T>::kElems, g2)) {
+  const NormPlan pl = norm_plan(rows, cols, dtype_of<T>(), kFused ? kNormFusedFwd : kNormFwd);
+  if (pl.gen == 3) {
+    run_fwd_v3<T, kRMS, kFused>(pl, x, gamma, beta, y, mean, rstd, rows, cols, eps, bias, residual, summed, p,
+                                keep_scale, seed, offset, stream);
+  } else if (pl.gen == 2) {
+    const NormGeom2 g2{rows, cols, pl.tpr, pl.nvec, pl.groups};
     auto fkern = norm_fwd_v2_kernel<T, kFwdR, kRMS, kFused>;
-    const size_t fsmem = (size_t)kNormStages * g2.groups * kFwdR * cols * sizeof(T) * (kFused ? 2 : 1) + 64;
+    const size_t fsmem = (size_t)kNormStages * pl.tile_rows * cols * sizeof(T) * (kFused ? 2 : 1) + 64;
     cudaFuncSetAttribute(fkern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem);
-    fkern<<<v2_grid(g2, kFwdR), g2.tpr * g2.groups, fsmem, stream>>>(
+    fkern<<<pl.grid, pl.threads, fsmem, stream>>>(
         (const T*)x, (const T*)gamma, (const T*)beta, (T*)y, mean, rstd, g2, eps, (const T*)bias, (const T*)residual,
         (T*)summed, p, keep_scale, seed, offset);
-    return;
+  } else if (pl.gen == 1) {
+    const NormGeom g{rows, cols, pl.tpr, pl.nvec};
+    UB_DISPATCH_VPT(pl.vpt, (norm_fwd_kernel<T, VPT, kRMS, kFused><<<pl.grid, kNormThreads, 0, stream>>>(
+                                (const T*)x, (const T*)gamma, (const T*)beta, (T*)y, mean, rstd, g, eps,
+                                (const T*)bias, (const T*)residual, (T*)summed, p, keep_scale, seed, offset)));
   }
-  int vpt;
-  NormGeom g = make_geom(rows, cols, VecTraits<T>::kElems, vpt);
-  const int grid = fwd_grid(g);
-  UB_DISPATCH_VPT(vpt, (norm_fwd_kernel<T, VPT, kRMS, kFused><<<grid, kNormThreads, 0, stream>>>(
-                           (const T*)x, (const T*)gamma, (const T*)beta, (T*)y, mean, rstd, g, eps, (const T*)bias,
-                           (const T*)residual, (T*)summed, p, keep_scale, seed, offset)));
 }
 
 template <typename T, bool kRMS, bool kFused>
@@ -1260,37 +1239,36 @@ static void run_bwd(const void* dy, const void* x, const float* mean, const floa
                     void* dgamma, void* dbeta, void* dbias, float* part, int rows, int cols, void* dx_drop, float p,
                     unsigned long long seed, unsigned long long offset, cudaStream_t stream) {
   const float keep_scale = p > 0.f ? 1.f / (1.f - p) : 1.f;
-  if (run_bwd_v3<T, kRMS, kFused>(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, dbias, part, rows, cols, dx_drop, p,
-                                  keep_scale, seed, offset, stream))
-    return;
-  NormGeom2 g2;
-  if (make_geom2(rows, cols, VecTraits<T>::kElems, g2)) {
-    const int grid = v2_grid(g2, kBwdR);
+  const NormPlan pl = norm_plan(rows, cols, dtype_of<T>(), kNormBwd);
+  if (pl.gen == 3) {
+    run_bwd_v3<T, kRMS, kFused>(pl, dy, x, mean, rstd, gamma, dx, dgamma, dbeta, dbias, part, rows, cols, dx_drop, p,
+                                keep_scale, seed, offset, stream);
+  } else if (pl.gen == 2) {
+    const NormGeom2 g2{rows, cols, pl.tpr, pl.nvec, pl.groups};
     const size_t smem2 = (((size_t)3 * cols * sizeof(float) + 127) & ~(size_t)127) +
-                         (size_t)kNormStages * g2.groups * kBwdR * cols * sizeof(T) * 2 + 64;
+                         (size_t)kNormStages * pl.tile_rows * cols * sizeof(T) * 2 + 64;
     auto kern = norm_bwd_v2_kernel<T, kBwdR, kRMS, kFused>;
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2);
-    kern<<<grid, g2.tpr * g2.groups, smem2, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx,
-                                                       part, g2, (T*)dx_drop, dbias != nullptr ? 1 : 0, p, keep_scale,
-                                                       seed, offset);
-    colsum_finalize_kernel<T><<<dim3((cols + 31) / 32, 3), 1024, 0, stream>>>(part, grid, cols, (T*)dgamma, (T*)dbeta,
-                                                                              (T*)dbias, g_acc_mask);
-    return;
+    kern<<<pl.grid, pl.threads, smem2, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx, part,
+                                                  g2, (T*)dx_drop, dbias != nullptr ? 1 : 0, p, keep_scale, seed,
+                                                  offset);
+    colsum_finalize_kernel<T><<<dim3((cols + 31) / 32, 3), 1024, 0, stream>>>(part, pl.grid, cols, (T*)dgamma,
+                                                                              (T*)dbeta, (T*)dbias, g_acc_mask);
+  } else if (pl.gen == 1) {
+    const NormGeom g{rows, cols, pl.tpr, pl.nvec};
+    const int parts = pl.grid;
+    float* dg_part = part;
+    float* db_part = part + (size_t)parts * cols;
+    const size_t smem = (size_t)(kRMS ? 1 : 2) * cols * sizeof(float);
+    UB_DISPATCH_VPT(pl.vpt, {
+      auto kern = norm_bwd_kernel<T, VPT, kRMS, kFused>;
+      if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      kern<<<parts, kNormThreads, smem, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx,
+                                                  dg_part, db_part, g, (T*)dx_drop, p, keep_scale, seed, offset);
+    });
+    norm_param_grad_kernel<T><<<(cols + 31) / 32, 256, 0, stream>>>(dg_part, kRMS ? nullptr : db_part, parts, cols,
+                                                                    (T*)dgamma, (T*)dbeta, g_acc_mask);
   }
-  int vpt;
-  NormGeom g = make_geom(rows, cols, VecTraits<T>::kElems, vpt);
-  const int parts = norm_bwd_parts(rows, cols, std::is_same<T, float>::value ? kF32 : kF16);
-  float* dg_part = part;
-  float* db_part = part + (size_t)parts * cols;
-  const size_t smem = (size_t)(kRMS ? 1 : 2) * cols * sizeof(float);
-  UB_DISPATCH_VPT(vpt, {
-    auto kern = norm_bwd_kernel<T, VPT, kRMS, kFused>;
-    if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<parts, kNormThreads, smem, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx,
-                                                dg_part, db_part, g, (T*)dx_drop, p, keep_scale, seed, offset);
-  });
-  norm_param_grad_kernel<T><<<(cols + 31) / 32, 256, 0, stream>>>(dg_part, kRMS ? nullptr : db_part, parts, cols,
-                                                                  (T*)dgamma, (T*)dbeta, g_acc_mask);
 }
 
 void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd,

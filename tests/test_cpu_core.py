@@ -459,3 +459,21 @@ def test_staged_logging_outputs_and_lazy_step_statistics():
     full = dict(stats.items())
     assert full["loss"] == 2.5 and abs(float(full["gnorm"]) - 1.25) < 1e-6 and "_hidden" not in full
     assert stats._values is not None and stats["loss"] == 2.5
+
+
+def test_norm_rows_are_16_byte_aligned():
+    """The norm kernels read rows with 16-byte vector loads and bulk copies: a contiguous view at an odd element
+    offset must reach them as an aligned copy, an aligned tensor as itself."""
+    from unicore_b200.ops._native import aligned_rows
+
+    for dtype in (torch.float32, torch.float16, torch.bfloat16):
+        buf = torch.randn(3 * 5 * 64 + 1).to(dtype)
+        for x in (buf[1:].view(3, 5, 64), buf[1:].view(15, 64)):
+            assert x.is_contiguous() and x.data_ptr() % 16 != 0
+            rows = aligned_rows(x)
+            assert rows.shape == (15, 64) and rows.is_contiguous() and rows.data_ptr() % 16 == 0
+            assert torch.equal(rows, x.reshape(15, 64))
+        aligned = torch.randn(4, 3, 64).to(dtype)
+        assert aligned.data_ptr() % 16 == 0 and aligned_rows(aligned).data_ptr() == aligned.data_ptr()
+        strided = torch.randn(64, 30).to(dtype).t()  # not contiguous: copied
+        assert torch.equal(aligned_rows(strided), strided) and aligned_rows(strided).is_contiguous()

@@ -594,3 +594,202 @@ def test_gaussian_basis(dtype):
     for got, ref in zip((mul_w, bias_w, means, stds), ref_in):
         scale = max(1.0, ref.grad.abs().max().item())
         assert (got.grad.float() - ref.grad.view_as(got.grad)).abs().max().item() < 3e-2 * scale
+
+
+# ---------------------------------------------------------------------------------------------------
+# softmax_dropout on every launch path, past the first sweep of the grid, against fp64
+# ---------------------------------------------------------------------------------------------------
+E32 = 2.0 ** -24
+UNIT = {torch.float32: 2.0 ** -24, torch.float16: 2.0 ** -11, torch.bfloat16: 2.0 ** -8}  # unit roundoff
+# row lengths in 16-byte vectors: threads per row < 32 (8), = 32 with 1..4 vectors per thread (32, 64, 96, 128),
+# 64 threads (160, 256: 3 and 4 vectors), 256 threads (640, 1024); the scalar kernels take K = 99 (not a multiple of
+# the vector width) and K past the longest vector row
+SM_NVECS = [8, 32, 64, 96, 128, 160, 256, 640, 1024]
+SM_SCALAR_K = [99, "long"]
+
+
+def _sm_k(spec, dtype):
+    epv = 16 // torch.empty((), dtype=dtype).element_size()
+    return 1024 * epv + epv if spec == "long" else spec
+
+
+def _sm_case(plan):
+    if not plan["vec"]:
+        return ("scalar",)
+    t = plan["tpr"]
+    return ("vec", "<32" if t < 32 else ("32" if t == 32 else ("256" if t == 256 else "64-128")), plan["vpt"])
+
+
+def _sm_keep_scale(p):
+    """1 / P(keep): the kernels compare 14 random bits against round(p * 2^14), so p is quantised to 1 / 16384."""
+    return 1.0 if p == 0 else 16384.0 / (16384.0 - round(p * 16384.0))
+
+
+def _sm_rows(K, dtype, Q):
+    """Rows (a multiple of Q) that make every CTA of both kernels take 3 sweeps or more, with a ragged last sweep.
+    Rows past the longest vector row run one sweep only: three would take gigabytes; the scalar kernels' later
+    sweeps are covered by K = 99."""
+    nat = _ops().native()
+    if K > 1024 * (16 // torch.empty((), dtype=dtype).element_size()):
+        return Q * 17
+    sweep = max(nat.softmax_plan(1 << 40, K, dtype, True, k)["rows_per_sweep"] for k in ("fwd", "bwd"))
+    rows = -(-(3 * sweep + sweep // 2 + 1) // Q) * Q
+    for k in ("fwd", "bwd"):
+        pl = nat.softmax_plan(rows, K, dtype, True, k)
+        while rows % pl["rows_per_sweep"] == 0:
+            rows += Q
+        assert pl["sweeps"] >= 4, pl
+    return rows
+
+
+def _sm_chunks(rows, K):
+    step = max(1, (1 << 21) // K)
+    for r0 in range(0, rows, step):
+        yield slice(r0, min(rows, r0 + step))
+
+
+def _within(got, ref, bound, what):
+    err = (got.double() - ref).abs()
+    bad = err > bound
+    if bad.any():
+        i = tuple(bad.nonzero()[0].tolist())
+        raise AssertionError("{}: {} elements out of bound, first at {}: got {}, want {} +- {}".format(
+            what, int(bad.sum()), i, got[i].item(), ref[i].item(), bound[i].item()))
+
+
+def _check_sm_forward(z, probs, out, p, dtype):
+    """probs = softmax(z), out = keep * probs / P(keep), with keep read from out; returns (keep, live) counts.
+    Bound: one rounding of the output type plus fp32 error relative to the probability: the exponent's argument
+    (2 |z - max| ulp), exp2 and the row sum (< 80 ulp)."""
+    u, tiny = UNIT[dtype], torch.finfo(dtype).tiny * UNIT[dtype]
+    scale = _sm_keep_scale(p)
+    kept = live = 0
+    for s in _sm_chunks(*z.shape):
+        zd = z[s].double()
+        yr = torch.softmax(zd, -1)
+        comp = yr * E32 * (2 * (zd - zd.max(-1, keepdim=True).values).abs() + 80)
+        if probs is not None:
+            _within(probs[s], yr, u * (yr + comp) + comp + tiny, "probs")
+        keep = out[s] != 0 if p > 0 else torch.ones_like(yr, dtype=torch.bool)
+        ref = yr * keep * scale
+        _within(out[s], ref, u * (ref + comp * scale) + comp * scale + tiny, "out")
+        alive = yr > 1e-3 / z.shape[1]  # probabilities that cannot round to zero
+        kept += int((keep & alive).sum())
+        live += int(alive.sum())
+    return kept, live
+
+
+def _check_sm_backward(dy, probs, out, dx, p, dtype, z=None, addend=None):
+    """dx = y * (d - sum(d * y)) (+ addend), d = keep * dy / P(keep), keep read from the forward's `out`.  y: the
+    stored probabilities `probs`, or (logits mode) softmax(z) rebuilt by backward from z and the row log-sum-exp,
+    with error e_y: one rounding (absolute below the normal range), the exponent's argument and the log-sum-exp."""
+    u, tiny = UNIT[dtype], torch.finfo(dtype).tiny * UNIT[dtype]
+    scale = _sm_keep_scale(p)
+    for s in _sm_chunks(*dy.shape):
+        if z is None:
+            yd, e_y = probs[s].double(), 0.0
+        else:
+            zd = z[s].double()
+            yd = torch.softmax(zd, -1)
+            lse = torch.logsumexp(zd, -1, keepdim=True)
+            e_y = yd * (u + E32 * (2 * (zd - lse).abs() + 2 * lse.abs() + 80)) + tiny
+        keep = (out[s] != 0) if p > 0 else 1.0
+        d = dy[s].double() * keep * scale
+        dot = (d * yd).sum(-1, keepdim=True)
+        ref = yd * (d - dot)
+        comp = ((d - dot).abs() * e_y + yd * ((d.abs() * e_y).sum(-1, keepdim=True)
+                                               + 72 * E32 * (d * yd).abs().sum(-1, keepdim=True))
+                + 4 * E32 * ((d * yd).abs() + (yd * dot).abs()))
+        if addend is not None:
+            ref = ref + addend[s].double()
+            comp = comp + 2 * E32 * addend[s].double().abs()
+        _within(dx[s], ref, u * (ref.abs() + comp) + comp + tiny, "dx")
+
+
+def _sm_rate(kept, live, p):
+    if p > 0:
+        q = 1 - 1 / _sm_keep_scale(p)
+        assert abs(kept / live - (1 - q)) < 6 * math.sqrt(q * (1 - q) / live), kept / live
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16, torch.float32])
+@pytest.mark.parametrize("k", SM_NVECS + SM_SCALAR_K)
+@pytest.mark.parametrize("mode", ["plain", "in_place", "logits"])
+def test_softmax_dropout_all_paths(mode, k, dtype):
+    """Every vector case (threads per row, vectors per thread) and the scalar kernels, plain / in-place / logits mode,
+    p in {0, 0.2}; each CTA runs several sweeps, and backward must regenerate exactly the forward's keep mask."""
+    nat = _ops().native()
+    epv = 16 // torch.empty((), dtype=dtype).element_size()
+    K = k * epv if isinstance(k, int) and k in SM_NVECS else _sm_k(k, dtype)
+    Q = 16
+    rows = _sm_rows(K, dtype, Q)
+    assert _sm_case(nat.softmax_plan(rows, K, dtype, True, "fwd"))[0] == ("vec" if k in SM_NVECS else "scalar")
+    g = torch.Generator(device="cuda").manual_seed(K)
+    x = (torch.randn(rows // Q, Q, K, device="cuda", generator=g) * 2).to(dtype)
+    bias = torch.randn(1, Q, K, device="cuda", generator=g).to(dtype)
+    dy = torch.randn(rows // Q, Q, K, device="cuda", generator=g).to(dtype)
+    addend = torch.randn(rows // Q, Q, K, device="cuda", generator=g).to(dtype)
+    for p in (0.0, 0.2):
+        if mode == "logits":
+            out, z, lse, seed, off = nat.softmax_dropout_logits_fwd(x, None, bias, p, True)
+            u = UNIT[dtype]
+            for s in _sm_chunks(rows // Q, Q * K):
+                zr = x[s].double() + bias.double()
+                _within(z[s], zr, u * zr.abs() + 2 * E32 * zr.abs(), "logits")
+            kept, live = _check_sm_forward(z.view(rows, K), None, out.view(rows, K), p, dtype)
+            dx = nat.softmax_dropout_logits_bwd(dy, z, lse, addend, p, seed, off)
+            _check_sm_backward(dy.view(rows, K), None, out.view(rows, K), dx.view(rows, K), p, dtype,
+                               z=z.view(rows, K), addend=addend.view(rows, K))
+        else:
+            xin = x.clone()
+            out, probs, seed, off = nat.softmax_dropout_fwd(xin, None, None, p, True, mode == "in_place")
+            assert (probs.data_ptr() == xin.data_ptr()) == (mode == "in_place")
+            kept, live = _check_sm_forward(x.view(rows, K), probs.view(rows, K), out.view(rows, K), p, dtype)
+            dx = nat.softmax_dropout_bwd(dy, probs, p, seed, off)
+            _check_sm_backward(dy.view(rows, K), probs.view(rows, K), out.view(rows, K), dx.view(rows, K), p, dtype)
+        _sm_rate(kept, live, p)
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16, torch.float32])
+@pytest.mark.parametrize("nvec", [8, 128, 256])
+def test_softmax_dropout_vector_and_scalar_paths_agree(dtype, nvec):
+    """The same rows and Philox state through the vector kernels (aligned buffers) and the scalar kernels (a
+    contiguous view at an odd element offset): identical keep masks, probabilities equal to rounding."""
+    nat = _ops().native()
+    epv = 16 // torch.empty((), dtype=dtype).element_size()
+    K, Q = nvec * epv, 8
+    rows = _sm_rows(K, dtype, Q)
+    assert nat.softmax_plan(rows, K, dtype, True, "fwd")["vec"] and nat.softmax_plan(rows, K, dtype, True, "bwd")["vec"]
+    assert not nat.softmax_plan(rows, K, dtype, False, "fwd")["vec"]
+    assert not nat.softmax_plan(rows, K, dtype, False, "bwd")["vec"]
+    g = torch.Generator(device="cuda").manual_seed(nvec)
+    xbuf = (torch.randn(rows * K + 1, device="cuda", generator=g) * 2).to(dtype)
+    dbuf = torch.randn(rows * K + 1, device="cuda", generator=g).to(dtype)
+    xm, dym = xbuf[1:].view(rows // Q, Q, K), dbuf[1:].view(rows // Q, Q, K)
+    assert xm.data_ptr() % 16 != 0
+    res = []
+    for xi, di in ((xm.clone(), dym.clone()), (xm, dym)):
+        torch.cuda.manual_seed(5)
+        out, probs, seed, off = nat.softmax_dropout_fwd(xi, None, None, 0.2, True, False)
+        dx = nat.softmax_dropout_bwd(di, probs, 0.2, seed, off)
+        res.append((out, probs, dx, (seed, off)))
+    (oa, pa, da, sa), (om, pm, dm, sm) = res
+    assert sa == sm
+    assert torch.equal(oa != 0, om != 0)
+    for probs, out, dx in ((pa, oa, da), (pm, om, dm)):
+        kept, live = _check_sm_forward(xm.reshape(rows, K), probs.view(rows, K), out.view(rows, K), 0.2, dtype)
+        _sm_rate(kept, live, 0.2)
+        _check_sm_backward(dym.reshape(rows, K), probs.view(rows, K), out.view(rows, K), dx.view(rows, K), 0.2, dtype)
+
+
+def test_softmax_dispatch_coverage():
+    """The test row lengths reach every case the softmax launchers can dispatch to (launches no kernel)."""
+    nat = _ops().native()
+    for dtype in (torch.float16, torch.bfloat16, torch.float32):
+        epv = 16 // torch.empty((), dtype=dtype).element_size()
+        reachable = {_sm_case(nat.softmax_plan(64, K, dtype, True, kind))
+                     for K in range(1, 1024 * epv + 2 * epv) for kind in ("fwd", "bwd")}
+        tested = {_sm_case(nat.softmax_plan(64, n * epv, dtype, True, kind)) for n in SM_NVECS for kind in ("fwd", "bwd")}
+        tested |= {_sm_case(nat.softmax_plan(64, _sm_k(k, dtype), dtype, True, "fwd")) for k in SM_SCALAR_K}
+        assert tested == reachable, (dtype, sorted(reachable - tested))
+        assert not nat.softmax_plan(64, 64 * epv, dtype, False, "fwd")["vec"]

@@ -56,6 +56,7 @@ _LAUNCHES_PER_CALL = {
     # not kernels: allocation / capability queries
     "SymmAllocation": 0, "symm_error_channel": 0, "symm_mem_supported": 0, "symm_multicast_supported": 0,
     "symm_tail_max_blocks": 0, "symm_pick_algo": 0, "norm_v2_supported": 0,
+    "norm_plan": 0, "softmax_plan": 0,
 }
 _launch_count = 0
 
@@ -118,6 +119,17 @@ def aligned_param(t, dtype=None):
     if not t.is_contiguous() or t.data_ptr() % 16 != 0:
         t = t.clone(memory_format=torch.contiguous_format)
     return t
+
+
+def aligned_rows(t):
+    """``t`` as a contiguous, 16-byte aligned ``[rows, t.shape[-1]]`` tensor.
+
+    The row kernels (norms, the fused bias + dropout + residual + LayerNorm) read with 16-byte vector loads and bulk
+    copies from the first element on, so a contiguous view at an odd element offset (``buf[1:].view(n, d)``) must
+    not reach them.  Such a view is copied once to a fresh (aligned) buffer: the kernel still runs, and the copy is
+    the same pass an eager fallback would have to make anyway.  Aligned rows are returned as a view, without a copy.
+    """
+    return aligned_param(t.reshape(-1, t.shape[-1]))
 
 
 def use_native(*tensors) -> bool:

@@ -19,7 +19,7 @@ import torch
 import torch.nn.functional as F
 
 from . import grad_sink
-from ._native import aligned_param, native, use_native
+from ._native import aligned_param, aligned_rows, native, use_native
 
 
 # ------------------------------------------------------------------------------------------------
@@ -147,8 +147,8 @@ class _BiasDropoutAddLNFn(torch.autograd.Function):
     def forward(ctx, x, bias, residual, ln_weight, ln_bias, p, eps, training):
         p = float(p) if training else 0.0
         shape = x.shape
-        x2 = x.contiguous().view(-1, shape[-1])
-        r2 = residual.contiguous().view(-1, shape[-1])
+        x2 = aligned_rows(x)
+        r2 = aligned_rows(residual)
         y, mean, rstd, summed, seed, offset = native().bias_dropout_add_ln_fwd(x2, bias, r2, ln_weight, ln_bias, p, eps)
         ctx.save_for_backward(summed, ln_weight, mean, rstd)
         ctx.p = p
@@ -162,7 +162,7 @@ class _BiasDropoutAddLNFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         summed, ln_weight, mean, rstd = ctx.saved_tensors
-        dy2 = dy.contiguous().view(summed.shape)
+        dy2 = aligned_rows(dy)
         # dsum: gradient w.r.t. (residual + dropout(x+bias)); dx = dropout-masked dsum
         b_sink, g_sink, be_sink = ctx.sinks
         dsum, dx, dgamma, dbeta, dbias = native().bias_dropout_add_ln_bwd(

@@ -13,14 +13,14 @@ import torch
 import torch.nn.functional as F
 
 from . import grad_sink
-from ._native import aligned_param, native, use_native
+from ._native import aligned_param, aligned_rows, native, use_native
 
 
 class _LayerNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, eps):
         shape = x.shape
-        x2 = x.contiguous().view(-1, shape[-1])
+        x2 = aligned_rows(x)
         y, mean, rstd = native().layernorm_fwd(x2, weight, bias, eps)
         ctx.save_for_backward(x2, weight, mean, rstd)
         ctx.has_bias = bias is not None
@@ -31,7 +31,7 @@ class _LayerNormFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x2, weight, mean, rstd = ctx.saved_tensors
-        dy2 = dy.contiguous().view(x2.shape)
+        dy2 = aligned_rows(dy)
         g_sink, b_sink = ctx.sinks
         dx, dgamma, dbeta = native().layernorm_bwd(dy2, x2, mean, rstd, weight, grad_sink.sink(g_sink), grad_sink.sink(b_sink))
         if g_sink is not None:
@@ -47,7 +47,7 @@ class _RMSNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, eps):
         shape = x.shape
-        x2 = x.contiguous().view(-1, shape[-1])
+        x2 = aligned_rows(x)
         y, rstd = native().rmsnorm_fwd(x2, weight, eps)
         ctx.save_for_backward(x2, weight, rstd)
         ctx.g_sink = grad_sink.claim(weight, ctx.needs_input_grad[1])
@@ -56,7 +56,7 @@ class _RMSNormFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x2, weight, rstd = ctx.saved_tensors
-        dy2 = dy.contiguous().view(x2.shape)
+        dy2 = aligned_rows(dy)
         dx, dgamma = native().rmsnorm_bwd(dy2, x2, rstd, weight, grad_sink.sink(ctx.g_sink))
         if ctx.g_sink is not None:
             grad_sink.done(ctx.g_sink)
