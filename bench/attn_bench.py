@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """Micro-benchmark of the wgmma fused attention vs the materialised PyTorch path.
 
-BERT-base shape by default: B=32, H=12, L=512, D=64, fp16, rel-pos bias [1,H,L,L], dropout 0.1.
+BERT-base shape by default: B=32, H=12, L=512, D=64, fp16, rel-pos bias [1,H,L,L], dropout 0.1; --D sets the
+head dim (softmax scale 1/sqrt(D)).
 Times forward and forward+backward with CUDA events (L2 flushed between iterations by writing a
 256 MB buffer) and prints one JSON line per variant with achieved TFLOP/s (4*B*H*L*L*D FLOPs forward,
 2.5x that backward) and the fraction of the dense 16-bit peak (MEASURED_PEAKS.json if present, else the H100
@@ -9,6 +10,7 @@ data sheet).
 """
 import argparse
 import json
+import math
 import os
 import sys
 
@@ -38,6 +40,7 @@ def main():
     ap.add_argument("--B", type=int, default=32)
     ap.add_argument("--H", type=int, default=12)
     ap.add_argument("--L", type=int, default=512)
+    ap.add_argument("--D", type=int, default=64)
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--dtype", default="float16")
     ap.add_argument("--only", default="")
@@ -46,7 +49,8 @@ def main():
 
     assert ops.USE_NATIVE
     dtype = getattr(torch, args.dtype)
-    B, H, L, D = args.B, args.H, args.L, 64
+    B, H, L, D = args.B, args.H, args.L, args.D
+    scale = 1.0 / math.sqrt(D)
     peak = 989.4   # H100 SXM data sheet, dense fp16 / bf16 TFLOP/s (700 W); a measured peak replaces it when present
     try:
         peak = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))["bf16_tflops"]
@@ -72,7 +76,7 @@ def main():
 
         def fwd():
             return ops.fused_attention(q, k, v, bias=cfg["bias"], key_padding_mask=cfg["kpm"], dropout_p=cfg["p"],
-                                       training=True, scale=0.125)
+                                       training=True, scale=scale)
 
         def fwd_bwd():
             qkv.grad = None
@@ -84,7 +88,7 @@ def main():
         t_fb = timeit(fwd_bwd, args.iters, flush)
         t_b = t_fb - t_f
         print(json.dumps({
-            "kernel": "fmha_sm90", "variant": name, "B": B, "H": H, "L": L, "dtype": args.dtype,
+            "kernel": "fmha_sm90", "variant": name, "B": B, "H": H, "L": L, "D": D, "dtype": args.dtype,
             "fwd_ms": round(t_f, 4), "bwd_ms": round(t_b, 4),
             "fwd_tflops": round(fwd_flops / t_f / 1e9, 1), "bwd_tflops": round(2.5 * fwd_flops / t_b / 1e9, 1),
             "fwd_frac_of_peak": round(fwd_flops / t_f / 1e9 / peak, 4),
@@ -93,7 +97,7 @@ def main():
     if not args.only:
         # materialised reference path (what the reference framework executes)
         def ref_fwd():
-            return ops.attention_reference(q, k, v, bias, kpm, 0.1, True, 0.125)
+            return ops.attention_reference(q, k, v, bias, kpm, 0.1, True, scale)
 
         def ref_fwd_bwd():
             qkv.grad = None
@@ -103,8 +107,11 @@ def main():
         with torch.no_grad():
             t_f = timeit(ref_fwd, max(2, args.iters // 3), flush)
         t_fb = timeit(ref_fwd_bwd, max(2, args.iters // 3), flush)
-        print(json.dumps({"kernel": "pytorch_materialised", "variant": "bias_mask_dropout", "fwd_ms": round(t_f, 4),
-                          "bwd_ms": round(t_fb - t_f, 4)}), flush=True)
+        t_b = t_fb - t_f
+        print(json.dumps({"kernel": "pytorch_materialised", "variant": "bias_mask_dropout", "D": D,
+                          "fwd_ms": round(t_f, 4), "bwd_ms": round(t_b, 4),
+                          "fwd_tflops": round(fwd_flops / t_f / 1e9, 1),
+                          "bwd_tflops": round(2.5 * fwd_flops / t_b / 1e9, 1)}), flush=True)
 
 
 if __name__ == "__main__":

@@ -6,15 +6,22 @@
 
 namespace ub {
 
-// rows of the TMA boxes of q / k / v (and dO): the forward walks 128-key tiles with 64 query rows per CTA, the
-// backward walks 64-row query tiles with 64 keys per CTA
-constexpr int kFwdQBoxRows = 64, kFwdKVBoxRows = 128, kBwdBoxRows = 64;
+// Head dims the kernels take: D % 8 == 0 and 8 <= D <= 128.  D <= 64 runs on the 64-column kernels, larger D on the
+// 128-column ones; the TMA unit zero-fills the columns D..63 / D..127 of every tile in shared memory.
+constexpr int kMaxHeadDim = 128;
+inline bool fmha_head_dim_supported(long long d) { return d >= 8 && d <= kMaxHeadDim && d % 8 == 0; }
+inline int fmha_padded_head_dim(int d) { return d <= 64 ? 64 : 128; }
+
+// rows of the TMA boxes of q / k / v (and dO): the forward walks 128-key tiles (64-key tiles at padded width 128)
+// with 64 query rows per CTA, the backward walks 64-row query tiles with 64 keys per CTA
+constexpr int kFwdQBoxRows = 64, kBwdBoxRows = 64;
+inline int fmha_fwd_kv_box_rows(int d) { return d <= 64 ? 128 : 64; }
 
 struct FmhaFwdParams {
-  const void* q;   // [B, Lq, H, 64] via strides (elements)
-  const void* k;   // [B, Lk, H, 64]
+  const void* q;   // [B, Lq, H, D] via strides (elements)
+  const void* k;   // [B, Lk, H, D]
   const void* v;
-  void* out;       // [B, Lq, H, 64] contiguous
+  void* out;       // [B, Lq, H, D] contiguous
   float* lse;      // [B, H, Lq]
   const void* bias;        // [bias_batch (1 or B), H, Lq, Lk] contiguous, same 16-bit type as q; may be null
   const uint8_t* kpm;      // [B, Lk] bool, nonzero = masked; may be null
@@ -22,7 +29,7 @@ struct FmhaFwdParams {
   // keys 32w .. 32w + 31: key 32w + 2i in bit i, key 32w + 2i + 1 in bit 16 + i.
   uint32_t* drop_bits;
   long long q_sb, q_sl, q_sh, k_sb, k_sl, k_sh, v_sb, v_sl, v_sh;
-  int B, H, Lq, Lk;
+  int B, H, Lq, Lk, D;
   int bias_batch, bias_is_f32, is_bf16;
   float scale, p_drop;
   unsigned long long seed, offset;
@@ -33,11 +40,12 @@ void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
 
 struct FmhaBwdParams {
   FmhaFwdParams f;   // same inputs as forward (out/lse hold the forward results)
-  const void* dout;  // [B, Lq, H, 64] contiguous
+  const void* dout;  // [B, Lq, H, D] contiguous
   float* delta;      // [B, H, Lq] scratch: rowsum(dO * O)
-  float* dq_acc;     // [B, H, ceil(Lq / 64) * 64, 64] fp32, zeroed: every key tile adds its dQ share with bulk reductions
-  void* dq;          // [B, Lq, H, 64] 16-bit results, addressed through (batch, seq, head) element strides so
-  void* dk;          // that they can be slices of one packed [B, L, 3, H, 64] gradient tensor
+  float* dq_acc;     // [B, H, ceil(Lq / 64) * 64, DP] fp32 (DP = padded head width), zeroed: every key tile adds its
+                     // dQ share with bulk reductions
+  void* dq;          // [B, Lq, H, D] 16-bit results, addressed through (batch, seq, head) element strides so
+  void* dk;          // that they can be slices of one packed [B, L, 3, H, D] gradient tensor
   void* dv;
   long long dq_sb, dq_sl, dq_sh, dk_sb, dk_sl, dk_sh, dv_sb, dv_sl, dv_sh;
   // Bias gradient: every CTA stores its 16-bit dS tile (already in shared memory for the dQ product) with one TMA
@@ -46,7 +54,7 @@ struct FmhaBwdParams {
   void* ds_buf;      // [B, H, Lq, Lk] 16-bit
   void* dbias;       // [bias_batch, H, Lq, Lk] 16-bit; == ds_buf when bias_batch == B
   CUtensorMap sw_ds;   // 128-byte-swizzled map of ds_buf (64 x 64 boxes)
-  CUtensorMap sw_do;   // 64 x 64 tiles of dO (128-byte swizzle)
+  CUtensorMap sw_do;   // 64-row x 64-column boxes of dO (128-byte swizzle)
 };
 void launch_fmha_bwd(const FmhaBwdParams& p, cudaStream_t stream);
 

@@ -26,10 +26,12 @@ std::pair<uint64_t, uint64_t> reserve_philox(uint64_t increment) {
 }
 
 void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const Tensor& v, const OptTensor& bias,
-                 const OptTensor& kpm, double p_drop, double scale, int q_box_rows, int kv_box_rows) {
+                 const OptTensor& kpm, double p_drop, double scale, bool forward) {
   TORCH_CHECK(q.is_cuda() && k.is_cuda() && v.is_cuda());
   TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, "q/k/v must be [B, L, H, D]");
-  TORCH_CHECK(q.size(3) == 64 && k.size(3) == 64 && v.size(3) == 64, "head_dim must be 64");
+  const int64_t D = q.size(3);
+  TORCH_CHECK(ub::fmha_head_dim_supported(D) && k.size(3) == D && v.size(3) == D,
+              "head_dim must be the same for q/k/v and a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
   TORCH_CHECK(q.stride(3) == 1 && k.stride(3) == 1 && v.stride(3) == 1, "last dim must be contiguous");
   TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16);
   TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type());
@@ -51,6 +53,7 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   p.Lq = (int)q.size(1);
   p.H = (int)q.size(2);
   p.Lk = (int)k.size(1);
+  p.D = (int)D;
   p.is_bf16 = q.scalar_type() == at::kBFloat16 ? 1 : 0;
   p.bias = nullptr;
   p.bias_batch = 1;
@@ -76,12 +79,14 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   // The driver API behind cuTensorMapEncodeTiled needs a current context in THIS thread; autograd worker
   // threads only have the c10 device guard's notion of the device, so bind the primary context explicitly.
   cudaSetDevice(q.get_device());
-  // TMA descriptors: heads must be contiguous (stride 64) so that (head, 16-byte chunk) is one dimension
-  TORCH_CHECK(q.stride(2) == 64 && k.stride(2) == 64 && v.stride(2) == 64, "q/k/v head stride must be 64");
+  // TMA descriptors: heads must be contiguous (stride D) so that (head, 16-byte chunk) is one dimension
+  TORCH_CHECK(q.stride(2) == D && k.stride(2) == D && v.stride(2) == D, "q/k/v head stride must be head_dim");
   const bool bf16 = p.is_bf16 != 0;
-  bool ok = ub::make_head_tile_map_sw128(&p.sw_q, p.q, bf16, p.B, p.Lq, p.H, p.q_sb, p.q_sl, p.q_sh, q_box_rows);
-  ok = ok && ub::make_head_tile_map_sw128(&p.sw_k, p.k, bf16, p.B, p.Lk, p.H, p.k_sb, p.k_sl, p.k_sh, kv_box_rows);
-  ok = ok && ub::make_head_tile_map_sw128(&p.sw_v, p.v, bf16, p.B, p.Lk, p.H, p.v_sb, p.v_sl, p.v_sh, kv_box_rows);
+  const int q_box_rows = forward ? ub::kFwdQBoxRows : ub::kBwdBoxRows;
+  const int kv_box_rows = forward ? ub::fmha_fwd_kv_box_rows(p.D) : ub::kBwdBoxRows;
+  bool ok = ub::make_head_tile_map_sw128(&p.sw_q, p.q, bf16, p.B, p.Lq, p.H, p.D, p.q_sb, p.q_sl, p.q_sh, q_box_rows);
+  ok = ok && ub::make_head_tile_map_sw128(&p.sw_k, p.k, bf16, p.B, p.Lk, p.H, p.D, p.k_sb, p.k_sl, p.k_sh, kv_box_rows);
+  ok = ok && ub::make_head_tile_map_sw128(&p.sw_v, p.v, bf16, p.B, p.Lk, p.H, p.D, p.v_sb, p.v_sl, p.v_sh, kv_box_rows);
   if (p.bias != nullptr) ok = ok && ub::make_bias_tile_map_sw128(&p.sw_bias, p.bias, bf16, p.bias_batch * p.H, p.Lq, p.Lk);
   TORCH_CHECK(ok, "cuTensorMapEncodeTiled failed for the attention operands");
 }
@@ -91,8 +96,8 @@ std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k,
                                                       double scale) {
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaFwdParams p{};
-  fill_common(p, q, k, v, bias, kpm, p_drop, scale, ub::kFwdQBoxRows, ub::kFwdKVBoxRows);
-  Tensor out = torch::empty({p.B, p.Lq, p.H, 64}, q.options());
+  fill_common(p, q, k, v, bias, kpm, p_drop, scale, /*forward=*/true);
+  Tensor out = torch::empty({p.B, p.Lq, p.H, p.D}, q.options());
   Tensor lse = torch::empty({p.B, p.H, p.Lq}, q.options().dtype(at::kFloat));
   p.out = out.data_ptr();
   p.lse = lse.data_ptr<float>();
@@ -117,13 +122,17 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
                                                        const OptTensor& bias, const OptTensor& kpm, double p_drop,
                                                        double scale, const OptTensor& drop_bits, bool need_dbias,
                                                        bool packed_grad) {
-  // packed_grad: q/k/v are slices [:, :, i] of one [B, L, 3, H, 64] tensor; the gradients are then
-  // written straight into one packed [B, L, 3, H, 64] tensor (returned three times as views), which
+  // packed_grad: q/k/v are slices [:, :, i] of one [B, L, 3, H, D] tensor; the gradients are then
+  // written straight into one packed [B, L, 3, H, D] tensor (returned three times as views), which
   // spares autograd three zero-filled select-backward tensors and two full-size adds per layer.
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaBwdParams p{};
-  fill_common(p.f, q, k, v, bias, kpm, p_drop, scale, ub::kBwdBoxRows, ub::kBwdBoxRows);
+  fill_common(p.f, q, k, v, bias, kpm, p_drop, scale, /*forward=*/false);
+  const int D = p.f.D;
   TORCH_CHECK(dout.is_contiguous() && out.is_contiguous() && lse.is_contiguous());
+  TORCH_CHECK(dout.dim() == 4 && dout.size(0) == p.f.B && dout.size(1) == p.f.Lq && dout.size(2) == p.f.H &&
+                  dout.size(3) == D && out.sizes() == dout.sizes(),
+              "dout / out must be [B, Lq, H, D]");
   p.f.out = out.data_ptr();
   p.f.lse = lse.data_ptr<float>();
   if (p_drop > 0.0) {
@@ -131,23 +140,24 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
     p.f.drop_bits = reinterpret_cast<uint32_t*>(drop_bits->data_ptr());
   }
   p.dout = dout.data_ptr();
-  TORCH_CHECK(ub::make_head_tile_map_sw128(&p.sw_do, p.dout, p.f.is_bf16 != 0, p.f.B, p.f.Lq, p.f.H,
-                                           (long long)p.f.Lq * p.f.H * 64, (long long)p.f.H * 64, 64, ub::kBwdBoxRows),
+  TORCH_CHECK(ub::make_head_tile_map_sw128(&p.sw_do, p.dout, p.f.is_bf16 != 0, p.f.B, p.f.Lq, p.f.H, D,
+                                           (long long)p.f.Lq * p.f.H * D, (long long)p.f.H * D, D, ub::kBwdBoxRows),
               "cuTensorMapEncodeTiled failed for dO");
   Tensor delta = torch::empty({p.f.B, p.f.H, p.f.Lq}, q.options().dtype(at::kFloat));
-  // zeroed by the launcher; padded to whole 64-row query tiles
-  Tensor dq_acc = torch::empty({p.f.B, p.f.H, (p.f.Lq + 63) / 64 * 64, 64}, q.options().dtype(at::kFloat));
+  // zeroed by the launcher; padded to whole 64-row query tiles and to the kernel's padded head width
+  Tensor dq_acc = torch::empty({p.f.B, p.f.H, (p.f.Lq + 63) / 64 * 64, ub::fmha_padded_head_dim(D)},
+                               q.options().dtype(at::kFloat));
   Tensor dq, dk, dv;
   if (packed_grad) {
     TORCH_CHECK(p.f.Lq == p.f.Lk, "packed gradients need self-attention shapes");
-    Tensor dqkv = torch::empty({p.f.B, p.f.Lq, 3, p.f.H, 64}, q.options());
+    Tensor dqkv = torch::empty({p.f.B, p.f.Lq, 3, p.f.H, D}, q.options());
     dq = dqkv.select(2, 0);
     dk = dqkv.select(2, 1);
     dv = dqkv.select(2, 2);
   } else {
-    dq = torch::empty({p.f.B, p.f.Lq, p.f.H, 64}, q.options());
-    dk = torch::empty({p.f.B, p.f.Lk, p.f.H, 64}, q.options());
-    dv = torch::empty({p.f.B, p.f.Lk, p.f.H, 64}, q.options());
+    dq = torch::empty({p.f.B, p.f.Lq, p.f.H, D}, q.options());
+    dk = torch::empty({p.f.B, p.f.Lk, p.f.H, D}, q.options());
+    dv = torch::empty({p.f.B, p.f.Lk, p.f.H, D}, q.options());
   }
   p.dq_sb = dq.stride(0); p.dq_sl = dq.stride(1); p.dq_sh = dq.stride(2);
   p.dk_sb = dk.stride(0); p.dk_sl = dk.stride(1); p.dk_sh = dk.stride(2);

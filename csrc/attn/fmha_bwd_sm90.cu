@@ -1,19 +1,24 @@
-// Fused multi-head attention backward for sm_90a (head_dim 64, fp16/bf16), flash-attention style
+// Fused multi-head attention backward for sm_90a (head_dim D % 8 == 0, 8 <= D <= 128, fp16/bf16), flash-attention style
 // (reference: autograd through unicore/modules/multihead_attention.py:47-113 + softmax_fast.h:513-666):
 // probabilities are recomputed from the saved log-sum-exp; the dropout keep bits come from the
 // forward pass (1 bit / element).
 //
+//   Templated on the padded head width DP (64 or 128): Q / K / V / dO tiles are DP / 64 column boxes whose columns
+//   D..DP-1 the TMA unit zero-fills, so they add nothing to S, dP or the products, and the epilogues store columns
+//   below D only.
 //   grid = (64-key tiles, H, B); one CTA = one warpgroup owns K_j, V_j and walks the 64-row query tiles i.  The
 //   products are computed transposed (keys are the M dimension), so that P^T and dS^T are accumulator tiles whose
 //   16-bit conversions are directly the register A operands of the dV / dK products:
 //     S^T  = K_j Q_i^T                      wgmma m64n64, both operands K-major from shared memory
 //     dP^T = V_j dO_i^T                     wgmma m64n64
 //     P = exp2((S*scale + bias + kmask) * log2e - LSE_i * log2e) ;  dS = P o (drop(dP) - delta_i)
-//     dV_j += drop(P)^T dO_i                wgmma, A from registers, dO MN-major
-//     dK_j += dS^T Q_i                      wgmma, A from registers, Q MN-major
-//     dQ_i += dS K_j                        wgmma, dS from shared memory (stmatrix.trans of the registers, written in
-//                                           place over the consumed bias tile), K MN-major; the fp32 tile is added to
-//                                           a global fp32 accumulator with ONE bulk reduction (cp.reduce.async.bulk)
+//     dV_j += drop(P)^T dO_i                wgmma m64n{DP}, A from registers, dO MN-major
+//     dK_j += dS^T Q_i                      wgmma m64n{DP}, A from registers, Q MN-major
+//     dQ_i += dS K_j                        wgmma m64n64 per 64-column half of K (one dq[32] reused, so that DP = 128
+//                                           fits the registers next to dV and dK), dS from shared memory
+//                                           (stmatrix.trans of the registers, written in place over the consumed bias
+//                                           tile), K MN-major; the fp32 tile is added to a global fp32 accumulator
+//                                           with ONE bulk reduction (cp.reduce.async.bulk)
 //     dS tile (16-bit, in shared memory for the dQ product) -> TMA store; a follow-up kernel sums it over the batch
 //     into dBias.
 //   Q_i, dO_i and the bias tile are fetched one query tile ahead (two stages), one thread issues every copy.
@@ -33,19 +38,27 @@ namespace {
 
 using namespace tc;
 
-constexpr int kBM = 64, kBN = 64, kD = 64;   // query rows per step, keys per CTA, head dim
+constexpr int kBM = 64, kBN = 64;   // query rows per step, keys per CTA
 constexpr int kBwdThreads = 128;
 
-// shared memory map (bytes); every operand tile is 64 rows x 128 B, 128-byte swizzled
-constexpr uint32_t kOffK = 0;
-constexpr uint32_t kOffV = 8192;
-constexpr uint32_t kOffQ = 16384;      // 2 stages x 8 KB
-constexpr uint32_t kOffDO = 32768;     // 2 stages x 8 KB
-constexpr uint32_t kOffDS = 49152;     // 2 stages x 8 KB: bias tile [q][key], then dS in place
-constexpr uint32_t kOffDQ = 65536;     // fp32 [64][64] dQ tile, row-major (the layout of the global accumulator)
-constexpr uint32_t kOffStats = 81920;  // 2 stages x {float lse2[64], float delta[64], uint32 bits[64][2]}
-constexpr uint32_t kOffBar = kOffStats + 2048;
-constexpr uint32_t kBwdSmemBytes = kOffBar + 32 + 1024;   // + alignment slack of the 1024-byte-aligned base
+// shared memory map (bytes) of the padded head width DP; every box is 64 rows x 128 B, 128-byte swizzled, and a
+// Q / K / V / dO tile is DP / 64 boxes of 8 KB
+template <int DP>
+struct BwdCfg {
+  static constexpr int kBoxes = DP / 64;
+  static constexpr uint32_t kTile = kBoxes * 8192;
+  static constexpr uint32_t kOffK = 0;
+  static constexpr uint32_t kOffV = kOffK + kTile;
+  static constexpr uint32_t kOffQ = kOffV + kTile;        // 2 stages
+  static constexpr uint32_t kOffDO = kOffQ + 2 * kTile;   // 2 stages
+  static constexpr uint32_t kOffDS = kOffDO + 2 * kTile;  // 2 stages x 8 KB: bias tile [q][key], then dS in place
+  static constexpr uint32_t kOffDQ = kOffDS + 2 * 8192;   // fp32 [64][DP] dQ tile, row-major (the global accumulator's)
+  static constexpr uint32_t kOffStats = kOffDQ + kBM * DP * 4;   // 2 stages x {float lse2[64], delta[64], bits[64][2]}
+  static constexpr uint32_t kOffBar = kOffStats + 2048;
+  static constexpr uint32_t kSmemBytes = kOffBar + 32 + 1024;   // + alignment slack of the 1024-byte-aligned base
+};
+static_assert(BwdCfg<64>::kOffStats == 81920 && BwdCfg<64>::kSmemBytes == 85024,
+              "DP = 64 keeps the shared memory map of the 64-only kernel");
 
 template <typename T>
 UB_DEVICE uint32_t bwd_pack2(float a, float b);
@@ -71,19 +84,21 @@ UB_DEVICE float2 bwd_unpack2(uint32_t w) {
 // ---- pre-pass: delta[b,h,q] = sum_d dO * O -----------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256) fmha_delta_kernel(const T* __restrict__ dout, const T* __restrict__ out,
-                                                           float* __restrict__ delta, int B, int H, int Lq) {
-  // 8 threads per (b, q, h) row of 64 elements
+                                                           float* __restrict__ delta, int B, int H, int Lq, int D) {
+  // 8 threads per (b, q, h) row of D elements; thread `part` sums the 8-element chunks part, part + 8
   const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long rowi = gid >> 3;
   const int part = (int)(gid & 7);
   const long long nrows = (long long)B * Lq * H;
   float acc = 0.f;
   if (rowi < nrows) {
-    float a[8], o[8];
-    unpack<T>(ld_global_nc_v4(dout + rowi * 64 + part * 8), a);
-    unpack<T>(ld_global_nc_v4(out + rowi * 64 + part * 8), o);
+    for (int ch = part; ch < D / 8; ch += 8) {
+      float a[8], o[8];
+      unpack<T>(ld_global_nc_v4(dout + rowi * D + ch * 8), a);
+      unpack<T>(ld_global_nc_v4(out + rowi * D + ch * 8), o);
 #pragma unroll
-    for (int e = 0; e < 8; ++e) acc += a[e] * o[e];
+      for (int e = 0; e < 8; ++e) acc += a[e] * o[e];
+    }
   }
   acc += __shfl_xor_sync(0xffffffffu, acc, 1);
   acc += __shfl_xor_sync(0xffffffffu, acc, 2);
@@ -99,18 +114,19 @@ __global__ void __launch_bounds__(256) fmha_delta_kernel(const T* __restrict__ d
 // ---- post-pass: dq = scale * fp32 accumulator, written through (batch, seq, head) strides -------------------------
 template <typename T>
 __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __restrict__ acc, T* __restrict__ out, int H,
-                                                                int Lq, int Lq_pad, long long nvec, float scale, long long sb,
-                                                                long long sl, long long sh) {
+                                                                int Lq, int Lq_pad, int D, int DP, long long nvec, float scale,
+                                                                long long sb, long long sl, long long sh) {
   const long long stride = (long long)gridDim.x * blockDim.x;
+  const int groups = D / 8;   // the accumulator rows are DP wide; columns D..DP-1 are not stored
   for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
-    // v enumerates [b][h][q][8 groups of 8 columns]
-    const int part = (int)(v & 7);
-    const long long row = v >> 3;
+    // v enumerates [b][h][q][D / 8 groups of 8 columns]
+    const int part = (int)(v % groups);
+    const long long row = v / groups;
     const int q = (int)(row % Lq);
     const long long bh = row / Lq;
     const int h = (int)(bh % H);
     const long long b = bh / H;
-    const float4* src = reinterpret_cast<const float4*>(acc + ((bh * Lq_pad + q) * 64 + part * 8));
+    const float4* src = reinterpret_cast<const float4*>(acc + ((bh * Lq_pad + q) * DP + part * 8));
     const float4 x0 = src[0], x1 = src[1];
     const float x[8] = {x0.x * scale, x0.y * scale, x0.z * scale, x0.w * scale,
                         x1.x * scale, x1.y * scale, x1.z * scale, x1.w * scale};
@@ -119,8 +135,11 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
 }
 
 // ---- main kernel ----------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(kBwdThreads, 2) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
+template <typename T, int DP>
+__global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
+  using C = BwdCfg<DP>;
+  constexpr uint32_t kOffK = C::kOffK, kOffV = C::kOffV, kOffQ = C::kOffQ, kOffDO = C::kOffDO, kOffDS = C::kOffDS,
+                     kOffDQ = C::kOffDQ, kOffStats = C::kOffStats, kOffBar = C::kOffBar, kTile = C::kTile;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_base + 1023u) & ~1023u;   // 128-byte swizzle: tiles must be 1024-byte aligned
@@ -137,13 +156,15 @@ __global__ void __launch_bounds__(kBwdThreads, 2) fmha_bwd_kernel(const __grid_c
   const long long bh = (long long)b * p.H + h;
   const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
   const int words_per_row = (p.Lk + 31) / 32;
-  constexpr uint32_t kTileBytes = kBM * kD * 2;
-
+  // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
   auto load_tile = [&](int i) {   // one thread: Q_i, dO_i (and the bias tile) -> stage i & 1
     const uint32_t st = (uint32_t)(i & 1), bar = bar_in0 + 8u * st;
-    mbar_expect_tx(bar, 2 * kTileBytes + (has_bias ? kTileBytes : 0u));
-    tma_load_4d(smem_base + kOffQ + st * 8192, &p.sw_q, 0, h, i * kBM, b, bar);
-    tma_load_4d(smem_base + kOffDO + st * 8192, &bp.sw_do, 0, h, i * kBM, b, bar);
+    mbar_expect_tx(bar, 2 * kTile + (has_bias ? 8192u : 0u));
+#pragma unroll
+    for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
+      tma_load_4d(smem_base + kOffQ + st * kTile + x * 8192, &p.sw_q, 64 * x, h, i * kBM, b, bar);
+      tma_load_4d(smem_base + kOffDO + st * kTile + x * 8192, &bp.sw_do, 64 * x, h, i * kBM, b, bar);
+    }
     if (has_bias) tma_load_3d(smem_base + kOffDS + st * 8192, &p.sw_bias, key0, i * kBM, bias_nb, bar);
   };
   auto load_stats = [&](int i) {  // all threads: LSE (log2 units, +inf = row contributes nothing), delta, keep bits
@@ -168,9 +189,12 @@ __global__ void __launch_bounds__(kBwdThreads, 2) fmha_bwd_kernel(const __grid_c
     mbar_init(bar_in0, 1);
     mbar_init(bar_in0 + 8, 1);
     fence_mbarrier_init();
-    mbar_expect_tx(bar_kv, 2 * kTileBytes);
-    tma_load_4d(smem_base + kOffK, &p.sw_k, 0, h, key0, b, bar_kv);
-    tma_load_4d(smem_base + kOffV, &p.sw_v, 0, h, key0, b, bar_kv);
+    mbar_expect_tx(bar_kv, 2 * kTile);
+#pragma unroll
+    for (int x = 0; x < C::kBoxes; ++x) {
+      tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, h, key0, b, bar_kv);
+      tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, h, key0, b, bar_kv);
+    }
     load_tile(0);
   }
   load_stats(0);
@@ -191,9 +215,9 @@ __global__ void __launch_bounds__(kBwdThreads, 2) fmha_bwd_kernel(const __grid_c
   const int lm = lane >> 3, lj = lane & 7;
   const int ld_q = (lm >> 1) * 8 + lj, ld_chunk = 2 * warp + (lm & 1);
 
-  float dv[32], dk[32];
+  float dv[DP / 2], dk[DP / 2];
 #pragma unroll
-  for (int e = 0; e < 32; ++e) {
+  for (int e = 0; e < DP / 2; ++e) {
     dv[e] = 0.f;
     dk[e] = 0.f;
   }
@@ -210,16 +234,21 @@ __global__ void __launch_bounds__(kBwdThreads, 2) fmha_bwd_kernel(const __grid_c
     if (i + 1 < n_qtiles) load_stats(i + 1);
     mbar_wait(bar_in0 + 8u * st, (uint32_t)((i >> 1) & 1));
 
-    const uint32_t sQ = smem_base + kOffQ + st * 8192, sDO = smem_base + kOffDO + st * 8192;
+    const uint32_t sQ = smem_base + kOffQ + st * kTile, sDO = smem_base + kOffDO + st * kTile;
     const uint32_t sDS = smem_base + kOffDS + st * 8192;
     float s[32], dp[32];
     wgmma_fence();
+    // k-step kk: box kk / 4, +32 bytes per step inside the box
 #pragma unroll
-    for (int kk = 0; kk < kD / 16; ++kk)
-      wgmma_m64n64_ss<T, 0>(s, make_desc_sw128(smem_base + kOffK + kk * 32), make_desc_sw128(sQ + kk * 32), kk > 0 ? 1u : 0u);
+    for (int kk = 0; kk < DP / 16; ++kk) {
+      const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
+      wgmma_m64n64_ss<T, 0>(s, make_desc_sw128(smem_base + kOffK + off), make_desc_sw128(sQ + off), kk > 0 ? 1u : 0u);
+    }
 #pragma unroll
-    for (int kk = 0; kk < kD / 16; ++kk)
-      wgmma_m64n64_ss<T, 0>(dp, make_desc_sw128(smem_base + kOffV + kk * 32), make_desc_sw128(sDO + kk * 32), kk > 0 ? 1u : 0u);
+    for (int kk = 0; kk < DP / 16; ++kk) {
+      const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
+      wgmma_m64n64_ss<T, 0>(dp, make_desc_sw128(smem_base + kOffV + off), make_desc_sw128(sDO + off), kk > 0 ? 1u : 0u);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     fence_operands(s);
@@ -268,38 +297,51 @@ __global__ void __launch_bounds__(kBwdThreads, 2) fmha_bwd_kernel(const __grid_c
 
     // ---- dV += drop(P)^T dO, dK += dS^T Q ---------------------------------------------------------------------
     wgmma_fence();
+    // 16 queries = 16 rows of 128 bytes per step; at DP = 128 the descriptor steps to the second box through its LBO
 #pragma unroll
-    for (int sb = 0; sb < 4; ++sb) wgmma_m64n64_rs<T, 1>(dv, pa[sb], make_desc_sw128(sDO + sb * 2048), 1u);
+    for (int sb = 0; sb < 4; ++sb) {
+      if constexpr (DP == 64) wgmma_m64n64_rs<T, 1>(dv, pa[sb], make_desc_sw128(sDO + sb * 2048), 1u);
+      else wgmma_m64n128_rs<T, 1>(dv, pa[sb], make_desc_sw128_mn(sDO + sb * 2048, 8192), 1u);
+    }
 #pragma unroll
-    for (int sb = 0; sb < 4; ++sb) wgmma_m64n64_rs<T, 1>(dk, da[sb], make_desc_sw128(sQ + sb * 2048), 1u);
+    for (int sb = 0; sb < 4; ++sb) {
+      if constexpr (DP == 64) wgmma_m64n64_rs<T, 1>(dk, da[sb], make_desc_sw128(sQ + sb * 2048), 1u);
+      else wgmma_m64n128_rs<T, 1>(dk, da[sb], make_desc_sw128_mn(sQ + sb * 2048, 8192), 1u);
+    }
     wgmma_commit();
     __syncthreads();   // (B) the whole dS tile is in shared memory
 
-    // ---- dQ = dS K ------------------------------------------------------------------------------------------
-    float dq[32];
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < kBN / 16; ++kk)
-      wgmma_m64n64_ss<T, 1>(dq, make_desc_sw128(sDS + kk * 32), make_desc_sw128(smem_base + kOffK + kk * 2048), kk > 0 ? 1u : 0u);
-    wgmma_commit();
-    if (tid == 0 && bp.ds_buf != nullptr) {   // bias gradient: the dS tile leaves through one TMA store
-      tma_store_3d(&bp.sw_ds, key0, i * kBM, (int)bh, sDS);
-      bulk_commit();
-    }
-    wgmma_wait<0>();
-    fence_operands(dv);
-    fence_operands(dk);
-    fence_operands(dq);
+    // ---- dQ = dS K, one 64-column box of K at a time ------------------------------------------------------------
     float* dq_s = reinterpret_cast<float*>(smem + kOffDQ);
 #pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      *reinterpret_cast<float2*>(dq_s + kl0 * 64 + 8 * n + 2 * c) = make_float2(dq[4 * n], dq[4 * n + 1]);
-      *reinterpret_cast<float2*>(dq_s + kl1 * 64 + 8 * n + 2 * c) = make_float2(dq[4 * n + 2], dq[4 * n + 3]);
+    for (int x = 0; x < C::kBoxes; ++x) {
+      float dq[32];
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kBN / 16; ++kk)
+        wgmma_m64n64_ss<T, 1>(dq, make_desc_sw128(sDS + kk * 32), make_desc_sw128(smem_base + kOffK + x * 8192 + kk * 2048),
+                              kk > 0 ? 1u : 0u);
+      wgmma_commit();
+      if (x == 0 && tid == 0 && bp.ds_buf != nullptr) {   // bias gradient: the dS tile leaves through one TMA store
+        tma_store_3d(&bp.sw_ds, key0, i * kBM, (int)bh, sDS);
+        bulk_commit();
+      }
+      wgmma_wait<0>();
+      if (x == 0) {
+        fence_operands(dv);
+        fence_operands(dk);
+      }
+      fence_operands(dq);
+#pragma unroll
+      for (int n = 0; n < 8; ++n) {
+        *reinterpret_cast<float2*>(dq_s + kl0 * DP + 64 * x + 8 * n + 2 * c) = make_float2(dq[4 * n], dq[4 * n + 1]);
+        *reinterpret_cast<float2*>(dq_s + kl1 * DP + 64 * x + 8 * n + 2 * c) = make_float2(dq[4 * n + 2], dq[4 * n + 3]);
+      }
     }
     fence_proxy_async_smem();
     __syncthreads();   // (C) the dQ tile is in shared memory
     if (tid == 0) {
-      bulk_reduce_add_f32(bp.dq_acc + (bh * Lq_pad + (long long)i * kBM) * kD, smem_base + kOffDQ, kBM * kD * 4);
+      bulk_reduce_add_f32(bp.dq_acc + (bh * Lq_pad + (long long)i * kBM) * DP, smem_base + kOffDQ, kBM * DP * 4);
       bulk_commit();
     }
   }
@@ -313,7 +355,8 @@ __global__ void __launch_bounds__(kBwdThreads, 2) fmha_bwd_kernel(const __grid_c
     T* dvg = reinterpret_cast<T*>(bp.dv) + (long long)b * bp.dv_sb + (long long)key * bp.dv_sl + (long long)h * bp.dv_sh;
     T* dkg = reinterpret_cast<T*>(bp.dk) + (long long)b * bp.dk_sb + (long long)key * bp.dk_sl + (long long)h * bp.dk_sh;
 #pragma unroll
-    for (int n = 0; n < 8; ++n) {
+    for (int n = 0; n < DP / 8; ++n) {
+      if (8 * n >= p.D) continue;   // columns 8n + 2c, +1 exist iff 8n < D (D % 8 == 0)
       const int e = 4 * n + 2 * half;
       *reinterpret_cast<uint32_t*>(dvg + 8 * n + 2 * c) = bwd_pack2<T>(dv[e] * keep_scale, dv[e + 1] * keep_scale);
       *reinterpret_cast<uint32_t*>(dkg + 8 * n + 2 * c) = bwd_pack2<T>(dk[e] * p.scale, dk[e + 1] * p.scale);
@@ -357,18 +400,18 @@ int device_sms() {
   return sms;
 }
 
-template <typename T>
+template <typename T, int DP>
 void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
   const FmhaFwdParams& p = bp.f;
   const long long nrows = (long long)p.B * p.Lq * p.H;
   const int n_qt = (p.Lq + kBM - 1) / kBM;
-  cudaMemsetAsync(bp.dq_acc, 0, (size_t)p.B * p.H * n_qt * kBM * kD * sizeof(float), stream);
+  cudaMemsetAsync(bp.dq_acc, 0, (size_t)p.B * p.H * n_qt * kBM * DP * sizeof(float), stream);
   fmha_delta_kernel<T><<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
-      reinterpret_cast<const T*>(bp.dout), reinterpret_cast<const T*>(p.out), bp.delta, p.B, p.H, p.Lq);
+      reinterpret_cast<const T*>(bp.dout), reinterpret_cast<const T*>(p.out), bp.delta, p.B, p.H, p.Lq, p.D);
   dim3 grid((p.Lk + kBN - 1) / kBN, p.H, p.B);
-  auto kern = fmha_bwd_kernel<T>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmemBytes);
-  kern<<<grid, kBwdThreads, kBwdSmemBytes, stream>>>(bp);
+  auto kern = fmha_bwd_kernel<T, DP>;
+  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BwdCfg<DP>::kSmemBytes);
+  kern<<<grid, kBwdThreads, BwdCfg<DP>::kSmemBytes, stream>>>(bp);
   const long long cap = (long long)device_sms() * 16;
   if (bp.ds_buf != nullptr && bp.dbias != bp.ds_buf) {
     const long long nv = (long long)p.H * p.Lq * p.Lk / 8;
@@ -376,17 +419,23 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
     fmha_dbias_reduce_kernel<T><<<(unsigned)rb, 256, 0, stream>>>(reinterpret_cast<const T*>(bp.ds_buf),
                                                                  reinterpret_cast<T*>(bp.dbias), p.B, nv);
   }
-  const long long nvec = nrows * 8;
+  const long long nvec = nrows * (p.D / 8);
   const long long blocks = std::min((nvec + 255) / 256, cap);
   fmha_dq_convert_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>(bp.dq_acc, reinterpret_cast<T*>(bp.dq), p.H, p.Lq,
-                                                                  n_qt * kBM, nvec, p.scale, bp.dq_sb, bp.dq_sl, bp.dq_sh);
+                                                                  n_qt * kBM, p.D, DP, nvec, p.scale, bp.dq_sb, bp.dq_sl,
+                                                                  bp.dq_sh);
 }
 
 }  // namespace
 
 void launch_fmha_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
-  if (bp.f.is_bf16) run_bwd<__nv_bfloat16>(bp, stream);
-  else run_bwd<__half>(bp, stream);
+  if (bp.f.D <= 64) {
+    if (bp.f.is_bf16) run_bwd<__nv_bfloat16, 64>(bp, stream);
+    else run_bwd<__half, 64>(bp, stream);
+  } else {
+    if (bp.f.is_bf16) run_bwd<__nv_bfloat16, 128>(bp, stream);
+    else run_bwd<__half, 128>(bp, stream);
+  }
 }
 
 }  // namespace ub

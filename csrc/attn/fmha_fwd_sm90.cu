@@ -1,20 +1,26 @@
-// Fused multi-head attention forward for sm_90a (head_dim 64, fp16/bf16):
+// Fused multi-head attention forward for sm_90a (head_dim D % 8 == 0, 8 <= D <= 128, fp16/bf16):
 //   O = dropout(softmax(scale * Q K^T + bias + key_padding)) V        LSE = logsumexp of the logits
 // One kernel for what the reference runs as bmm -> masked_fill -> softmax_dropout -> bmm plus four transposes
 // (unicore/modules/multihead_attention.py:47-113, csrc/softmax_dropout/softmax_fast.h:207-434).
 //
-// One CTA = one warpgroup (128 threads) = one 64-row query tile of one (batch, head); it walks the 128-key tiles:
+// The kernel is a template on the padded head width DP (64 or 128 columns = one or two 128-byte-swizzled boxes per
+// row); the head dim D is a runtime value.  The TMA maps span D columns, so the unit zero-fills columns D..DP-1 in
+// shared memory: zero columns of Q and K add nothing to S, zero columns of V give zero columns of O, which the
+// epilogue does not store.
+// One CTA = one warpgroup (128 threads) = one 64-row query tile of one (batch, head); it walks the key tiles
+// (kBlockN = 128 keys at DP = 64, 64 keys at DP = 128, which keeps o[64] + s[32] in registers):
 //   1. TMA (128-byte-swizzled boxes, csrc/attn/tma_map.h): K, V and the bias tile of key tile j+1 are requested into
 //      the other of two stages while tile j is computed; one thread issues every copy, completion on an mbarrier.
-//   2. S = Q K_j^T           4 x wgmma m64n128k16, both operands K-major from shared memory, fp32 in registers
+//   2. S = Q K_j^T           DP/16 x wgmma m64n{kBlockN}k16, both operands K-major from shared memory, fp32 in registers
 //   3. softmax in registers: logits = S*scale + bias + key mask, row max across the 4 threads of a quad, online
 //      rescaling of O and of the row sum, Philox dropout on packed 16-bit pairs (the keep bits are stored for the
 //      backward pass), P converted in place into the register A operand of the next product
-//   4. O += P V_j            8 x wgmma m64n64k16, A (P) from registers, V presented MN-major from its row-major bytes
-//   q/k/v are read through strides straight out of the packed in_proj output; O is written as [B, Lq, H, 64] so
+//   4. O += P V_j            kBlockN/16 x wgmma m64n{DP}k16, A (P) from registers, V presented MN-major from its
+//                            row-major bytes (at DP = 128 the descriptor steps to the second box through its LBO)
+//   q/k/v are read through strides straight out of the packed in_proj output; O is written as [B, Lq, H, D] so
 //   that out_proj consumes it without a transpose.
-// 104 KB of shared memory and <= 255 registers per thread: two CTAs (8 warps) per SM, so one CTA's softmax overlaps
-// the other's tensor-core work and copies.
+// 106 KB (DP = 64) / 98 KB (DP = 128) of shared memory and <= 255 registers per thread: two CTAs (8 warps) per SM,
+// so one CTA's softmax overlaps the other's tensor-core work and copies.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math_constants.h>
@@ -29,17 +35,26 @@ namespace {
 using namespace tc;
 
 constexpr int kBlockM = 64;    // query rows per CTA
-constexpr int kBlockN = 128;   // keys per tile
-constexpr int kHeadDim = 64;
 constexpr int kFwdThreads = 128;
 
-constexpr uint32_t kSmemQ = 0;                       // 64 x 64 x 2   = 8 KB
-constexpr uint32_t kSmemK = 8192;                    // 2 stages x 16 KB
-constexpr uint32_t kSmemV = kSmemK + 2 * 16384;      // 2 stages x 16 KB
-constexpr uint32_t kSmemBias = kSmemV + 2 * 16384;   // 2 stages x (two 64-key boxes of 64 rows = 16 KB)
-constexpr uint32_t kSmemKAdd = kSmemBias + 2 * 16384;  // 2 stages x float[128]: 0 or -inf per key
-constexpr uint32_t kSmemBar = kSmemKAdd + 1024;
-constexpr uint32_t kFwdSmemBytes = kSmemBar + 64 + 1024;   // + alignment slack of the 1024-byte-aligned base
+// Tile geometry and shared memory map of the padded head width DP; every box is 128-byte-swizzled rows of 64 columns
+template <int DP>
+struct FwdCfg {
+  static constexpr int kBlockN = DP == 64 ? 128 : 64;            // keys per tile
+  static constexpr int kBoxes = DP / 64;                         // 64-column boxes per row
+  static constexpr uint32_t kQBox = kBlockM * 128;               // one 64-column box of the Q tile
+  static constexpr uint32_t kKVBox = kBlockN * 128;              // one 64-column box of a K / V tile
+  static constexpr uint32_t kKVStage = kBoxes * kKVBox;
+  static constexpr uint32_t kBiasStage = kBlockM * kBlockN * 2;  // kBlockN / 64 boxes of 64 rows x 64 keys
+  static constexpr uint32_t kSmemQ = 0;
+  static constexpr uint32_t kSmemK = kSmemQ + kBoxes * kQBox;    // 2 stages
+  static constexpr uint32_t kSmemV = kSmemK + 2 * kKVStage;      // 2 stages
+  static constexpr uint32_t kSmemBias = kSmemV + 2 * kKVStage;   // 2 stages
+  static constexpr uint32_t kSmemKAdd = kSmemBias + 2 * kBiasStage;   // 2 stages x float[kBlockN]: 0 or -inf per key
+  static constexpr uint32_t kSmemBar = kSmemKAdd + 2 * kBlockN * 4;
+  static constexpr uint32_t kSmemBytes = kSmemBar + 64 + 1024;   // + alignment slack of the 1024-byte-aligned base
+};
+static_assert(FwdCfg<64>::kSmemBytes == 108608, "DP = 64 keeps the shared memory map of the 64-only kernel");
 
 template <typename T>
 UB_DEVICE uint32_t pack2(float a, float b);
@@ -64,8 +79,11 @@ UB_DEVICE float2 unpack2(uint32_t w) {
 
 UB_DEVICE uint32_t select4(const Philox4& r, int i) { return i == 0 ? r.x : (i == 1 ? r.y : (i == 2 ? r.z : r.w)); }
 
-template <typename T>
+template <typename T, int DP>
 __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
+  using C = FwdCfg<DP>;
+  constexpr int kBlockN = C::kBlockN;
+  constexpr int kWords = kBlockN / 32;   // keep-bit words per row of a key tile
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_base + 1023u) & ~1023u;   // 128-byte swizzle: tiles must be 1024-byte aligned
@@ -73,22 +91,28 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, c = lane & 3;
   const int q0 = blockIdx.x * kBlockM, h = blockIdx.y, b = blockIdx.z;
-  const uint32_t bar0 = smem_base + kSmemBar;   // bar0 + 8 * stage: K / V / bias of a key tile (+ Q on the first)
-  float* kadd = reinterpret_cast<float*>(smem + kSmemKAdd);
+  const uint32_t bar0 = smem_base + C::kSmemBar;   // bar0 + 8 * stage: K / V / bias of a key tile (+ Q on the first)
+  float* kadd = reinterpret_cast<float*>(smem + C::kSmemKAdd);
 
   const bool has_bias = p.bias != nullptr;
   const int n_tiles = (p.Lk + kBlockN - 1) / kBlockN;
   const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
-  constexpr uint32_t kKVBytes = kBlockN * kHeadDim * 2, kBiasBytes = kBlockM * kBlockN * 2, kQBytes = kBlockM * kHeadDim * 2;
+  // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
+  constexpr uint32_t kKVBytes = C::kKVStage, kBiasBytes = C::kBiasStage, kQBytes = C::kBoxes * C::kQBox;
   auto load_tile = [&](int j) {   // one thread; the first tile's phase also covers Q (one arrival per phase)
     const uint32_t st = (uint32_t)(j & 1), bar = bar0 + 8u * st;
     mbar_expect_tx(bar, 2 * kKVBytes + (has_bias ? kBiasBytes : 0u) + (j == 0 ? kQBytes : 0u));
-    if (j == 0) tma_load_4d(smem_base + kSmemQ, &p.sw_q, 0, h, q0, b, bar);
-    tma_load_4d(smem_base + kSmemK + st * 16384, &p.sw_k, 0, h, j * kBlockN, b, bar);
-    tma_load_4d(smem_base + kSmemV + st * 16384, &p.sw_v, 0, h, j * kBlockN, b, bar);
-    if (has_bias) {   // 64 rows x 128 keys = two 64-key boxes
-      tma_load_3d(smem_base + kSmemBias + st * 16384, &p.sw_bias, j * kBlockN, q0, bias_nb, bar);
-      tma_load_3d(smem_base + kSmemBias + st * 16384 + 8192, &p.sw_bias, j * kBlockN + 64, q0, bias_nb, bar);
+#pragma unroll
+    for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
+      if (j == 0) tma_load_4d(smem_base + C::kSmemQ + x * C::kQBox, &p.sw_q, 64 * x, h, q0, b, bar);
+      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, h, j * kBlockN, b, bar);
+      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, h, j * kBlockN, b, bar);
+    }
+    if (has_bias) {   // 64 rows x kBlockN keys = kBlockN / 64 boxes of 64 keys
+#pragma unroll
+      for (int x = 0; x < kBlockN / 64; ++x)
+        tma_load_3d(smem_base + C::kSmemBias + st * C::kBiasStage + x * 8192, &p.sw_bias, j * kBlockN + 64 * x, q0, bias_nb,
+                    bar);
     }
   };
   if (tid == 0) {
@@ -112,18 +136,18 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 
   constexpr float kLog2e = 1.4426950408889634f;
   float m0 = -CUDART_INF_F, m1 = -CUDART_INF_F, l0 = 0.f, l1 = 0.f;   // running max (in use) and partial row sums
-  float o[32];
+  float o[DP / 2];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  for (int i = 0; i < DP / 2; ++i) o[i] = 0.f;
 
   for (int j = 0; j < n_tiles; ++j) {
     const uint32_t st = (uint32_t)(j & 1);
     const int key0 = j * kBlockN;
     bool masked = false;
-    {
+    if (tid < kBlockN) {
       const int key = key0 + tid;
       masked = key >= p.Lk || (kpm_row != nullptr && kpm_row[key] != 0);
-      kadd[st * 128 + tid] = masked ? -CUDART_INF_F : 0.f;
+      kadd[st * kBlockN + tid] = masked ? -CUDART_INF_F : 0.f;
     }
     // barrier: every thread is done with tile j-1, so its stage may be refilled with tile j+1
     const bool tile_masked = __syncthreads_or(masked) != 0;
@@ -131,21 +155,24 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     mbar_wait(bar0 + 8u * st, (uint32_t)((j >> 1) & 1));
 
     // ---- S = Q K^T --------------------------------------------------------------------------------------
-    float s[64];
+    float s[kBlockN / 2];
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < kHeadDim / 16; ++kk)
-      wgmma_m64n128_ss<T, 0>(s, make_desc_sw128(smem_base + kSmemQ + kk * 32),
-                             make_desc_sw128(smem_base + kSmemK + st * 16384 + kk * 32), kk > 0 ? 1u : 0u);
+    for (int kk = 0; kk < DP / 16; ++kk) {   // k-step kk: box kk / 4, +32 bytes per step inside the box
+      const uint64_t da = make_desc_sw128(smem_base + C::kSmemQ + (kk >> 2) * C::kQBox + (kk & 3) * 32);
+      const uint64_t db = make_desc_sw128(smem_base + C::kSmemK + st * C::kKVStage + (kk >> 2) * C::kKVBox + (kk & 3) * 32);
+      if constexpr (kBlockN == 128) wgmma_m64n128_ss<T, 0>(s, da, db, kk > 0 ? 1u : 0u);
+      else wgmma_m64n64_ss<T, 0>(s, da, db, kk > 0 ? 1u : 0u);
+    }
     wgmma_commit();
     wgmma_wait<0>();
     fence_operands(s);
 
     // ---- logits, row max ----------------------------------------------------------------------------------
     float mx0 = -CUDART_INF_F, mx1 = -CUDART_INF_F;
-    const uint8_t* bias_tile = smem + kSmemBias + st * 16384;
+    const uint8_t* bias_tile = smem + C::kSmemBias + st * C::kBiasStage;
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
+    for (int i = 0; i < kBlockN / 8; ++i) {
       const int col = 8 * i + 2 * c;
       float2 b0 = make_float2(0.f, 0.f), b1 = make_float2(0.f, 0.f);
       if (has_bias) {
@@ -154,7 +181,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
         b1 = unpack2<T>(*reinterpret_cast<const uint32_t*>(box + sw128_off(rl1, i & 7)));
       }
       if (tile_masked) {
-        const float2 ka = *reinterpret_cast<const float2*>(kadd + st * 128 + col);
+        const float2 ka = *reinterpret_cast<const float2*>(kadd + st * kBlockN + col);
         b0.x += ka.x; b0.y += ka.y; b1.x += ka.x; b1.y += ka.y;
       }
       s[4 * i + 0] = fmaf(s[4 * i + 0], p.scale, b0.x);
@@ -178,7 +205,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     l0 *= alpha0;
     l1 *= alpha1;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < DP / 8; ++i) {
       o[4 * i + 0] *= alpha0;
       o[4 * i + 1] *= alpha0;
       o[4 * i + 2] *= alpha1;
@@ -187,10 +214,12 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 
     // ---- probabilities, dropout, P -> register A operand ---------------------------------------------------------
     const float nm0 = -mu0 * kLog2e, nm1 = -mu1 * kLog2e;
-    uint32_t pa[32];                 // pa[2i] = row rl0, keys 8i + 2c, +1; pa[2i + 1] = row rl1
-    uint32_t kw0[4] = {0u, 0u, 0u, 0u}, kw1[4] = {0u, 0u, 0u, 0u};   // keep bits, one word per 32 keys
+    uint32_t pa[kBlockN / 4];        // pa[2i] = row rl0, keys 8i + 2c, +1; pa[2i + 1] = row rl1
+    uint32_t kw0[kWords], kw1[kWords];   // keep bits, one word per 32 keys
 #pragma unroll
-    for (int i = 0; i < 16; ++i) {
+    for (int w = 0; w < kWords; ++w) kw0[w] = kw1[w] = 0u;
+#pragma unroll
+    for (int i = 0; i < kBlockN / 8; ++i) {
       const float p00 = ex2_approx(fmaf(s[4 * i + 0], kLog2e, nm0)), p01 = ex2_approx(fmaf(s[4 * i + 1], kLog2e, nm0));
       const float p10 = ex2_approx(fmaf(s[4 * i + 2], kLog2e, nm1)), p11 = ex2_approx(fmaf(s[4 * i + 3], kLog2e, nm1));
       l0 += p00 + p01;
@@ -210,16 +239,22 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     }
     if (drop && p.drop_bits != nullptr) {
 #pragma unroll
-      for (int w = 0; w < 4; ++w) {
+      for (int w = 0; w < kWords; ++w) {
         kw0[w] |= __shfl_xor_sync(0xffffffffu, kw0[w], 1);
         kw0[w] |= __shfl_xor_sync(0xffffffffu, kw0[w], 2);
         kw1[w] |= __shfl_xor_sync(0xffffffffu, kw1[w], 1);
         kw1[w] |= __shfl_xor_sync(0xffffffffu, kw1[w], 2);
       }
       // thread c of the quad stores word c of both rows
-      const uint32_t w0 = c == 0 ? kw0[0] : (c == 1 ? kw0[1] : (c == 2 ? kw0[2] : kw0[3]));
-      const uint32_t w1 = c == 0 ? kw1[0] : (c == 1 ? kw1[1] : (c == 2 ? kw1[2] : kw1[3]));
-      if (key0 + 32 * c < p.Lk) {
+      uint32_t w0, w1;
+      if constexpr (kWords == 4) {
+        w0 = c == 0 ? kw0[0] : (c == 1 ? kw0[1] : (c == 2 ? kw0[2] : kw0[3]));
+        w1 = c == 0 ? kw1[0] : (c == 1 ? kw1[1] : (c == 2 ? kw1[2] : kw1[3]));
+      } else {
+        w0 = c == 0 ? kw0[0] : kw0[1];
+        w1 = c == 0 ? kw1[0] : kw1[1];
+      }
+      if (c < kWords && key0 + 32 * c < p.Lk) {
         const int wi = (key0 >> 5) + c;
         if (row0 < p.Lq) p.drop_bits[lin0 * words_per_row + wi] = w0;
         if (row1 < p.Lq) p.drop_bits[lin1 * words_per_row + wi] = w1;
@@ -229,9 +264,11 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     // ---- O += P V ---------------------------------------------------------------------------------------
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < kBlockN / 16; ++kk) {
+    for (int kk = 0; kk < kBlockN / 16; ++kk) {   // 16 keys = 16 rows of 128 bytes per step
       const uint32_t a[4] = {pa[4 * kk], pa[4 * kk + 1], pa[4 * kk + 2], pa[4 * kk + 3]};
-      wgmma_m64n64_rs<T, 1>(o, a, make_desc_sw128(smem_base + kSmemV + st * 16384 + kk * 2048), 1u);
+      const uint32_t v_addr = smem_base + C::kSmemV + st * C::kKVStage + kk * 2048;
+      if constexpr (DP == 64) wgmma_m64n64_rs<T, 1>(o, a, make_desc_sw128(v_addr), 1u);
+      else wgmma_m64n128_rs<T, 1>(o, a, make_desc_sw128_mn(v_addr, C::kKVBox), 1u);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -245,16 +282,19 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
   const float inv0 = l0 > 0.f ? keep_scale / l0 : 0.f, inv1 = l1 > 0.f ? keep_scale / l1 : 0.f;
   T* out = reinterpret_cast<T*>(p.out);
+  const int D = p.D;   // columns 8i + 2c, +1 exist iff 8i < D (D % 8 == 0)
   if (row0 < p.Lq) {
-    uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row0) * p.H + h) * kHeadDim + 2 * c);
+    uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row0) * p.H + h) * D + 2 * c);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) og[4 * i] = pack2<T>(o[4 * i + 0] * inv0, o[4 * i + 1] * inv0);
+    for (int i = 0; i < DP / 8; ++i)
+      if (8 * i < D) og[4 * i] = pack2<T>(o[4 * i + 0] * inv0, o[4 * i + 1] * inv0);
     if (c == 0) p.lse[lin0] = l0 > 0.f ? m0 + __logf(l0) : -CUDART_INF_F;   // natural-log LSE of the logits
   }
   if (row1 < p.Lq) {
-    uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row1) * p.H + h) * kHeadDim + 2 * c);
+    uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row1) * p.H + h) * D + 2 * c);
 #pragma unroll
-    for (int i = 0; i < 8; ++i) og[4 * i] = pack2<T>(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
+    for (int i = 0; i < DP / 8; ++i)
+      if (8 * i < D) og[4 * i] = pack2<T>(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
     if (c == 0) p.lse[lin1] = l1 > 0.f ? m1 + __logf(l1) : -CUDART_INF_F;
   }
 }
@@ -263,12 +303,17 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream) {
   dim3 grid((p.Lq + kBlockM - 1) / kBlockM, p.H, p.B);
-  auto run = [&](auto kern) {
-    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFwdSmemBytes);
-    kern<<<grid, kFwdThreads, kFwdSmemBytes, stream>>>(p);
+  auto run = [&](auto kern, uint32_t smem_bytes) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    kern<<<grid, kFwdThreads, smem_bytes, stream>>>(p);
   };
-  if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16>);
-  else run(fmha_fwd_kernel<__half>);
+  if (p.D <= 64) {
+    if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64>, FwdCfg<64>::kSmemBytes);
+    else run(fmha_fwd_kernel<__half, 64>, FwdCfg<64>::kSmemBytes);
+  } else {
+    if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128>, FwdCfg<128>::kSmemBytes);
+    else run(fmha_fwd_kernel<__half, 128>, FwdCfg<128>::kSmemBytes);
+  }
 }
 
 }  // namespace ub

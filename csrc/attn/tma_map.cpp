@@ -37,9 +37,10 @@ bool encode_sw128(CUtensorMap* map, const void* base, bool bf16, int rank, const
 
 }  // namespace
 
-bool make_head_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int B, int L, int H, long long sb,
+bool make_head_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int B, int L, int H, int D, long long sb,
                               long long sl, long long sh, int box_rows) {
-  const cuuint64_t dims[4] = {64, (cuuint64_t)H, (cuuint64_t)L, (cuuint64_t)B};
+  // columns D..127 of a box lie outside the tensor: the TMA unit fills them with zeros
+  const cuuint64_t dims[4] = {(cuuint64_t)D, (cuuint64_t)H, (cuuint64_t)L, (cuuint64_t)B};
   const cuuint64_t strides[3] = {(cuuint64_t)sh * 2, (cuuint64_t)sl * 2, (cuuint64_t)sb * 2};
   const cuuint32_t box[4] = {64, 1, (cuuint32_t)box_rows, 1};
   return encode_sw128(map, base, bf16, 4, dims, strides, box);

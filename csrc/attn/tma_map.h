@@ -9,8 +9,9 @@
 
 namespace ub {
 
-// [B, L, H, 64] tensor, box = box_rows x 64 of one (batch, head); coordinates {0, head, row0, batch}.
-bool make_head_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int B, int L, int H, long long sb,
+// [B, L, H, D] tensor (D % 8 == 0, heads contiguous), box = box_rows x 64 columns of one (batch, head); coordinates
+// {col0 (0 or 64), head, row0, batch}.  Columns at or past D read as zeros.
+bool make_head_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int B, int L, int H, int D, long long sb,
                               long long sl, long long sh, int box_rows);
 // bias [NB, Lq, Lk]: box = 64 rows x 64 columns (a 64 x 128 tile is two boxes); coordinates {key0, q0, nb}.
 bool make_bias_tile_map_sw128(CUtensorMap* map, const void* base, bool bf16, int NB, int Lq, int Lk);

@@ -6,9 +6,11 @@ boolean ``key_padding_mask``, ``return_attn`` yielding ``(out, pre-softmax logit
 probabilities)``) and ``CrossMultiheadAttention:121``.
 
 GPU path: unless ``return_attn`` is requested, the whole ``QK^T -> +bias/mask -> softmax ->
-dropout -> @V`` chain runs in the wgmma kernel behind ``ops.fused_attention``; q/k/v are strided
+dropout -> @V`` chain runs in the wgmma kernel behind ``ops.fused_attention`` for every head dim the
+kernel takes (a multiple of 8 up to 128, ``ops.fused_head_dim_supported``); q/k/v are strided
 views of the projection output (no transpose/contiguous copies) and the bias is *not* expanded over
-the batch.  With ``return_attn`` the materialised path (bmm + ``softmax_dropout`` kernel) is used.
+the batch.  With ``return_attn``, or another head dim, the materialised path (bmm +
+``softmax_dropout`` kernel) is used.
 """
 from typing import Optional
 

@@ -302,7 +302,7 @@ class _StackMixin:
                 fm = future_mask[:seq_len, :seq_len]
                 bias = fm.view(1, 1, seq_len, seq_len).expand(1, heads, seq_len, seq_len) if bias is None else bias + fm
             fused_capable = x.is_cuda and ops.USE_NATIVE and x.dtype in (torch.float16, torch.bfloat16) \
-                and (self.embed_dim // heads) == 64
+                and ops.fused_head_dim_supported(self.embed_dim // heads)
             if bias is None or fused_capable or padding_mask is None:
                 return bias, padding_mask
             merged = bias.expand(bsz, heads, seq_len, seq_len).clone()

@@ -97,7 +97,8 @@ class BertModel(BaseUnicoreModel):
     def _padding_mask(self, src_tokens, embedded):
         mask = src_tokens.eq(self.padding_idx)
         head_dim = self.args.encoder_embed_dim // self.args.encoder_attention_heads
-        fused = ops.use_native(embedded) and embedded.dtype in (torch.float16, torch.bfloat16) and head_dim == 64
+        fused = ops.use_native(embedded) and embedded.dtype in (torch.float16, torch.bfloat16) \
+            and ops.fused_head_dim_supported(head_dim)
         if fused:
             return mask  # consumed inside the attention kernel: no reason to sync on mask.any()
         return mask if bool(mask.any()) else None

@@ -8,6 +8,9 @@ dropout in registers, and P is the register operand of a second ``wgmma`` that a
 q/k/v are consumed directly from the packed ``in_proj`` output through strides (no transposes) and O is
 written as ``[B, L, H*D]``.  Backward recomputes P from the saved log-sum-exp (flash-attention style) and
 reads the dropout keep bits the forward kernel stored.
+
+The kernels take every head dim ``D`` with ``D % 8 == 0`` and ``8 <= D <= 128`` (``fused_head_dim_supported``);
+other head dims, and callers that need the probabilities (``return_attn``), use ``attention_reference``.
 """
 import math
 
@@ -15,6 +18,13 @@ import torch
 import torch.nn.functional as F
 
 from ._native import native, use_native
+
+FUSED_MAX_HEAD_DIM = 128
+
+
+def fused_head_dim_supported(head_dim: int) -> bool:
+    """True when the fused attention kernels take this head dim: a multiple of 8 from 8 to 128."""
+    return 8 <= head_dim <= FUSED_MAX_HEAD_DIM and head_dim % 8 == 0
 
 
 def attention_reference(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None):
@@ -58,7 +68,7 @@ class _FusedAttentionFn(torch.autograd.Function):
 
 
 class _FusedAttentionPackedFn(torch.autograd.Function):
-    """Self-attention on a packed ``[B, L, 3, H, 64]`` projection: q/k/v are strided slices on the way
+    """Self-attention on a packed ``[B, L, 3, H, D]`` projection: q/k/v are strided slices on the way
     in, and the backward kernels write dq/dk/dv directly into ONE packed gradient tensor."""
 
     @staticmethod
@@ -79,7 +89,7 @@ class _FusedAttentionPackedFn(torch.autograd.Function):
         dq, _dk, _dv, dbias = native().fmha_bwd(
             dout.contiguous(), q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, True
         )
-        dqkv = dq._base  # the packed [B, L, 3, H, 64] tensor the three gradients are views of
+        dqkv = dq._base  # the packed [B, L, 3, H, D] tensor the three gradients are views of
         if dbias is not None and dbias.dtype != bias.dtype:
             dbias = dbias.to(bias.dtype)
         return dqkv, dbias, None, None, None, None
@@ -90,12 +100,15 @@ def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool
         return False
     if key_padding_mask is not None and key_padding_mask.dtype != torch.bool:
         return False
+    if q.dim() != 4 or k.dim() != 4 or v.dim() != 4:
+        return False
+    head_dim = q.shape[-1]
+    if not fused_head_dim_supported(head_dim) or k.shape[-1] != head_dim or v.shape[-1] != head_dim:
+        return False
     for t in (q, k, v):
-        if t.data_ptr() % 16 != 0 or any(s % 8 != 0 for s in t.stride()[:3]) or t.stride(2) != 64:
+        if t.data_ptr() % 16 != 0 or any(s % 8 != 0 for s in t.stride()[:3]) or t.stride(2) != head_dim:
             return False
     if q.dtype not in (torch.float16, torch.bfloat16) or k.dtype != q.dtype or v.dtype != q.dtype:
-        return False
-    if q.dim() != 4 or q.shape[-1] != 64 or k.shape[-1] != 64:
         return False
     if q.stride(-1) != 1 or k.stride(-1) != 1 or v.stride(-1) != 1:
         return False
