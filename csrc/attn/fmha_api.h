@@ -35,6 +35,10 @@ struct FmhaFwdParams {
   unsigned long long seed, offset;
   // TMA descriptors (csrc/attn/tma_map.h), 128-byte swizzle: row tiles of q / k / v, 64 x 64 tiles of the bias
   CUtensorMap sw_q, sw_k, sw_v, sw_bias;
+  // Logits mode (forward only): z = scale * Q K^T + bias + key mask, [B, H, Lq, Lk] contiguous in the dtype of q,
+  // -inf at masked keys; null otherwise.  sw_logits: 64 x 64 boxes of z (the bias map's layout, B * H matrices).
+  void* logits;
+  CUtensorMap sw_logits;
 };
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
 
@@ -55,6 +59,10 @@ struct FmhaBwdParams {
   void* dbias;       // [bias_batch, H, Lq, Lk] 16-bit; == ds_buf when bias_batch == B
   CUtensorMap sw_ds;   // 128-byte-swizzled map of ds_buf (64 x 64 boxes)
   CUtensorMap sw_do;   // 64-row x 64-column boxes of dO (128-byte swizzle)
+  // Logits mode: the incoming gradient dz of the forward's logits output, [B, H, Lq, Lk] contiguous 16-bit, added to
+  // dS everywhere (dS_total = P o (drop(dP) - delta) + dz feeds dQ, dK and dBias); null runs the plain backward.
+  const void* dlogits;
+  CUtensorMap sw_dz;   // 64 x 64 boxes of dlogits (the bias map's layout, B * H matrices)
 };
 void launch_fmha_bwd(const FmhaBwdParams& p, cudaStream_t stream);
 

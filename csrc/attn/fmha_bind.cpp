@@ -91,9 +91,10 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   TORCH_CHECK(ok, "cuTensorMapEncodeTiled failed for the attention operands");
 }
 
-std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k, const Tensor& v,
-                                                      const OptTensor& bias, const OptTensor& kpm, double p_drop,
-                                                      double scale) {
+// (out, lse, keep bits, logits); the logits z = scale * q k^T + bias + key mask only when `logits` is set
+std::tuple<Tensor, Tensor, OptTensor, OptTensor> fwd_impl(const Tensor& q, const Tensor& k, const Tensor& v,
+                                                          const OptTensor& bias, const OptTensor& kpm, double p_drop,
+                                                          double scale, bool logits) {
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaFwdParams p{};
   fill_common(p, q, k, v, bias, kpm, p_drop, scale, /*forward=*/true);
@@ -101,6 +102,14 @@ std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k,
   Tensor lse = torch::empty({p.B, p.H, p.Lq}, q.options().dtype(at::kFloat));
   p.out = out.data_ptr();
   p.lse = lse.data_ptr<float>();
+  OptTensor z;
+  p.logits = nullptr;
+  if (logits) {
+    z = torch::empty({p.B, p.H, p.Lq, p.Lk}, q.options());
+    p.logits = z->data_ptr();
+    TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_logits, p.logits, p.is_bf16 != 0, p.B * p.H, p.Lq, p.Lk),
+                "cuTensorMapEncodeTiled failed for the logits");
+  }
   p.seed = p.offset = 0;
   OptTensor bits;
   if (p_drop > 0.0) {
@@ -114,17 +123,34 @@ std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k,
   ub::launch_fmha_fwd(p, at::cuda::getCurrentCUDAStream().stream());
   cudaError_t err = cudaGetLastError();
   TORCH_CHECK(err == cudaSuccess, "fmha_fwd launch failed: ", cudaGetErrorString(err));
-  return {out, lse, bits};
+  return {out, lse, bits, z};
+}
+
+std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k, const Tensor& v,
+                                                      const OptTensor& bias, const OptTensor& kpm, double p_drop,
+                                                      double scale) {
+  auto r = fwd_impl(q, k, v, bias, kpm, p_drop, scale, /*logits=*/false);
+  return {std::get<0>(r), std::get<1>(r), std::get<2>(r)};
+}
+
+// also returns the logits z [B, H, Lq, Lk] (dtype of q, -inf at masked keys); z is [B, H, ...] even for a [1, H, ...]
+// bias
+std::tuple<Tensor, Tensor, OptTensor, Tensor> fmha_fwd_logits(const Tensor& q, const Tensor& k, const Tensor& v,
+                                                              const OptTensor& bias, const OptTensor& kpm,
+                                                              double p_drop, double scale) {
+  auto r = fwd_impl(q, k, v, bias, kpm, p_drop, scale, /*logits=*/true);
+  return {std::get<0>(r), std::get<1>(r), std::get<2>(r), *std::get<3>(r)};
 }
 
 std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const Tensor& q, const Tensor& k,
                                                        const Tensor& v, const Tensor& out, const Tensor& lse,
                                                        const OptTensor& bias, const OptTensor& kpm, double p_drop,
                                                        double scale, const OptTensor& drop_bits, bool need_dbias,
-                                                       bool packed_grad) {
+                                                       bool packed_grad, const OptTensor& dlogits) {
   // packed_grad: q/k/v are slices [:, :, i] of one [B, L, 3, H, D] tensor; the gradients are then
   // written straight into one packed [B, L, 3, H, D] tensor (returned three times as views), which
   // spares autograd three zero-filled select-backward tensors and two full-size adds per layer.
+  // dlogits: gradient of the logits output of fmha_fwd_logits, [B, H, Lq, Lk]; None means zero.
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaBwdParams p{};
   fill_common(p.f, q, k, v, bias, kpm, p_drop, scale, /*forward=*/false);
@@ -174,6 +200,17 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
     TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_ds, p.ds_buf, p.f.is_bf16 != 0, p.f.B * p.f.H, p.f.Lq, p.f.Lk),
                 "cuTensorMapEncodeTiled failed for the dS scratch tensor");
   }
+  p.dlogits = nullptr;
+  if (dlogits.has_value() && dlogits->defined()) {
+    TORCH_CHECK(dlogits->is_cuda() && dlogits->is_contiguous() && dlogits->dim() == 4 && dlogits->size(0) == p.f.B &&
+                    dlogits->size(1) == p.f.H && dlogits->size(2) == p.f.Lq && dlogits->size(3) == p.f.Lk,
+                "dlogits must be contiguous [B, H, Lq, Lk]");
+    TORCH_CHECK(dlogits->scalar_type() == q.scalar_type(), "dlogits must have the dtype of q");
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(dlogits->data_ptr()) & 15) == 0, "dlogits must be 16-byte aligned");
+    p.dlogits = dlogits->data_ptr();
+    TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_dz, p.dlogits, p.f.is_bf16 != 0, p.f.B * p.f.H, p.f.Lq, p.f.Lk),
+                "cuTensorMapEncodeTiled failed for dlogits");
+  }
   p.delta = delta.data_ptr<float>();
   p.dq_acc = dq_acc.data_ptr<float>();
   p.dq = dq.data_ptr();
@@ -187,6 +224,10 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
 }  // namespace
 
 void register_fmha(pybind11::module_& m) {
+  namespace py = pybind11;
   m.def("fmha_fwd", &fmha_fwd);
-  m.def("fmha_bwd", &fmha_bwd);
+  m.def("fmha_fwd_logits", &fmha_fwd_logits);
+  m.def("fmha_bwd", &fmha_bwd, py::arg("dout"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("out"),
+        py::arg("lse"), py::arg("bias"), py::arg("kpm"), py::arg("p_drop"), py::arg("scale"), py::arg("drop_bits"),
+        py::arg("need_dbias"), py::arg("packed_grad"), py::arg("dlogits") = py::none());
 }

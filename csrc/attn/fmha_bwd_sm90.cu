@@ -23,6 +23,9 @@
 //     into dBias.
 //   Q_i, dO_i and the bias tile are fetched one query tile ahead (two stages), one thread issues every copy.
 // Pre-pass: delta = rowsum(dO o O).   Post-pass: dq = scale * the fp32 accumulator (and dbias = batch sum of dS).
+// Logits mode (template flag kLogits, bp.dlogits set): the gradient dz of the forward's logits output arrives by TMA next
+// to the bias tile (two more 8 KB stages) and is added to dS in fp32, so dS_total = P o (drop(dP) - delta) + dz reaches
+// dK, dQ and dBias.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math_constants.h>
@@ -42,8 +45,8 @@ constexpr int kBM = 64, kBN = 64;   // query rows per step, keys per CTA
 constexpr int kBwdThreads = 128;
 
 // shared memory map (bytes) of the padded head width DP; every box is 64 rows x 128 B, 128-byte swizzled, and a
-// Q / K / V / dO tile is DP / 64 boxes of 8 KB
-template <int DP>
+// Q / K / V / dO tile is DP / 64 boxes of 8 KB.  Logits mode adds two 8 KB stages of the incoming logits gradient dz.
+template <int DP, bool kLogits = false>
 struct BwdCfg {
   static constexpr int kBoxes = DP / 64;
   static constexpr uint32_t kTile = kBoxes * 8192;
@@ -52,7 +55,8 @@ struct BwdCfg {
   static constexpr uint32_t kOffQ = kOffV + kTile;        // 2 stages
   static constexpr uint32_t kOffDO = kOffQ + 2 * kTile;   // 2 stages
   static constexpr uint32_t kOffDS = kOffDO + 2 * kTile;  // 2 stages x 8 KB: bias tile [q][key], then dS in place
-  static constexpr uint32_t kOffDQ = kOffDS + 2 * 8192;   // fp32 [64][DP] dQ tile, row-major (the global accumulator's)
+  static constexpr uint32_t kOffDZ = kOffDS + 2 * 8192;   // logits mode: 2 stages x 8 KB dz tile [q][key]
+  static constexpr uint32_t kOffDQ = kOffDZ + (kLogits ? 2 * 8192 : 0);   // fp32 [64][DP] dQ tile, row-major
   static constexpr uint32_t kOffStats = kOffDQ + kBM * DP * 4;   // 2 stages x {float lse2[64], delta[64], bits[64][2]}
   static constexpr uint32_t kOffBar = kOffStats + 2048;
   static constexpr uint32_t kSmemBytes = kOffBar + 32 + 1024;   // + alignment slack of the 1024-byte-aligned base
@@ -135,9 +139,11 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
 }
 
 // ---- main kernel ----------------------------------------------------------------------------------------------
-template <typename T, int DP>
+// kLogits: the forward also returned z, and dz (fmha_api.h) is added to dS before it is packed, so that the dK operand,
+// the dQ tile and the dBias store all carry dS_total = P o (drop(dP) - delta) + dz
+template <typename T, int DP, bool kLogits>
 __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
-  using C = BwdCfg<DP>;
+  using C = BwdCfg<DP, kLogits>;
   constexpr uint32_t kOffK = C::kOffK, kOffV = C::kOffV, kOffQ = C::kOffQ, kOffDO = C::kOffDO, kOffDS = C::kOffDS,
                      kOffDQ = C::kOffDQ, kOffStats = C::kOffStats, kOffBar = C::kOffBar, kTile = C::kTile;
   extern __shared__ uint8_t smem_raw[];
@@ -157,15 +163,16 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
   const int words_per_row = (p.Lk + 31) / 32;
   // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
-  auto load_tile = [&](int i) {   // one thread: Q_i, dO_i (and the bias tile) -> stage i & 1
+  auto load_tile = [&](int i) {   // one thread: Q_i, dO_i (and the bias and dz tiles) -> stage i & 1
     const uint32_t st = (uint32_t)(i & 1), bar = bar_in0 + 8u * st;
-    mbar_expect_tx(bar, 2 * kTile + (has_bias ? 8192u : 0u));
+    mbar_expect_tx(bar, 2 * kTile + (has_bias ? 8192u : 0u) + (kLogits ? 8192u : 0u));
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
       tma_load_4d(smem_base + kOffQ + st * kTile + x * 8192, &p.sw_q, 64 * x, h, i * kBM, b, bar);
       tma_load_4d(smem_base + kOffDO + st * kTile + x * 8192, &bp.sw_do, 64 * x, h, i * kBM, b, bar);
     }
     if (has_bias) tma_load_3d(smem_base + kOffDS + st * 8192, &p.sw_bias, key0, i * kBM, bias_nb, bar);
+    if constexpr (kLogits) tma_load_3d(smem_base + C::kOffDZ + st * 8192, &bp.sw_dz, key0, i * kBM, (int)bh, bar);
   };
   auto load_stats = [&](int i) {  // all threads: LSE (log2 units, +inf = row contributes nothing), delta, keep bits
     uint8_t* s = smem + kOffStats + (i & 1) * 1024;
@@ -265,6 +272,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
       uint32_t bias_r[4] = {0u, 0u, 0u, 0u};
       const uint32_t addr = sDS + sw128_off(16 * sb + ld_q, ld_chunk);
       if (has_bias) ldmatrix_x4_trans(addr, bias_r);
+      uint32_t dz_r[4];   // dz has the bias tile's layout
+      if constexpr (kLogits) ldmatrix_x4_trans(smem_base + C::kOffDZ + st * 8192 + sw128_off(16 * sb + ld_q, ld_chunk), dz_r);
 #pragma unroll
       for (int r = 0; r < 4; ++r) {   // r: rows (key kl0 or kl1) x query half (16sb + 2c or 16sb + 8 + 2c)
         const int e = 8 * sb + 2 * r;
@@ -282,8 +291,13 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
           k0 = (bits_s[ql * 2 + kword] >> bit) & 1u;
           k1 = (bits_s[(ql + 1) * 2 + kword] >> bit) & 1u;
         }
-        const float ds0 = p0 * (dp[e] * (k0 ? keep_scale : 0.f) - dl.x);
-        const float ds1 = p1 * (dp[e + 1] * (k1 ? keep_scale : 0.f) - dl.y);
+        float ds0 = p0 * (dp[e] * (k0 ? keep_scale : 0.f) - dl.x);
+        float ds1 = p1 * (dp[e + 1] * (k1 ? keep_scale : 0.f) - dl.y);
+        if constexpr (kLogits) {
+          const float2 dz = bwd_unpack2<T>(dz_r[r]);
+          ds0 += dz.x;
+          ds1 += dz.y;
+        }
         pa[sb][r] = bwd_pack2<T>(k0 ? p0 : 0.f, k1 ? p1 : 0.f);   // keep_scale is applied to dV in the epilogue
         da[sb][r] = bwd_pack2<T>(ds0, ds1);                         // the softmax scale to dQ / dK at read-out
       }
@@ -409,9 +423,12 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
   fmha_delta_kernel<T><<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
       reinterpret_cast<const T*>(bp.dout), reinterpret_cast<const T*>(p.out), bp.delta, p.B, p.H, p.Lq, p.D);
   dim3 grid((p.Lk + kBN - 1) / kBN, p.H, p.B);
-  auto kern = fmha_bwd_kernel<T, DP>;
-  cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BwdCfg<DP>::kSmemBytes);
-  kern<<<grid, kBwdThreads, BwdCfg<DP>::kSmemBytes, stream>>>(bp);
+  auto run = [&](auto kern, uint32_t smem_bytes) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    kern<<<grid, kBwdThreads, smem_bytes, stream>>>(bp);
+  };
+  if (bp.dlogits != nullptr) run(fmha_bwd_kernel<T, DP, true>, BwdCfg<DP, true>::kSmemBytes);
+  else run(fmha_bwd_kernel<T, DP, false>, BwdCfg<DP, false>::kSmemBytes);
   const long long cap = (long long)device_sms() * 16;
   if (bp.ds_buf != nullptr && bp.dbias != bp.ds_buf) {
     const long long nv = (long long)p.H * p.Lq * p.Lk / 8;

@@ -21,6 +21,8 @@
 //   that out_proj consumes it without a transpose.
 // 106 KB (DP = 64) / 98 KB (DP = 128) of shared memory and <= 255 registers per thread: two CTAs (8 warps) per SM,
 // so one CTA's softmax overlaps the other's tensor-core work and copies.
+// Logits mode (template flag kLogits, p.logits set) also writes z = S*scale + bias + key mask as [B, H, Lq, Lk]: the
+// 16-bit logits go back over the bias tile in shared memory and leave by TMA store while P V runs (same shared memory).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math_constants.h>
@@ -79,7 +81,11 @@ UB_DEVICE float2 unpack2(uint32_t w) {
 
 UB_DEVICE uint32_t select4(const Philox4& r, int i) { return i == 0 ? r.x : (i == 1 ? r.y : (i == 2 ? r.z : r.w)); }
 
-template <typename T, int DP>
+// kLogits: also write z = scale * Q K^T + bias + key mask (fmha_api.h).  Each thread writes its 16-bit logits back over
+// the bias elements it has just read from the swizzled bias stage (no other thread touches them; the region exists
+// without a bias too), and one thread stores the tile with a TMA store, clipped at Lq / Lk.  The stage is refilled
+// by the prefetch of tile j + 2, so that prefetch first waits until the store has read shared memory.
+template <typename T, int DP, bool kLogits>
 __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
   using C = FwdCfg<DP>;
   constexpr int kBlockN = C::kBlockN;
@@ -151,6 +157,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     }
     // barrier: every thread is done with tile j-1, so its stage may be refilled with tile j+1
     const bool tile_masked = __syncthreads_or(masked) != 0;
+    if (kLogits && tid == 0) bulk_wait_read();   // the logits store of tile j-1 has read the stage tile j+1 fills
     if (tid == 0 && j + 1 < n_tiles) load_tile(j + 1);
     mbar_wait(bar0 + 8u * st, (uint32_t)((j >> 1) & 1));
 
@@ -170,7 +177,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 
     // ---- logits, row max ----------------------------------------------------------------------------------
     float mx0 = -CUDART_INF_F, mx1 = -CUDART_INF_F;
-    const uint8_t* bias_tile = smem + C::kSmemBias + st * C::kBiasStage;
+    uint8_t* bias_tile = smem + C::kSmemBias + st * C::kBiasStage;
 #pragma unroll
     for (int i = 0; i < kBlockN / 8; ++i) {
       const int col = 8 * i + 2 * c;
@@ -188,6 +195,11 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
       s[4 * i + 1] = fmaf(s[4 * i + 1], p.scale, b0.y);
       s[4 * i + 2] = fmaf(s[4 * i + 2], p.scale, b1.x);
       s[4 * i + 3] = fmaf(s[4 * i + 3], p.scale, b1.y);
+      if constexpr (kLogits) {   // the same swizzled positions as the bias elements above
+        uint8_t* box = bias_tile + (i >> 3) * 8192 + c * 4;
+        *reinterpret_cast<uint32_t*>(box + sw128_off(rl0, i & 7)) = pack2<T>(s[4 * i + 0], s[4 * i + 1]);
+        *reinterpret_cast<uint32_t*>(box + sw128_off(rl1, i & 7)) = pack2<T>(s[4 * i + 2], s[4 * i + 3]);
+      }
       mx0 = fmaxf(mx0, fmaxf(s[4 * i + 0], s[4 * i + 1]));
       mx1 = fmaxf(mx1, fmaxf(s[4 * i + 2], s[4 * i + 3]));
     }
@@ -271,6 +283,16 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
       else wgmma_m64n128_rs<T, 1>(o, a, make_desc_sw128_mn(v_addr, C::kKVBox), 1u);
     }
     wgmma_commit();
+    if constexpr (kLogits) {   // while the product runs: the logits tile leaves through one TMA store per 64 keys
+      fence_proxy_async_smem();
+      __syncthreads();
+      if (tid == 0) {
+#pragma unroll
+        for (int x = 0; x < kBlockN / 64; ++x)
+          tma_store_3d(&p.sw_logits, key0 + 64 * x, q0, (int)bh, smem_base + C::kSmemBias + st * C::kBiasStage + x * 8192);
+        bulk_commit();
+      }
+    }
     wgmma_wait<0>();
     fence_operands(o);
   }
@@ -297,6 +319,9 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
       if (8 * i < D) og[4 * i] = pack2<T>(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
     if (c == 0) p.lse[lin1] = l1 > 0.f ? m1 + __logf(l1) : -CUDART_INF_F;
   }
+  if constexpr (kLogits) {
+    if (tid == 0) bulk_wait_all();   // shared memory must outlive the last logits store's reads
+  }
 }
 
 }  // namespace
@@ -307,13 +332,18 @@ void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
     kern<<<grid, kFwdThreads, smem_bytes, stream>>>(p);
   };
-  if (p.D <= 64) {
-    if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64>, FwdCfg<64>::kSmemBytes);
-    else run(fmha_fwd_kernel<__half, 64>, FwdCfg<64>::kSmemBytes);
-  } else {
-    if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128>, FwdCfg<128>::kSmemBytes);
-    else run(fmha_fwd_kernel<__half, 128>, FwdCfg<128>::kSmemBytes);
-  }
+  auto dispatch = [&](auto logits) {
+    constexpr bool kLogits = decltype(logits)::value;
+    if (p.D <= 64) {
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits>, FwdCfg<64>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 64, kLogits>, FwdCfg<64>::kSmemBytes);
+    } else {
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits>, FwdCfg<128>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 128, kLogits>, FwdCfg<128>::kSmemBytes);
+    }
+  };
+  if (p.logits != nullptr) dispatch(std::true_type{});
+  else dispatch(std::false_type{});
 }
 
 }  // namespace ub

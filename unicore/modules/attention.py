@@ -5,12 +5,14 @@ Parity: reference ``unicore/modules/multihead_attention.py`` - ``SelfMultiheadAt
 boolean ``key_padding_mask``, ``return_attn`` yielding ``(out, pre-softmax logits incl. bias,
 probabilities)``) and ``CrossMultiheadAttention:121``.
 
-GPU path: unless ``return_attn`` is requested, the whole ``QK^T -> +bias/mask -> softmax ->
-dropout -> @V`` chain runs in the wgmma kernel behind ``ops.fused_attention`` for every head dim the
-kernel takes (a multiple of 8 up to 128, ``ops.fused_head_dim_supported``); q/k/v are strided
-views of the projection output (no transpose/contiguous copies) and the bias is *not* expanded over
-the batch.  With ``return_attn``, or another head dim, the materialised path (bmm +
-``softmax_dropout`` kernel) is used.
+GPU path: the whole ``QK^T -> +bias/mask -> softmax -> dropout -> @V`` chain runs in the wgmma kernel
+behind ``ops.fused_attention`` for every head dim the kernel takes (a multiple of 8 up to 128,
+``ops.fused_head_dim_supported``); q/k/v are strided views of the projection output (no
+transpose/contiguous copies) and the bias is *not* expanded over the batch.  ``return_attn=True,
+need_probs=False`` (the caller wants the logits but not the probabilities, as Uni-Mol's pair stack does)
+runs in the same kernel in its logits mode, which also writes the logits; its third result is ``None``.
+With the probabilities requested (``return_attn`` and the default ``need_probs=True``), or another head
+dim, or on the CPU, the materialised path (bmm + ``softmax_dropout`` kernel) is used.
 """
 from typing import Optional
 
@@ -78,8 +80,11 @@ class SelfMultiheadAttention(nn.Module):
         self.in_proj = nn.Linear(embed_dim, embed_dim * 3, bias=bias)
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
 
-    def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False):
-        """Everything up to (not including) ``out_proj``: returns ``(o [B, L, E], logits, probs)``."""
+    def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False, need_probs=True):
+        """Everything up to (not including) ``out_proj``: returns ``(o [B, L, E], logits, probs)``.
+
+        ``need_probs=False`` returns ``probs = None``; with ``return_attn`` the fused kernel then also computes the
+        logits ``[B*H, L, L]`` where it takes the shapes."""
         bsz, tgt_len, embed_dim = query.size()
         if embed_dim != self.embed_dim:
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
@@ -89,14 +94,19 @@ class SelfMultiheadAttention(nn.Module):
         qkv = qkv.view(bsz, tgt_len, 3, self.num_heads, self.head_dim)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]  # strided views [B, L, H, D]
         bias4 = _bias_as_4d(attn_bias, bsz, self.num_heads, tgt_len, tgt_len)
-        if not return_attn and ops.fused_attention_supported(q, k, v, bias4, key_padding_mask):
-            o = ops.fused_attention_qkvpacked(
+        if (not return_attn or not need_probs) and ops.fused_attention_supported(q, k, v, bias4, key_padding_mask):
+            res = ops.fused_attention_qkvpacked(
                 qkv, bias=bias4, key_padding_mask=key_padding_mask,
-                dropout_p=self.dropout, training=self.training, scale=self.scaling,
-            ).reshape(bsz, tgt_len, embed_dim)
-            return o, None, None
+                dropout_p=self.dropout, training=self.training, scale=self.scaling, return_logits=return_attn,
+            )
+            if not return_attn:
+                return res.reshape(bsz, tgt_len, embed_dim), None, None
+            o, logits = res
+            return o.reshape(bsz, tgt_len, embed_dim), logits.view(bsz * self.num_heads, tgt_len, tgt_len), None
         qh, kh, vh = ops.split_heads(qkv.view(bsz, tgt_len, 3 * embed_dim), 3, self.num_heads, self.scaling)
-        return _materialised_attention(qh, kh, vh, key_padding_mask, bias4, self.dropout, self.training, return_attn)
+        o, logits, probs = _materialised_attention(qh, kh, vh, key_padding_mask, bias4, self.dropout, self.training,
+                                                   return_attn)
+        return o, logits, (probs if need_probs else None)
 
     def forward(
         self,
@@ -104,8 +114,9 @@ class SelfMultiheadAttention(nn.Module):
         key_padding_mask: Optional[Tensor] = None,
         attn_bias: Optional[Tensor] = None,
         return_attn: bool = False,
+        need_probs: bool = True,
     ) -> Tensor:
-        o, logits, probs = self.attend(query, key_padding_mask, attn_bias, return_attn)
+        o, logits, probs = self.attend(query, key_padding_mask, attn_bias, return_attn, need_probs)
         o = self.out_proj(o)
         return (o, logits, probs) if return_attn else o
 

@@ -99,10 +99,12 @@ class _BlockMixin:
     def _attn_residual(self, attn_module, norm, residual, attn_in, **kw):
         """post-LN: LN(residual + drop(attn(x)));  pre-LN: residual + drop(attn(LN(x)))."""
         return_attn = kw.pop("return_attn", False)
+        need_probs = kw.pop("need_probs", True)
         h = attn_in if self.post_ln else norm(attn_in)
         extra = None
         if isinstance(attn_module, SelfMultiheadAttention):
-            o, logits, probs = attn_module.attend(h, kw.get("key_padding_mask"), kw.get("attn_bias"), return_attn)
+            o, logits, probs = attn_module.attend(h, kw.get("key_padding_mask"), kw.get("attn_bias"), return_attn,
+                                                  need_probs)
             if return_attn:
                 extra = (logits, probs)
         else:
@@ -175,10 +177,13 @@ class TransformerEncoderLayer(nn.Module, _BlockMixin):
         attn_bias: Optional[torch.Tensor] = None,
         padding_mask: Optional[torch.Tensor] = None,
         return_attn: bool = False,
+        need_probs: bool = True,
     ) -> torch.Tensor:
+        """With ``return_attn`` returns ``(x, logits, probs)``; ``need_probs=False`` makes ``probs`` None and lets the
+        fused attention kernel produce the logits."""
         x, extra = self._attn_residual(
             self.self_attn, self.self_attn_layer_norm, x, x,
-            key_padding_mask=padding_mask, attn_bias=attn_bias, return_attn=return_attn,
+            key_padding_mask=padding_mask, attn_bias=attn_bias, return_attn=return_attn, need_probs=need_probs,
         )
         x = self._ffn_residual(x)
         if not return_attn:

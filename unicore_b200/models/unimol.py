@@ -12,8 +12,10 @@ full ``[B*H, N, N]`` bias.  This file implements the publicly described architec
   logits, which become the next layer's bias (pair update);
 * heads: masked-atom LM, pair-distance regression, SE(3)-equivariant coordinate update.
 
-Hot ops on the GPU: ``ops.softmax_dropout`` (materialised, head_dim 8 is not an MMA shape), LayerNorm(512)
-and LayerNorm(64) kernels, bias+GELU; the GEMMs go to cuBLAS.
+Hot ops on the GPU: the fused wgmma attention in its logits mode (``ops.fused_attention_qkvpacked(...,
+return_logits=True)``: head dim 8 runs on the 64-column kernels; each layer writes its logits and takes their
+gradient, and the ``[B, H, N, N]`` probabilities are never materialised), LayerNorm(512) and LayerNorm(64)
+kernels, bias+GELU; the GEMMs go to cuBLAS.
 """
 import math
 
@@ -153,11 +155,13 @@ class TransformerEncoderWithPair(nn.Module):
         input_padding_mask = padding_mask
 
         # The reference writes -inf into the padded key columns of the pair bias up front (a full pass over
-        # [B, H, L, L] and another in backward).  Here the first layer's softmax kernel adds the [B, 1, 1, L]
+        # [B, H, L, L] and another in backward).  Here the first layer's attention kernel adds the [B, 1, 1, L]
         # padding mask while it forms the logits; those logits ARE the next layer's bias, so the -inf columns
         # travel with the pair representation from then on.
+        # Only the logits are threaded on (need_probs=False), so on the GPU each layer's attention runs fused.
         for layer in self.layers:
-            x, attn_mask, _ = layer(x, padding_mask=padding_mask, attn_bias=attn_mask, return_attn=True)
+            x, attn_mask, _ = layer(x, padding_mask=padding_mask, attn_bias=attn_mask, return_attn=True,
+                                    need_probs=False)
             padding_mask = None
 
         def norm_loss(t, tolerance=1.0):

@@ -11,6 +11,12 @@ reads the dropout keep bits the forward kernel stored.
 
 The kernels take every head dim ``D`` with ``D % 8 == 0`` and ``8 <= D <= 128`` (``fused_head_dim_supported``);
 other head dims, and callers that need the probabilities (``return_attn``), use ``attention_reference``.
+
+``return_logits=True`` also returns the logits ``z = scale * q k^T + bias + key_mask`` as ``[B, H, Lq, Lk]`` (the
+contract of ``softmax_dropout_with_logits``): the key padding mask is additive, so ``z`` is ``-inf`` at masked keys,
+and the gradient ``dz`` of ``z`` is added to the softmax gradient at every position before it reaches q, k and the
+bias.  The kernels write ``z`` from the forward pass and take ``dz`` in the backward pass; the probabilities are never
+materialised.  Uni-Mol threads ``z`` through its layers as the pair representation.
 """
 import math
 
@@ -27,11 +33,13 @@ def fused_head_dim_supported(head_dim: int) -> bool:
     return 8 <= head_dim <= FUSED_MAX_HEAD_DIM and head_dim % 8 == 0
 
 
-def attention_reference(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None):
+def attention_reference(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
+                        return_logits=False):
     """Plain PyTorch implementation with the same signature (fallback + test oracle).
 
     q: [B, Lq, H, D], k/v: [B, Lk, H, D]; bias broadcastable to [B, H, Lq, Lk];
-    key_padding_mask: [B, Lk] bool (True = masked). Returns [B, Lq, H, D].
+    key_padding_mask: [B, Lk] bool (True = masked). Returns [B, Lq, H, D], or with ``return_logits``
+    ``(out, z)`` with ``z [B, H, Lq, Lk]`` built with an additive ``-inf`` mask (its gradient reaches masked keys).
     """
     B, Lq, H, D = q.shape
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
@@ -39,32 +47,57 @@ def attention_reference(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0
     if bias is not None:
         scores = scores + bias.to(scores.dtype)
     if key_padding_mask is not None:
-        scores = scores.masked_fill(key_padding_mask[:, None, None, :].to(torch.bool), float("-inf"))
+        if return_logits:
+            pad = torch.zeros(B, 1, 1, k.shape[1], dtype=scores.dtype, device=scores.device)
+            scores = scores + pad.masked_fill(key_padding_mask[:, None, None, :].to(torch.bool), float("-inf"))
+        else:
+            scores = scores.masked_fill(key_padding_mask[:, None, None, :].to(torch.bool), float("-inf"))
     probs = F.softmax(scores.float(), dim=-1).to(q.dtype)
     probs = F.dropout(probs, p=dropout_p, training=training)
-    return torch.einsum("bhqk,bkhd->bqhd", probs, v)
+    out = torch.einsum("bhqk,bkhd->bqhd", probs, v)
+    return (out, scores) if return_logits else out
+
+
+def _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits):
+    """Shared forward of the two Functions: runs the kernel, records what the backward needs, returns
+    ``(out, lse, bits, logits)`` (logits None without ``return_logits``)."""
+    p = float(dropout_p) if training else 0.0
+    logits = None
+    if return_logits:
+        out, lse, bits, logits = native().fmha_fwd_logits(q, k, v, bias, key_padding_mask, p, float(scale))
+        # a logits gradient that autograd never produced stays None (= zero) instead of a zero-filled [B, H, Lq, Lk]
+        ctx.set_materialize_grads(False)
+    else:
+        out, lse, bits = native().fmha_fwd(q, k, v, bias, key_padding_mask, p, float(scale))
+    ctx.p = p
+    ctx.scale = float(scale)
+    ctx.need_dbias = bias is not None and bias.requires_grad
+    return out, lse, bits, logits
+
+
+def _bwd_grads(out, dout, dlogits):
+    """(dout, dlogits) for the kernel; a missing gradient is zero, and a missing dlogits runs the plain backward."""
+    dout = torch.zeros_like(out) if dout is None else dout.contiguous()
+    return dout, (None if dlogits is None else dlogits.contiguous())
 
 
 class _FusedAttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale):
-        p = float(dropout_p) if training else 0.0
-        out, lse, bits = native().fmha_fwd(q, k, v, bias, key_padding_mask, p, float(scale))
+    def forward(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits=False):
+        out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
         ctx.save_for_backward(q, k, v, out, lse, bias, key_padding_mask, bits)
-        ctx.p = p
-        ctx.scale = float(scale)
-        ctx.need_dbias = bias is not None and bias.requires_grad
-        return out
+        return (out, logits) if return_logits else out
 
     @staticmethod
-    def backward(ctx, dout):
+    def backward(ctx, dout, dlogits=None):
         q, k, v, out, lse, bias, kpm, bits = ctx.saved_tensors
+        dout, dlogits = _bwd_grads(out, dout, dlogits)
         dq, dk, dv, dbias = native().fmha_bwd(
-            dout.contiguous(), q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, False
+            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, False, dlogits
         )
         if dbias is not None and dbias.dtype != bias.dtype:
             dbias = dbias.to(bias.dtype)
-        return dq, dk, dv, dbias, None, None, None, None
+        return dq, dk, dv, dbias, None, None, None, None, None
 
 
 class _FusedAttentionPackedFn(torch.autograd.Function):
@@ -72,27 +105,24 @@ class _FusedAttentionPackedFn(torch.autograd.Function):
     in, and the backward kernels write dq/dk/dv directly into ONE packed gradient tensor."""
 
     @staticmethod
-    def forward(ctx, qkv, bias, key_padding_mask, dropout_p, training, scale):
-        p = float(dropout_p) if training else 0.0
+    def forward(ctx, qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits=False):
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-        out, lse, bits = native().fmha_fwd(q, k, v, bias, key_padding_mask, p, float(scale))
+        out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
         ctx.save_for_backward(qkv, out, lse, bias, key_padding_mask, bits)
-        ctx.p = p
-        ctx.scale = float(scale)
-        ctx.need_dbias = bias is not None and bias.requires_grad
-        return out
+        return (out, logits) if return_logits else out
 
     @staticmethod
-    def backward(ctx, dout):
+    def backward(ctx, dout, dlogits=None):
         qkv, out, lse, bias, kpm, bits = ctx.saved_tensors
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+        dout, dlogits = _bwd_grads(out, dout, dlogits)
         dq, _dk, _dv, dbias = native().fmha_bwd(
-            dout.contiguous(), q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, True
+            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, True, dlogits
         )
         dqkv = dq._base  # the packed [B, L, 3, H, D] tensor the three gradients are views of
         if dbias is not None and dbias.dtype != bias.dtype:
             dbias = dbias.to(bias.dtype)
-        return dqkv, dbias, None, None, None, None
+        return dqkv, dbias, None, None, None, None, None
 
 
 def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool:
@@ -126,8 +156,11 @@ def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool
     return True
 
 
-def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None):
-    """Dispatch to the wgmma kernel when shapes/dtypes allow, else to the PyTorch reference."""
+def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
+                    return_logits=False):
+    """Dispatch to the wgmma kernel when shapes/dtypes allow, else to the PyTorch reference.
+
+    Returns ``[B, Lq, H, D]``, or ``(out, z [B, H, Lq, Lk])`` with ``return_logits`` (see the module docstring)."""
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
     if fused_attention_supported(q, k, v, bias, key_padding_mask):
@@ -136,12 +169,14 @@ def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, tr
             bias = bias.to(q.dtype).contiguous()
         if key_padding_mask is not None:
             key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
-        return _FusedAttentionFn.apply(q, k, v, bias, key_padding_mask, dropout_p, training, scale)
-    return attention_reference(q, k, v, bias, key_padding_mask, dropout_p, training, scale)
+        return _FusedAttentionFn.apply(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
+    return attention_reference(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
 
 
-def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None):
-    """Self-attention on the packed in_proj output ``qkv [B, L, 3, H, D]`` (returns ``[B, L, H, D]``)."""
+def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
+                              return_logits=False):
+    """Self-attention on the packed in_proj output ``qkv [B, L, 3, H, D]`` (returns ``[B, L, H, D]``, or
+    ``(out, z [B, H, L, L])`` with ``return_logits``)."""
     q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
@@ -150,5 +185,5 @@ def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0
             bias = bias.to(q.dtype).contiguous()
         if key_padding_mask is not None:
             key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
-        return _FusedAttentionPackedFn.apply(qkv, bias, key_padding_mask, dropout_p, training, scale)
-    return fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale)
+        return _FusedAttentionPackedFn.apply(qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits)
+    return fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
