@@ -47,7 +47,8 @@ struct FmhaBwdParams {
   const void* dout;  // [B, Lq, H, D] contiguous
   float* delta;      // [B, H, Lq] scratch: rowsum(dO * O)
   float* dq_acc;     // [B, H, ceil(Lq / 64) * 64, DP] fp32 (DP = padded head width), zeroed: every key tile adds its
-                     // dQ share with bulk reductions
+                     // dQ share with bulk reductions.  Row q keeps its 8-column groups in the order group ^ (q & 7)
+                     // (the conflict-free layout of the tile in shared memory); only the dQ convert kernel reads it.
   void* dq;          // [B, Lq, H, D] 16-bit results, addressed through (batch, seq, head) element strides so
   void* dk;          // that they can be slices of one packed [B, L, 3, H, D] gradient tensor
   void* dv;

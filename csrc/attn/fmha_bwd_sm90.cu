@@ -10,14 +10,16 @@
 //   products are computed transposed (keys are the M dimension), so that P^T and dS^T are accumulator tiles whose
 //   16-bit conversions are directly the register A operands of the dV / dK products:
 //     S^T  = K_j Q_i^T                      wgmma m64n64, both operands K-major from shared memory
-//     dP^T = V_j dO_i^T                     wgmma m64n64
+//     dP^T = V_j dO_i^T                     wgmma m64n64, a commit group of its own: P is formed while it runs
 //     P = exp2((S*scale + bias + kmask) * log2e - LSE_i * log2e) ;  dS = P o (drop(dP) - delta_i)
+//                                           (keep bits read once per tile into registers, applied as selects)
 //     dV_j += drop(P)^T dO_i                wgmma m64n{DP}, A from registers, dO MN-major
 //     dK_j += dS^T Q_i                      wgmma m64n{DP}, A from registers, Q MN-major
 //     dQ_i += dS K_j                        wgmma m64n64 per 64-column half of K (one dq[32] reused, so that DP = 128
 //                                           fits the registers next to dV and dK), dS from shared memory
 //                                           (stmatrix.trans of the registers, written in place over the consumed bias
-//                                           tile), K MN-major; the fp32 tile is added to a global fp32 accumulator
+//                                           tile), K MN-major; the fp32 tile (bank-conflict-free column order,
+//                                           dq_swz_col) is added to a global fp32 accumulator of the same order
 //                                           with ONE bulk reduction (cp.reduce.async.bulk)
 //     dS tile (16-bit, in shared memory for the dQ product) -> TMA store; a follow-up kernel sums it over the batch
 //     into dBias.
@@ -56,8 +58,8 @@ struct BwdCfg {
   static constexpr uint32_t kOffDO = kOffQ + 2 * kTile;   // 2 stages
   static constexpr uint32_t kOffDS = kOffDO + 2 * kTile;  // 2 stages x 8 KB: bias tile [q][key], then dS in place
   static constexpr uint32_t kOffDZ = kOffDS + 2 * 8192;   // logits mode: 2 stages x 8 KB dz tile [q][key]
-  static constexpr uint32_t kOffDQ = kOffDZ + (kLogits ? 2 * 8192 : 0);   // fp32 [64][DP] dQ tile, row-major
-  static constexpr uint32_t kOffStats = kOffDQ + kBM * DP * 4;   // 2 stages x {float lse2[64], delta[64], bits[64][2]}
+  static constexpr uint32_t kOffDQ = kOffDZ + (kLogits ? 2 * 8192 : 0);   // fp32 [64][DP] dQ tile (dq_swz_col)
+  static constexpr uint32_t kOffStats = kOffDQ + kBM * DP * 4;   // 2 stages x {float lse2[64], delta[64], bits[2][64]}
   static constexpr uint32_t kOffBar = kOffStats + 2048;
   static constexpr uint32_t kSmemBytes = kOffBar + 32 + 1024;   // + alignment slack of the 1024-byte-aligned base
 };
@@ -84,6 +86,12 @@ UB_DEVICE float2 bwd_unpack2(uint32_t w) {
     return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
   }
 }
+
+// Column layout of the fp32 dQ tile in shared memory and of its accumulator rows in global memory (the bulk reduction
+// copies the tile linearly): the 8-column (32-byte) group of column `col` in row q is stored at group ^ (q & 7).  A
+// warp's float2 stores cover 8 rows x 8 columns of one group; unswizzled, every row of 256 or 512 bytes starts in the
+// same bank and the store takes 8 wavefronts, swizzled it takes the minimum, 2.
+UB_DEVICE int dq_swz_col(int q, int col) { return (((col >> 3) ^ (q & 7)) << 3) | (col & 7); }
 
 // ---- pre-pass: delta[b,h,q] = sum_d dO * O -----------------------------------------------------------------
 template <typename T>
@@ -130,7 +138,7 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
     const long long bh = row / Lq;
     const int h = (int)(bh % H);
     const long long b = bh / H;
-    const float4* src = reinterpret_cast<const float4*>(acc + ((bh * Lq_pad + q) * DP + part * 8));
+    const float4* src = reinterpret_cast<const float4*>(acc + ((bh * Lq_pad + q) * DP + dq_swz_col(q, part * 8)));
     const float4 x0 = src[0], x1 = src[1];
     const float x[8] = {x0.x * scale, x0.y * scale, x0.z * scale, x0.w * scale,
                         x1.x * scale, x1.y * scale, x1.z * scale, x1.w * scale};
@@ -184,9 +192,9 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     } else {
       reinterpret_cast<float*>(s + 256)[tid - 64] = ok ? bp.delta[bh * p.Lq + q] : 0.f;
     }
-    if (drop) {
+    if (drop) {   // bits[w][q]: word w of the tile's two for query q, so that queries q, q + 1 are one 8-byte load
       const int qb = i * kBM + (tid >> 1), wi = (key0 >> 5) + (tid & 1);
-      reinterpret_cast<uint32_t*>(s + 512)[tid] =
+      reinterpret_cast<uint32_t*>(s + 512)[(tid & 1) * 64 + (tid >> 1)] =
           (qb < p.Lq && wi < words_per_row) ? p.drop_bits[(bh * p.Lq + qb) * words_per_row + wi] : 0xffffffffu;
     }
   };
@@ -251,46 +259,64 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
       const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
       wgmma_m64n64_ss<T, 0>(s, make_desc_sw128(smem_base + kOffK + off), make_desc_sw128(sQ + off), kk > 0 ? 1u : 0u);
     }
+    wgmma_commit();   // S^T and dP^T are separate groups: P is formed while dP^T is still on the tensor cores
 #pragma unroll
     for (int kk = 0; kk < DP / 16; ++kk) {
       const uint32_t off = (kk >> 2) * 8192 + (kk & 3) * 32;
       wgmma_m64n64_ss<T, 0>(dp, make_desc_sw128(smem_base + kOffV + off), make_desc_sw128(sDO + off), kk > 0 ? 1u : 0u);
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    fence_operands(s);
-    fence_operands(dp);
 
-    // ---- P^T, dS^T in registers ---------------------------------------------------------------------------------
     const uint8_t* stats = smem + kOffStats + st * 1024;
     const float* lse2_s = reinterpret_cast<const float*>(stats);
     const float* delta_s = reinterpret_cast<const float*>(stats + 256);
-    const uint32_t* bits_s = reinterpret_cast<const uint32_t*>(stats + 512);
-    uint32_t pa[4][4], da[4][4];   // [16-query block][A-operand register] of drop(P)^T and dS^T
+    const uint32_t* bits_s = reinterpret_cast<const uint32_t*>(stats + 512) + 64 * kword;
+
+    // ---- P^T = exp2(logits - LSE), in place over S^T ------------------------------------------------------------
+    wgmma_wait<1>();
+    fence_operands(s);
 #pragma unroll
     for (int sb = 0; sb < 4; ++sb) {
       uint32_t bias_r[4] = {0u, 0u, 0u, 0u};
       const uint32_t addr = sDS + sw128_off(16 * sb + ld_q, ld_chunk);
       if (has_bias) ldmatrix_x4_trans(addr, bias_r);
-      uint32_t dz_r[4];   // dz has the bias tile's layout
-      if constexpr (kLogits) ldmatrix_x4_trans(smem_base + C::kOffDZ + st * 8192 + sw128_off(16 * sb + ld_q, ld_chunk), dz_r);
 #pragma unroll
       for (int r = 0; r < 4; ++r) {   // r: rows (key kl0 or kl1) x query half (16sb + 2c or 16sb + 8 + 2c)
         const int e = 8 * sb + 2 * r;
-        const bool hi_key = (r & 1) != 0;
         const int ql = 16 * sb + 8 * (r >> 1) + 2 * c;
         const float2 bb = has_bias ? bwd_unpack2<T>(bias_r[r]) : make_float2(0.f, 0.f);
-        const float ka = hi_key ? kadd1 : kadd0;
+        const float ka = (r & 1) ? kadd1 : kadd0;
         const float2 l2 = *reinterpret_cast<const float2*>(lse2_s + ql);
-        const float2 dl = *reinterpret_cast<const float2*>(delta_s + ql);
         const float x0 = fmaf(s[e], p.scale, bb.x + ka), x1 = fmaf(s[e + 1], p.scale, bb.y + ka);
-        const float p0 = ex2_approx(fmaf(x0, kLog2e, -l2.x)), p1 = ex2_approx(fmaf(x1, kLog2e, -l2.y));
-        bool k0 = true, k1 = true;
-        if (drop) {
-          const int bit = hi_key ? bit1 : bit0;
-          k0 = (bits_s[ql * 2 + kword] >> bit) & 1u;
-          k1 = (bits_s[(ql + 1) * 2 + kword] >> bit) & 1u;
-        }
+        s[e] = ex2_approx(fmaf(x0, kLog2e, -l2.x));
+        s[e + 1] = ex2_approx(fmaf(x1, kLog2e, -l2.y));
+      }
+    }
+
+    // ---- dS^T = P o (drop(dP) - delta) (+ dz), both packed into register A operands ----------------------------------
+    wgmma_wait<0>();
+    fence_operands(s);
+    fence_operands(dp);
+    uint32_t pa[4][4], da[4][4];   // [16-query block][A-operand register] of drop(P)^T and dS^T
+#pragma unroll
+    for (int sb = 0; sb < 4; ++sb) {
+      uint32_t dz_r[4];   // dz has the bias tile's layout
+      if constexpr (kLogits) ldmatrix_x4_trans(smem_base + C::kOffDZ + st * 8192 + sw128_off(16 * sb + ld_q, ld_chunk), dz_r);
+      // keep bits of my queries 16sb + 2c, +1 and 16sb + 8 + 2c, +1 in word kword: two 8-byte loads, read once per
+      // tile and applied below as selects
+      uint2 kb[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh)
+        kb[hh] = drop ? *reinterpret_cast<const uint2*>(bits_s + 16 * sb + 8 * hh + 2 * c) : make_uint2(~0u, ~0u);
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int e = 8 * sb + 2 * r;
+        const int ql = 16 * sb + 8 * (r >> 1) + 2 * c;
+        const int bit = (r & 1) ? bit1 : bit0;
+        const uint2 w = kb[r >> 1];   // queries ql, ql + 1
+        const bool k0 = (w.x >> bit) & 1u, k1 = (w.y >> bit) & 1u;
+        const float2 dl = *reinterpret_cast<const float2*>(delta_s + ql);
+        const float p0 = s[e], p1 = s[e + 1];
         float ds0 = p0 * (dp[e] * (k0 ? keep_scale : 0.f) - dl.x);
         float ds1 = p1 * (dp[e + 1] * (k1 ? keep_scale : 0.f) - dl.y);
         if constexpr (kLogits) {
@@ -346,10 +372,12 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
         fence_operands(dk);
       }
       fence_operands(dq);
+      // rows kl0 and kl1 are both = g (mod 8), and so are the global rows i * 64 + kl0 / kl1
 #pragma unroll
       for (int n = 0; n < 8; ++n) {
-        *reinterpret_cast<float2*>(dq_s + kl0 * DP + 64 * x + 8 * n + 2 * c) = make_float2(dq[4 * n], dq[4 * n + 1]);
-        *reinterpret_cast<float2*>(dq_s + kl1 * DP + 64 * x + 8 * n + 2 * c) = make_float2(dq[4 * n + 2], dq[4 * n + 3]);
+        const int col = dq_swz_col(g, 64 * x + 8 * n + 2 * c);
+        *reinterpret_cast<float2*>(dq_s + kl0 * DP + col) = make_float2(dq[4 * n], dq[4 * n + 1]);
+        *reinterpret_cast<float2*>(dq_s + kl1 * DP + col) = make_float2(dq[4 * n + 2], dq[4 * n + 3]);
       }
     }
     fence_proxy_async_smem();

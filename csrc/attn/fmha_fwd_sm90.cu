@@ -14,7 +14,9 @@
 //   2. S = Q K_j^T           DP/16 x wgmma m64n{kBlockN}k16, both operands K-major from shared memory, fp32 in registers
 //   3. softmax in registers: logits = S*scale + bias + key mask, row max across the 4 threads of a quad, online
 //      rescaling of O and of the row sum, Philox dropout on packed 16-bit pairs (the keep bits are stored for the
-//      backward pass), P converted in place into the register A operand of the next product
+//      backward pass), P converted in place into the register A operand of the next product.  Each Philox call is
+//      made by one thread of the quad that needs its words, and a 4 x 4 word transpose in the quad (quad_transpose4)
+//      distributes them.
 //   4. O += P V_j            kBlockN/16 x wgmma m64n{DP}k16, A (P) from registers, V presented MN-major from its
 //                            row-major bytes (at DP = 128 the descriptor steps to the second box through its LBO)
 //   q/k/v are read through strides straight out of the packed in_proj output; O is written as [B, Lq, H, D] so
@@ -79,7 +81,27 @@ UB_DEVICE float2 unpack2(uint32_t w) {
   }
 }
 
-UB_DEVICE uint32_t select4(const Philox4& r, int i) { return i == 0 ? r.x : (i == 1 ? r.y : (i == 2 ? r.z : r.w)); }
+// w[j] <- w[j ^ x] for x in 0..3 (per-thread), as two conditional swaps: 8 selects, no runtime-indexed array
+UB_DEVICE void xor_permute4(uint32_t (&w)[4], int x) {
+  const bool s1 = (x & 1) != 0, s2 = (x & 2) != 0;
+  uint32_t a0 = s1 ? w[1] : w[0], a1 = s1 ? w[0] : w[1], a2 = s1 ? w[3] : w[2], a3 = s1 ? w[2] : w[3];
+  w[0] = s2 ? a2 : a0;
+  w[1] = s2 ? a3 : a1;
+  w[2] = s2 ? a0 : a2;
+  w[3] = s2 ? a1 : a3;
+}
+
+// 4 x 4 word transpose inside a quad: thread c holds the four words of Philox call c and leaves with word c of calls
+// 0..3 (w[k] = word c of call k).  After the first permutation w[m] is the word that partner c ^ m needs, so each of the
+// three shuffles sends a fixed register; the received w[m] is word c of call c ^ m, and the second permutation puts
+// it in place.
+UB_DEVICE void quad_transpose4(uint32_t (&w)[4], int c) {
+  xor_permute4(w, c);
+  w[1] = __shfl_xor_sync(0xffffffffu, w[1], 1);
+  w[2] = __shfl_xor_sync(0xffffffffu, w[2], 2);
+  w[3] = __shfl_xor_sync(0xffffffffu, w[3], 3);
+  xor_permute4(w, c);
+}
 
 // kLogits: also write z = scale * Q K^T + bias + key mask (fmha_api.h).  Each thread writes its 16-bit logits back over
 // the bias elements it has just read from the swizzled bias stage (no other thread touches them; the region exists
@@ -139,6 +161,11 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   const unsigned long long bh = (unsigned long long)b * p.H + h;
   const unsigned long long lin0 = bh * p.Lq + (row0 < p.Lq ? row0 : 0), lin1 = bh * p.Lq + (row1 < p.Lq ? row1 : 0);
   const int words_per_row = (p.Lk + 31) / 32;
+  // Philox counter of element (lin, key) is (lin * Lk + key) >> 3, one call per (row, 8 keys).  For each pair of 8-key
+  // groups (i, i + 1) the quad needs four calls - rows rl0 / rl1 x groups i / i + 1 - and thread c computes call c:
+  // row rl0 for even c, rl1 for odd c, group i + (c >> 1).  ctr_c is that call's (lin * Lk + key) at group pair 0 of
+  // tile 0; a tile adds kBlockN, a group pair 16.
+  const unsigned long long ctr_c = ((c & 1) ? lin1 : lin0) * p.Lk + 8 * (c >> 1);
 
   constexpr float kLog2e = 1.4426950408889634f;
   float m0 = -CUDART_INF_F, m1 = -CUDART_INF_F, l0 = 0.f, l1 = 0.f;   // running max (in use) and partial row sums
@@ -230,24 +257,33 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     uint32_t kw0[kWords], kw1[kWords];   // keep bits, one word per 32 keys
 #pragma unroll
     for (int w = 0; w < kWords; ++w) kw0[w] = kw1[w] = 0u;
+    const unsigned long long ctr_tile = ctr_c + (unsigned long long)key0;
 #pragma unroll
-    for (int i = 0; i < kBlockN / 8; ++i) {
-      const float p00 = ex2_approx(fmaf(s[4 * i + 0], kLog2e, nm0)), p01 = ex2_approx(fmaf(s[4 * i + 1], kLog2e, nm0));
-      const float p10 = ex2_approx(fmaf(s[4 * i + 2], kLog2e, nm1)), p11 = ex2_approx(fmaf(s[4 * i + 3], kLog2e, nm1));
-      l0 += p00 + p01;
-      l1 += p10 + p11;
-      uint32_t km0 = 0xffffffffu, km1 = 0xffffffffu;
+    for (int i2 = 0; i2 < kBlockN / 16; ++i2) {   // 8-key groups i = 2 i2, 2 i2 + 1
+      // km[2h + r]: keep masks of group 2 i2 + h, row rl0 (r = 0) / rl1 (r = 1); word c decides the pair of keys
+      // 8i + 2c, +1 (bit layout of fmha_api.h)
+      uint32_t km[4] = {0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu};
       if (drop) {
-        // one Philox call per (row, 8 keys): word c decides the pair of keys 8i + 2c, +1 (bit layout of fmha_api.h)
-        const unsigned long long k8 = (unsigned long long)(key0 + 8 * i);
-        km0 = keep_mask2(select4(philox4x32<7>(p.seed, p.offset, (lin0 * p.Lk + k8) >> 3), c), t14x2);
-        km1 = keep_mask2(select4(philox4x32<7>(p.seed, p.offset, (lin1 * p.Lk + k8) >> 3), c), t14x2);
+        const Philox4 r = philox4x32<7>(p.seed, p.offset, (ctr_tile + 16u * i2) >> 3);
+        uint32_t w[4] = {r.x, r.y, r.z, r.w};
+        quad_transpose4(w, c);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) km[k] = keep_mask2(w[k], t14x2);
+      }
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int i = 2 * i2 + hh;
+        const float p00 = ex2_approx(fmaf(s[4 * i + 0], kLog2e, nm0)), p01 = ex2_approx(fmaf(s[4 * i + 1], kLog2e, nm0));
+        const float p10 = ex2_approx(fmaf(s[4 * i + 2], kLog2e, nm1)), p11 = ex2_approx(fmaf(s[4 * i + 3], kLog2e, nm1));
+        l0 += p00 + p01;
+        l1 += p10 + p11;
+        const uint32_t km0 = km[2 * hh], km1 = km[2 * hh + 1];
         const uint32_t bit = 0x00010001u << (4 * (i & 3) + c);
         kw0[i >> 2] |= km0 & bit;
         kw1[i >> 2] |= km1 & bit;
+        pa[2 * i] = pack2<T>(p00, p01) & km0;
+        pa[2 * i + 1] = pack2<T>(p10, p11) & km1;
       }
-      pa[2 * i] = pack2<T>(p00, p01) & km0;
-      pa[2 * i + 1] = pack2<T>(p10, p11) & km1;
     }
     if (drop && p.drop_bits != nullptr) {
 #pragma unroll
