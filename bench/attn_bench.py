@@ -7,6 +7,11 @@ Times forward and forward+backward with CUDA events (L2 flushed between iteratio
 256 MB buffer) and prints one JSON line per variant with achieved TFLOP/s (4*B*H*L*L*D FLOPs forward,
 2.5x that backward) and the fraction of the dense 16-bit peak (MEASURED_PEAKS.json if present, else the H100
 data sheet).
+
+--causal adds three variants with dropout 0.1: ``causal_dropout`` (no bias), ``causal_bias_mask_dropout`` (the kernels'
+causal flag) and ``future_bias_mask_dropout`` (the same bias plus an explicit [L, L] -inf future mask, added once
+outside the timed region, in the non-causal kernels).  Their FLOP/s count only the visible (query, key) pairs,
+4*B*H*D*sum_i min(i+1, L), for all three, so that the numbers compare the work each path has to do.
 """
 import argparse
 import json
@@ -44,6 +49,7 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--dtype", default="float16")
     ap.add_argument("--only", default="")
+    ap.add_argument("--causal", action="store_true", help="also time the causal variants (FLOPs of visible pairs)")
     args = ap.parse_args()
     from unicore import ops
 
@@ -63,24 +69,36 @@ def main():
     kpm = torch.zeros(B, L, dtype=torch.bool, device="cuda")
     dout = torch.randn(B, L, H, D, device="cuda").to(dtype)
     flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")
-    fwd_flops = 4.0 * B * H * L * L * D
+    dense_flops = 4.0 * B * H * L * L * D
     variants = {
         "plain": dict(bias=None, kpm=None, p=0.0),
         "bias": dict(bias=bias, kpm=None, p=0.0),
         "bias_mask": dict(bias=bias, kpm=kpm, p=0.0),
         "bias_mask_dropout": dict(bias=bias, kpm=kpm, p=0.1),
     }
+    if args.causal:
+        future = torch.full((L, L), float("-inf"), device="cuda").triu(1)
+        future_bias = (bias.detach().float() + future).to(dtype).requires_grad_(True)
+        variants.update({
+            "causal_dropout": dict(bias=None, kpm=None, p=0.1, causal=True),
+            "causal_bias_mask_dropout": dict(bias=bias, kpm=kpm, p=0.1, causal=True),
+            "future_bias_mask_dropout": dict(bias=future_bias, kpm=kpm, p=0.1, visible=True),
+        })
     for name, cfg in variants.items():
         if args.only and name != args.only:
             continue
+        causal = cfg.get("causal", False)
+        # visible (query, key) pairs only for the causal variants: sum_i min(i + 1, L) = L (L + 1) / 2
+        fwd_flops = 4.0 * B * H * D * L * (L + 1) / 2 if causal or cfg.get("visible") else dense_flops
 
         def fwd():
             return ops.fused_attention(q, k, v, bias=cfg["bias"], key_padding_mask=cfg["kpm"], dropout_p=cfg["p"],
-                                       training=True, scale=scale)
+                                       training=True, scale=scale, causal=causal)
 
         def fwd_bwd():
             qkv.grad = None
-            bias.grad = None
+            if cfg["bias"] is not None:
+                cfg["bias"].grad = None
             fwd().backward(dout)
 
         with torch.no_grad():
@@ -94,6 +112,7 @@ def main():
             "fwd_frac_of_peak": round(fwd_flops / t_f / 1e9 / peak, 4),
             "bwd_frac_of_peak": round(2.5 * fwd_flops / t_b / 1e9 / peak, 4),
         }), flush=True)
+    fwd_flops = dense_flops
     if not args.only:
         # materialised reference path (what the reference framework executes)
         def ref_fwd():

@@ -38,6 +38,9 @@ struct FmhaFwdParams {
   // Logits mode (forward only): z = scale * Q K^T + bias + key mask, [B, H, Lq, Lk] contiguous in the dtype of q,
   // -inf at masked keys; null otherwise.  sw_logits: 64 x 64 boxes of z (the bias map's layout, B * H matrices).
   void* logits;
+  // Causal: key j is visible to query i iff j <= i (top-left aligned for any Lq, Lk, the mask
+  // triu(full((Lq, Lk), -inf), 1)).  Key tiles wholly above the diagonal are skipped; not combined with logits mode.
+  int causal;
   CUtensorMap sw_logits;
 };
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);

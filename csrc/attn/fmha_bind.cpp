@@ -94,10 +94,12 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
 // (out, lse, keep bits, logits); the logits z = scale * q k^T + bias + key mask only when `logits` is set
 std::tuple<Tensor, Tensor, OptTensor, OptTensor> fwd_impl(const Tensor& q, const Tensor& k, const Tensor& v,
                                                           const OptTensor& bias, const OptTensor& kpm, double p_drop,
-                                                          double scale, bool logits) {
+                                                          double scale, bool logits, bool causal) {
+  TORCH_CHECK(!(logits && causal), "fmha: causal attention does not return logits");
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaFwdParams p{};
   fill_common(p, q, k, v, bias, kpm, p_drop, scale, /*forward=*/true);
+  p.causal = causal ? 1 : 0;
   Tensor out = torch::empty({p.B, p.Lq, p.H, p.D}, q.options());
   Tensor lse = torch::empty({p.B, p.H, p.Lq}, q.options().dtype(at::kFloat));
   p.out = out.data_ptr();
@@ -126,10 +128,11 @@ std::tuple<Tensor, Tensor, OptTensor, OptTensor> fwd_impl(const Tensor& q, const
   return {out, lse, bits, z};
 }
 
+// causal: key j is visible to query i iff j <= i (fmha_api.h)
 std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k, const Tensor& v,
                                                       const OptTensor& bias, const OptTensor& kpm, double p_drop,
-                                                      double scale) {
-  auto r = fwd_impl(q, k, v, bias, kpm, p_drop, scale, /*logits=*/false);
+                                                      double scale, bool causal) {
+  auto r = fwd_impl(q, k, v, bias, kpm, p_drop, scale, /*logits=*/false, causal);
   return {std::get<0>(r), std::get<1>(r), std::get<2>(r)};
 }
 
@@ -138,7 +141,7 @@ std::tuple<Tensor, Tensor, OptTensor> fmha_fwd(const Tensor& q, const Tensor& k,
 std::tuple<Tensor, Tensor, OptTensor, Tensor> fmha_fwd_logits(const Tensor& q, const Tensor& k, const Tensor& v,
                                                               const OptTensor& bias, const OptTensor& kpm,
                                                               double p_drop, double scale) {
-  auto r = fwd_impl(q, k, v, bias, kpm, p_drop, scale, /*logits=*/true);
+  auto r = fwd_impl(q, k, v, bias, kpm, p_drop, scale, /*logits=*/true, /*causal=*/false);
   return {std::get<0>(r), std::get<1>(r), std::get<2>(r), *std::get<3>(r)};
 }
 
@@ -146,14 +149,18 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
                                                        const Tensor& v, const Tensor& out, const Tensor& lse,
                                                        const OptTensor& bias, const OptTensor& kpm, double p_drop,
                                                        double scale, const OptTensor& drop_bits, bool need_dbias,
-                                                       bool packed_grad, const OptTensor& dlogits) {
+                                                       bool packed_grad, const OptTensor& dlogits, bool causal) {
   // packed_grad: q/k/v are slices [:, :, i] of one [B, L, 3, H, D] tensor; the gradients are then
   // written straight into one packed [B, L, 3, H, D] tensor (returned three times as views), which
   // spares autograd three zero-filled select-backward tensors and two full-size adds per layer.
   // dlogits: gradient of the logits output of fmha_fwd_logits, [B, H, Lq, Lk]; None means zero.
+  // causal: the backward of fmha_fwd(..., causal=True); its keep bits cover only the key tiles that forward walked.
+  const bool has_dlogits = dlogits.has_value() && dlogits->defined();
+  TORCH_CHECK(!(causal && has_dlogits), "fmha_bwd: causal attention has no logits output, so dlogits must be None");
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaBwdParams p{};
   fill_common(p.f, q, k, v, bias, kpm, p_drop, scale, /*forward=*/false);
+  p.f.causal = causal ? 1 : 0;
   const int D = p.f.D;
   TORCH_CHECK(dout.is_contiguous() && out.is_contiguous() && lse.is_contiguous());
   TORCH_CHECK(dout.dim() == 4 && dout.size(0) == p.f.B && dout.size(1) == p.f.Lq && dout.size(2) == p.f.H &&
@@ -201,7 +208,7 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
                 "cuTensorMapEncodeTiled failed for the dS scratch tensor");
   }
   p.dlogits = nullptr;
-  if (dlogits.has_value() && dlogits->defined()) {
+  if (has_dlogits) {
     TORCH_CHECK(dlogits->is_cuda() && dlogits->is_contiguous() && dlogits->dim() == 4 && dlogits->size(0) == p.f.B &&
                     dlogits->size(1) == p.f.H && dlogits->size(2) == p.f.Lq && dlogits->size(3) == p.f.Lk,
                 "dlogits must be contiguous [B, H, Lq, Lk]");
@@ -225,9 +232,10 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
 
 void register_fmha(pybind11::module_& m) {
   namespace py = pybind11;
-  m.def("fmha_fwd", &fmha_fwd);
+  m.def("fmha_fwd", &fmha_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("bias"), py::arg("kpm"),
+        py::arg("p_drop"), py::arg("scale"), py::arg("causal") = false);
   m.def("fmha_fwd_logits", &fmha_fwd_logits);
   m.def("fmha_bwd", &fmha_bwd, py::arg("dout"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("out"),
         py::arg("lse"), py::arg("bias"), py::arg("kpm"), py::arg("p_drop"), py::arg("scale"), py::arg("drop_bits"),
-        py::arg("need_dbias"), py::arg("packed_grad"), py::arg("dlogits") = py::none());
+        py::arg("need_dbias"), py::arg("packed_grad"), py::arg("dlogits") = py::none(), py::arg("causal") = false);
 }

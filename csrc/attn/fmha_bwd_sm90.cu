@@ -149,8 +149,14 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
 // ---- main kernel ----------------------------------------------------------------------------------------------
 // kLogits: the forward also returned z, and dz (fmha_api.h) is added to dS before it is packed, so that the dK operand,
 // the dQ tile and the dBias store all carry dS_total = P o (drop(dP) - delta) + dz
-template <typename T, int DP, bool kLogits>
+// kCausal: only queries >= key0 see the CTA's keys, so the query-tile loop starts at i0 = key0 / 64 (kBM == kBN: tile i0
+// is the diagonal one, where P = dS = 0 at key > query through an additive -inf, as the future mask gives).  Stages and
+// mbarrier phases count from i0.  A CTA with key0 >= Lq has no query tile: it loads nothing and stores dK = dV = 0.
+// dBias above the diagonal is exactly 0: with a per-batch bias (ds_buf == dbias) the CTA stores a zero tile for each
+// skipped query tile i < i0; with a shared bias the reduction kernel writes the zeros and never reads those tiles.
+template <typename T, int DP, bool kLogits, bool kCausal>
 __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
+  static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
   using C = BwdCfg<DP, kLogits>;
   constexpr uint32_t kOffK = C::kOffK, kOffV = C::kOffV, kOffQ = C::kOffQ, kOffDO = C::kOffDO, kOffDS = C::kOffDS,
                      kOffDQ = C::kOffDQ, kOffStats = C::kOffStats, kOffBar = C::kOffBar, kTile = C::kTile;
@@ -167,12 +173,14 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   const bool drop = p.p_drop > 0.f && p.drop_bits != nullptr;
   const int n_qtiles = (p.Lq + kBM - 1) / kBM;
   const int Lq_pad = n_qtiles * kBM;
+  // first query tile: causal CTAs skip the tiles whose queries all precede key0 (i0 == n_qtiles: none is left)
+  const int i0 = kCausal ? min(key0 / kBM, n_qtiles) : 0;
   const long long bh = (long long)b * p.H + h;
   const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
   const int words_per_row = (p.Lk + 31) / 32;
   // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
-  auto load_tile = [&](int i) {   // one thread: Q_i, dO_i (and the bias and dz tiles) -> stage i & 1
-    const uint32_t st = (uint32_t)(i & 1), bar = bar_in0 + 8u * st;
+  auto load_tile = [&](int i) {   // one thread: Q_i, dO_i (and the bias and dz tiles) -> stage (i - i0) & 1
+    const uint32_t st = (uint32_t)((i - i0) & 1), bar = bar_in0 + 8u * st;
     mbar_expect_tx(bar, 2 * kTile + (has_bias ? 8192u : 0u) + (kLogits ? 8192u : 0u));
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
@@ -182,8 +190,10 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     if (has_bias) tma_load_3d(smem_base + kOffDS + st * 8192, &p.sw_bias, key0, i * kBM, bias_nb, bar);
     if constexpr (kLogits) tma_load_3d(smem_base + C::kOffDZ + st * 8192, &bp.sw_dz, key0, i * kBM, (int)bh, bar);
   };
+  // causal: the keep words (key0 >> 5) + {0, 1} are read for query tiles i >= key0 / 64 only; the causal forward of such
+  // a tile walked the keys up to at least i * 64 + 63 >= key0 + 63, so it wrote both words of every row it read here
   auto load_stats = [&](int i) {  // all threads: LSE (log2 units, +inf = row contributes nothing), delta, keep bits
-    uint8_t* s = smem + kOffStats + (i & 1) * 1024;
+    uint8_t* s = smem + kOffStats + ((i - i0) & 1) * 1024;
     const int q = i * kBM + (tid & 63);
     const bool ok = q < p.Lq;
     if (tid < 64) {
@@ -199,20 +209,33 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     }
   };
 
+  const bool any_q = !kCausal || i0 < n_qtiles;   // a copy must not outlive the CTA: no query tile, no load
   if (tid == 0) {
     mbar_init(bar_kv, 1);
     mbar_init(bar_in0, 1);
     mbar_init(bar_in0 + 8, 1);
     fence_mbarrier_init();
-    mbar_expect_tx(bar_kv, 2 * kTile);
+    if (any_q) {
+      mbar_expect_tx(bar_kv, 2 * kTile);
 #pragma unroll
-    for (int x = 0; x < C::kBoxes; ++x) {
-      tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, h, key0, b, bar_kv);
-      tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, h, key0, b, bar_kv);
+      for (int x = 0; x < C::kBoxes; ++x) {
+        tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, h, key0, b, bar_kv);
+        tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, h, key0, b, bar_kv);
+      }
+      load_tile(i0);
     }
-    load_tile(0);
   }
-  load_stats(0);
+  if (any_q) load_stats(i0);
+  // causal, per-batch dBias: the skipped tiles (i < i0, every key above every query) are zero.  The first 8 KB of the
+  // dQ staging tile are zeroed and stored over each of them; the first dQ tile is written after the bulk_wait_read of
+  // the loop's first barrier (A), when the stores have read it.
+  const bool zero_ds = kCausal && i0 > 0 && bp.ds_buf != nullptr && bp.ds_buf == bp.dbias;
+  if (zero_ds) {
+    uint4* zt = reinterpret_cast<uint4*>(smem + kOffDQ);
+#pragma unroll
+    for (int e = 0; e < 8192 / 16 / kBwdThreads; ++e) zt[e * kBwdThreads + tid] = make_uint4(0u, 0u, 0u, 0u);
+    fence_proxy_async_smem();
+  }
 
   // my two keys (accumulator rows) and their additive masks
   const int kl0 = warp * 16 + g, kl1 = kl0 + 8;
@@ -236,18 +259,22 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     dv[e] = 0.f;
     dk[e] = 0.f;
   }
-  __syncthreads();   // barriers initialised, stats of tile 0 in shared memory
-  mbar_wait(bar_kv, 0);
+  __syncthreads();   // barriers initialised, stats of tile i0 in shared memory
+  if (zero_ds && tid == 0) {
+    for (int i = 0; i < i0; ++i) tma_store_3d(&bp.sw_ds, key0, i * kBM, (int)bh, smem_base + kOffDQ);
+    bulk_commit();
+  }
+  if (any_q) mbar_wait(bar_kv, 0);
 
-  for (int i = 0; i < n_qtiles; ++i) {
-    const uint32_t st = (uint32_t)(i & 1);
+  for (int i = i0; i < n_qtiles; ++i) {
+    const uint32_t st = (uint32_t)((i - i0) & 1);
     __syncthreads();   // (A) tile i-1 is finished by every thread: its stage, stats and dQ staging may be reused
     if (tid == 0) {
       bulk_wait_read();   // the dS store and the dQ reduction of tile i-1 have read shared memory
       if (i + 1 < n_qtiles) load_tile(i + 1);
     }
     if (i + 1 < n_qtiles) load_stats(i + 1);
-    mbar_wait(bar_in0 + 8u * st, (uint32_t)((i >> 1) & 1));
+    mbar_wait(bar_in0 + 8u * st, (uint32_t)(((i - i0) >> 1) & 1));
 
     const uint32_t sQ = smem_base + kOffQ + st * kTile, sDO = smem_base + kOffDO + st * kTile;
     const uint32_t sDS = smem_base + kOffDS + st * 8192;
@@ -287,7 +314,15 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
         const float2 bb = has_bias ? bwd_unpack2<T>(bias_r[r]) : make_float2(0.f, 0.f);
         const float ka = (r & 1) ? kadd1 : kadd0;
         const float2 l2 = *reinterpret_cast<const float2*>(lse2_s + ql);
-        const float x0 = fmaf(s[e], p.scale, bb.x + ka), x1 = fmaf(s[e + 1], p.scale, bb.y + ka);
+        float ka0 = ka, ka1 = ka;
+        if constexpr (kCausal) {   // diagonal tile (key0 == i0 * 64): local key index > local query index is future
+          const int kl = (r & 1) ? kl1 : kl0;
+          if (i == i0) {
+            if (kl > ql) ka0 = -CUDART_INF_F;
+            if (kl > ql + 1) ka1 = -CUDART_INF_F;
+          }
+        }
+        const float x0 = fmaf(s[e], p.scale, bb.x + ka0), x1 = fmaf(s[e + 1], p.scale, bb.y + ka1);
         s[e] = ex2_approx(fmaf(x0, kLog2e, -l2.x));
         s[e + 1] = ex2_approx(fmaf(x1, kLog2e, -l2.y));
       }
@@ -406,12 +441,21 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   }
 }
 
-// dbias[n] = sum_b ds[b, n] (fp32 accumulate), n over H * Lq * Lk in 16-byte vectors
-template <typename T>
+// dbias[n] = sum_b ds[b, n] (fp32 accumulate), n over H * Lq * Lk in 16-byte vectors.  kCausal: a vector whose 8 keys
+// are all past its query lies in a dS tile the causal kernel skipped (never written); it is stored as 0 unread.
+template <typename T, bool kCausal>
 __global__ void __launch_bounds__(256) fmha_dbias_reduce_kernel(const T* __restrict__ ds, T* __restrict__ dbias, int B,
-                                                                  long long nvec) {
+                                                                  long long nvec, int Lq, int Lk) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
+    if constexpr (kCausal) {
+      const long long vpr = Lk / 8;   // vectors per row (Lk % 8 == 0)
+      const int key = (int)(v % vpr) * 8, q = (int)((v / vpr) % Lq);
+      if (key > q) {
+        st_global_v4(dbias + v * 8, Vec16{});
+        continue;
+      }
+    }
     float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
     for (int b0 = 0; b0 < B; b0 += 4) {
       Vec16 in[4];
@@ -455,14 +499,17 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
     kern<<<grid, kBwdThreads, smem_bytes, stream>>>(bp);
   };
-  if (bp.dlogits != nullptr) run(fmha_bwd_kernel<T, DP, true>, BwdCfg<DP, true>::kSmemBytes);
-  else run(fmha_bwd_kernel<T, DP, false>, BwdCfg<DP, false>::kSmemBytes);
+  // causal + logits is refused by the binding (fmha_bind.cpp)
+  if (bp.dlogits != nullptr) run(fmha_bwd_kernel<T, DP, true, false>, BwdCfg<DP, true>::kSmemBytes);
+  else if (p.causal) run(fmha_bwd_kernel<T, DP, false, true>, BwdCfg<DP, false>::kSmemBytes);
+  else run(fmha_bwd_kernel<T, DP, false, false>, BwdCfg<DP, false>::kSmemBytes);
   const long long cap = (long long)device_sms() * 16;
   if (bp.ds_buf != nullptr && bp.dbias != bp.ds_buf) {
     const long long nv = (long long)p.H * p.Lq * p.Lk / 8;
     const long long rb = std::min((nv + 255) / 256, cap);
-    fmha_dbias_reduce_kernel<T><<<(unsigned)rb, 256, 0, stream>>>(reinterpret_cast<const T*>(bp.ds_buf),
-                                                                 reinterpret_cast<T*>(bp.dbias), p.B, nv);
+    auto reduce = p.causal ? fmha_dbias_reduce_kernel<T, true> : fmha_dbias_reduce_kernel<T, false>;
+    reduce<<<(unsigned)rb, 256, 0, stream>>>(reinterpret_cast<const T*>(bp.ds_buf), reinterpret_cast<T*>(bp.dbias), p.B,
+                                             nv, p.Lq, p.Lk);
   }
   const long long nvec = nrows * (p.D / 8);
   const long long blocks = std::min((nvec + 255) / 256, cap);

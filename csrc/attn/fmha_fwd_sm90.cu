@@ -107,8 +107,14 @@ UB_DEVICE void quad_transpose4(uint32_t (&w)[4], int c) {
 // the bias elements it has just read from the swizzled bias stage (no other thread touches them; the region exists
 // without a bias too), and one thread stores the tile with a TMA store, clipped at Lq / Lk.  The stage is refilled
 // by the prefetch of tile j + 2, so that prefetch first waits until the store has read shared memory.
-template <typename T, int DP, bool kLogits>
+// kCausal: key j is visible to row i iff j <= i.  The tile loop (and with it the prefetch of tile j + 1) stops at the
+// last key tile with key0 <= q0 + 63; the 64 keys q0 .. q0 + 63 of the diagonal lie in that one tile (q0 is a multiple
+// of 64, kBlockN of 64), so only there do some elements get -inf, by index, in registers.  The skipped tiles would
+// have added exact zeros (alpha = ex2(0) = 1, l += 0, P = +0), so O, LSE and the keep words written are bitwise those
+// of the plain kernel given bias + the future mask.  The CTAs take the query tiles longest first.
+template <typename T, int DP, bool kLogits, bool kCausal>
 __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
+  static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
   using C = FwdCfg<DP>;
   constexpr int kBlockN = C::kBlockN;
   constexpr int kWords = kBlockN / 32;   // keep-bit words per row of a key tile
@@ -118,12 +124,15 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   uint8_t* smem = smem_raw + (smem_base - raw_base);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, c = lane & 3;
-  const int q0 = blockIdx.x * kBlockM, h = blockIdx.y, b = blockIdx.z;
+  const int q_tile = kCausal ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
+  const int q0 = q_tile * kBlockM, h = blockIdx.y, b = blockIdx.z;
   const uint32_t bar0 = smem_base + C::kSmemBar;   // bar0 + 8 * stage: K / V / bias of a key tile (+ Q on the first)
   float* kadd = reinterpret_cast<float*>(smem + C::kSmemKAdd);
 
   const bool has_bias = p.bias != nullptr;
-  const int n_tiles = (p.Lk + kBlockN - 1) / kBlockN;
+  const int n_key_tiles = (p.Lk + kBlockN - 1) / kBlockN;
+  // causal: key tiles 0 .. (q0 + 63) / kBlockN hold a key visible to one of the rows q0 .. q0 + 63
+  const int n_tiles = kCausal ? min(n_key_tiles, (q0 + kBlockM - 1) / kBlockN + 1) : n_key_tiles;
   const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
   // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
   constexpr uint32_t kKVBytes = C::kKVStage, kBiasBytes = C::kBiasStage, kQBytes = C::kBoxes * C::kQBox;
@@ -222,6 +231,15 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
       s[4 * i + 1] = fmaf(s[4 * i + 1], p.scale, b0.y);
       s[4 * i + 2] = fmaf(s[4 * i + 2], p.scale, b1.x);
       s[4 * i + 3] = fmaf(s[4 * i + 3], p.scale, b1.y);
+      if constexpr (kCausal) {   // the diagonal tile: keys past the row are -inf, as the future mask would make them
+        if (j == n_tiles - 1) {
+          const int key = key0 + col;
+          if (key > row0) s[4 * i + 0] = -CUDART_INF_F;
+          if (key + 1 > row0) s[4 * i + 1] = -CUDART_INF_F;
+          if (key > row1) s[4 * i + 2] = -CUDART_INF_F;
+          if (key + 1 > row1) s[4 * i + 3] = -CUDART_INF_F;
+        }
+      }
       if constexpr (kLogits) {   // the same swizzled positions as the bias elements above
         uint8_t* box = bias_tile + (i >> 3) * 8192 + c * 4;
         *reinterpret_cast<uint32_t*>(box + sw128_off(rl0, i & 7)) = pack2<T>(s[4 * i + 0], s[4 * i + 1]);
@@ -368,18 +386,20 @@ void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
     kern<<<grid, kFwdThreads, smem_bytes, stream>>>(p);
   };
-  auto dispatch = [&](auto logits) {
-    constexpr bool kLogits = decltype(logits)::value;
+  auto dispatch = [&](auto logits, auto causal) {
+    constexpr bool kLogits = decltype(logits)::value, kCausal = decltype(causal)::value;
     if (p.D <= 64) {
-      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits>, FwdCfg<64>::kSmemBytes);
-      else run(fmha_fwd_kernel<__half, 64, kLogits>, FwdCfg<64>::kSmemBytes);
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits, kCausal>, FwdCfg<64>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 64, kLogits, kCausal>, FwdCfg<64>::kSmemBytes);
     } else {
-      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits>, FwdCfg<128>::kSmemBytes);
-      else run(fmha_fwd_kernel<__half, 128, kLogits>, FwdCfg<128>::kSmemBytes);
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits, kCausal>, FwdCfg<128>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 128, kLogits, kCausal>, FwdCfg<128>::kSmemBytes);
     }
   };
-  if (p.logits != nullptr) dispatch(std::true_type{});
-  else dispatch(std::false_type{});
+  // causal + logits is refused by the binding (fmha_bind.cpp)
+  if (p.logits != nullptr) dispatch(std::true_type{}, std::false_type{});
+  else if (p.causal) dispatch(std::false_type{}, std::true_type{});
+  else dispatch(std::false_type{}, std::false_type{});
 }
 
 }  // namespace ub

@@ -13,6 +13,10 @@ need_probs=False`` (the caller wants the logits but not the probabilities, as Un
 runs in the same kernel in its logits mode, which also writes the logits; its third result is ``None``.
 With the probabilities requested (``return_attn`` and the default ``need_probs=True``), or another head
 dim, or on the CPU, the materialised path (bmm + ``softmax_dropout`` kernel) is used.
+
+``causal=True`` on ``SelfMultiheadAttention`` hides key ``j`` from query ``i`` when ``j > i``.  The fused path passes it
+to the kernel as a flag (no mask tensor); the materialised path adds the future mask ``triu(-inf, 1)`` to the bias, so
+its logits are those of the same call with that mask in ``attn_bias``.
 """
 from typing import Optional
 
@@ -37,6 +41,14 @@ def _bias_as_4d(attn_bias: Optional[Tensor], bsz: int, heads: int, tgt: int, src
     if attn_bias.dim() == 2:
         return attn_bias.view(1, 1, tgt, src).expand(1, heads, tgt, src)
     raise ValueError("unsupported attn_bias shape {}".format(tuple(attn_bias.shape)))
+
+
+def _add_future_mask(bias4: Optional[Tensor], heads: int, seq_len: int, like: Tensor) -> Tensor:
+    """``bias4`` (``[1|B, H, L, L]`` or None) plus the causal mask: ``-inf`` where key > query."""
+    fm = torch.full((seq_len, seq_len), float("-inf"), dtype=like.dtype, device=like.device).triu(1)
+    if bias4 is None:
+        return fm.view(1, 1, seq_len, seq_len).expand(1, heads, seq_len, seq_len)
+    return bias4 + fm
 
 
 def _materialised_attention(qh, kh, vh, key_padding_mask, attn_bias4, dropout, training, return_attn):
@@ -80,11 +92,12 @@ class SelfMultiheadAttention(nn.Module):
         self.in_proj = nn.Linear(embed_dim, embed_dim * 3, bias=bias)
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
 
-    def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False, need_probs=True):
+    def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False, need_probs=True, causal=False):
         """Everything up to (not including) ``out_proj``: returns ``(o [B, L, E], logits, probs)``.
 
         ``need_probs=False`` returns ``probs = None``; with ``return_attn`` the fused kernel then also computes the
-        logits ``[B*H, L, L]`` where it takes the shapes."""
+        logits ``[B*H, L, L]`` where it takes the shapes.  ``causal`` hides key j from query i when j > i (see the module
+        docstring)."""
         bsz, tgt_len, embed_dim = query.size()
         if embed_dim != self.embed_dim:
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
@@ -98,12 +111,15 @@ class SelfMultiheadAttention(nn.Module):
             res = ops.fused_attention_qkvpacked(
                 qkv, bias=bias4, key_padding_mask=key_padding_mask,
                 dropout_p=self.dropout, training=self.training, scale=self.scaling, return_logits=return_attn,
+                causal=causal,
             )
             if not return_attn:
                 return res.reshape(bsz, tgt_len, embed_dim), None, None
             o, logits = res
             return o.reshape(bsz, tgt_len, embed_dim), logits.view(bsz * self.num_heads, tgt_len, tgt_len), None
         qh, kh, vh = ops.split_heads(qkv.view(bsz, tgt_len, 3 * embed_dim), 3, self.num_heads, self.scaling)
+        if causal:
+            bias4 = _add_future_mask(bias4, self.num_heads, tgt_len, qh)
         o, logits, probs = _materialised_attention(qh, kh, vh, key_padding_mask, bias4, self.dropout, self.training,
                                                    return_attn)
         return o, logits, (probs if need_probs else None)
@@ -115,8 +131,9 @@ class SelfMultiheadAttention(nn.Module):
         attn_bias: Optional[Tensor] = None,
         return_attn: bool = False,
         need_probs: bool = True,
+        causal: bool = False,
     ) -> Tensor:
-        o, logits, probs = self.attend(query, key_padding_mask, attn_bias, return_attn, need_probs)
+        o, logits, probs = self.attend(query, key_padding_mask, attn_bias, return_attn, need_probs, causal)
         o = self.out_proj(o)
         return (o, logits, probs) if return_attn else o
 

@@ -13,6 +13,9 @@ GPU execution plan for one layer (post-LN shown; pre-LN analogous):
 The relative-position bias stays ``[1, H, L, L]`` (never repeated over the batch) and the key
 padding mask stays ``[B, L]`` (never merged into a ``[B*H, L, L]`` tensor of ``-inf``) whenever the
 fused attention kernel is usable; otherwise the reference's merged-mask formulation is used.
+The auto-regressive decoder's future mask is not a tensor either on that path: its layers run self-attention with
+``causal=True``, and the kernels skip the key tiles above the diagonal.  On the CPU, in fp32 or at a head dim the
+kernels do not take, the future mask is added into the bias as in the reference.
 """
 import math
 from typing import Optional
@@ -100,11 +103,12 @@ class _BlockMixin:
         """post-LN: LN(residual + drop(attn(x)));  pre-LN: residual + drop(attn(LN(x)))."""
         return_attn = kw.pop("return_attn", False)
         need_probs = kw.pop("need_probs", True)
+        causal = kw.pop("causal", False)
         h = attn_in if self.post_ln else norm(attn_in)
         extra = None
         if isinstance(attn_module, SelfMultiheadAttention):
             o, logits, probs = attn_module.attend(h, kw.get("key_padding_mask"), kw.get("attn_bias"), return_attn,
-                                                  need_probs)
+                                                  need_probs, causal)
             if return_attn:
                 extra = (logits, probs)
         else:
@@ -229,9 +233,13 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
         padding_mask: Optional[torch.Tensor] = None,
         encoder_attn_bias: Optional[torch.Tensor] = None,
         encoder_padding_mask: Optional[torch.Tensor] = None,
+        causal: bool = False,
     ) -> torch.Tensor:
+        """``causal`` masks future keys in the self-attention (key j > query i), without a mask tensor on the fused
+        path; the encoder attention is unaffected."""
         x, _ = self._attn_residual(
-            self.self_attn, self.self_attn_layer_norm, x, x, key_padding_mask=padding_mask, attn_bias=attn_bias
+            self.self_attn, self.self_attn_layer_norm, x, x, key_padding_mask=padding_mask, attn_bias=attn_bias,
+            causal=causal,
         )
         if encoder_out is not None:
             x, _ = self._attn_residual(
@@ -246,6 +254,12 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
 # stacks
 # ------------------------------------------------------------------------------------------------
 class _StackMixin:
+    def _fused_attention_capable(self, x):
+        """True when the layers' attention runs in the fused kernels: CUDA input, native kernels, 16-bit dtype and a
+        head dim the kernels take."""
+        return x.is_cuda and ops.USE_NATIVE and x.dtype in (torch.float16, torch.bfloat16) \
+            and ops.fused_head_dim_supported(self.embed_dim // self.attention_heads)
+
     def _init_rel_pos(self, rel_pos, rel_pos_bins, max_rel_pos):
         self.rel_pos = rel_pos
         if not rel_pos:
@@ -306,9 +320,7 @@ class _StackMixin:
             if future_mask is not None:
                 fm = future_mask[:seq_len, :seq_len]
                 bias = fm.view(1, 1, seq_len, seq_len).expand(1, heads, seq_len, seq_len) if bias is None else bias + fm
-            fused_capable = x.is_cuda and ops.USE_NATIVE and x.dtype in (torch.float16, torch.bfloat16) \
-                and ops.fused_head_dim_supported(self.embed_dim // heads)
-            if bias is None or fused_capable or padding_mask is None:
+            if bias is None or self._fused_attention_capable(x) or padding_mask is None:
                 return bias, padding_mask
             merged = bias.expand(bsz, heads, seq_len, seq_len).clone()
         else:
@@ -454,7 +466,10 @@ class TransformerDecoder(nn.Module, _StackMixin):
         encoder_attn_mask: Optional[torch.Tensor] = None,
     ) -> torch.Tensor:
         x = self._embed_prologue(emb, padding_mask)
-        attn_bias, key_padding = self._compose_bias(x, attn_mask, padding_mask, future_mask=self._future(x))
+        # on the fused path the kernels apply the future mask themselves (causal=True); it joins no bias tensor
+        causal = self.auto_regressive and self._fused_attention_capable(x)
+        future_mask = None if causal else self._future(x)
+        attn_bias, key_padding = self._compose_bias(x, attn_mask, padding_mask, future_mask=future_mask)
         for layer in self.layers:
             x = layer(
                 x,
@@ -463,6 +478,7 @@ class TransformerDecoder(nn.Module, _StackMixin):
                 attn_bias=attn_bias,
                 encoder_padding_mask=encoder_padding_mask,
                 encoder_attn_bias=encoder_attn_mask,
+                causal=causal,
             )
         if self.final_layer_norm is not None:
             x = self.final_layer_norm(x)

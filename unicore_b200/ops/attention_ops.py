@@ -17,6 +17,12 @@ contract of ``softmax_dropout_with_logits``): the key padding mask is additive, 
 and the gradient ``dz`` of ``z`` is added to the softmax gradient at every position before it reaches q, k and the
 bias.  The kernels write ``z`` from the forward pass and take ``dz`` in the backward pass; the probabilities are never
 materialised.  Uni-Mol threads ``z`` through its layers as the pair representation.
+
+``causal=True`` lets key ``j`` reach query ``i`` only when ``j <= i``, for any ``Lq`` and ``Lk``: the top-left aligned
+mask ``torch.triu(full((Lq, Lk), -inf), 1)``, as the future mask of ``TransformerDecoder`` (not flash-attn's
+bottom-right convention when ``Lq != Lk``).  It combines with the bias, the key padding mask and dropout.  The kernels
+take it as a flag: no mask tensor is read, and the key tiles above the diagonal are never computed, in the forward or
+the backward pass.  ``causal=True`` with ``return_logits=True`` runs ``attention_reference``.
 """
 import math
 
@@ -34,12 +40,13 @@ def fused_head_dim_supported(head_dim: int) -> bool:
 
 
 def attention_reference(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
-                        return_logits=False):
+                        return_logits=False, causal=False):
     """Plain PyTorch implementation with the same signature (fallback + test oracle).
 
     q: [B, Lq, H, D], k/v: [B, Lk, H, D]; bias broadcastable to [B, H, Lq, Lk];
-    key_padding_mask: [B, Lk] bool (True = masked). Returns [B, Lq, H, D], or with ``return_logits``
-    ``(out, z)`` with ``z [B, H, Lq, Lk]`` built with an additive ``-inf`` mask (its gradient reaches masked keys).
+    key_padding_mask: [B, Lk] bool (True = masked); ``causal`` masks key j > query i. Returns [B, Lq, H, D], or with
+    ``return_logits`` ``(out, z)`` with ``z [B, H, Lq, Lk]`` built with additive ``-inf`` masks (its gradient reaches
+    masked keys).
     """
     B, Lq, H, D = q.shape
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
@@ -52,15 +59,22 @@ def attention_reference(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0
             scores = scores + pad.masked_fill(key_padding_mask[:, None, None, :].to(torch.bool), float("-inf"))
         else:
             scores = scores.masked_fill(key_padding_mask[:, None, None, :].to(torch.bool), float("-inf"))
+    if causal:
+        future = torch.ones(Lq, k.shape[1], dtype=torch.bool, device=scores.device).triu(1)
+        if return_logits:
+            scores = scores + torch.zeros(future.shape, dtype=scores.dtype, device=scores.device).masked_fill(
+                future, float("-inf"))
+        else:
+            scores = scores.masked_fill(future, float("-inf"))
     probs = F.softmax(scores.float(), dim=-1).to(q.dtype)
     probs = F.dropout(probs, p=dropout_p, training=training)
     out = torch.einsum("bhqk,bkhd->bqhd", probs, v)
     return (out, scores) if return_logits else out
 
 
-def _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits):
+def _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal):
     """Shared forward of the two Functions: runs the kernel, records what the backward needs, returns
-    ``(out, lse, bits, logits)`` (logits None without ``return_logits``)."""
+    ``(out, lse, bits, logits)`` (logits None without ``return_logits``; never both logits and ``causal``)."""
     p = float(dropout_p) if training else 0.0
     logits = None
     if return_logits:
@@ -68,8 +82,9 @@ def _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, retur
         # a logits gradient that autograd never produced stays None (= zero) instead of a zero-filled [B, H, Lq, Lk]
         ctx.set_materialize_grads(False)
     else:
-        out, lse, bits = native().fmha_fwd(q, k, v, bias, key_padding_mask, p, float(scale))
+        out, lse, bits = native().fmha_fwd(q, k, v, bias, key_padding_mask, p, float(scale), causal=causal)
     ctx.p = p
+    ctx.causal = causal
     ctx.scale = float(scale)
     ctx.need_dbias = bias is not None and bias.requires_grad
     return out, lse, bits, logits
@@ -83,8 +98,9 @@ def _bwd_grads(out, dout, dlogits):
 
 class _FusedAttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits=False):
-        out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
+    def forward(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits=False, causal=False):
+        out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits,
+                                      causal)
         ctx.save_for_backward(q, k, v, out, lse, bias, key_padding_mask, bits)
         return (out, logits) if return_logits else out
 
@@ -93,11 +109,11 @@ class _FusedAttentionFn(torch.autograd.Function):
         q, k, v, out, lse, bias, kpm, bits = ctx.saved_tensors
         dout, dlogits = _bwd_grads(out, dout, dlogits)
         dq, dk, dv, dbias = native().fmha_bwd(
-            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, False, dlogits
+            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, False, dlogits, causal=ctx.causal
         )
         if dbias is not None and dbias.dtype != bias.dtype:
             dbias = dbias.to(bias.dtype)
-        return dq, dk, dv, dbias, None, None, None, None, None
+        return dq, dk, dv, dbias, None, None, None, None, None, None
 
 
 class _FusedAttentionPackedFn(torch.autograd.Function):
@@ -105,9 +121,10 @@ class _FusedAttentionPackedFn(torch.autograd.Function):
     in, and the backward kernels write dq/dk/dv directly into ONE packed gradient tensor."""
 
     @staticmethod
-    def forward(ctx, qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits=False):
+    def forward(ctx, qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits=False, causal=False):
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
-        out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
+        out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits,
+                                      causal)
         ctx.save_for_backward(qkv, out, lse, bias, key_padding_mask, bits)
         return (out, logits) if return_logits else out
 
@@ -117,12 +134,12 @@ class _FusedAttentionPackedFn(torch.autograd.Function):
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
         dout, dlogits = _bwd_grads(out, dout, dlogits)
         dq, _dk, _dv, dbias = native().fmha_bwd(
-            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, True, dlogits
+            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, True, dlogits, causal=ctx.causal
         )
         dqkv = dq._base  # the packed [B, L, 3, H, D] tensor the three gradients are views of
         if dbias is not None and dbias.dtype != bias.dtype:
             dbias = dbias.to(bias.dtype)
-        return dqkv, dbias, None, None, None, None, None
+        return dqkv, dbias, None, None, None, None, None, None
 
 
 def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool:
@@ -157,33 +174,37 @@ def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool
 
 
 def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
-                    return_logits=False):
+                    return_logits=False, causal=False):
     """Dispatch to the wgmma kernel when shapes/dtypes allow, else to the PyTorch reference.
 
-    Returns ``[B, Lq, H, D]``, or ``(out, z [B, H, Lq, Lk])`` with ``return_logits`` (see the module docstring)."""
+    Returns ``[B, Lq, H, D]``, or ``(out, z [B, H, Lq, Lk])`` with ``return_logits`` (see the module docstring).
+    ``causal`` masks key j > query i; with ``return_logits`` it runs the reference."""
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
-    if fused_attention_supported(q, k, v, bias, key_padding_mask):
+    if not (causal and return_logits) and fused_attention_supported(q, k, v, bias, key_padding_mask):
         if bias is not None:
             # the kernel stages the bias tile next to P in shared memory in the compute dtype
             bias = bias.to(q.dtype).contiguous()
         if key_padding_mask is not None:
             key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
-        return _FusedAttentionFn.apply(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
-    return attention_reference(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
+        return _FusedAttentionFn.apply(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits,
+                                       causal)
+    return attention_reference(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal)
 
 
 def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
-                              return_logits=False):
+                              return_logits=False, causal=False):
     """Self-attention on the packed in_proj output ``qkv [B, L, 3, H, D]`` (returns ``[B, L, H, D]``, or
-    ``(out, z [B, H, L, L])`` with ``return_logits``)."""
+    ``(out, z [B, H, L, L])`` with ``return_logits``); ``causal`` as in ``fused_attention``."""
     q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
-    if qkv.is_contiguous() and fused_attention_supported(q, k, v, bias, key_padding_mask):
+    if not (causal and return_logits) and qkv.is_contiguous() and fused_attention_supported(q, k, v, bias,
+                                                                                            key_padding_mask):
         if bias is not None:
             bias = bias.to(q.dtype).contiguous()
         if key_padding_mask is not None:
             key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
-        return _FusedAttentionPackedFn.apply(qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits)
-    return fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits)
+        return _FusedAttentionPackedFn.apply(qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits,
+                                             causal)
+    return fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal)
