@@ -87,13 +87,15 @@ void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, vo
 int norm_bwd_parts(int rows, int cols, int dtype);
 bool norm_v2_supported(int cols, int dtype);  // geometries for which the fused op can also emit dbias
 // accumulate (bit 0: dgamma, bit 1: dbeta, bit 2: dbias): add to what the output already holds (gradient arena)
+// deterministic: the per-CTA column partials are combined in a fixed order on every launch path
 void launch_layernorm_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const void* gamma,
                           void* dx, void* dgamma, void* dbeta, float* part, int rows, int cols, int dtype,
-                          cudaStream_t stream, int accumulate = 0);
+                          cudaStream_t stream, int accumulate = 0, bool deterministic = false);
 void launch_rmsnorm_fwd(const void* x, const void* gamma, void* y, float* rstd, int rows, int cols, float eps,
                         int dtype, cudaStream_t stream);
 void launch_rmsnorm_bwd(const void* dy, const void* x, const float* rstd, const void* gamma, void* dx, void* dgamma,
-                        float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate = 0);
+                        float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate = 0,
+                        bool deterministic = false);
 
 // ---- softmax + dropout ---------------------------------------------------------------------------------------
 // Launch plan of the softmax-dropout kernels (the launchers run exactly this plan).  `aligned`: every buffer of the
@@ -136,7 +138,8 @@ void launch_bias_dropout_add_ln_fwd(const void* x, const void* bias, const void*
 void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const float* mean, const float* rstd,
                                     const void* gamma, void* dsum, void* dx, void* dgamma, void* dbeta,
                                     void* dbias, float* part, int rows, int cols, float p, unsigned long long seed,
-                                    unsigned long long offset, int dtype, cudaStream_t stream, int accumulate = 0);
+                                    unsigned long long offset, int dtype, cudaStream_t stream, int accumulate = 0,
+                                    bool deterministic = false);
 // ---- Gaussian radial basis of (mul[edge] * d + bias[edge]) (Uni-Mol pair features), csrc/fused/gaussian.cu ----------
 // y: [n, K] in `dtype` (fp16 / bf16), K a multiple of 8 with K / 8 a power of two <= 32
 // token-major [B, L, T, H, D] <-> T head-major [B, H, L, D] tensors (null head pointer = zeros when gathering);
@@ -158,6 +161,12 @@ void launch_pair_tail_bwd(const void* d_pair, const void* d_delta, const void* z
 void launch_embedding_bwd(const void* dy, const long long* tokens, float* scratch, unsigned char* touched, void* grad,
                           long long rows, int cols, long long vocab, long long padding_idx, int accumulate, int dtype,
                           cudaStream_t stream);
+// The same gradient in a fixed summation order (deterministic mode): `sorted` [rows] are the token ids stable-sorted
+// ascending and `perm` [rows] their original row indices; vocabulary row v sums dy over its run in ascending row order
+// in fp32 from 0, then adds the 16-bit grad (accumulate) and rounds once.  Padding and out-of-range ids are skipped.
+void launch_embedding_bwd_sorted(const void* dy, const long long* sorted, const long long* perm, void* grad,
+                                 long long rows, int cols, long long vocab, long long padding_idx, int accumulate,
+                                 int dtype, cudaStream_t stream);
 
 void launch_gbf_fwd(const void* d, const long long* edge, const void* mul_w, const void* bias_w, const void* means,
                     const void* stds, void* y, long long n, int K, int dtype, cudaStream_t stream);
@@ -166,6 +175,11 @@ int gbf_parts(long long n, int K);
 void launch_gbf_bwd(const void* dy, const void* d, const long long* edge, const void* mul_w, const void* bias_w,
                     const void* means, const void* stds, float* part, float* hist, long long n, int K, int E, int dtype,
                     cudaStream_t stream);
+// The same gradients in a fixed summation order (deterministic mode): rowg float[n][2] scratch; sorted / perm: the
+// edge types stable-sorted and their row indices; d mul / d bias of a type sum its rows in ascending order
+void launch_gbf_bwd_det(const void* dy, const void* d, const long long* edge, const void* mul_w, const void* bias_w,
+                        const void* means, const void* stds, float* part, float* rowg, const long long* sorted,
+                        const long long* perm, float* hist, long long n, int K, int E, int dtype, cudaStream_t stream);
 // loss_rows[i] = lse_i - logit_i[target_i] (0 when target == ignore_index); lse saved for backward
 void launch_softmax_xent_fwd(const void* logits, const long long* target, float* loss_rows, float* lse, int rows,
                              int cols, int stride, long long ignore_index, int dtype, cudaStream_t stream);

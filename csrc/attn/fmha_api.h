@@ -67,7 +67,15 @@ struct FmhaBwdParams {
   // dS everywhere (dS_total = P o (drop(dP) - delta) + dz feeds dQ, dK and dBias); null runs the plain backward.
   const void* dlogits;
   CUtensorMap sw_dz;   // 64 x 64 boxes of dlogits (the bias map's layout, B * H matrices)
+  // Deterministic mode (torch.use_deterministic_algorithms): one int32 turn counter per (b, h, query tile),
+  // [B, H, ceil(Lq / 64)], stored right after dq_acc in the same allocation and zeroed with it.  The key tiles then add
+  // their dQ shares into each query tile in ascending key-tile order, so dQ does not depend on the CTA schedule.
+  // Null runs the default kernels, which add in completion order.
+  int* dq_turn;
 };
 void launch_fmha_bwd(const FmhaBwdParams& p, cudaStream_t stream);
+// Number of deterministic-mode waits for a turn that gave up after ~10 s (and added out of order) on the current
+// device since the last call; reading resets it.  Any value other than 0 is a bug.
+unsigned int fmha_det_timeouts_take();
 
 }  // namespace ub

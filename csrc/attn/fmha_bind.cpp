@@ -177,9 +177,14 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
                                            (long long)p.f.Lq * p.f.H * D, (long long)p.f.H * D, D, ub::kBwdBoxRows),
               "cuTensorMapEncodeTiled failed for dO");
   Tensor delta = torch::empty({p.f.B, p.f.H, p.f.Lq}, q.options().dtype(at::kFloat));
-  // zeroed by the launcher; padded to whole 64-row query tiles and to the kernel's padded head width
-  Tensor dq_acc = torch::empty({p.f.B, p.f.H, (p.f.Lq + 63) / 64 * 64, ub::fmha_padded_head_dim(D)},
-                               q.options().dtype(at::kFloat));
+  // zeroed by the launcher; padded to whole 64-row query tiles and to the kernel's padded head width.  Under
+  // torch.use_deterministic_algorithms (warn-only included) the int32 turn counters of the ordered dQ reductions,
+  // one per (b, h, query tile), follow in the same allocation.
+  const bool det = at::globalContext().deterministicAlgorithms();
+  const int64_t n_qt = (p.f.Lq + 63) / 64;
+  const int64_t acc_floats = (int64_t)p.f.B * p.f.H * n_qt * 64 * ub::fmha_padded_head_dim(D);
+  Tensor dq_acc = torch::empty({acc_floats + (det ? (int64_t)p.f.B * p.f.H * n_qt : 0)}, q.options().dtype(at::kFloat));
+  p.dq_turn = det ? reinterpret_cast<int*>(dq_acc.data_ptr<float>() + acc_floats) : nullptr;
   Tensor dq, dk, dv;
   if (packed_grad) {
     TORCH_CHECK(p.f.Lq == p.f.Lk, "packed gradients need self-attention shapes");
@@ -238,4 +243,6 @@ void register_fmha(pybind11::module_& m) {
   m.def("fmha_bwd", &fmha_bwd, py::arg("dout"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("out"),
         py::arg("lse"), py::arg("bias"), py::arg("kpm"), py::arg("p_drop"), py::arg("scale"), py::arg("drop_bits"),
         py::arg("need_dbias"), py::arg("packed_grad"), py::arg("dlogits") = py::none(), py::arg("causal") = false);
+  m.def("fmha_det_timeouts", [] { return (int64_t)ub::fmha_det_timeouts_take(); },
+        "deterministic-mode dQ turn waits that timed out on the current device since the last call (reset on read)");
 }

@@ -93,6 +93,45 @@ UB_DEVICE float2 bwd_unpack2(uint32_t w) {
 // same bank and the store takes 8 wavefronts, swizzled it takes the minimum, 2.
 UB_DEVICE int dq_swz_col(int q, int col) { return (((col >> 3) ^ (q & 7)) << 3) | (col & 7); }
 
+// ---- deterministic mode: ordered dQ reductions -----------------------------------------------------------------
+__device__ unsigned int g_det_timeouts;   // waits that gave up (fmha_det_timeouts_take)
+
+UB_DEVICE int ld_acquire_gpu(const int* p) {
+  int v;
+  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+UB_DEVICE void red_release_gpu_add(int* p, int v) {
+  asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// orders this thread's generic-proxy accesses of global memory with its async-proxy (bulk copy) accesses
+UB_DEVICE void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
+UB_DEVICE unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
+// One thread: wait until the turn counter of a query tile reaches `turn` (the CTA's key tile index).  The wait is
+// bounded: after ~10 s it gives up, counts a timeout and lets the caller add out of order rather than hang the GPU.
+UB_DEVICE void det_wait_turn(const int* counter, int turn) {
+  if (ld_acquire_gpu(counter) != turn) {
+    const unsigned long long t0 = globaltimer_ns();
+    unsigned int ns = 32;
+    while (ld_acquire_gpu(counter) != turn) {
+      __nanosleep(ns);
+      ns = ns < 1024 ? 2 * ns : ns;
+      if (globaltimer_ns() - t0 > 10000000000ull) {
+        atomicAdd(&g_det_timeouts, 1u);
+        break;
+      }
+    }
+  }
+  // the acquire made the previous key tile's reduction visible to this thread; the proxy fence orders it before the
+  // reduction this thread issues next through the async proxy
+  fence_proxy_async_global();
+}
+
 // ---- pre-pass: delta[b,h,q] = sum_d dO * O -----------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256) fmha_delta_kernel(const T* __restrict__ dout, const T* __restrict__ out,
@@ -154,7 +193,16 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
 // mbarrier phases count from i0.  A CTA with key0 >= Lq has no query tile: it loads nothing and stores dK = dV = 0.
 // dBias above the diagonal is exactly 0: with a per-batch bias (ds_buf == dbias) the CTA stores a zero tile for each
 // skipped query tile i < i0; with a shared bias the reduction kernel writes the zeros and never reads those tiles.
-template <typename T, int DP, bool kLogits, bool kCausal>
+// kDet (deterministic mode, bp.dq_turn set): the key tiles add their dQ shares into query tile i strictly in ascending
+// key-tile order j, so dQ_i = ((0 + dQ_i^0) + dQ_i^1) + ... whatever the schedule.  Before its reduction, thread 0 of
+// key tile j waits until the turn counter of (b, h, i) is j; after the reduction has completed it increments the
+// counter.  The chain has no gap: every key tile walks every query tile, and in causal mode key tile j starts at query
+// tile j, so the tiles that reach query tile i are exactly 0 .. min(i, n_kt - 1).  Forward progress: a CTA only ever
+// waits on the CTA of the same (b, h) with the next lower blockIdx.x, whose linear block index is lower, so the
+// hardware dispatched it before this one; by induction down to key tile 0, which never waits, the chain completes.
+// The wait is at the last point, with the dQ tile already staged, so a CTA does not hold up the chain while it
+// computes.  dK, dV and dS are computed exactly as in the default mode.
+template <typename T, int DP, bool kLogits, bool kCausal, bool kDet = false>
 __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
   using C = BwdCfg<DP, kLogits>;
@@ -418,8 +466,14 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     fence_proxy_async_smem();
     __syncthreads();   // (C) the dQ tile is in shared memory
     if (tid == 0) {
+      if constexpr (kDet) det_wait_turn(bp.dq_turn + bh * n_qtiles + i, (int)blockIdx.x);
       bulk_reduce_add_f32(bp.dq_acc + (bh * Lq_pad + (long long)i * kBM) * DP, smem_base + kOffDQ, kBM * DP * 4);
       bulk_commit();
+      if constexpr (kDet) {
+        bulk_wait_all();             // the reduction's writes are performed (not only its reads of shared memory) ...
+        fence_proxy_async_global();  // ... and ordered before the generic-proxy release that passes the turn on
+        red_release_gpu_add(bp.dq_turn + bh * n_qtiles + i, 1);
+      }
     }
   }
   if (tid == 0) bulk_wait_all();   // shared memory must outlive the last store's and reduction's reads
@@ -491,7 +545,8 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
   const FmhaFwdParams& p = bp.f;
   const long long nrows = (long long)p.B * p.Lq * p.H;
   const int n_qt = (p.Lq + kBM - 1) / kBM;
-  cudaMemsetAsync(bp.dq_acc, 0, (size_t)p.B * p.H * n_qt * kBM * DP * sizeof(float), stream);
+  const bool det = bp.dq_turn != nullptr;   // the turn counters follow dq_acc: one memset zeroes both
+  cudaMemsetAsync(bp.dq_acc, 0, (size_t)p.B * p.H * n_qt * (kBM * DP * sizeof(float) + (det ? sizeof(int) : 0)), stream);
   fmha_delta_kernel<T><<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
       reinterpret_cast<const T*>(bp.dout), reinterpret_cast<const T*>(p.out), bp.delta, p.B, p.H, p.Lq, p.D);
   dim3 grid((p.Lk + kBN - 1) / kBN, p.H, p.B);
@@ -500,7 +555,11 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
     kern<<<grid, kBwdThreads, smem_bytes, stream>>>(bp);
   };
   // causal + logits is refused by the binding (fmha_bind.cpp)
-  if (bp.dlogits != nullptr) run(fmha_bwd_kernel<T, DP, true, false>, BwdCfg<DP, true>::kSmemBytes);
+  if (det) {
+    if (bp.dlogits != nullptr) run(fmha_bwd_kernel<T, DP, true, false, true>, BwdCfg<DP, true>::kSmemBytes);
+    else if (p.causal) run(fmha_bwd_kernel<T, DP, false, true, true>, BwdCfg<DP, false>::kSmemBytes);
+    else run(fmha_bwd_kernel<T, DP, false, false, true>, BwdCfg<DP, false>::kSmemBytes);
+  } else if (bp.dlogits != nullptr) run(fmha_bwd_kernel<T, DP, true, false>, BwdCfg<DP, true>::kSmemBytes);
   else if (p.causal) run(fmha_bwd_kernel<T, DP, false, true>, BwdCfg<DP, false>::kSmemBytes);
   else run(fmha_bwd_kernel<T, DP, false, false>, BwdCfg<DP, false>::kSmemBytes);
   const long long cap = (long long)device_sms() * 16;
@@ -528,6 +587,15 @@ void launch_fmha_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
     if (bp.f.is_bf16) run_bwd<__nv_bfloat16, 128>(bp, stream);
     else run_bwd<__half, 128>(bp, stream);
   }
+}
+
+unsigned int fmha_det_timeouts_take() {
+  unsigned int n = 0;
+  const unsigned int zero = 0;
+  cudaDeviceSynchronize();   // every backward launched so far has finished counting
+  cudaMemcpyFromSymbol(&n, g_det_timeouts, sizeof(n));
+  cudaMemcpyToSymbol(g_det_timeouts, &zero, sizeof(zero));
+  return n;
 }
 
 }  // namespace ub

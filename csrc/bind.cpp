@@ -269,7 +269,8 @@ std::tuple<Tensor, Tensor, Tensor> layernorm_bwd(const Tensor& dy, const Tensor&
   Tensor part = torch::empty({3, parts, cols}, x.options().dtype(at::kFloat));
   ub::launch_layernorm_bwd(dy.data_ptr(), x.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
                            gamma.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(),
-                           part.data_ptr<float>(), rows, cols, dtype_tag(x), cur_stream(), acc);
+                           part.data_ptr<float>(), rows, cols, dtype_tag(x), cur_stream(), acc,
+                           at::globalContext().deterministicAlgorithms());
   check_launch("layernorm_bwd");
   return {dx, dgamma, dbeta};
 }
@@ -304,7 +305,8 @@ std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& x, const 
   const int parts = ub::norm_bwd_parts(rows, cols, dtype_tag(x));
   Tensor part = torch::empty({3, parts, cols}, x.options().dtype(at::kFloat));
   ub::launch_rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), rstd.data_ptr<float>(), gamma.data_ptr(), dx.data_ptr(),
-                         dgamma.data_ptr(), part.data_ptr<float>(), rows, cols, dtype_tag(x), cur_stream(), acc);
+                         dgamma.data_ptr(), part.data_ptr<float>(), rows, cols, dtype_tag(x), cur_stream(), acc,
+                         at::globalContext().deterministicAlgorithms());
   check_launch("rmsnorm_bwd");
   return {dx, dgamma};
 }
@@ -536,6 +538,18 @@ void embedding_bwd(const Tensor& dy, const Tensor& tokens, int64_t padding_idx, 
   TORCH_CHECK(scratch.is_cuda() && scratch.is_contiguous() && scratch.scalar_type() == at::kFloat && scratch.numel() == vocab * cols);
   TORCH_CHECK(touched.is_cuda() && touched.is_contiguous() && touched.scalar_type() == at::kByte && touched.numel() == vocab);
   const c10::cuda::CUDAGuard guard(dy.device());
+  if (at::globalContext().deterministicAlgorithms()) {
+    // fixed summation order: each vocabulary row sums its rows in ascending original order (scratch / touched unused)
+    const auto sorted = at::sort(tokens.reshape({-1}), /*stable=*/true, /*dim=*/0, /*descending=*/false);
+    const Tensor& ids = std::get<0>(sorted);
+    const Tensor& perm = std::get<1>(sorted);
+    ub::launch_embedding_bwd_sorted(dy.data_ptr(), reinterpret_cast<const long long*>(ids.data_ptr<int64_t>()),
+                                    reinterpret_cast<const long long*>(perm.data_ptr<int64_t>()), grad.data_ptr(),
+                                    tokens.numel(), cols, vocab, padding_idx, accumulate ? 1 : 0, dtype_tag(dy),
+                                    cur_stream());
+    check_launch("embedding_bwd");
+    return;
+  }
   ub::launch_embedding_bwd(dy.data_ptr(), tokens.data_ptr<int64_t>() == nullptr ? nullptr : reinterpret_cast<const long long*>(tokens.data_ptr<int64_t>()),
                            scratch.data_ptr<float>(), touched.data_ptr<uint8_t>(), grad.data_ptr(), tokens.numel(), cols, vocab,
                            padding_idx, accumulate ? 1 : 0, dtype_tag(dy), cur_stream());
@@ -604,7 +618,8 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, OptTensor> bias_dropout_add_ln_bwd(co
                                      rstd.data_ptr<float>(), gamma.data_ptr(), dsum.data_ptr(), dx.data_ptr(),
                                      dgamma.data_ptr(), dbeta.data_ptr(), dbias.has_value() ? dbias->data_ptr() : nullptr,
                                      part.data_ptr<float>(), rows, cols, (float)p, (uint64_t)seed, (uint64_t)offset,
-                                     dtype_tag(summed), cur_stream(), acc);
+                                     dtype_tag(summed), cur_stream(), acc,
+                                     at::globalContext().deterministicAlgorithms());
   check_launch("bias_dropout_add_ln_bwd");
   return {dsum, dx, dgamma, dbeta, dbias};
 }
@@ -803,6 +818,19 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> gbf_bwd(const Tensor& dy, const Tenso
   const int parts = ub::gbf_parts(d.numel(), K);
   Tensor part = torch::empty({parts, 2 * K}, d.options().dtype(at::kFloat));
   Tensor hist = torch::zeros({2, E}, d.options().dtype(at::kFloat));
+  if (at::globalContext().deterministicAlgorithms()) {
+    // fixed summation order: per-row (dt * dist, dt) summed per edge type over the stable-sorted ids
+    Tensor rowg = torch::empty({d.numel(), 2}, d.options().dtype(at::kFloat));
+    const auto sorted = at::sort(edge.reshape({-1}), /*stable=*/true, /*dim=*/0, /*descending=*/false);
+    ub::launch_gbf_bwd_det(dy.data_ptr(), d.data_ptr(), (const long long*)edge.data_ptr<int64_t>(), mul_w.data_ptr(),
+                           bias_w.data_ptr(), means.data_ptr(), stds.data_ptr(), part.data_ptr<float>(),
+                           rowg.data_ptr<float>(), (const long long*)std::get<0>(sorted).data_ptr<int64_t>(),
+                           (const long long*)std::get<1>(sorted).data_ptr<int64_t>(), hist.data_ptr<float>(), d.numel(),
+                           K, E, dtype_tag(d), cur_stream());
+    check_launch("gbf_bwd");
+    Tensor cols = part.sum(0);
+    return {hist[0], hist[1], cols.slice(0, 0, K), cols.slice(0, K, 2 * K)};
+  }
   ub::launch_gbf_bwd(dy.data_ptr(), d.data_ptr(), (const long long*)edge.data_ptr<int64_t>(), mul_w.data_ptr(),
                      bias_w.data_ptr(), means.data_ptr(), stds.data_ptr(), part.data_ptr<float>(), hist.data_ptr<float>(),
                      d.numel(), K, E, dtype_tag(d), cur_stream());

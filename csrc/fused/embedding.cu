@@ -8,6 +8,9 @@
 //   finalize: a warp per vocabulary row; touched rows are added to (or written into) the 16-bit gradient and their
 //             scratch + flag are cleared again, so the scratch buffer is persistent and never needs a memset.
 // The 16-bit gradient is the optimizer's flat arena view when the parameter is claimed (ops/grad_sink.py).
+// The red-adds land in scheduler order, so the fp32 sums can differ in the last bits from run to run.  Under
+// torch.use_deterministic_algorithms the binding sorts the ids instead and embedding_sorted_kernel sums each row's run
+// in a fixed order (no scratch, no flags).
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -81,7 +84,88 @@ __global__ void __launch_bounds__(kEmbThreads) embedding_finalize_kernel(float* 
   }
 }
 
+// Deterministic mode: `sorted` / `perm` are the token ids stable-sorted and their original row indices, so the rows of
+// vocabulary row v are the run perm[lo .. hi) in ascending original order.  A CTA per vocabulary row, threads over
+// 8-column vectors: each column is summed in fp32 strictly in that order, starting from 0.0f; with `accumulate` the
+// existing 16-bit gradient is then added in fp32 and the result rounded once.  A float32 loop on the host over the rows
+// in ascending order reproduces it bit for bit.
+UB_DEVICE long long lower_bound_ll(const long long* __restrict__ a, long long n, long long key) {
+  long long lo = 0, hi = n;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (a[mid] < key) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+constexpr int kEmbDetThreads = 128;
+
+template <typename T>
+__global__ void __launch_bounds__(kEmbDetThreads) embedding_sorted_kernel(const T* __restrict__ dy,
+                                                                         const long long* __restrict__ sorted,
+                                                                         const long long* __restrict__ perm,
+                                                                         T* __restrict__ grad, long long rows, int cols,
+                                                                         long long vocab, long long padding_idx,
+                                                                         int accumulate) {
+  __shared__ long long run[2];
+  const int vecs = cols >> 3;
+  for (long long row = blockIdx.x; row < vocab; row += gridDim.x) {
+    if (row == padding_idx) continue;
+    if (threadIdx.x < 2) run[threadIdx.x] = lower_bound_ll(sorted, rows, row + threadIdx.x);
+    __syncthreads();
+    const long long lo = run[0], hi = run[1];
+    __syncthreads();   // run[] is rewritten for the next row
+    if (lo == hi) continue;
+    for (int v = threadIdx.x; v < vecs; v += kEmbDetThreads) {
+      float f[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      long long r = lo;
+      for (; r + 4 <= hi; r += 4) {   // four loads in flight, added in order
+        Vec16 in[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) in[u] = ld_global_nc_v4(dy + perm[r + u] * cols + v * 8);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          float x[8];
+          unpack<T>(in[u], x);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) f[e] += x[e];
+        }
+      }
+      for (; r < hi; ++r) {
+        float x[8];
+        unpack<T>(ld_global_nc_v4(dy + perm[r] * cols + v * 8), x);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) f[e] += x[e];
+      }
+      T* dst = grad + row * cols + v * 8;
+      if (accumulate) {
+        float g[8];
+        unpack<T>(*reinterpret_cast<const Vec16*>(dst), g);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) f[e] += g[e];
+      }
+      *reinterpret_cast<Vec16*>(dst) = pack<T>(f);
+    }
+  }
+}
+
 }  // namespace
+
+void launch_embedding_bwd_sorted(const void* dy, const long long* sorted, const long long* perm, void* grad,
+                                 long long rows, int cols, long long vocab, long long padding_idx, int accumulate,
+                                 int dtype, cudaStream_t stream) {
+  if (rows == 0 || vocab == 0) return;
+  const unsigned grid = (unsigned)(vocab < 132 * 16 ? vocab : 132 * 16);
+  if (dtype == kBF16)
+    embedding_sorted_kernel<__nv_bfloat16><<<grid, kEmbDetThreads, 0, stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(dy), sorted, perm, reinterpret_cast<__nv_bfloat16*>(grad), rows, cols,
+        vocab, padding_idx, accumulate);
+  else
+    embedding_sorted_kernel<__half><<<grid, kEmbDetThreads, 0, stream>>>(reinterpret_cast<const __half*>(dy), sorted, perm,
+                                                                         reinterpret_cast<__half*>(grad), rows, cols,
+                                                                         vocab, padding_idx, accumulate);
+}
 
 void launch_embedding_bwd(const void* dy, const long long* tokens, float* scratch, unsigned char* touched, void* grad,
                           long long rows, int cols, long long vocab, long long padding_idx, int accumulate, int dtype,

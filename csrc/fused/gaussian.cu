@@ -51,7 +51,10 @@ __global__ void __launch_bounds__(kGbfThreads) gbf_fwd_kernel(const T* __restric
 }
 
 // part: float[gridDim.x][2 * K] (d mean, d std partial column sums); hist: float[2 * E] global (d mul, d bias), zeroed
-template <typename T>
+// kDet (deterministic mode): no atomics.  hist is then float[n][2], each row's (dt * dist, dt), which
+// gbf_edge_sum_kernel sums per edge type in a fixed order; shared memory holds every thread's column accumulators
+// [rows_per_cta][2 * K], and each column of the CTA's partial row is their sum in row-group order.
+template <typename T, bool kDet = false>
 __global__ void __launch_bounds__(kGbfThreads) gbf_bwd_kernel(const T* __restrict__ dy, const T* __restrict__ d,
                                                                const long long* __restrict__ edge,
                                                                const T* __restrict__ mul_w, const T* __restrict__ bias_w,
@@ -61,8 +64,10 @@ __global__ void __launch_bounds__(kGbfThreads) gbf_bwd_kernel(const T* __restric
   extern __shared__ float sm[];            // [2 * E] histogram, then [2 * K] column accumulators
   float* sm_hist = sm;
   float* sm_col = sm + 2 * E;
-  for (int i = threadIdx.x; i < 2 * E + 2 * K; i += kGbfThreads) sm[i] = 0.f;
-  __syncthreads();
+  if constexpr (!kDet) {
+    for (int i = threadIdx.x; i < 2 * E + 2 * K; i += kGbfThreads) sm[i] = 0.f;
+    __syncthreads();
+  }
   const int kvec = K / 8;
   const int rows_per_cta = kGbfThreads / kvec;
   const int j = threadIdx.x % kvec, rl = threadIdx.x / kvec;
@@ -106,9 +111,29 @@ __global__ void __launch_bounds__(kGbfThreads) gbf_bwd_kernel(const T* __restric
     // the kvec threads of a row sit in one warp segment (kvec is a power of two <= 32): reduce dt among them
     for (int o = kvec >> 1; o > 0; o >>= 1) dt += __shfl_xor_sync(0xffffffffu, dt, o);
     if (active && row < n && j == 0) {
-      atomicAdd(&sm_hist[e_idx], dt * dist);
-      atomicAdd(&sm_hist[E + e_idx], dt);
+      if constexpr (kDet) {
+        *reinterpret_cast<float2*>(hist + 2 * row) = make_float2(dt * dist, dt);
+      } else {
+        atomicAdd(&sm_hist[e_idx], dt * dist);
+        atomicAdd(&sm_hist[E + e_idx], dt);
+      }
     }
+  }
+  if constexpr (kDet) {
+    if (active) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        sm[(size_t)rl * 2 * K + j * 8 + e] = dm[e];
+        sm[(size_t)rl * 2 * K + K + j * 8 + e] = ds[e];
+      }
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 2 * K; i += kGbfThreads) {
+      float s = 0.f;
+      for (int r = 0; r < rows_per_cta; ++r) s += sm[(size_t)r * 2 * K + i];
+      part[(size_t)blockIdx.x * 2 * K + i] = s;
+    }
+    return;
   }
   if (active) {
 #pragma unroll
@@ -122,6 +147,53 @@ __global__ void __launch_bounds__(kGbfThreads) gbf_bwd_kernel(const T* __restric
   for (int i = threadIdx.x; i < 2 * E; i += kGbfThreads) {
     const float v = sm_hist[i];
     if (v != 0.f) atomicAdd(&hist[i], v);
+  }
+}
+
+// Deterministic d mul / d bias: `rowg` [n][2] from gbf_bwd_kernel<T, true>; `sorted` / `perm` the stable-sorted edge
+// types and their row indices.  A CTA per edge type e finds its run by binary search and sums (dt * dist, dt) over it
+// in ascending row order, from 0: the CTA stages 256 rows in shared memory, thread 0 adds them in order.
+// hist: float[2 * E], zeroed (types with no row, and ids outside [0, E), contribute nothing).
+constexpr int kGbfSumThreads = 256;
+
+__global__ void __launch_bounds__(kGbfSumThreads) gbf_edge_sum_kernel(const float* __restrict__ rowg,
+                                                                       const long long* __restrict__ sorted,
+                                                                       const long long* __restrict__ perm,
+                                                                       float* __restrict__ hist, long long n, int E) {
+  __shared__ long long run[2];
+  __shared__ float2 stage[kGbfSumThreads];
+  for (int e = blockIdx.x; e < E; e += gridDim.x) {
+    if (threadIdx.x < 2) {
+      long long lo = 0, hi = n;
+      const long long key = e + threadIdx.x;
+      while (lo < hi) {
+        const long long mid = (lo + hi) >> 1;
+        if (sorted[mid] < key) lo = mid + 1;
+        else hi = mid;
+      }
+      run[threadIdx.x] = lo;
+    }
+    __syncthreads();
+    const long long r0 = run[0], r1 = run[1];
+    __syncthreads();   // run[] is rewritten for the next edge type
+    float a = 0.f, b = 0.f;
+    for (long long c = r0; c < r1; c += kGbfSumThreads) {
+      const long long r = c + threadIdx.x;
+      if (r < r1) stage[threadIdx.x] = *reinterpret_cast<const float2*>(rowg + 2 * perm[r]);
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        const int m = (int)(r1 - c < kGbfSumThreads ? r1 - c : kGbfSumThreads);
+        for (int u = 0; u < m; ++u) {
+          a += stage[u].x;
+          b += stage[u].y;
+        }
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x == 0 && r1 > r0) {
+      hist[e] = a;
+      hist[E + e] = b;
+    }
   }
 }
 
@@ -170,6 +242,24 @@ void launch_gbf_bwd(const void* dy, const void* d, const long long* edge, const 
                                               (const __nv_bfloat16*)mul_w, (const __nv_bfloat16*)bias_w,
                                               (const __nv_bfloat16*)means, (const __nv_bfloat16*)stds, part, hist, n, K, E);
   }
+}
+
+void launch_gbf_bwd_det(const void* dy, const void* d, const long long* edge, const void* mul_w, const void* bias_w,
+                        const void* means, const void* stds, float* part, float* rowg, const long long* sorted,
+                        const long long* perm, float* hist, long long n, int K, int E, int dtype, cudaStream_t stream) {
+  if (n <= 0) return;
+  const int grid = gbf_grid(n, K);
+  const size_t smem = (size_t)kGbfThreads * 16 * sizeof(float);   // [rows_per_cta][2 * K] = 256 / (K / 8) * 2 * K
+  if (dtype == kF16)
+    gbf_bwd_kernel<__half, true><<<grid, kGbfThreads, smem, stream>>>(
+        (const __half*)dy, (const __half*)d, edge, (const __half*)mul_w, (const __half*)bias_w, (const __half*)means,
+        (const __half*)stds, part, rowg, n, K, E);
+  else
+    gbf_bwd_kernel<__nv_bfloat16, true><<<grid, kGbfThreads, smem, stream>>>(
+        (const __nv_bfloat16*)dy, (const __nv_bfloat16*)d, edge, (const __nv_bfloat16*)mul_w,
+        (const __nv_bfloat16*)bias_w, (const __nv_bfloat16*)means, (const __nv_bfloat16*)stds, part, rowg, n, K, E);
+  const int egrid = E < 132 * 8 ? E : 132 * 8;
+  if (egrid > 0) gbf_edge_sum_kernel<<<egrid, kGbfSumThreads, 0, stream>>>(rowg, sorted, perm, hist, n, E);
 }
 
 }  // namespace ub

@@ -166,7 +166,7 @@ __global__ void __launch_bounds__(kNormThreads) norm_fwd_kernel(
 // ------------------------------------------------------------------------------------------------
 // backward: dx (+ optional dropout-masked copy for the fused op) and per-CTA dgamma/dbeta partials
 // ------------------------------------------------------------------------------------------------
-template <typename T, int VPT, bool kRMS, bool kFused>
+template <typename T, int VPT, bool kRMS, bool kFused, bool kDet = false>
 __global__ void __launch_bounds__(kNormThreads) norm_bwd_kernel(
     const T* __restrict__ dy, const T* __restrict__ x, const float* __restrict__ mean,
     const float* __restrict__ rstd, const T* __restrict__ gamma, T* __restrict__ dx, float* __restrict__ dgamma_part,
@@ -247,20 +247,30 @@ __global__ void __launch_bounds__(kNormThreads) norm_bwd_kernel(
     }
   }
 
-  // combine the row groups of this CTA, then publish one fp32 partial row per CTA
+  // combine the row groups of this CTA, then publish one fp32 partial row per CTA.  kDet: group 0, 1, ... add in turn
+  // (each column belongs to one thread of a group), so the order is fixed; otherwise shared atomics in arrival order.
   __syncthreads();
+  for (int r = 0; r < (kDet ? rows_per_cta : 1); ++r) {
+    if (!kDet || grp == r) {
 #pragma unroll
-  for (int k = 0; k < VPT; ++k) {
-    const int vi = j + k * tpr;
-    if (vi < g.nvec) {
+      for (int k = 0; k < VPT; ++k) {
+        const int vi = j + k * tpr;
+        if (vi < g.nvec) {
 #pragma unroll
-      for (int e = 0; e < EPV; ++e) {
-        atomicAdd(&sm_acc[vi * EPV + e], dg[k][e]);
-        if (!kRMS) atomicAdd(&sm_acc[g.cols + vi * EPV + e], db[k][e]);
+          for (int e = 0; e < EPV; ++e) {
+            if constexpr (kDet) {
+              sm_acc[vi * EPV + e] += dg[k][e];
+              if (!kRMS) sm_acc[g.cols + vi * EPV + e] += db[k][e];
+            } else {
+              atomicAdd(&sm_acc[vi * EPV + e], dg[k][e]);
+              if (!kRMS) atomicAdd(&sm_acc[g.cols + vi * EPV + e], db[k][e]);
+            }
+          }
+        }
       }
     }
+    __syncthreads();
   }
-  __syncthreads();
   for (int c = threadIdx.x; c < g.cols; c += kNormThreads) {
     dgamma_part[(size_t)blockIdx.x * g.cols + c] = sm_acc[c];
     if (!kRMS) dbeta_part[(size_t)blockIdx.x * g.cols + c] = sm_acc[g.cols + c];
@@ -1041,6 +1051,9 @@ __global__ void __launch_bounds__(kNormV3BwdThreads, (VPL <= 1 ? 2 : 1)) norm_bw
 // ------------------------------------------------------------------------------------------------
 // set by the launch_* entry points for the duration of one call (the host side of a stream is single-threaded)
 static thread_local int g_acc_mask = 0;
+// deterministic mode (torch.use_deterministic_algorithms), set the same way: the gen-1 backward combines its row groups
+// in a fixed order
+static thread_local bool g_det = false;
 
 static int sm_count() {
   static int sms = 0;
@@ -1261,7 +1274,7 @@ static void run_bwd(const void* dy, const void* x, const float* mean, const floa
     float* db_part = part + (size_t)parts * cols;
     const size_t smem = (size_t)(kRMS ? 1 : 2) * cols * sizeof(float);
     UB_DISPATCH_VPT(pl.vpt, {
-      auto kern = norm_bwd_kernel<T, VPT, kRMS, kFused>;
+      auto kern = g_det ? norm_bwd_kernel<T, VPT, kRMS, kFused, true> : norm_bwd_kernel<T, VPT, kRMS, kFused>;
       if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       kern<<<parts, kNormThreads, smem, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx,
                                                   dg_part, db_part, g, (T*)dx_drop, p, keep_scale, seed, offset);
@@ -1279,11 +1292,13 @@ void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, vo
 
 void launch_layernorm_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const void* gamma,
                           void* dx, void* dgamma, void* dbeta, float* part, int rows, int cols, int dtype,
-                          cudaStream_t stream, int accumulate) {
+                          cudaStream_t stream, int accumulate, bool deterministic) {
   g_acc_mask = accumulate;
+  g_det = deterministic;
   UB_DISPATCH_DTYPE(dtype, (run_bwd<T, false, false>(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, nullptr, part, rows,
                                                      cols, nullptr, 0.f, 0, 0, stream)));
   g_acc_mask = 0;
+  g_det = false;
 }
 
 void launch_rmsnorm_fwd(const void* x, const void* gamma, void* y, float* rstd, int rows, int cols, float eps,
@@ -1293,11 +1308,13 @@ void launch_rmsnorm_fwd(const void* x, const void* gamma, void* y, float* rstd, 
 }
 
 void launch_rmsnorm_bwd(const void* dy, const void* x, const float* rstd, const void* gamma, void* dx, void* dgamma,
-                        float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate) {
+                        float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate, bool deterministic) {
   g_acc_mask = accumulate;
+  g_det = deterministic;
   UB_DISPATCH_DTYPE(dtype, (run_bwd<T, true, false>(dy, x, nullptr, rstd, gamma, dx, dgamma, nullptr, nullptr, part,
                                                     rows, cols, nullptr, 0.f, 0, 0, stream)));
   g_acc_mask = 0;
+  g_det = false;
 }
 
 void launch_bias_dropout_add_ln_fwd(const void* x, const void* bias, const void* residual, const void* gamma,
@@ -1316,9 +1333,10 @@ void launch_bias_dropout_add_ln_fwd(const void* x, const void* bias, const void*
 void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const float* mean, const float* rstd,
                                     const void* gamma, void* dsum, void* dx, void* dgamma, void* dbeta,
                                     void* dbias, float* part, int rows, int cols, float p, unsigned long long seed,
-                                    unsigned long long offset, int dtype, cudaStream_t stream, int accumulate) {
+                                    unsigned long long offset, int dtype, cudaStream_t stream, int accumulate, bool deterministic) {
   // dbias (optional, v2 geometries only): column sums of dx, produced by the same pass
   g_acc_mask = accumulate;
+  g_det = deterministic;
   if (dtype == kF16) {
     run_bwd<__half, false, true>(dy, summed, mean, rstd, gamma, dsum, dgamma, dbeta, dbias, part, rows, cols, dx, p,
                                  seed, offset, stream);
@@ -1327,6 +1345,7 @@ void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const fl
                                         dx, p, seed, offset, stream);
   }
   g_acc_mask = 0;
+  g_det = false;
 }
 
 }  // namespace ub

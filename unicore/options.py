@@ -44,6 +44,9 @@ def _global_rows():
         _flag("--wandb-project", metavar="DIR", default="", help="Weights&Biases project name"),
         _flag("--wandb-name", metavar="DIR", default="", help="Weights&Biases run name"),
         _flag("--seed", default=1, type=int, metavar="N", help="pseudo random number generator seed"),
+        _flag("--deterministic", action="store_true",
+              help="bitwise reproducible training on one GPU: torch.use_deterministic_algorithms(True), which also "
+                   "switches the native kernels to their fixed-order reductions (slower backward)"),
         _flag("--cpu", action="store_true", help="use CPU instead of CUDA"),
         _flag("--fp16", action="store_true", help="fp16 model + fp32 master weights + dynamic loss scaling"),
         _flag("--bf16", action="store_true", help="bf16 model + fp32 master weights (no loss scaling)"),

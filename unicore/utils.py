@@ -691,6 +691,18 @@ def set_jit_fusion_options() -> None:
         pass
 
 
+def set_deterministic(enabled: bool) -> None:
+    """``--deterministic``: bitwise reproducible runs on one GPU.  Turns on PyTorch's
+    ``use_deterministic_algorithms``, which the native kernels read at every call to pick their fixed-order
+    reductions, and gives cuBLAS the fixed workspace it needs for reproducible GEMMs.  Call it before the first
+    cuBLAS handle exists (``CUBLAS_WORKSPACE_CONFIG`` is read when a handle is created); an existing
+    ``CUBLAS_WORKSPACE_CONFIG`` is kept."""
+    if not enabled:
+        return
+    os.environ.setdefault("CUBLAS_WORKSPACE_CONFIG", ":4096:8")
+    torch.use_deterministic_algorithms(True)
+
+
 @contextlib.contextmanager
 def validate_with_ema(trainer, ema=False):
     """Temporarily swap the trainer's model for (a half/bf16 copy of) the EMA weights."""

@@ -223,6 +223,7 @@ class TrainingSession:
 
 
 def main(args) -> None:
+    utils.set_deterministic(getattr(args, "deterministic", False))
     utils.import_user_module(args)
     utils.set_jit_fusion_options()
     if args.batch_size is None:
