@@ -78,4 +78,36 @@ void launch_fmha_bwd(const FmhaBwdParams& p, cudaStream_t stream);
 // device since the last call; reading resets it.  Any value other than 0 is a bug.
 unsigned int fmha_det_timeouts_take();
 
+// Decode attention (fmha_decode_sm90.cu): one query row per (b, h) against the first n_b rows of a [B, C, H, D] key /
+// value cache, n_b = min(seqlens[b], C) (all C rows without seqlens), plus row seqlens[b] itself when k_new / v_new
+// are given: that row is first written with k_new / v_new, bitwise.  n_b is also clamped to the columns of the bias
+// and of the key mask, so no device value of seqlens reaches outside a tensor.
+struct FmhaDecodeParams {
+  const void* q;           // [B, 1, H, D] via strides (elements)
+  const void* k_new;       // [B, 1, H, D] via strides, or null (no append)
+  const void* v_new;
+  void* k_cache;           // [B, C, H, D] via strides
+  void* v_cache;
+  const int* seqlens;      // [B] int32 on the device, or null (all C rows visible)
+  const void* bias;        // [bias_batch, H, 1, bias_cols] via (batch, head) strides, contiguous rows; may be null
+  const uint8_t* kpm;      // [B, kpm_cols] bool rows, nonzero = masked; may be null
+  void* out;               // [B, 1, H, D] contiguous
+  float* part_o;           // [B, H, num_splits, D] fp32 partials (num_splits > 1)
+  float* part_ml;          // [B, H, num_splits, 2] (row max in log2 units, row sum)
+  long long q_sb, q_sh, kn_sb, kn_sh, vn_sb, vn_sh;
+  long long kc_sb, kc_sl, kc_sh, vc_sb, vc_sl, vc_sh;
+  long long bias_sb, bias_sh, kpm_sb;
+  int B, H, D, C;
+  int bias_batch, bias_cols, kpm_cols;
+  int num_splits, chunk;   // split s takes keys [s * chunk, (s + 1) * chunk); the last one runs to n_b
+  int is_bf16;
+  float scale;
+};
+constexpr int kDecodeCtasPerSm = 3;        // 72 KB of shared memory each
+constexpr int kDecodeMinSplitKeys = 256;   // the split heuristic makes no shorter split
+constexpr int kDecodeMaxSplits = 128;
+// split count for B x H rows and at most len_bound visible keys (a host bound: the device lengths are never read)
+int fmha_decode_num_splits(int B, int H, int len_bound, int num_sms);
+void launch_fmha_decode(const FmhaDecodeParams& p, cudaStream_t stream);
+
 }  // namespace ub

@@ -233,6 +233,116 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   TORCH_CHECK(err == cudaSuccess, "fmha_bwd launch failed: ", cudaGetErrorString(err));
   return {dq, dk, dv, dbias};
 }
+
+void check_decode_operand(const Tensor& t, const Tensor& q) {
+  TORCH_CHECK(t.is_cuda() && t.device() == q.device(), "fmha_decode: every tensor must be on the device of q");
+  TORCH_CHECK(t.dim() == 4 && t.size(0) == q.size(0) && t.size(2) == q.size(2) && t.size(3) == q.size(3),
+              "fmha_decode: q / k_cache / v_cache / k_new / v_new must be [B, L, H, D] with the B, H, D of q");
+  TORCH_CHECK(t.scalar_type() == q.scalar_type(), "fmha_decode: k_cache / v_cache / k_new / v_new need the dtype of q");
+  TORCH_CHECK(t.stride(3) == 1, "fmha_decode: the last dim of q / k / v must be contiguous");
+  TORCH_CHECK(t.stride(0) % 8 == 0 && t.stride(1) % 8 == 0 && t.stride(2) % 8 == 0 &&
+                  (reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) == 0,
+              "fmha_decode: q / k / v must be 16-byte aligned with strides that are multiples of 8 elements");
+}
+
+// One query row per (b, h) against a [B, C, H, D] key / value cache (fmha_api.h).  max_len is a host bound on
+// seqlens (the device values are never read here, so a decode step does not synchronise); with k_new / v_new the row
+// seqlens[b] is appended first and counts as visible, so up to max_len + 1 keys are.  num_splits = 0 picks the split
+// count from the shapes; any other value forces it.
+Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& seqlens,
+                   int64_t max_len, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
+                   const OptTensor& kpm, double scale, int64_t num_splits) {
+  TORCH_CHECK(q.is_cuda() && q.dim() == 4 && q.size(1) == 1, "q must be [B, 1, H, D] on the GPU");
+  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be fp16 or bf16");
+  const int64_t D = q.size(3);
+  TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
+  check_decode_operand(q, q);
+  check_decode_operand(k_cache, q);
+  check_decode_operand(v_cache, q);
+  const int64_t C = k_cache.size(1);
+  TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
+  const bool append = k_new.has_value() && k_new->defined();
+  TORCH_CHECK(append == (v_new.has_value() && v_new->defined()), "k_new and v_new go together");
+  const bool has_len = seqlens.has_value() && seqlens->defined();
+  if (append) {
+    TORCH_CHECK(has_len, "appending needs seqlens (the row to write)");
+    check_decode_operand(*k_new, q);
+    check_decode_operand(*v_new, q);
+    TORCH_CHECK(k_new->size(1) == 1 && v_new->size(1) == 1, "k_new / v_new must be [B, 1, H, D]");
+  }
+  if (has_len) {
+    TORCH_CHECK(seqlens->is_cuda() && seqlens->device() == q.device() && seqlens->scalar_type() == at::kInt &&
+                    seqlens->dim() == 1 && seqlens->size(0) == q.size(0) && seqlens->is_contiguous(),
+                "seqlens must be a contiguous int32 [B] tensor on the device of q");
+  } else {
+    max_len = C;
+  }
+  const int64_t bound = max_len + (append ? 1 : 0);   // visible keys of any batch
+  TORCH_CHECK(max_len >= 0, "max_len must not be negative");
+  TORCH_CHECK(bound <= C, "max_len (+ 1 when appending) exceeds the cache capacity");
+  const c10::cuda::CUDAGuard guard(q.device());
+  ub::FmhaDecodeParams p{};
+  p.B = (int)q.size(0);
+  p.H = (int)q.size(2);
+  p.D = (int)D;
+  p.C = (int)C;
+  p.is_bf16 = q.scalar_type() == at::kBFloat16 ? 1 : 0;
+  p.scale = (float)scale;
+  p.q = q.data_ptr();
+  p.q_sb = q.stride(0); p.q_sh = q.stride(2);
+  p.k_cache = k_cache.data_ptr();
+  p.kc_sb = k_cache.stride(0); p.kc_sl = k_cache.stride(1); p.kc_sh = k_cache.stride(2);
+  p.v_cache = v_cache.data_ptr();
+  p.vc_sb = v_cache.stride(0); p.vc_sl = v_cache.stride(1); p.vc_sh = v_cache.stride(2);
+  if (append) {
+    p.k_new = k_new->data_ptr();
+    p.kn_sb = k_new->stride(0); p.kn_sh = k_new->stride(2);
+    p.v_new = v_new->data_ptr();
+    p.vn_sb = v_new->stride(0); p.vn_sh = v_new->stride(2);
+  }
+  p.seqlens = has_len ? seqlens->data_ptr<int>() : nullptr;
+  if (bias.has_value() && bias->defined()) {
+    TORCH_CHECK(bias->is_cuda() && bias->device() == q.device() && bias->dim() == 4 &&
+                    (bias->size(0) == 1 || bias->size(0) == p.B) && bias->size(1) == p.H && bias->size(2) == 1 &&
+                    bias->stride(3) == 1,
+                "bias must be [1|B, H, 1, Lb] with a contiguous last dim");
+    TORCH_CHECK(bias->scalar_type() == q.scalar_type(), "bias must have the dtype of q");
+    TORCH_CHECK(bias->size(3) >= bound, "bias must have a column for every key that can be visible");
+    p.bias = bias->data_ptr();
+    p.bias_batch = (int)bias->size(0);
+    p.bias_sb = bias->stride(0); p.bias_sh = bias->stride(1);
+    p.bias_cols = (int)bias->size(3);
+  }
+  if (kpm.has_value() && kpm->defined()) {
+    TORCH_CHECK(kpm->is_cuda() && kpm->device() == q.device() && kpm->scalar_type() == at::kBool && kpm->dim() == 2 &&
+                    kpm->size(0) == p.B && kpm->stride(1) == 1 && kpm->size(1) >= bound,
+                "key_padding_mask must be bool [B, Lk] with a contiguous last dim and Lk >= the visible keys");
+    p.kpm = reinterpret_cast<const uint8_t*>(kpm->data_ptr());
+    p.kpm_sb = kpm->stride(0);
+    p.kpm_cols = (int)kpm->size(1);
+  }
+  if (num_splits == 0) {
+    const int sms = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
+    num_splits = ub::fmha_decode_num_splits(p.B, p.H, (int)bound, sms);
+  }
+  TORCH_CHECK(num_splits >= 1 && num_splits <= ub::kDecodeMaxSplits,
+              "num_splits must be 0 (heuristic) or 1 .. fmha_decode_max_splits()");
+  p.num_splits = (int)num_splits;
+  p.chunk = (int)std::max<int64_t>(1, (bound + num_splits - 1) / num_splits);
+  Tensor out = torch::empty({p.B, 1, p.H, p.D}, q.options());
+  p.out = out.data_ptr();
+  Tensor work;
+  if (p.num_splits > 1) {
+    const int64_t parts = (int64_t)p.B * p.H * p.num_splits;
+    work = torch::empty({parts * (D + 2)}, q.options().dtype(at::kFloat));
+    p.part_o = work.data_ptr<float>();
+    p.part_ml = p.part_o + parts * D;
+  }
+  ub::launch_fmha_decode(p, at::cuda::getCurrentCUDAStream().stream());
+  cudaError_t err = cudaGetLastError();
+  TORCH_CHECK(err == cudaSuccess, "fmha_decode launch failed: ", cudaGetErrorString(err));
+  return out;
+}
 }  // namespace
 
 void register_fmha(pybind11::module_& m) {
@@ -243,6 +353,14 @@ void register_fmha(pybind11::module_& m) {
   m.def("fmha_bwd", &fmha_bwd, py::arg("dout"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("out"),
         py::arg("lse"), py::arg("bias"), py::arg("kpm"), py::arg("p_drop"), py::arg("scale"), py::arg("drop_bits"),
         py::arg("need_dbias"), py::arg("packed_grad"), py::arg("dlogits") = py::none(), py::arg("causal") = false);
+  m.def("fmha_decode", &fmha_decode, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("seqlens"),
+        py::arg("max_len"), py::arg("k_new"), py::arg("v_new"), py::arg("bias"), py::arg("key_padding_mask"),
+        py::arg("scale"), py::arg("num_splits") = 0);
+  m.def("fmha_decode_max_splits", [] { return (int64_t)ub::kDecodeMaxSplits; });
+  m.def("fmha_decode_num_splits", [](int64_t B, int64_t H, int64_t len_bound) {
+    return (int64_t)ub::fmha_decode_num_splits((int)B, (int)H, (int)len_bound,
+                                               at::cuda::getCurrentDeviceProperties()->multiProcessorCount);
+  }, "split count fmha_decode picks with num_splits = 0 for B x H rows and at most len_bound visible keys");
   m.def("fmha_det_timeouts", [] { return (int64_t)ub::fmha_det_timeouts_take(); },
         "deterministic-mode dQ turn waits that timed out on the current device since the last call (reset on read)");
 }

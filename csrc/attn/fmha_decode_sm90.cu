@@ -1,0 +1,302 @@
+// Decode attention for sm_90a: one query row per (batch, head) against the first n_b rows of a key / value cache,
+//   O[b, h] = softmax(scale * q k^T + bias + key mask) V          (fp16 / bf16 in and out, fp32 math)
+// with an optional append of the new token's key / value into row seqlens[b] of the caches in the same launch.
+//
+// M = 1 leaves nothing for wgmma: each key is a dot product and an axpy, and a step has to stream K and V once at HBM
+// bandwidth.  So the kernel is a copy pipeline feeding the CUDA cores:
+//   * Split-KV: CTA (s, h, b) takes the contiguous key range [s * chunk, (s + 1) * chunk) of (b, h) (the last split
+//     runs to n_b).  With one split it writes O; otherwise it writes an fp32 partial (o[D] unnormalised, m, l) and
+//     fmha_decode_combine_kernel merges the splits in ascending order.  No atomics: for a given split count the
+//     result does not depend on the schedule.
+//   * Streaming: warp 0 requests the K and V rows of key tile t + kStages with one cp.async.bulk per row (rows are
+//     D * 2 bytes, a multiple of 16; no tensor map to encode on the host) into stage t % kStages, completion on that
+//     stage's mbarrier.  kStages * 16 KB are in flight per CTA, three CTAs per SM.
+//   * Math: 16 groups of 8 lanes; lane j of a group holds 16-byte chunks j and j + 8 of the pre-scaled query
+//     (scale * log2e) in fp32.  Group g takes keys g, g + 16, ... of a tile: partial dot products, three xor
+//     shuffles, then the online softmax with ex2 over the group's keys of the tile and P V into the lane's fp32
+//     chunks.  At the end the 16 group states are merged in shared memory in group order.
+//   * Append (k_new / v_new set): the new token's key and value are row pos = seqlens[b] of the caches, and that row
+//     is always the last visible key (n_b = pos + 1).  The CTA whose range holds pos bulk-copies that row into its
+//     stage straight from k_new / v_new (not from the cache) and stores it bitwise into the caches.  No other CTA
+//     reads row pos of (b, h) - every other key range ends before it - so the write needs no ordering against any
+//     read, and one launch both appends and attends.
+//   * Bounds: n_b is clamped to the cache capacity C (and to the columns of the bias / key mask), pos to n_b - 1, for
+//     any device value of seqlens: no read or write outside the tensors.  A row whose visible keys are all masked
+//     gives O = 0.
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <math_constants.h>
+
+#include <algorithm>
+
+#include "../common.cuh"
+#include "fmha_api.h"
+
+namespace ub {
+namespace {
+
+constexpr int kThreads = 128;
+constexpr int kGroups = kThreads / 8;   // 8 lanes per key
+constexpr int kStages = 4;
+constexpr float kLog2e = 1.4426950408889634f;
+
+// NC = 16-byte chunks per lane: 1 for D <= 64, 2 for D <= 128.  A stage holds kTile K rows and kTile V rows of at
+// most 64 * NC columns: 16 KB either way.
+template <int NC>
+struct DecCfg {
+  static constexpr int kTile = NC == 1 ? 64 : 32;               // keys per tile
+  static constexpr int kKeysPerGroup = kTile / kGroups;          // 4 or 2
+  static constexpr uint32_t kRowMax = 64 * NC * 2;               // bytes of the widest row
+  static constexpr uint32_t kStageBytes = 2 * kTile * kRowMax;   // K rows, then V rows
+  static constexpr uint32_t kSmemRedO = kStages * kStageBytes;   // float[kGroups][64 * NC]
+  static constexpr uint32_t kSmemRedML = kSmemRedO + kGroups * 64 * NC * 4;   // float[2][kGroups]
+  static constexpr uint32_t kSmemBar = kSmemRedML + 2 * kGroups * 4;
+  static constexpr uint32_t kSmemBytes = kSmemBar + kStages * 8;
+};
+
+UB_DEVICE int clampi(int x, int lo, int hi) { return x < lo ? lo : (x > hi ? hi : x); }
+
+template <typename T, int NC>
+__global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeParams p) {
+  using C = DecCfg<NC>;
+  extern __shared__ __align__(16) unsigned char smem[];
+  const int tid = threadIdx.x, lane = tid & 31, g = tid >> 3, j8 = tid & 7;
+  const int s = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int D = p.D, nch = D / 8;
+  const uint32_t row_bytes = (uint32_t)D * 2;
+
+  // ---- visible keys of (b, h) and this CTA's range --------------------------------------------------------------
+  int cap = p.C;
+  if (p.bias != nullptr) cap = min(cap, p.bias_cols);
+  if (p.kpm != nullptr) cap = min(cap, p.kpm_cols);
+  const bool append = p.k_new != nullptr;
+  const int len = p.seqlens != nullptr ? p.seqlens[b] : cap;
+  const int pos = append ? clampi(len, 0, cap - 1) : -1;   // row of the new token
+  const int n = append ? pos + 1 : clampi(len, 0, cap);
+  const int start = s * p.chunk;
+  const int end = s == p.num_splits - 1 ? n : min(start + p.chunk, n);
+
+  const T* kc = reinterpret_cast<const T*>(p.k_cache) + (long long)b * p.kc_sb + (long long)h * p.kc_sh;
+  const T* vc = reinterpret_cast<const T*>(p.v_cache) + (long long)b * p.vc_sb + (long long)h * p.vc_sh;
+  const T* kn = append ? reinterpret_cast<const T*>(p.k_new) + (long long)b * p.kn_sb + (long long)h * p.kn_sh : nullptr;
+  const T* vn = append ? reinterpret_cast<const T*>(p.v_new) + (long long)b * p.vn_sb + (long long)h * p.vn_sh : nullptr;
+  const bool owner = append && start <= pos && pos < end;
+  if (owner && tid < 2 * nch) {
+    // bitwise copy of the new row into the caches (see the append invariant above)
+    const int c = tid % nch;
+    const bool is_v = tid >= nch;
+    const Vec16 w = ld_global_v4((is_v ? vn : kn) + 8 * c);
+    T* dst = const_cast<T*>(is_v ? vc + (long long)pos * p.vc_sl : kc + (long long)pos * p.kc_sl);
+    st_global_v4(dst + 8 * c, w);
+  }
+
+  const int ntiles = end > start ? (end - start + C::kTile - 1) / C::kTile : 0;
+  const uint32_t smem0 = smem_addr_u32(smem);
+  const uint32_t bar0 = smem0 + C::kSmemBar;
+  auto issue = [&](int t) {   // warp 0: K and V rows of tile t into stage t % kStages
+    const int st = t % kStages, r0 = start + t * C::kTile, nrows = min(C::kTile, end - r0);
+    const uint32_t bar = bar0 + 8 * st, dk = smem0 + st * C::kStageBytes, dv = dk + C::kTile * row_bytes;
+    if (lane == 0) bulk_expect_tx(bar, 2u * nrows * row_bytes);
+    __syncwarp();
+    for (int r = lane; r < nrows; r += 32) {
+      const int key = r0 + r;
+      const bool is_new = key == pos;
+      bulk_g2s(dk + r * row_bytes, is_new ? kn : kc + (long long)key * p.kc_sl, row_bytes, bar);
+      bulk_g2s(dv + r * row_bytes, is_new ? vn : vc + (long long)key * p.vc_sl, row_bytes, bar);
+    }
+  };
+  if (tid == 0) {
+    for (int st = 0; st < kStages; ++st) bulk_bar_init(bar0 + 8 * st, 1);
+    bulk_bar_init_fence();
+  }
+  __syncthreads();
+  if (tid < 32)
+    for (int t = 0; t < min(kStages, ntiles); ++t) issue(t);
+
+  // ---- query chunks of this lane, pre-scaled by scale * log2e ------------------------------------------------------
+  const float qs = p.scale * kLog2e;
+  float qf[8 * NC], acc[8 * NC];
+  const T* q = reinterpret_cast<const T*>(p.q) + (long long)b * p.q_sb + (long long)h * p.q_sh;
+#pragma unroll
+  for (int c = 0; c < NC; ++c) {
+    const int ch = j8 + 8 * c;
+    if (ch < nch) {
+      unpack<T>(ld_global_v4(q + 8 * ch), qf + 8 * c);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) qf[8 * c + e] = 0.f;
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      qf[8 * c + e] *= qs;
+      acc[8 * c + e] = 0.f;
+    }
+  }
+  const T* bias = p.bias != nullptr
+                      ? reinterpret_cast<const T*>(p.bias) + (p.bias_batch > 1 ? (long long)b * p.bias_sb : 0LL) +
+                            (long long)h * p.bias_sh
+                      : nullptr;
+  const uint8_t* kpm = p.kpm != nullptr ? p.kpm + (long long)b * p.kpm_sb : nullptr;
+
+  float m = -CUDART_INF_F, l = 0.f;
+  for (int t = 0; t < ntiles; ++t) {
+    const int st = t % kStages, r0 = start + t * C::kTile, nrows = min(C::kTile, end - r0);
+    bulk_wait(bar0 + 8 * st, (t / kStages) & 1);
+    const unsigned char* sk = smem + st * C::kStageBytes;
+    const unsigned char* sv = sk + C::kTile * row_bytes;
+    float sc[C::kKeysPerGroup];
+#pragma unroll
+    for (int i = 0; i < C::kKeysPerGroup; ++i) {
+      const int r = g + kGroups * i;
+      float d = 0.f;
+#pragma unroll
+      for (int c = 0; c < NC; ++c) {
+        const int ch = j8 + 8 * c;
+        if (ch < nch) {
+          float kf[8];
+          unpack<T>(*reinterpret_cast<const Vec16*>(sk + r * row_bytes + 16 * ch), kf);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) d = fmaf(qf[8 * c + e], kf[e], d);
+        }
+      }
+      d += __shfl_xor_sync(0xffffffffu, d, 1);
+      d += __shfl_xor_sync(0xffffffffu, d, 2);
+      d += __shfl_xor_sync(0xffffffffu, d, 4);
+      // rows past the range hold stale bytes: their score is replaced, and their V row is never read
+      const int key = r0 + r;
+      if (r < nrows) {
+        if (bias != nullptr) d = fmaf(to_f32<T>(bias[key]), kLog2e, d);
+        if (kpm != nullptr && kpm[key] != 0) d = -CUDART_INF_F;
+      } else {
+        d = -CUDART_INF_F;
+      }
+      sc[i] = d;
+    }
+    float mt = sc[0];
+#pragma unroll
+    for (int i = 1; i < C::kKeysPerGroup; ++i) mt = fmaxf(mt, sc[i]);
+    const float m_new = fmaxf(m, mt);
+    if (m_new != -CUDART_INF_F) {   // else every key so far is masked: l and acc stay 0
+      const float alpha = ex2_approx(m - m_new);   // m = -inf -> 0
+      l *= alpha;
+#pragma unroll
+      for (int e = 0; e < 8 * NC; ++e) acc[e] *= alpha;
+#pragma unroll
+      for (int i = 0; i < C::kKeysPerGroup; ++i) {
+        const int r = g + kGroups * i;
+        if (r < nrows) {
+          const float pk = ex2_approx(sc[i] - m_new);
+          l += pk;
+#pragma unroll
+          for (int c = 0; c < NC; ++c) {
+            const int ch = j8 + 8 * c;
+            if (ch < nch) {
+              float vf[8];
+              unpack<T>(*reinterpret_cast<const Vec16*>(sv + r * row_bytes + 16 * ch), vf);
+#pragma unroll
+              for (int e = 0; e < 8; ++e) acc[8 * c + e] = fmaf(pk, vf[e], acc[8 * c + e]);
+            }
+          }
+        }
+      }
+      m = m_new;
+    }
+    __syncthreads();   // every thread is done with stage st
+    if (tid < 32 && t + kStages < ntiles) issue(t + kStages);
+  }
+
+  // ---- merge the 16 group states in group order --------------------------------------------------------------------
+  float* red_o = reinterpret_cast<float*>(smem + C::kSmemRedO);
+  float* red_m = reinterpret_cast<float*>(smem + C::kSmemRedML);
+  float* red_l = red_m + kGroups;
+  if (j8 == 0) {
+    red_m[g] = m;
+    red_l[g] = l;
+  }
+#pragma unroll
+  for (int c = 0; c < NC; ++c) {
+    const int ch = j8 + 8 * c;
+    if (ch < nch) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) red_o[g * 64 * NC + 8 * ch + e] = acc[8 * c + e];
+    }
+  }
+  __syncthreads();
+  float mm = red_m[0];
+#pragma unroll
+  for (int i = 1; i < kGroups; ++i) mm = fmaxf(mm, red_m[i]);
+  if (tid < D) {
+    float o = 0.f, ls = 0.f;
+    if (mm != -CUDART_INF_F) {
+#pragma unroll
+      for (int i = 0; i < kGroups; ++i) {
+        const float w = ex2_approx(red_m[i] - mm);
+        ls = fmaf(red_l[i], w, ls);
+        o = fmaf(red_o[i * 64 * NC + tid], w, o);
+      }
+    }
+    const long long bh = (long long)b * p.H + h;
+    if (p.num_splits == 1) {
+      reinterpret_cast<T*>(p.out)[bh * D + tid] = from_f32<T>(ls > 0.f ? o / ls : 0.f);
+    } else {
+      const long long part = bh * p.num_splits + s;
+      p.part_o[part * D + tid] = o;   // o = 0, m = -inf, l = 0: the neutral partial of an empty range
+      if (tid == 0) {
+        p.part_ml[2 * part] = mm;
+        p.part_ml[2 * part + 1] = ls;
+      }
+    }
+  }
+}
+
+// O[b, h] from the num_splits partials of (b, h), added in ascending split order.  One CTA per (b, h), thread d owns
+// column d.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) fmha_decode_combine_kernel(const FmhaDecodeParams p) {
+  const int h = blockIdx.x, b = blockIdx.y, d = threadIdx.x;
+  if (d >= p.D) return;
+  const long long bh = (long long)b * p.H + h;
+  const float* ml = p.part_ml + 2 * bh * p.num_splits;
+  const float* po = p.part_o + bh * p.num_splits * p.D + d;
+  float mm = -CUDART_INF_F;
+  for (int s = 0; s < p.num_splits; ++s) mm = fmaxf(mm, ml[2 * s]);
+  float o = 0.f, ls = 0.f;
+  if (mm != -CUDART_INF_F) {
+    for (int s = 0; s < p.num_splits; ++s) {
+      const float w = ex2_approx(ml[2 * s] - mm);
+      ls = fmaf(ml[2 * s + 1], w, ls);
+      o = fmaf(po[(long long)s * p.D], w, o);
+    }
+  }
+  reinterpret_cast<T*>(p.out)[bh * p.D + d] = from_f32<T>(ls > 0.f ? o / ls : 0.f);
+}
+
+}  // namespace
+
+int fmha_decode_num_splits(int B, int H, int len_bound, int num_sms) {
+  // As many splits as fit the num_sms * kDecodeCtasPerSm resident CTAs in one wave (a partial second wave would
+  // leave most SMs idle at its end); no split shorter than kDecodeMinSplitKeys (its partial and the second launch
+  // would cost more than its keys).  B * H above half the resident slots runs with one split.
+  const long long bh = (long long)B * H, slots = (long long)num_sms * kDecodeCtasPerSm;
+  long long s = slots / bh;
+  s = std::min<long long>(s, (len_bound + kDecodeMinSplitKeys - 1) / kDecodeMinSplitKeys);
+  return (int)std::max<long long>(1, std::min<long long>(s, kDecodeMaxSplits));
+}
+
+void launch_fmha_decode(const FmhaDecodeParams& p, cudaStream_t stream) {
+  const dim3 grid(p.num_splits, p.H, p.B);
+  auto run = [&](auto kern, auto combine, uint32_t smem_bytes) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
+    kern<<<grid, kThreads, smem_bytes, stream>>>(p);
+    if (p.num_splits > 1) combine<<<dim3(p.H, p.B), kThreads, 0, stream>>>(p);
+  };
+  if (p.D <= 64) {
+    if (p.is_bf16) run(fmha_decode_kernel<__nv_bfloat16, 1>, fmha_decode_combine_kernel<__nv_bfloat16>, DecCfg<1>::kSmemBytes);
+    else run(fmha_decode_kernel<__half, 1>, fmha_decode_combine_kernel<__half>, DecCfg<1>::kSmemBytes);
+  } else {
+    if (p.is_bf16) run(fmha_decode_kernel<__nv_bfloat16, 2>, fmha_decode_combine_kernel<__nv_bfloat16>, DecCfg<2>::kSmemBytes);
+    else run(fmha_decode_kernel<__half, 2>, fmha_decode_combine_kernel<__half>, DecCfg<2>::kSmemBytes);
+  }
+}
+
+}  // namespace ub

@@ -5,7 +5,7 @@ import types as _types
 
 from .norm import FusedLayerNormFastFunction, FusedRMSNormFastFunction, LayerNorm, RMSNorm
 from .softmax_dropout import softmax_dropout
-from .attention import CrossMultiheadAttention, SelfMultiheadAttention
+from .attention import CrossMultiheadAttention, DecoderCache, LayerKVCache, SelfMultiheadAttention
 from .transformer import (
     TransformerDecoder,
     TransformerDecoderLayer,
@@ -20,7 +20,7 @@ from .transformer import (
 __all__ = [
     "LayerNorm", "RMSNorm", "softmax_dropout", "SelfMultiheadAttention", "CrossMultiheadAttention",
     "TransformerEncoderLayer", "TransformerEncoder", "init_bert_params", "relative_position_bucket",
-    "TransformerDecoderLayer", "TransformerDecoder",
+    "TransformerDecoderLayer", "TransformerDecoder", "DecoderCache", "LayerKVCache",
 ]
 
 _LEGACY = {

@@ -17,6 +17,9 @@ dim, or on the CPU, the materialised path (bmm + ``softmax_dropout`` kernel) is 
 ``causal=True`` on ``SelfMultiheadAttention`` hides key ``j`` from query ``i`` when ``j > i``.  The fused path passes it
 to the kernel as a flag (no mask tensor); the materialised path adds the future mask ``triu(-inf, 1)`` to the bias, so
 its logits are those of the same call with that mask in ``attn_bias``.
+
+``DecoderCache`` holds what incremental decoding keeps between steps: per layer the self-attention keys and values
+``[B, C, H, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.
 """
 from typing import Optional
 
@@ -92,12 +95,16 @@ class SelfMultiheadAttention(nn.Module):
         self.in_proj = nn.Linear(embed_dim, embed_dim * 3, bias=bias)
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
 
-    def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False, need_probs=True, causal=False):
+    def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False, need_probs=True, causal=False,
+               cache=None):
         """Everything up to (not including) ``out_proj``: returns ``(o [B, L, E], logits, probs)``.
 
         ``need_probs=False`` returns ``probs = None``; with ``return_attn`` the fused kernel then also computes the
         logits ``[B*H, L, L]`` where it takes the shapes.  ``causal`` hides key j from query i when j > i (see the module
-        docstring)."""
+        docstring).  ``cache`` (a ``LayerKVCache`` of a ``DecoderCache``): on the prefill the keys and values of the L
+        positions are also stored in it; on a decoding step (``query [B, 1, E]``) the new token's key and value are
+        appended and its query attends to the cached keys (``ops.attention_with_kv_cache``), with ``attn_bias`` the
+        ``[B, H, 1, Lb]`` row of the new queries."""
         bsz, tgt_len, embed_dim = query.size()
         if embed_dim != self.embed_dim:
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
@@ -106,6 +113,14 @@ class SelfMultiheadAttention(nn.Module):
         qkv = ops.linear(query, self.in_proj.weight, self.in_proj.bias)
         qkv = qkv.view(bsz, tgt_len, 3, self.num_heads, self.head_dim)
         q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]  # strided views [B, L, H, D]
+        if cache is not None and cache.stepping:
+            if return_attn:
+                raise ValueError("a decoding step does not return attention weights")
+            o = ops.attention_with_kv_cache(q, cache.k, cache.v, cache.seqlens, cache.max_len, k_new=k, v_new=v,
+                                            bias=attn_bias, scale=self.scaling)
+            return o.reshape(bsz, tgt_len, embed_dim), None, None
+        if cache is not None:
+            cache.store_prefix(k, v)
         bias4 = _bias_as_4d(attn_bias, bsz, self.num_heads, tgt_len, tgt_len)
         if (not return_attn or not need_probs) and ops.fused_attention_supported(q, k, v, bias4, key_padding_mask):
             res = ops.fused_attention_qkvpacked(
@@ -153,17 +168,29 @@ class CrossMultiheadAttention(nn.Module):
         self.v_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
 
-    def attend(self, query, key, value, key_padding_mask=None, attn_bias=None):
-        """Everything up to (not including) ``out_proj``."""
+    def attend(self, query, key, value, key_padding_mask=None, attn_bias=None, cache=None):
+        """Everything up to (not including) ``out_proj``.
+
+        ``cache`` (a ``LayerKVCache``): the projected keys and values are computed once, on the prefill, and kept in
+        it; a decoding step (``query [B, 1, E]``, ``key`` / ``value`` unused) attends to them with
+        ``ops.attention_with_kv_cache``."""
         bsz, tgt_len, embed_dim = query.size()
         if embed_dim != self.embed_dim:
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
-        src_len = key.size(1)
         if key_padding_mask is not None and key_padding_mask.dim() == 0:
             key_padding_mask = None
         q = self.q_proj(query).view(bsz, tgt_len, self.num_heads, self.head_dim)
+        if cache is not None and cache.stepping:
+            src_len = cache.enc_k.size(1)
+            bias4 = _bias_as_4d(attn_bias, bsz, self.num_heads, tgt_len, src_len)
+            o = ops.attention_with_kv_cache(q, cache.enc_k, cache.enc_v, bias=bias4,
+                                            key_padding_mask=key_padding_mask, scale=self.scaling)
+            return o.reshape(bsz, tgt_len, embed_dim)
+        src_len = key.size(1)
         k = self.k_proj(key).view(bsz, src_len, self.num_heads, self.head_dim)
         v = self.v_proj(value).view(bsz, src_len, self.num_heads, self.head_dim)
+        if cache is not None:
+            cache.store_encoder(k, v)
         bias4 = _bias_as_4d(attn_bias, bsz, self.num_heads, tgt_len, src_len)
         if ops.fused_attention_supported(q, k, v, bias4, key_padding_mask):
             return ops.fused_attention(
@@ -185,3 +212,65 @@ class CrossMultiheadAttention(nn.Module):
         attn_bias: Optional[Tensor] = None,
     ) -> Tensor:
         return self.out_proj(self.attend(query, key, value, key_padding_mask, attn_bias))
+
+
+class LayerKVCache:
+    """One decoder layer's share of a ``DecoderCache``: self-attention keys / values ``k``, ``v`` ``[B, C, H, D]`` and
+    the projected encoder keys / values ``enc_k``, ``enc_v`` ``[B, S, H, D]`` (None until the prefill stores them)."""
+
+    def __init__(self, owner, k, v):
+        self.owner = owner
+        self.k, self.v = k, v
+        self.enc_k = self.enc_v = None
+
+    @property
+    def stepping(self):
+        """False on the prefill (the first call on an empty cache), True on every decoding step after it."""
+        return self.owner.max_len > 0
+
+    @property
+    def seqlens(self):
+        return self.owner.seqlens
+
+    @property
+    def max_len(self):
+        return self.owner.max_len
+
+    def store_prefix(self, k, v):
+        """Rows ``0 .. L-1`` of the self-attention cache from the prefill's ``[B, L, H, D]`` keys and values."""
+        with torch.no_grad():
+            self.k[:, :k.size(1)].copy_(k)
+            self.v[:, :v.size(1)].copy_(v)
+
+    def store_encoder(self, k, v):
+        self.enc_k, self.enc_v = k.detach(), v.detach()
+
+    def reorder(self, index):
+        self.k, self.v = self.k.index_select(0, index), self.v.index_select(0, index)
+        if self.enc_k is not None:
+            self.enc_k, self.enc_v = self.enc_k.index_select(0, index), self.enc_v.index_select(0, index)
+
+
+class DecoderCache:
+    """State of incremental decoding for a ``TransformerDecoder`` (made by ``TransformerDecoder.new_cache``).
+
+    ``layers``: one ``LayerKVCache`` per layer.  ``seqlens``: int32 ``[B]`` on the device, the tokens decoded so far per
+    sequence (the position of the next one).  ``max_len``: a host-side upper bound on ``seqlens`` (0 = empty cache), so
+    that no step has to read the device lengths.  ``capacity``: rows of the self-attention buffers."""
+
+    def __init__(self, num_layers, batch_size, capacity, heads, head_dim, dtype, device):
+        self.capacity = capacity
+        self.seqlens = torch.zeros(batch_size, dtype=torch.int32, device=device)
+        self.max_len = 0
+        shape = (batch_size, capacity, heads, head_dim)
+        self.layers = [
+            LayerKVCache(self, torch.zeros(shape, dtype=dtype, device=device),
+                         torch.zeros(shape, dtype=dtype, device=device))
+            for _ in range(num_layers)
+        ]
+
+    def reorder(self, index):
+        """Select (and repeat) sequences of the batch along ``index`` in every buffer, as beam search does."""
+        self.seqlens = self.seqlens.index_select(0, index)
+        for layer in self.layers:
+            layer.reorder(index)

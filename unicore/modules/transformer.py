@@ -26,7 +26,7 @@ import torch.nn.functional as F
 
 from unicore import ops, utils
 
-from .attention import CrossMultiheadAttention, SelfMultiheadAttention
+from .attention import CrossMultiheadAttention, DecoderCache, SelfMultiheadAttention
 from .norm import LayerNorm
 
 
@@ -104,15 +104,17 @@ class _BlockMixin:
         return_attn = kw.pop("return_attn", False)
         need_probs = kw.pop("need_probs", True)
         causal = kw.pop("causal", False)
+        cache = kw.pop("cache", None)
         h = attn_in if self.post_ln else norm(attn_in)
         extra = None
         if isinstance(attn_module, SelfMultiheadAttention):
             o, logits, probs = attn_module.attend(h, kw.get("key_padding_mask"), kw.get("attn_bias"), return_attn,
-                                                  need_probs, causal)
+                                                  need_probs, causal, cache=cache)
             if return_attn:
                 extra = (logits, probs)
         else:
-            o = attn_module.attend(h, kw["key"], kw["value"], kw.get("key_padding_mask"), kw.get("attn_bias"))
+            o = attn_module.attend(h, kw["key"], kw["value"], kw.get("key_padding_mask"), kw.get("attn_bias"),
+                                   cache=cache)
         proj = attn_module.out_proj
         if self.post_ln and self._fused_ok(o):
             # out_proj bias + dropout + residual + LayerNorm in one pass over the GEMM output
@@ -234,18 +236,21 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
         encoder_attn_bias: Optional[torch.Tensor] = None,
         encoder_padding_mask: Optional[torch.Tensor] = None,
         causal: bool = False,
+        cache=None,
     ) -> torch.Tensor:
         """``causal`` masks future keys in the self-attention (key j > query i), without a mask tensor on the fused
-        path; the encoder attention is unaffected."""
+        path; the encoder attention is unaffected.  ``cache``: this layer's ``LayerKVCache`` of a ``DecoderCache``
+        (see ``TransformerDecoder.forward``); on a decoding step the encoder attention uses the encoder keys and values
+        it stored on the prefill, and ``encoder_out`` may be None."""
         x, _ = self._attn_residual(
             self.self_attn, self.self_attn_layer_norm, x, x, key_padding_mask=padding_mask, attn_bias=attn_bias,
-            causal=causal,
+            causal=causal, cache=cache,
         )
-        if encoder_out is not None:
+        if encoder_out is not None or (cache is not None and cache.stepping and cache.enc_k is not None):
             x, _ = self._attn_residual(
                 self.encoder_attn, self.encoder_attn_layer_norm, x, x,
                 key=encoder_out, value=encoder_out,
-                key_padding_mask=encoder_padding_mask, attn_bias=encoder_attn_bias,
+                key_padding_mask=encoder_padding_mask, attn_bias=encoder_attn_bias, cache=cache,
             )
         return self._ffn_residual(x)
 
@@ -464,7 +469,22 @@ class TransformerDecoder(nn.Module, _StackMixin):
         encoder_padding_mask: Optional[torch.Tensor] = None,
         attn_mask: Optional[torch.Tensor] = None,
         encoder_attn_mask: Optional[torch.Tensor] = None,
+        cache: Optional[DecoderCache] = None,
     ) -> torch.Tensor:
+        """Without ``cache`` the whole sequence is decoded at once.  With a ``DecoderCache`` (``new_cache``):
+
+        * the first call (the prefill) takes the prompts ``emb [B, L, E]``, right-padded as ``padding_mask`` says, runs
+          exactly the path above and stores every layer's keys / values of the L positions and its projected encoder
+          keys / values; the cache then holds the unpadded lengths;
+        * every later call (a step) takes one token per sequence, ``emb [B, 1, E]`` at position ``seqlens[b]``, and
+          returns ``[B, 1, E]``.  Its self-attention appends the token's key / value and attends to the cache; the
+          encoder attention uses the stored encoder keys / values (``encoder_out`` may be None) with
+          ``encoder_padding_mask``, and ``encoder_attn_mask``, if given, holds the rows of the new queries
+          ``[B*H, 1, S]``.  ``padding_mask`` and ``attn_mask`` are not supported on a step.
+        """
+        if cache is not None:
+            return self._forward_cached(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
+                                        encoder_attn_mask, cache)
         x = self._embed_prologue(emb, padding_mask)
         # on the fused path the kernels apply the future mask themselves (causal=True); it joins no bias tensor
         causal = self.auto_regressive and self._fused_attention_capable(x)
@@ -480,6 +500,76 @@ class TransformerDecoder(nn.Module, _StackMixin):
                 encoder_attn_bias=encoder_attn_mask,
                 causal=causal,
             )
+        if self.final_layer_norm is not None:
+            x = self.final_layer_norm(x)
+        return x
+
+    # ---- incremental decoding ------------------------------------------------------------------------------------
+    def new_cache(self, batch_size, capacity, dtype=None, device=None) -> DecoderCache:
+        """An empty ``DecoderCache`` for ``batch_size`` sequences of up to ``capacity`` tokens (prompt included).
+        ``capacity <= max_seq_len``: the relative-position table and the future mask end there."""
+        if not self.auto_regressive:
+            raise ValueError("incremental decoding needs an auto-regressive decoder")
+        if capacity > self.max_seq_len:
+            raise ValueError("capacity {} exceeds max_seq_len {}".format(capacity, self.max_seq_len))
+        weight = self.emb_layer_norm.weight
+        heads = self.attention_heads
+        return DecoderCache(len(self.layers), batch_size, capacity, heads, self.embed_dim // heads,
+                            dtype or weight.dtype, device or weight.device)
+
+    def _dropout_active(self):
+        rates = [self.emb_dropout]
+        for layer in self.layers:
+            rates += [layer.dropout, layer.attention_dropout, layer.activation_dropout]
+        return self.training and any(r > 0 for r in rates)
+
+    def _step_rel_pos_bias(self, cache, like):
+        """``[B, H, 1, max_len + 1]``: the relative-position bias row of each sequence's new token, gathered on the
+        device at its position ``seqlens[b]`` (keys past it are not visible)."""
+        if self.rp_bucket.device != like.device:
+            self.rp_bucket = self.rp_bucket.to(like.device)
+        idx = self.rp_bucket[cache.seqlens.long(), : cache.max_len + 1]   # [B, max_len + 1]
+        values = F.embedding(idx, self.relative_attention_bias.weight)   # [B, max_len + 1, H]
+        return values.permute(0, 2, 1).unsqueeze(2).to(like.dtype).contiguous()
+
+    def _forward_cached(self, emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask,
+                        cache):
+        if self._dropout_active():
+            raise RuntimeError("incremental decoding runs without dropout: call eval() or set the dropout rates to 0")
+        if cache.max_len == 0:
+            # prefill: the ordinary path, with every layer storing its keys / values on the way
+            L = emb.size(1)
+            if L > cache.capacity:
+                raise ValueError("the prompt ({} tokens) exceeds the cache capacity {}".format(L, cache.capacity))
+            x = self._embed_prologue(emb, padding_mask)
+            causal = self.auto_regressive and self._fused_attention_capable(x)
+            future_mask = None if causal else self._future(x)
+            attn_bias, key_padding = self._compose_bias(x, attn_mask, padding_mask, future_mask=future_mask)
+            for layer, lc in zip(self.layers, cache.layers):
+                x = layer(x, encoder_out=encoder_out, padding_mask=key_padding, attn_bias=attn_bias,
+                          encoder_padding_mask=encoder_padding_mask, encoder_attn_bias=encoder_attn_mask,
+                          causal=causal, cache=lc)
+            if padding_mask is None:
+                cache.seqlens.fill_(L)
+            else:
+                cache.seqlens.copy_(L - padding_mask.to(torch.int32).sum(1))
+            cache.max_len = L
+        else:
+            if emb.size(1) != 1:
+                raise ValueError("a decoding step takes one token per sequence: emb must be [B, 1, E]")
+            if attn_mask is not None:
+                raise NotImplementedError("attn_mask is not supported on a decoding step")
+            if padding_mask is not None:
+                raise NotImplementedError("padding_mask is not supported on a decoding step")
+            if cache.max_len + 1 > cache.capacity:
+                raise ValueError("the cache is full: capacity {}".format(cache.capacity))
+            x = self._embed_prologue(emb, None)
+            attn_bias = self._step_rel_pos_bias(cache, x) if self.rel_pos else None
+            for layer, lc in zip(self.layers, cache.layers):
+                x = layer(x, encoder_out=encoder_out, attn_bias=attn_bias, encoder_padding_mask=encoder_padding_mask,
+                          encoder_attn_bias=encoder_attn_mask, cache=lc)
+            cache.seqlens += 1
+            cache.max_len += 1
         if self.final_layer_norm is not None:
             x = self.final_layer_norm(x)
         return x

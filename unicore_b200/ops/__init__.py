@@ -2,6 +2,8 @@
 from ._native import HAS_CUDA_EXT, USE_NATIVE, native, use_native  # noqa: F401
 from .attention_ops import (  # noqa: F401
     attention_reference,
+    attention_with_kv_cache,
+    attention_with_kv_cache_reference,
     fused_attention,
     fused_attention_qkvpacked,
     fused_attention_supported,

@@ -23,6 +23,10 @@ mask ``torch.triu(full((Lq, Lk), -inf), 1)``, as the future mask of ``Transforme
 bottom-right convention when ``Lq != Lk``).  It combines with the bias, the key padding mask and dropout.  The kernels
 take it as a flag: no mask tensor is read, and the key tiles above the diagonal are never computed, in the forward or
 the backward pass.  ``causal=True`` with ``return_logits=True`` runs ``attention_reference``.
+
+``attention_with_kv_cache`` is the decoding step: one query per sequence against a ``[B, C, H, D]`` key / value cache,
+optionally appending the new token's key and value first.  It runs in ``csrc/attn/fmha_decode_sm90.cu`` (split-KV,
+fp32 on the CUDA cores) for every head dim the fused kernels take, and has no backward.
 """
 import math
 
@@ -208,3 +212,116 @@ def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0
         return _FusedAttentionPackedFn.apply(qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits,
                                              causal)
     return fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal)
+
+
+def _check_no_grad(*tensors):
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
+        raise RuntimeError("attention_with_kv_cache has no backward: call it under torch.no_grad() or "
+                           "torch.inference_mode(), or detach the inputs")
+
+
+def _visible_bound(C, max_len, append, bias, key_padding_mask):
+    """Host bound on the visible keys of any batch: ``max_len`` (+1 when appending), else ``C``; never more than the
+    columns of the bias and of the key mask (the kernel clamps to them as well)."""
+    bound = C if max_len is None else min(C, int(max_len) + (1 if append else 0))
+    if bias is not None:
+        bound = min(bound, bias.shape[-1])
+    if key_padding_mask is not None:
+        bound = min(bound, key_padding_mask.shape[-1])
+    return bound
+
+
+def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len=None, k_new=None, v_new=None,
+                                      bias=None, key_padding_mask=None, scale=None):
+    """Plain PyTorch implementation of ``attention_with_kv_cache`` (CPU path, fallback and test oracle).
+
+    Performs the append in place like the kernel: row ``seqlens[b]`` (clamped to ``C - 1``) of the caches becomes
+    ``k_new[b] / v_new[b]``.  Keys past the visible length are masked; a row with no visible unmasked key gives 0.
+    """
+    B, _, H, D = q.shape
+    C = k_cache.shape[1]
+    scale = scale if scale is not None else 1.0 / math.sqrt(D)
+    append = k_new is not None
+    if append:
+        if seqlens is None:
+            raise ValueError("appending needs seqlens (the row to write)")
+        pos = seqlens.long().clamp(0, C - 1)
+        rows = torch.arange(B, device=k_cache.device)
+        k_cache[rows, pos] = k_new[:, 0].to(k_cache.dtype)
+        v_cache[rows, pos] = v_new[:, 0].to(v_cache.dtype)
+        n = pos + 1
+    elif seqlens is not None:
+        n = seqlens.long().clamp(0, C)
+    else:
+        n = torch.full((B,), C, dtype=torch.long, device=q.device)
+    K = _visible_bound(C, max_len if seqlens is not None else None, append, bias, key_padding_mask)
+    k, v = k_cache[:, :K], v_cache[:, :K]
+    scores = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale   # [B, H, 1, K]
+    if bias is not None:
+        scores = scores + bias[..., :K].to(scores.dtype)
+    hidden = torch.arange(K, device=q.device)[None, :] >= n.to(q.device)[:, None]   # [B, K]
+    # rows past the visible length are never read by the kernel: whatever they hold (NaN included) must not matter
+    v = v.masked_fill(hidden[:, :, None, None], 0)
+    if key_padding_mask is not None:
+        hidden = hidden | key_padding_mask[:, :K].to(torch.bool)
+    scores = scores.masked_fill(hidden[:, None, None, :], float("-inf"))
+    probs = torch.nan_to_num(F.softmax(scores.float(), dim=-1), nan=0.0).to(q.dtype)   # all masked -> 0
+    return torch.einsum("bhqk,bkhd->bqhd", probs, v)
+
+
+def _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask) -> bool:
+    if not use_native(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask) \
+            or not hasattr(native(), "fmha_decode"):
+        return False
+    if q.dim() != 4 or q.shape[1] != 1 or q.dtype not in (torch.float16, torch.bfloat16):
+        return False
+    if not fused_head_dim_supported(q.shape[-1]):
+        return False
+    for t in (q, k_cache, v_cache, k_new, v_new):
+        if t is None:
+            continue
+        if t.dim() != 4 or t.dtype != q.dtype or t.shape[-1] != q.shape[-1] or t.stride(-1) != 1:
+            return False
+        if t.data_ptr() % 16 != 0 or any(s % 8 != 0 for s in t.stride()[:3]):
+            return False
+    if bias is not None and bias.stride(-1) != 1 and bias.shape[-1] > 1:
+        return False
+    return True
+
+
+def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_new=None, v_new=None, bias=None,
+                            key_padding_mask=None, scale=None):
+    """One decoding step of attention against a key / value cache.
+
+    q: ``[B, 1, H, D]``; k_cache / v_cache: ``[B, C, H, D]`` (strided views are fine, the last dim contiguous).
+    The visible keys of batch b are rows ``0 .. seqlens[b] - 1``, plus row ``seqlens[b]`` when appending; with
+    ``seqlens=None`` all C rows are (cross-attention).  ``k_new`` / ``v_new`` ``[B, 1, H, D]``: the new token's key
+    and value, written bitwise into row ``seqlens[b]`` of the caches before the attention (needs ``seqlens``).
+    ``max_len``: a host-side upper bound on ``seqlens`` (default: the most the capacity allows); the device lengths are
+    never read on the host, so a step does not synchronise.  bias: ``[1|B, H, 1, Lb]``, ``Lb`` covering the visible
+    keys (columns past them are ignored); key_padding_mask: bool ``[B, Lk]``, True = masked.  A row whose visible keys
+    are all masked gives 0.  Returns ``[B, 1, H, D]``.  No dropout and no backward."""
+    _check_no_grad(q, k_cache, v_cache, k_new, v_new, bias)
+    append = k_new is not None
+    if append != (v_new is not None):
+        raise ValueError("k_new and v_new go together")
+    if append and seqlens is None:
+        raise ValueError("appending needs seqlens (the row to write)")
+    C = k_cache.shape[1]
+    if scale is None:
+        scale = 1.0 / math.sqrt(q.shape[-1])
+    if seqlens is not None and max_len is None:
+        max_len = C - (1 if append else 0)
+    if max_len is not None and int(max_len) + (1 if append else 0) > C:
+        raise ValueError("max_len {} {}exceeds the cache capacity {}".format(max_len, "+ 1 " if append else "", C))
+    if not _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask):
+        return attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
+                                                 key_padding_mask, scale)
+    if seqlens is not None and (seqlens.dtype != torch.int32 or not seqlens.is_contiguous()):
+        seqlens = seqlens.to(torch.int32).contiguous()
+    if bias is not None and (bias.dtype != q.dtype or bias.stride(-1) != 1):
+        bias = bias.to(q.dtype).contiguous()
+    if key_padding_mask is not None and (key_padding_mask.dtype != torch.bool or key_padding_mask.stride(-1) != 1):
+        key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
+    return native().fmha_decode(q, k_cache, v_cache, seqlens, 0 if max_len is None else int(max_len), k_new, v_new,
+                                bias, key_padding_mask, float(scale))
