@@ -120,6 +120,16 @@ void launch_softmax_dropout_bwd(const void* dy, void* dx, const void* probs, lon
                                 const float* lse = nullptr, const void* addend = nullptr);
 
 // ---- fused element-wise ---------------------------------------------------------------------------------------
+// Launch plan of bias_gelu fwd / bwd and column_sum (the launchers run exactly this plan): a grid of (col_blocks,
+// slices) CTAs.  A thread owns one 16-byte column vector (nvec per row, 128 per column block: the last block is
+// partial unless nvec % 128 == 0) in one of a CTA's two row lanes, and walks the rows of its (slice, lane) in groups
+// of 4; one pass of every slice over its rows covers rows_per_sweep rows, `sweeps` passes cover all rows.  `fwd`:
+// the plan of bias_gelu's forward, else the one of its backward and of column_sum.
+struct ColumnPlan {
+  int nvec, col_blocks, slices;
+  long long rows_per_sweep, sweeps;
+};
+ColumnPlan bias_gelu_plan(long long rows, int cols, bool fwd);
 void launch_bias_gelu_fwd(const void* x, const void* bias, void* y, long long rows, int cols, int dtype,
                           cudaStream_t stream);
 // dbias (nullable) = column sums of dx; part = float[bias_gelu_parts(rows, cols) * cols] scratch
@@ -170,6 +180,15 @@ void launch_embedding_bwd_sorted(const void* dy, const long long* sorted, const 
 
 void launch_gbf_fwd(const void* d, const long long* edge, const void* mul_w, const void* bias_w, const void* means,
                     const void* stds, void* y, long long n, int K, int dtype, cudaStream_t stream);
+// Launch plan of the Gaussian-basis kernels: `grid` CTAs of 256 threads, a row of K outputs per kvec = K / 8 threads
+// (rows_per_cta rows per CTA), grid-stride over the rows in `sweeps` passes of rows_per_sweep rows.  The backward's
+// shared memory (histogram of E edge types + 2K column sums) is `smem` bytes, above 48 KB it needs the opt-in.
+struct GbfPlan {
+  int grid, kvec, rows_per_cta;
+  long long rows_per_sweep, sweeps;
+  int smem;
+};
+GbfPlan gbf_plan(long long n, int K, int E);
 // part: float[gbf_parts(n, K)][2 * K] per-CTA partial (d mean, d std); hist: float[2 * E] zero-initialised (d mul, d bias)
 int gbf_parts(long long n, int K);
 void launch_gbf_bwd(const void* dy, const void* d, const long long* edge, const void* mul_w, const void* bias_w,

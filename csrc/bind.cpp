@@ -354,6 +354,34 @@ pybind11::dict softmax_plan(int64_t rows, int64_t K, at::ScalarType dtype, bool 
   return d;
 }
 
+// bias_gelu's forward (kind "fwd"), or its backward and column_sum (kind "bwd")
+pybind11::dict bias_gelu_plan(int64_t rows, int64_t cols, const std::string& kind) {
+  TORCH_CHECK(kind == "fwd" || kind == "bwd", "kind must be fwd or bwd (the backward and column_sum)");
+  TORCH_CHECK(rows >= 1 && cols > 0 && cols % 8 == 0, "bias_gelu_plan needs rows >= 1 and a positive multiple of 8 columns");
+  const ub::ColumnPlan p = ub::bias_gelu_plan(rows, (int)cols, kind == "fwd");
+  pybind11::dict d;
+  d["nvec"] = p.nvec;
+  d["col_blocks"] = p.col_blocks;
+  d["slices"] = p.slices;
+  d["rows_per_sweep"] = p.rows_per_sweep;
+  d["sweeps"] = p.sweeps;
+  return d;
+}
+
+pybind11::dict gbf_plan(int64_t n, int64_t K, int64_t E) {
+  TORCH_CHECK(n >= 1 && K % 8 == 0 && K / 8 >= 1 && K / 8 <= 32 && ((K / 8) & (K / 8 - 1)) == 0 && E >= 1 && E <= 8192,
+              "gbf_plan needs n >= 1, K = 8 * 2^i <= 256 and 1 <= E <= 8192");
+  const ub::GbfPlan p = ub::gbf_plan(n, (int)K, (int)E);
+  pybind11::dict d;
+  d["grid"] = p.grid;
+  d["kvec"] = p.kvec;
+  d["rows_per_cta"] = p.rows_per_cta;
+  d["rows_per_sweep"] = p.rows_per_sweep;
+  d["sweeps"] = p.sweeps;
+  d["smem"] = p.smem;
+  return d;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // softmax + dropout
 // ---------------------------------------------------------------------------------------------------
@@ -467,11 +495,25 @@ Tensor softmax_dropout_bwd(Tensor dy, const Tensor& probs, double p, int64_t see
 // ---------------------------------------------------------------------------------------------------
 // fused element-wise
 // ---------------------------------------------------------------------------------------------------
-Tensor bias_gelu_fwd(const Tensor& x, const OptTensor& bias) {
+// The bias + GELU kernels read x, dy and the bias as 16-byte vectors of 8 elements from the first element on.
+static int check_bias_gelu_operands(const Tensor& x, const OptTensor& bias) {
   check_cuda_contig(x, "x");
-  const c10::cuda::CUDAGuard guard(x.device());
+  TORCH_CHECK(x.scalar_type() == at::kHalf || x.scalar_type() == at::kBFloat16, "bias_gelu supports fp16 / bf16");
+  TORCH_CHECK(x.dim() >= 1 && x.size(-1) > 0 && x.size(-1) % 8 == 0, "bias_gelu needs a positive multiple of 8 columns");
   const int cols = (int)x.size(-1);
-  TORCH_CHECK(cols % 8 == 0 && (x.scalar_type() == at::kHalf || x.scalar_type() == at::kBFloat16));
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(x.data_ptr()) & 15) == 0, "bias_gelu: x must be 16-byte aligned");
+  if (bias.has_value() && bias->defined()) {
+    check_cuda_contig(*bias, "bias");
+    TORCH_CHECK(bias->scalar_type() == x.scalar_type() && bias->numel() == cols,
+                "bias_gelu: bias must have the dtype of x and one element per column");
+    TORCH_CHECK((reinterpret_cast<uintptr_t>(bias->data_ptr()) & 15) == 0, "bias_gelu: bias must be 16-byte aligned");
+  }
+  return cols;
+}
+
+Tensor bias_gelu_fwd(const Tensor& x, const OptTensor& bias) {
+  const int cols = check_bias_gelu_operands(x, bias);
+  const c10::cuda::CUDAGuard guard(x.device());
   Tensor y = torch::empty_like(x);
   ub::launch_bias_gelu_fwd(x.data_ptr(), opt_ptr(bias), y.data_ptr(), x.numel() / cols, cols, dtype_tag(x),
                            cur_stream());
@@ -482,10 +524,11 @@ Tensor bias_gelu_fwd(const Tensor& x, const OptTensor& bias) {
 // returns (dx, dbias); dbias (column sums of dx, produced by the same pass) only when a bias was given
 std::tuple<Tensor, OptTensor> bias_gelu_bwd(const Tensor& dy, const Tensor& x, const OptTensor& bias,
                                             const OptTensor& dbias_sink) {
+  const int cols = check_bias_gelu_operands(x, bias);
   check_cuda_contig(dy, "dy");
-  check_cuda_contig(x, "x");
+  TORCH_CHECK(dy.sizes() == x.sizes() && dy.scalar_type() == x.scalar_type(), "bias_gelu_bwd: dy must match x");
+  TORCH_CHECK((reinterpret_cast<uintptr_t>(dy.data_ptr()) & 15) == 0, "bias_gelu_bwd: dy must be 16-byte aligned");
   const c10::cuda::CUDAGuard guard(x.device());
-  const int cols = (int)x.size(-1);
   const long long rows = x.numel() / cols;
   Tensor dx = torch::empty_like(x);
   OptTensor dbias;
@@ -862,6 +905,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("norm_plan", &norm_plan, pybind11::arg("rows"), pybind11::arg("cols"), pybind11::arg("dtype"), pybind11::arg("kind"));
   m.def("softmax_plan", &softmax_plan, pybind11::arg("rows"), pybind11::arg("K"), pybind11::arg("dtype"),
         pybind11::arg("aligned") = true, pybind11::arg("kind") = "fwd");
+  m.def("bias_gelu_plan", &bias_gelu_plan, pybind11::arg("rows"), pybind11::arg("cols"), pybind11::arg("kind"));
+  m.def("gbf_plan", &gbf_plan, pybind11::arg("n"), pybind11::arg("K"), pybind11::arg("E"));
   m.def("softmax_dropout_fwd", &softmax_dropout_fwd);
   m.def("softmax_dropout_bwd", &softmax_dropout_bwd);
   m.def("softmax_dropout_logits_fwd", &softmax_dropout_logits_fwd);

@@ -27,10 +27,13 @@ static int sm_count3() {
 //
 // exact (erf) GELU = x * Phi(x).  CUDA's erff costs ~40 issued instructions per element, which made
 // the first version of this kernel issue-bound at 2x its HBM time.  Phi is evaluated instead with
-// the classic 5-term rational/exponential form (Abramowitz-Stegun 26.2.17, |error| < 7.5e-8, far
-// below 16-bit output resolution), on element pairs (common.cuh F2):
+// the classic 5-term rational/exponential form (Abramowitz-Stegun 26.2.17), on element pairs (common.cuh F2):
 //   t = 1 / (1 + 0.2316419 |x|),  pdf = exp(-x^2/2) / sqrt(2 pi),
-//   Q = pdf * t (b1 + t (b2 + t (b3 + t (b4 + t b5)))),  Phi(x) = 0.5 + copysign(0.5 - Q, x).
+//   Q = pdf * t (b1 + t (b2 + t (b3 + t (b4 + t b5)))),  Phi(x) = 1 - Q for x >= 0,  Q for x < 0.
+// The formula's absolute error is < 7.5e-8, but GELU's negative tail is far smaller than that in
+// absolute terms, so what matters there is the relative error of Q: 0.16 % at x = -5, 0.36 % at -6,
+// 1.0 % at -8, 3.7 % at -13 (under one bf16 ulp down to -6; |GELU| < 5e-15 below -8).  Forming the
+// tail as 0.5 - (0.5 - Q) instead cancels to an absolute fp32 error of ~2^-25 and returns 0 for x < -5.75.
 // Layout: a thread owns one 8-wide column vector (its bias slice lives in registers) and walks
 // rows; the backward also accumulates the bias gradient (column sums of dx) in registers, so no
 // separate reduction pass over dx is needed.
@@ -58,8 +61,9 @@ UB_DEVICE PhiPdf normal_cdf_pdf2(F2 x) {
   r.pdf = mul2(e, f2(0.39894228040143267794f));
   const F2 q = mul2(r.pdf, poly);                      // upper tail of |x|, in (0, 0.5]
   const F2 d = fma2(q, f2(-1.f), f2(0.5f));             // 0.5 - Q >= 0
-  const F2 ds = f2_from_bits(f2_bits(d) | (xb & 0x8000000080000000ull));
-  r.phi = add2(ds, f2(0.5f));
+  const F2 p = add2(d, f2(0.5f));                       // x >= 0: 1 - Q
+  r.phi.x = x.x < 0.f ? q.x : p.x;                       // x < 0: Q itself (see above)
+  r.phi.y = x.y < 0.f ? q.y : p.y;
   return r;
 }
 
@@ -218,33 +222,42 @@ __global__ void __launch_bounds__(256) column_sum_kernel(const T* __restrict__ x
   }
 }
 
-int bias_gelu_parts(long long rows, int cols) {
-  const int col_blocks = (cols / 8 + kGeluColsPerCta - 1) / kGeluColsPerCta;
-  long long slices = ((long long)sm_count3() * 6 + col_blocks - 1) / col_blocks;
+ColumnPlan bias_gelu_plan(long long rows, int cols, bool fwd) {
+  ColumnPlan p;
+  p.nvec = cols / 8;
+  p.col_blocks = (p.nvec + kGeluColsPerCta - 1) / kGeluColsPerCta;
+  // The forward fits 5 CTAs per SM (48 registers): a grid of 16 CTAs per SM keeps the tail of the last wave short
+  // (with 6, the 32 x 512 x 3072 fp16 forward ran 1.2 waves in 92 us, with 16 in 76 us: H100 80GB HBM3, 400 W limit).
+  // The backward and the column sum keep 6 per SM: each slice adds a partial row to the final column pass.
+  long long slices = ((long long)sm_count3() * (fwd ? 16 : 6) + p.col_blocks - 1) / p.col_blocks;
   const long long max_slices = (rows + 2 * kGeluUnroll - 1) / (2 * kGeluUnroll);
   if (slices > max_slices) slices = max_slices;
-  return (int)(slices < 1 ? 1 : slices);
+  p.slices = (int)(slices < 1 ? 1 : slices);
+  p.rows_per_sweep = 2LL * kGeluUnroll * p.slices;
+  p.sweeps = (rows + p.rows_per_sweep - 1) / p.rows_per_sweep;
+  return p;
 }
+
+int bias_gelu_parts(long long rows, int cols) { return bias_gelu_plan(rows, cols, false).slices; }
 
 template <typename T, bool kBwd>
 static void run_bias_gelu_t(const void* dy, const void* x, const void* bias, void* out, void* dbias, float* part,
                             long long rows, int cols, cudaStream_t stream, int accumulate = 0) {
-  const int nvec = cols / 8;
-  const int slices = bias_gelu_parts(rows, cols);
-  dim3 grid((nvec + kGeluColsPerCta - 1) / kGeluColsPerCta, slices);
+  const ColumnPlan p = bias_gelu_plan(rows, cols, !kBwd);
+  dim3 grid(p.col_blocks, p.slices);
   const bool want = kBwd && dbias != nullptr && part != nullptr;
   bias_gelu_kernel<T, kBwd><<<grid, 256, 0, stream>>>((const T*)dy, (const T*)x, (const T*)bias, (T*)out,
-                                                      want ? part : nullptr, (int)rows, nvec);
-  if (want) colsum_kernel<T><<<(cols + 31) / 32, 1024, 0, stream>>>(part, slices, cols, (T*)dbias, accumulate);
+                                                      want ? part : nullptr, (int)rows, p.nvec);
+  if (want) colsum_kernel<T><<<(cols + 31) / 32, 1024, 0, stream>>>(part, p.slices, cols, (T*)dbias, accumulate);
 }
 
 // out[cols] = column sums of x[rows, cols]; part = float[bias_gelu_parts(rows, cols) * cols] scratch
 void launch_column_sum(const void* x, void* out, float* part, long long rows, int cols, int dtype, cudaStream_t stream,
                        int accumulate) {
   if (rows <= 0 || cols <= 0) return;
-  const int nvec = cols / 8;
-  const int slices = bias_gelu_parts(rows, cols);
-  dim3 grid((nvec + kGeluColsPerCta - 1) / kGeluColsPerCta, slices);
+  const ColumnPlan p = bias_gelu_plan(rows, cols, false);
+  const int nvec = p.nvec, slices = p.slices;
+  dim3 grid(p.col_blocks, slices);
   if (dtype == kF16) {
     column_sum_kernel<__half><<<grid, 256, 0, stream>>>((const __half*)x, part, (int)rows, nvec);
     colsum_kernel<__half><<<(cols + 31) / 32, 1024, 0, stream>>>(part, slices, cols, (__half*)out, accumulate);
@@ -287,6 +300,18 @@ UB_DEVICE void online_merge(float& m, float& s, float m2, float s2) {
   m = mn;
 }
 
+// The exponentials of the online sum are taken relative to the running max, or to 0 while that max is -inf (every
+// element seen so far is -inf): exp(-inf - -inf) would be NaN, and a row with masked (-inf) logits is ordinary input.
+// The state then stays (-inf, 0), as in online_merge; a NaN element still makes the sum NaN.
+UB_DEVICE float online_ref(float mn) { return mn == -CUDART_INF_F ? 0.f : mn; }
+
+UB_DEVICE void online_add(float& m, float& s, float v) {
+  const float mn = fmaxf(m, v);
+  const float r = online_ref(mn);
+  s = s * __expf(m - r) + __expf(v - r);
+  m = mn;
+}
+
 template <typename T>
 UB_DEVICE void row_max_sum(const T* row, int cols, float& m, float& s) {
   // per-thread online softmax statistics, widest aligned access that the row start allows
@@ -298,12 +323,7 @@ UB_DEVICE void row_max_sum(const T* row, int cols, float& m, float& s) {
   if (head > cols) head = cols;
   const int nvec = (cols - head) / EPV;
   const int tail_begin = head + nvec * EPV;
-  for (int c = threadIdx.x; c < head; c += blockDim.x) {
-    const float v = to_f32<T>(row[c]);
-    const float mn = fmaxf(m, v);
-    s = s * __expf(m - mn) + __expf(v - mn);
-    m = mn;
-  }
+  for (int c = threadIdx.x; c < head; c += blockDim.x) online_add(m, s, to_f32<T>(row[c]));
   for (int vi = threadIdx.x; vi < nvec; vi += blockDim.x) {
     float xs[EPV];
     unpack<T>(ld_global_nc_v4(row + head + vi * EPV), xs);
@@ -311,18 +331,14 @@ UB_DEVICE void row_max_sum(const T* row, int cols, float& m, float& s) {
 #pragma unroll
     for (int e = 1; e < EPV; ++e) lm = fmaxf(lm, xs[e]);
     const float mn = fmaxf(m, lm);
+    const float r = online_ref(mn);
     float acc = 0.f;
 #pragma unroll
-    for (int e = 0; e < EPV; ++e) acc += __expf(xs[e] - mn);
-    s = s * __expf(m - mn) + acc;
+    for (int e = 0; e < EPV; ++e) acc += __expf(xs[e] - r);
+    s = s * __expf(m - r) + acc;
     m = mn;
   }
-  for (int c = tail_begin + threadIdx.x; c < cols; c += blockDim.x) {
-    const float v = to_f32<T>(row[c]);
-    const float mn = fmaxf(m, v);
-    s = s * __expf(m - mn) + __expf(v - mn);
-    m = mn;
-  }
+  for (int c = tail_begin + threadIdx.x; c < cols; c += blockDim.x) online_add(m, s, to_f32<T>(row[c]));
 }
 
 template <typename T>

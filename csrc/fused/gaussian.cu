@@ -197,15 +197,23 @@ __global__ void __launch_bounds__(kGbfSumThreads) gbf_edge_sum_kernel(const floa
   }
 }
 
-static int gbf_grid(long long n, int K) {
+GbfPlan gbf_plan(long long n, int K, int E) {
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int rows_per_cta = kGbfThreads / (K / 8);
-  const long long need = (n + rows_per_cta - 1) / rows_per_cta;
+  GbfPlan p;
+  p.kvec = K / 8;
+  p.rows_per_cta = kGbfThreads / p.kvec;
+  const long long need = (n + p.rows_per_cta - 1) / p.rows_per_cta;
   const long long cap = (long long)sms * 4;
-  return (int)(need < cap ? (need < 1 ? 1 : need) : cap);
+  p.grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
+  p.rows_per_sweep = (long long)p.grid * p.rows_per_cta;
+  p.sweeps = (n + p.rows_per_sweep - 1) / p.rows_per_sweep;
+  p.smem = (2 * E + 2 * K) * (int)sizeof(float);
+  return p;
 }
+
+static int gbf_grid(long long n, int K) { return gbf_plan(n, K, 0).grid; }
 
 int gbf_parts(long long n, int K) { return gbf_grid(n, K); }
 
@@ -227,8 +235,9 @@ void launch_gbf_bwd(const void* dy, const void* d, const long long* edge, const 
                     const void* means, const void* stds, float* part, float* hist, long long n, int K, int E, int dtype,
                     cudaStream_t stream) {
   if (n <= 0) return;
-  const int grid = gbf_grid(n, K);
-  const size_t smem = (size_t)(2 * E + 2 * K) * sizeof(float);
+  const GbfPlan plan = gbf_plan(n, K, E);
+  const int grid = plan.grid;
+  const size_t smem = (size_t)plan.smem;
   if (dtype == kF16) {
     auto kern = gbf_bwd_kernel<__half>;
     if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -36,7 +36,7 @@ class _BiasGeluFn(torch.autograd.Function):
     def backward(ctx, dy):
         x, bias = ctx.saved_tensors
         claimed = ctx.bias_sink
-        dx, dbias = native().bias_gelu_bwd(dy.contiguous(), x, bias, grad_sink.sink(claimed))
+        dx, dbias = native().bias_gelu_bwd(aligned_param(dy), x, bias, grad_sink.sink(claimed))
         if claimed is not None:  # the bias gradient went straight into the arena
             grad_sink.done(claimed)
             dbias = None
@@ -44,8 +44,10 @@ class _BiasGeluFn(torch.autograd.Function):
 
 
 def bias_gelu(x: torch.Tensor, bias: Optional[torch.Tensor]) -> torch.Tensor:
-    if use_native(x, bias) and x.dtype in (torch.float16, torch.bfloat16) and x.is_contiguous() and x.shape[-1] % 8 == 0:
-        return _BiasGeluFn.apply(x, aligned_param(bias, x.dtype))
+    if use_native(x, bias) and x.dtype in (torch.float16, torch.bfloat16) and x.is_contiguous() and x.shape[-1] % 8 == 0 \
+            and x.numel() > 0:
+        # the kernels read 16-byte vectors: a view at an odd element offset is copied once (aligned_param)
+        return _BiasGeluFn.apply(aligned_param(x), aligned_param(bias, x.dtype))
     return F.gelu(x + bias if bias is not None else x)
 
 
