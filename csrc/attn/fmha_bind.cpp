@@ -1,48 +1,38 @@
 // PyTorch bindings of the fused attention kernels.
-#include <ATen/cuda/CUDAContext.h>
-#include <ATen/cuda/CUDAGeneratorImpl.h>
 #include <c10/cuda/CUDAGuard.h>
-#include <torch/extension.h>
 
-#include <cstdio>
-#include <cstdlib>
-#include <mutex>
-#include <optional>
-
+#include "../bind_util.h"
 #include "fmha_api.h"
 #include "tma_map.h"
 
 namespace {
-using torch::Tensor;
-using OptTensor = std::optional<Tensor>;
+using namespace ub_bind;
 
-std::pair<uint64_t, uint64_t> reserve_philox(uint64_t increment) {
-  auto gen = at::get_generator_or_default<at::CUDAGeneratorImpl>(std::nullopt,
-                                                                 at::cuda::detail::getDefaultCUDAGenerator());
-  std::lock_guard<std::mutex> lock(gen->mutex_);
-  at::PhiloxCudaState st = gen->philox_cuda_state(increment);
-  TORCH_CHECK(!st.captured_, "fmha: RNG under CUDA graph capture is not supported yet");
-  return {st.seed_.val, st.offset_.val};
-}
-
-void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const Tensor& v, const OptTensor& bias,
-                 const OptTensor& kpm, double p_drop, double scale, bool forward) {
-  TORCH_CHECK(q.is_cuda() && k.is_cuda() && v.is_cuda());
-  TORCH_CHECK(q.dim() == 4 && k.dim() == 4 && v.dim() == 4, "q/k/v must be [B, L, H, D]");
-  const int64_t D = q.size(3);
+// q / k / v [B, L, H, D] (heads contiguous, strides that are multiples of 8 elements), bias [1|B, H, Lq, Lk] and the
+// bool key_padding_mask [B, Lk]: what the TMA tile maps of fill_common need.
+void check_common(const Tensor& q, const Tensor& k, const Tensor& v, const OptTensor& bias, const OptTensor& kpm) {
+  check_operand(q, "q", q.device(), k16Bit, any_shape(4), kAligned);
+  check_operand(k, "k", q.device(), {q.scalar_type()}, any_shape(4), kAligned);
+  check_operand(v, "v", q.device(), {q.scalar_type()}, any_shape(4), kAligned);
+  const int64_t B = q.size(0), Lq = q.size(1), H = q.size(2), D = q.size(3), Lk = k.size(1);
   TORCH_CHECK(ub::fmha_head_dim_supported(D) && k.size(3) == D && v.size(3) == D,
               "head_dim must be the same for q/k/v and a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
-  TORCH_CHECK(q.stride(3) == 1 && k.stride(3) == 1 && v.stride(3) == 1, "last dim must be contiguous");
-  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16);
-  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type());
-  TORCH_CHECK(k.size(0) == q.size(0) && v.size(0) == q.size(0) && k.size(2) == q.size(2) && v.size(2) == q.size(2));
-  TORCH_CHECK(k.size(1) == v.size(1));
-  TORCH_CHECK(q.size(1) % 8 == 0 && k.size(1) % 8 == 0, "sequence lengths must be multiples of 8");
+  TORCH_CHECK(k.size(0) == B && v.size(0) == B && k.size(2) == H && v.size(2) == H && v.size(1) == Lk,
+              "k / v must be [B, Lk, H, D] with the B, H and D of q");
+  TORCH_CHECK(Lq % 8 == 0 && Lk % 8 == 0, "sequence lengths must be multiples of 8");
   for (const Tensor* t : {&q, &k, &v}) {
-    TORCH_CHECK(t->stride(0) % 8 == 0 && t->stride(1) % 8 == 0 && t->stride(2) % 8 == 0 &&
-                    (reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0,
-                "q/k/v must be 16-byte aligned with strides that are multiples of 8 elements");
+    // TMA descriptors: heads must be contiguous (stride D) so that (head, 16-byte chunk) is one dimension
+    TORCH_CHECK(t->stride(3) == 1 && t->stride(2) == D, "q/k/v head stride must be head_dim");
+    TORCH_CHECK(t->stride(0) % 8 == 0 && t->stride(1) % 8 == 0, "q/k/v strides must be multiples of 8 elements");
   }
+  check_operand(bias, "bias", q.device(), {q.scalar_type()}, {kAnySize, H, Lq, Lk}, kVec);
+  TORCH_CHECK(!has(bias) || bias->size(0) == 1 || bias->size(0) == B, "bias must be [1|B, H, Lq, Lk]");
+  check_operand(kpm, "key_padding_mask", q.device(), {at::kBool}, {B, Lk});
+}
+
+// The parameters and TMA tile maps of operands check_common accepted.
+void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const Tensor& v, const OptTensor& bias,
+                 const OptTensor& kpm, double p_drop, double scale, bool forward) {
   p.q = q.data_ptr();
   p.k = k.data_ptr();
   p.v = v.data_ptr();
@@ -53,34 +43,18 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   p.Lq = (int)q.size(1);
   p.H = (int)q.size(2);
   p.Lk = (int)k.size(1);
-  p.D = (int)D;
+  p.D = (int)q.size(3);
   p.is_bf16 = q.scalar_type() == at::kBFloat16 ? 1 : 0;
-  p.bias = nullptr;
-  p.bias_batch = 1;
+  p.bias = has(bias) ? bias->data_ptr() : nullptr;
+  p.bias_batch = has(bias) ? (int)bias->size(0) : 1;
   p.bias_is_f32 = 0;
-  if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->is_cuda() && bias->is_contiguous() && bias->dim() == 4);
-    TORCH_CHECK((bias->size(0) == 1 || bias->size(0) == p.B) && bias->size(1) == p.H && bias->size(2) == p.Lq &&
-                bias->size(3) == p.Lk, "bias must be [1|B, H, Lq, Lk]");
-    TORCH_CHECK(bias->scalar_type() == q.scalar_type(), "bias must have the dtype of q");
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(bias->data_ptr()) & 15) == 0, "bias must be 16-byte aligned");
-    p.bias = bias->data_ptr();
-    p.bias_batch = (int)bias->size(0);
-  }
   p.drop_bits = nullptr;
-  p.kpm = nullptr;
-  if (kpm.has_value() && kpm->defined()) {
-    TORCH_CHECK(kpm->is_cuda() && kpm->is_contiguous() && kpm->scalar_type() == at::kBool && kpm->dim() == 2 &&
-                kpm->size(0) == p.B && kpm->size(1) == p.Lk, "key_padding_mask must be bool [B, Lk]");
-    p.kpm = reinterpret_cast<const uint8_t*>(kpm->data_ptr());
-  }
+  p.kpm = static_cast<const uint8_t*>(opt_ptr(kpm));
   p.p_drop = (float)p_drop;
   p.scale = (float)scale;
   // The driver API behind cuTensorMapEncodeTiled needs a current context in THIS thread; autograd worker
   // threads only have the c10 device guard's notion of the device, so bind the primary context explicitly.
   cudaSetDevice(q.get_device());
-  // TMA descriptors: heads must be contiguous (stride D) so that (head, 16-byte chunk) is one dimension
-  TORCH_CHECK(q.stride(2) == D && k.stride(2) == D && v.stride(2) == D, "q/k/v head stride must be head_dim");
   const bool bf16 = p.is_bf16 != 0;
   const int q_box_rows = forward ? ub::kFwdQBoxRows : ub::kBwdBoxRows;
   const int kv_box_rows = forward ? ub::fmha_fwd_kv_box_rows(p.D) : ub::kBwdBoxRows;
@@ -96,6 +70,7 @@ std::tuple<Tensor, Tensor, OptTensor, OptTensor> fwd_impl(const Tensor& q, const
                                                           const OptTensor& bias, const OptTensor& kpm, double p_drop,
                                                           double scale, bool logits, bool causal) {
   TORCH_CHECK(!(logits && causal), "fmha: causal attention does not return logits");
+  check_common(q, k, v, bias, kpm);
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaFwdParams p{};
   fill_common(p, q, k, v, bias, kpm, p_drop, scale, /*forward=*/true);
@@ -115,16 +90,13 @@ std::tuple<Tensor, Tensor, OptTensor, OptTensor> fwd_impl(const Tensor& q, const
   p.seed = p.offset = 0;
   OptTensor bits;
   if (p_drop > 0.0) {
-    auto so = reserve_philox(4);
-    p.seed = so.first;
-    p.offset = so.second;
+    std::tie(p.seed, p.offset) = philox_reserve(4);
     // 1 keep-bit per (query, key): 1/16 of the size of a 16-bit score tensor
     bits = torch::empty({p.B, p.H, p.Lq, (p.Lk + 31) / 32}, q.options().dtype(at::kInt));
     p.drop_bits = reinterpret_cast<uint32_t*>(bits->data_ptr());
   }
-  ub::launch_fmha_fwd(p, at::cuda::getCurrentCUDAStream().stream());
-  cudaError_t err = cudaGetLastError();
-  TORCH_CHECK(err == cudaSuccess, "fmha_fwd launch failed: ", cudaGetErrorString(err));
+  ub::launch_fmha_fwd(p, cur_stream());
+  check_launch("fmha_fwd");
   return {out, lse, bits, z};
 }
 
@@ -155,23 +127,25 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   // spares autograd three zero-filled select-backward tensors and two full-size adds per layer.
   // dlogits: gradient of the logits output of fmha_fwd_logits, [B, H, Lq, Lk]; None means zero.
   // causal: the backward of fmha_fwd(..., causal=True); its keep bits cover only the key tiles that forward walked.
-  const bool has_dlogits = dlogits.has_value() && dlogits->defined();
-  TORCH_CHECK(!(causal && has_dlogits), "fmha_bwd: causal attention has no logits output, so dlogits must be None");
+  TORCH_CHECK(!(causal && has(dlogits)), "fmha_bwd: causal attention has no logits output, so dlogits must be None");
+  check_common(q, k, v, bias, kpm);
+  const int64_t B = q.size(0), Lq = q.size(1), H = q.size(2), Lk = k.size(1);
+  // dO is read through a TMA tile map, so it is kVec like dlogits
+  check_operand(dout, "dout", q.device(), {q.scalar_type()}, q.sizes(), kVec);
+  check_operand(out, "out", q.device(), {q.scalar_type()}, q.sizes());
+  check_operand(lse, "lse", q.device(), {at::kFloat}, {B, H, Lq});
+  TORCH_CHECK(p_drop <= 0.0 || has(drop_bits), "dropout bits missing");
+  if (p_drop > 0.0) check_operand(drop_bits, "drop_bits", q.device(), {at::kInt}, {B, H, Lq, (Lk + 31) / 32});
+  check_operand(dlogits, "dlogits", q.device(), {q.scalar_type()}, {B, H, Lq, Lk}, kVec);
+  TORCH_CHECK(!packed_grad || Lq == Lk, "packed gradients need self-attention shapes");
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaBwdParams p{};
   fill_common(p.f, q, k, v, bias, kpm, p_drop, scale, /*forward=*/false);
   p.f.causal = causal ? 1 : 0;
   const int D = p.f.D;
-  TORCH_CHECK(dout.is_contiguous() && out.is_contiguous() && lse.is_contiguous());
-  TORCH_CHECK(dout.dim() == 4 && dout.size(0) == p.f.B && dout.size(1) == p.f.Lq && dout.size(2) == p.f.H &&
-                  dout.size(3) == D && out.sizes() == dout.sizes(),
-              "dout / out must be [B, Lq, H, D]");
   p.f.out = out.data_ptr();
   p.f.lse = lse.data_ptr<float>();
-  if (p_drop > 0.0) {
-    TORCH_CHECK(drop_bits.has_value() && drop_bits->defined() && drop_bits->is_contiguous(), "dropout bits missing");
-    p.f.drop_bits = reinterpret_cast<uint32_t*>(drop_bits->data_ptr());
-  }
+  if (p_drop > 0.0) p.f.drop_bits = reinterpret_cast<uint32_t*>(drop_bits->data_ptr());
   p.dout = dout.data_ptr();
   TORCH_CHECK(ub::make_head_tile_map_sw128(&p.sw_do, p.dout, p.f.is_bf16 != 0, p.f.B, p.f.Lq, p.f.H, D,
                                            (long long)p.f.Lq * p.f.H * D, (long long)p.f.H * D, D, ub::kBwdBoxRows),
@@ -187,7 +161,6 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   p.dq_turn = det ? reinterpret_cast<int*>(dq_acc.data_ptr<float>() + acc_floats) : nullptr;
   Tensor dq, dk, dv;
   if (packed_grad) {
-    TORCH_CHECK(p.f.Lq == p.f.Lk, "packed gradients need self-attention shapes");
     Tensor dqkv = torch::empty({p.f.B, p.f.Lq, 3, p.f.H, D}, q.options());
     dq = dqkv.select(2, 0);
     dk = dqkv.select(2, 1);
@@ -213,12 +186,7 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
                 "cuTensorMapEncodeTiled failed for the dS scratch tensor");
   }
   p.dlogits = nullptr;
-  if (has_dlogits) {
-    TORCH_CHECK(dlogits->is_cuda() && dlogits->is_contiguous() && dlogits->dim() == 4 && dlogits->size(0) == p.f.B &&
-                    dlogits->size(1) == p.f.H && dlogits->size(2) == p.f.Lq && dlogits->size(3) == p.f.Lk,
-                "dlogits must be contiguous [B, H, Lq, Lk]");
-    TORCH_CHECK(dlogits->scalar_type() == q.scalar_type(), "dlogits must have the dtype of q");
-    TORCH_CHECK((reinterpret_cast<uintptr_t>(dlogits->data_ptr()) & 15) == 0, "dlogits must be 16-byte aligned");
+  if (has(dlogits)) {
     p.dlogits = dlogits->data_ptr();
     TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_dz, p.dlogits, p.f.is_bf16 != 0, p.f.B * p.f.H, p.f.Lq, p.f.Lk),
                 "cuTensorMapEncodeTiled failed for dlogits");
@@ -228,21 +196,16 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   p.dq = dq.data_ptr();
   p.dk = dk.data_ptr();
   p.dv = dv.data_ptr();
-  ub::launch_fmha_bwd(p, at::cuda::getCurrentCUDAStream().stream());
-  cudaError_t err = cudaGetLastError();
-  TORCH_CHECK(err == cudaSuccess, "fmha_bwd launch failed: ", cudaGetErrorString(err));
+  ub::launch_fmha_bwd(p, cur_stream());
+  check_launch("fmha_bwd");
   return {dq, dk, dv, dbias};
 }
 
-void check_decode_operand(const Tensor& t, const Tensor& q) {
-  TORCH_CHECK(t.is_cuda() && t.device() == q.device(), "fmha_decode: every tensor must be on the device of q");
-  TORCH_CHECK(t.dim() == 4 && t.size(0) == q.size(0) && t.size(2) == q.size(2) && t.size(3) == q.size(3),
-              "fmha_decode: q / k_cache / v_cache / k_new / v_new must be [B, L, H, D] with the B, H, D of q");
-  TORCH_CHECK(t.scalar_type() == q.scalar_type(), "fmha_decode: k_cache / v_cache / k_new / v_new need the dtype of q");
-  TORCH_CHECK(t.stride(3) == 1, "fmha_decode: the last dim of q / k / v must be contiguous");
-  TORCH_CHECK(t.stride(0) % 8 == 0 && t.stride(1) % 8 == 0 && t.stride(2) % 8 == 0 &&
-                  (reinterpret_cast<uintptr_t>(t.data_ptr()) & 15) == 0,
-              "fmha_decode: q / k / v must be 16-byte aligned with strides that are multiples of 8 elements");
+// q / k_cache / v_cache / k_new / v_new: [B, L, H, D] with the B, H, D and dtype of q, read as 16-byte vectors
+void check_decode_operand(const Tensor& t, const char* name, const Tensor& q, int64_t L = kAnySize) {
+  check_operand(t, name, q.device(), {q.scalar_type()}, {q.size(0), L, q.size(2), q.size(3)}, kAligned);
+  TORCH_CHECK(t.stride(3) == 1 && t.stride(0) % 8 == 0 && t.stride(1) % 8 == 0 && t.stride(2) % 8 == 0, name,
+              " needs a contiguous last dim and strides that are multiples of 8 elements");
 }
 
 // One query row per (b, h) against a [B, C, H, D] key / value cache (fmha_api.h).  max_len is a host bound on
@@ -252,38 +215,39 @@ void check_decode_operand(const Tensor& t, const Tensor& q) {
 Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& seqlens,
                    int64_t max_len, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
                    const OptTensor& kpm, double scale, int64_t num_splits) {
-  TORCH_CHECK(q.is_cuda() && q.dim() == 4 && q.size(1) == 1, "q must be [B, 1, H, D] on the GPU");
-  TORCH_CHECK(q.scalar_type() == at::kHalf || q.scalar_type() == at::kBFloat16, "q must be fp16 or bf16");
-  const int64_t D = q.size(3);
+  check_operand(q, "q", q.device(), k16Bit, {kAnySize, 1, kAnySize, kAnySize}, kAligned);
+  const int64_t B = q.size(0), H = q.size(2), D = q.size(3);
   TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
-  check_decode_operand(q, q);
-  check_decode_operand(k_cache, q);
-  check_decode_operand(v_cache, q);
+  check_decode_operand(q, "q", q);
+  check_decode_operand(k_cache, "k_cache", q);
+  check_decode_operand(v_cache, "v_cache", q);
   const int64_t C = k_cache.size(1);
   TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
-  const bool append = k_new.has_value() && k_new->defined();
-  TORCH_CHECK(append == (v_new.has_value() && v_new->defined()), "k_new and v_new go together");
-  const bool has_len = seqlens.has_value() && seqlens->defined();
+  const bool append = has(k_new);
+  TORCH_CHECK(append == has(v_new), "k_new and v_new go together");
+  TORCH_CHECK(!append || has(seqlens), "appending needs seqlens (the row to write)");
   if (append) {
-    TORCH_CHECK(has_len, "appending needs seqlens (the row to write)");
-    check_decode_operand(*k_new, q);
-    check_decode_operand(*v_new, q);
-    TORCH_CHECK(k_new->size(1) == 1 && v_new->size(1) == 1, "k_new / v_new must be [B, 1, H, D]");
+    check_decode_operand(*k_new, "k_new", q, 1);
+    check_decode_operand(*v_new, "v_new", q, 1);
   }
-  if (has_len) {
-    TORCH_CHECK(seqlens->is_cuda() && seqlens->device() == q.device() && seqlens->scalar_type() == at::kInt &&
-                    seqlens->dim() == 1 && seqlens->size(0) == q.size(0) && seqlens->is_contiguous(),
-                "seqlens must be a contiguous int32 [B] tensor on the device of q");
-  } else {
-    max_len = C;
-  }
+  check_operand(seqlens, "seqlens", q.device(), {at::kInt}, {B});
+  if (!has(seqlens)) max_len = C;
   const int64_t bound = max_len + (append ? 1 : 0);   // visible keys of any batch
   TORCH_CHECK(max_len >= 0, "max_len must not be negative");
   TORCH_CHECK(bound <= C, "max_len (+ 1 when appending) exceeds the cache capacity");
+  check_operand(bias, "bias", q.device(), {q.scalar_type()}, {kAnySize, H, 1, kAnySize}, 0);
+  if (has(bias)) {
+    TORCH_CHECK((bias->size(0) == 1 || bias->size(0) == B) && bias->stride(3) == 1,
+                "bias must be [1|B, H, 1, Lb] with a contiguous last dim");
+    TORCH_CHECK(bias->size(3) >= bound, "bias must have a column for every key that can be visible");
+  }
+  check_operand(kpm, "key_padding_mask", q.device(), {at::kBool}, {B, kAnySize}, 0);
+  TORCH_CHECK(!has(kpm) || (kpm->stride(1) == 1 && kpm->size(1) >= bound),
+              "key_padding_mask must have a contiguous last dim and a column for every key that can be visible");
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaDecodeParams p{};
-  p.B = (int)q.size(0);
-  p.H = (int)q.size(2);
+  p.B = (int)B;
+  p.H = (int)H;
   p.D = (int)D;
   p.C = (int)C;
   p.is_bf16 = q.scalar_type() == at::kBFloat16 ? 1 : 0;
@@ -300,23 +264,14 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
     p.v_new = v_new->data_ptr();
     p.vn_sb = v_new->stride(0); p.vn_sh = v_new->stride(2);
   }
-  p.seqlens = has_len ? seqlens->data_ptr<int>() : nullptr;
-  if (bias.has_value() && bias->defined()) {
-    TORCH_CHECK(bias->is_cuda() && bias->device() == q.device() && bias->dim() == 4 &&
-                    (bias->size(0) == 1 || bias->size(0) == p.B) && bias->size(1) == p.H && bias->size(2) == 1 &&
-                    bias->stride(3) == 1,
-                "bias must be [1|B, H, 1, Lb] with a contiguous last dim");
-    TORCH_CHECK(bias->scalar_type() == q.scalar_type(), "bias must have the dtype of q");
-    TORCH_CHECK(bias->size(3) >= bound, "bias must have a column for every key that can be visible");
+  p.seqlens = has(seqlens) ? seqlens->data_ptr<int>() : nullptr;
+  if (has(bias)) {
     p.bias = bias->data_ptr();
     p.bias_batch = (int)bias->size(0);
     p.bias_sb = bias->stride(0); p.bias_sh = bias->stride(1);
     p.bias_cols = (int)bias->size(3);
   }
-  if (kpm.has_value() && kpm->defined()) {
-    TORCH_CHECK(kpm->is_cuda() && kpm->device() == q.device() && kpm->scalar_type() == at::kBool && kpm->dim() == 2 &&
-                    kpm->size(0) == p.B && kpm->stride(1) == 1 && kpm->size(1) >= bound,
-                "key_padding_mask must be bool [B, Lk] with a contiguous last dim and Lk >= the visible keys");
+  if (has(kpm)) {
     p.kpm = reinterpret_cast<const uint8_t*>(kpm->data_ptr());
     p.kpm_sb = kpm->stride(0);
     p.kpm_cols = (int)kpm->size(1);
@@ -338,9 +293,8 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
     p.part_o = work.data_ptr<float>();
     p.part_ml = p.part_o + parts * D;
   }
-  ub::launch_fmha_decode(p, at::cuda::getCurrentCUDAStream().stream());
-  cudaError_t err = cudaGetLastError();
-  TORCH_CHECK(err == cudaSuccess, "fmha_decode launch failed: ", cudaGetErrorString(err));
+  ub::launch_fmha_decode(p, cur_stream());
+  check_launch("fmha_decode");
   return out;
 }
 }  // namespace

@@ -1,16 +1,14 @@
 // Bindings of the peer-memory collective kernels.
-#include <ATen/cuda/CUDAContext.h>
 #include <c10/cuda/CUDAGuard.h>
-#include <torch/extension.h>
 
-#include <cmath>
-#include <optional>
 #include <vector>
 
 #include "../api.h"
+#include "../bind_util.h"
 #include "comm_api.h"
 
 namespace {
+using namespace ub_bind;
 
 // buffer_ptrs / flag_ptrs: integer device addresses of every rank's (peer-mapped) buffers as returned
 // by the symmetric-memory rendezvous; multicast_ptr: NVLS alias or 0.
@@ -33,9 +31,8 @@ void symm_reduce_impl(const std::vector<int64_t>& buffer_ptrs, const std::vector
   peers.rank = (int)rank;
   peers.world = world;
   ub::launch_allreduce(peers, byte_offset, bytes, (int)dtype, (float)scale, (int)algo, (int)blocks,
-                       reinterpret_cast<float*>(sq_acc_ptr), at::cuda::getCurrentCUDAStream().stream(), scatter_only);
-  cudaError_t err = cudaGetLastError();
-  TORCH_CHECK(err == cudaSuccess, "symm_allreduce launch failed: ", cudaGetErrorString(err));
+                       reinterpret_cast<float*>(sq_acc_ptr), cur_stream(), scatter_only);
+  check_launch("symm_allreduce");
 }
 
 void symm_allreduce(const std::vector<int64_t>& buffer_ptrs, const std::vector<int64_t>& flag_ptrs,
@@ -75,14 +72,14 @@ ub::CommPeers make_sync(const std::vector<int64_t>& buf_ptrs, const std::vector<
 // K doubles summed over ranks through the symmetric exchange buffer (see comm_api.h); src / dst are local tensors.
 void symm_stats_allreduce(const std::vector<int64_t>& xchg_ptrs, const std::vector<int64_t>& flag_ptrs, int64_t err_ptr,
                           int64_t rank, int64_t tag, const at::Tensor& src, at::Tensor dst, int64_t parity) {
-  TORCH_CHECK(src.is_cuda() && dst.is_cuda() && src.scalar_type() == at::kDouble && dst.scalar_type() == at::kDouble);
-  TORCH_CHECK(src.is_contiguous() && dst.is_contiguous() && src.numel() == dst.numel() && src.numel() <= ub::kMaxStats);
+  check_operand(src, "src", src.device(), {at::kDouble});
+  check_operand(dst, "dst", src.device(), {at::kDouble}, {src.numel()}, kContig | kNumel);
+  TORCH_CHECK(src.numel() <= ub::kMaxStats, "at most SYMM_MAX_STATS statistics");
   const c10::cuda::CUDAGuard guard(src.device());
   ub::CommPeers x = make_sync(xchg_ptrs, flag_ptrs, err_ptr, rank, tag);
   ub::launch_stats_allreduce(x, src.data_ptr<double>(), dst.data_ptr<double>(), (int)src.numel(), (int)(parity & 1),
-                             at::cuda::getCurrentCUDAStream().stream());
-  cudaError_t err = cudaGetLastError();
-  TORCH_CHECK(err == cudaSuccess, "symm_stats_allreduce launch failed: ", cudaGetErrorString(err));
+                             cur_stream());
+  check_launch("symm_stats_allreduce");
 }
 
 // The fused optimizer tail (csrc/comm/fused_step.cu).  Per flat parameter group g: peer addresses + multicast alias of
@@ -106,17 +103,42 @@ void symm_fused_tail(const std::vector<int64_t>& xchg_ptrs, const std::vector<in
   TORCH_CHECK((int)param_ptrs.size() == ng && (int)grad_mc.size() == ng && (int)param_mc.size() == ng &&
               (int)master.size() == ng && (int)exp_avg.size() == ng && (int)exp_avg_sq.size() == ng &&
               (int)ema.size() == ng && (int)numel.size() == ng && (int)dtypes.size() == ng && (int)hyper.size() == ng);
-  TORCH_CHECK(ranges.is_cuda() && ranges.scalar_type() == at::kLong && ranges.is_contiguous() && ranges.dim() == 2 &&
-              ranges.size(1) == 6 && ranges.size(0) >= 1 && ranges.size(0) <= ub::kMaxTailRanges, "bad range table");
+  const c10::Device dev = state.device();
+  check_operand(state, "state", dev, {at::kFloat});
+  check_operand(ranges, "ranges", dev, {at::kLong}, {kAnySize, 6});
+  TORCH_CHECK(ranges.size(0) >= 1 && ranges.size(0) <= ub::kMaxTailRanges, "bad range table");
   const int nr = (int)ranges.size(0);
-  TORCH_CHECK(bucket_sq.is_cuda() && bucket_sq.scalar_type() == at::kFloat && bucket_sq.is_contiguous() &&
-              bucket_sq.numel() >= (int64_t)nr * ub::kMaxCommBlocks);
   const int cap = ub::fused_tail_max_blocks();
   if (blocks <= 0 || blocks > cap) blocks = cap;
-  TORCH_CHECK(block_sq.is_cuda() && block_sq.scalar_type() == at::kFloat && block_sq.numel() >= blocks);
-  TORCH_CHECK(grid_sync.is_cuda() && grid_sync.scalar_type() == at::kInt && grid_sync.numel() >= 4);
-  TORCH_CHECK(state.is_cuda() && state.scalar_type() == at::kFloat && state.numel() >= 4);
-  const c10::cuda::CUDAGuard guard(state.device());
+  check_operand(bucket_sq, "bucket_sq", dev, {at::kFloat});
+  check_operand(block_sq, "block_sq", dev, {at::kFloat});
+  check_operand(grid_sync, "grid_sync", dev, {at::kInt});
+  TORCH_CHECK(bucket_sq.numel() >= (int64_t)nr * ub::kMaxCommBlocks, "bucket_sq must hold SYMM_MAX_BLOCKS per range");
+  TORCH_CHECK(block_sq.numel() >= blocks, "block_sq must hold one float per block");
+  TORCH_CHECK(grid_sync.numel() >= 4, "grid_sync must hold 4 words");
+  TORCH_CHECK(state.numel() >= 4, "state must hold 4 words");
+  const bool stats = has(stats_src) && stats_src->numel() > 0;
+  TORCH_CHECK(!stats || has(stats_dst), "stats_src needs stats_dst");
+  if (stats) {
+    check_operand(stats_src, "stats_src", dev, {at::kDouble});
+    check_operand(stats_dst, "stats_dst", dev, {at::kDouble}, {stats_src->numel()}, kContig | kNumel);
+    TORCH_CHECK(stats_src->numel() <= ub::kMaxStats, "at most SYMM_MAX_STATS statistics");
+  }
+  for (int g = 0; g < ng; ++g) {
+    check_operand(master[g], "master", dev, {at::kFloat}, {}, kVec);
+    check_operand(exp_avg[g], "exp_avg", dev, {at::kFloat}, {master[g].numel()}, kVec | kNumel);
+    check_operand(exp_avg_sq[g], "exp_avg_sq", dev, {at::kFloat}, {master[g].numel()}, kVec | kNumel);
+    // (the arena view may end a few elements before the padded length; its STORAGE must cover the padding)
+    check_operand(ema[g], "ema", dev, {at::kFloat}, {}, kVec);
+    if (has(ema[g])) {
+      const int64_t room = (int64_t)(ema[g]->storage().nbytes() / sizeof(float)) - ema[g]->storage_offset();
+      TORCH_CHECK(room >= numel[g], "ema must have storage for the padded arena length");
+    }
+    TORCH_CHECK(numel[g] % 8 == 0, "arena lengths must be multiples of 8 elements");
+    TORCH_CHECK(dtypes[g] == ub::kF16 || dtypes[g] == ub::kBF16, "16-bit arenas expected");
+    TORCH_CHECK(hyper[g].size() == 5, "hyper: {beta1, beta2, eps, step_size, decay_mul} per group");
+  }
+  const c10::cuda::CUDAGuard guard(dev);
   ub::TailArgs a{};
   a.sync = make_sync(xchg_ptrs, flag_ptrs, err_ptr, rank, tag);
   const int world = a.sync.world;
@@ -124,34 +146,18 @@ void symm_fused_tail(const std::vector<int64_t>& xchg_ptrs, const std::vector<in
     ub::TailGroup& G = a.groups[g];
     TORCH_CHECK((int)grad_ptrs[g].size() == world && (int)param_ptrs[g].size() == world);
     for (int r = 0; r < world; ++r) {
-      TORCH_CHECK((grad_ptrs[g][r] & 15) == 0 && (param_ptrs[g][r] & 15) == 0, "arenas must be 16-byte aligned");
       G.grad[r] = reinterpret_cast<void*>(grad_ptrs[g][r]);
       G.param[r] = reinterpret_cast<void*>(param_ptrs[g][r]);
+      TORCH_CHECK(aligned16(G.grad[r]) && aligned16(G.param[r]), "arenas must be 16-byte aligned");
     }
     G.grad_mc = reinterpret_cast<void*>(grad_mc[g]);
     G.param_mc = reinterpret_cast<void*>(param_mc[g]);
-    for (const at::Tensor* t : {&master[g], &exp_avg[g], &exp_avg_sq[g]}) {
-      TORCH_CHECK(t->is_cuda() && t->is_contiguous() && t->scalar_type() == at::kFloat, "fp32 optimizer state expected");
-      TORCH_CHECK((reinterpret_cast<uintptr_t>(t->data_ptr()) & 15) == 0, "optimizer state must be 16-byte aligned");
-      TORCH_CHECK(t->numel() == master[g].numel(), "master / exp_avg / exp_avg_sq shards differ in length");
-    }
     G.master = master[g].data_ptr<float>();
     G.exp_avg = exp_avg[g].data_ptr<float>();
     G.exp_avg_sq = exp_avg_sq[g].data_ptr<float>();
-    G.ema = nullptr;
-    if (ema[g].has_value() && ema[g]->defined()) {
-      // (the arena view may end a few elements before the padded length; its STORAGE must cover the padding)
-      const int64_t room = (int64_t)(ema[g]->storage().nbytes() / sizeof(float)) - ema[g]->storage_offset();
-      TORCH_CHECK(ema[g]->is_cuda() && ema[g]->scalar_type() == at::kFloat && ema[g]->is_contiguous() &&
-                      room >= numel[g] && (reinterpret_cast<uintptr_t>(ema[g]->data_ptr()) & 15) == 0,
-                  "EMA arena: fp32, 16-byte aligned, storage of at least the padded arena length");
-      G.ema = ema[g]->data_ptr<float>();
-    }
-    TORCH_CHECK(numel[g] % 8 == 0, "arena lengths must be multiples of 8 elements");
+    G.ema = has(ema[g]) ? ema[g]->data_ptr<float>() : nullptr;
     G.numel = numel[g];
-    TORCH_CHECK(dtypes[g] == ub::kF16 || dtypes[g] == ub::kBF16, "16-bit arenas expected");
     G.dtype = (int)dtypes[g];
-    TORCH_CHECK(hyper[g].size() == 5);
     G.beta1 = (float)hyper[g][0];
     G.beta2 = (float)hyper[g][1];
     G.eps = (float)hyper[g][2];
@@ -165,18 +171,9 @@ void symm_fused_tail(const std::vector<int64_t>& xchg_ptrs, const std::vector<in
   a.bucket_sq = bucket_sq.data_ptr<float>();
   a.block_sq = block_sq.data_ptr<float>();
   a.grid_sync = reinterpret_cast<unsigned int*>(grid_sync.data_ptr<int>());
-  a.stats_src = nullptr;
-  a.stats_dst = nullptr;
-  a.nstats = 0;
-  if (stats_src.has_value() && stats_src->defined() && stats_src->numel() > 0) {
-    TORCH_CHECK(stats_dst.has_value() && stats_dst->defined());
-    TORCH_CHECK(stats_src->is_cuda() && stats_src->scalar_type() == at::kDouble && stats_src->is_contiguous() &&
-                stats_dst->is_cuda() && stats_dst->scalar_type() == at::kDouble && stats_dst->is_contiguous() &&
-                stats_src->numel() == stats_dst->numel() && stats_src->numel() <= ub::kMaxStats);
-    a.stats_src = stats_src->data_ptr<double>();
-    a.stats_dst = stats_dst->data_ptr<double>();
-    a.nstats = (int)stats_src->numel();
-  }
+  a.stats_src = stats ? stats_src->data_ptr<double>() : nullptr;
+  a.stats_dst = stats ? stats_dst->data_ptr<double>() : nullptr;
+  a.nstats = stats ? (int)stats_src->numel() : 0;
   a.parity = (int)(parity & 1);
   a.denom_index = (int)denom_index;
   a.factor = (float)factor;
@@ -188,9 +185,8 @@ void symm_fused_tail(const std::vector<int64_t>& xchg_ptrs, const std::vector<in
   a.seed = (unsigned long long)seed;
   a.offset = (unsigned long long)offset;
   a.state = state.data_ptr<float>();
-  ub::launch_fused_tail(a, (int)blocks, at::cuda::getCurrentCUDAStream().stream());
-  cudaError_t err = cudaGetLastError();
-  TORCH_CHECK(err == cudaSuccess, "symm_fused_tail launch failed: ", cudaGetErrorString(err));
+  ub::launch_fused_tail(a, (int)blocks, cur_stream());
+  check_launch("symm_fused_tail");
 }
 
 // Pinned, device-mapped host words for the communicator's error channel: returns (host tensor view, device address).

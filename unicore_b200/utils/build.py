@@ -121,6 +121,10 @@ def build_inplace(verbose=False, force=False):
         cuda_lib = os.path.join(os.path.dirname(os.path.dirname(nvcc)), "lib64")
         link += ["-L", cuda_lib, "-Wl,-rpath," + cuda_lib]
         link += ["-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch_cuda", "-ltorch", "-ltorch_python", "-lcudart", "-lcuda"]
+        # The shared libstdc++ that torch uses, named explicitly: where the compiler's own libstdc++.so link is missing,
+        # g++'s implicit -lstdc++ falls back to libstdc++.a, and a second, static copy of the stream and locale code
+        # in the extension crashes the process as soon as an error message formats a number.
+        link += ["-l:libstdc++.so.6"]
         _run(link)
     # only a complete build (compiled and linked with these flags) is recorded
     with open(stamp, "w") as f:
@@ -139,6 +143,7 @@ def cuda_extension():
         include_dirs=[CSRC],
         extra_compile_args={"cxx": CXX_FLAGS, "nvcc": NVCC_FLAGS},
         libraries=["cuda"],
+        extra_link_args=["-l:libstdc++.so.6"],  # (see build_inplace)
     )
 
 
