@@ -42,8 +42,31 @@ struct FmhaFwdParams {
   // triu(full((Lq, Lk), -inf), 1)).  Key tiles wholly above the diagonal are skipped; not combined with logits mode.
   int causal;
   CUtensorMap sw_logits;
+  // KV-cache mode (fmha_kvcache_fwd; appended so that no earlier field moves): q is a chunk of Lq = T queries per
+  // sequence, k / v are [B, C, H, D] caches (Lk = C).  With p_b = clamp(seqlens[b], 0, C) and
+  // n_b = min(p_b + T, kv_cap), query i of sequence b sees key j iff j < n_b and j <= p_b + i (the future mask of the
+  // whole sequence, aligned bottom-right per sequence); with seqlens null, p_b = C: every row below kv_cap is visible
+  // to every query (cross-attention).  kv_cap = min(C, bias columns, key-mask columns); the bias map is
+  // [bias_batch * H, T, Lb], the key mask [B, kpm_cols] contiguous.  No dropout, no keep bits, lse may be null.
+  const int* seqlens;
+  int kvcache, kv_cap, kpm_cols;
 };
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
+
+// Copies the T new rows of k_new / v_new [B, T, H, D] into rows p_b + i of the [B, C, H, D] caches, p_b =
+// clamp(seqlens[b], 0, C), bitwise, with 16-byte vectors; rows at or past C are skipped.  It runs as a launch of its
+// own before the KV-cache forward, which reads those rows from every query tile of a (b, h).
+struct KvCacheAppendParams {
+  const void* k_new;       // [B, T, H, D] via strides (elements)
+  const void* v_new;
+  void* k_cache;           // [B, C, H, D] via strides
+  void* v_cache;
+  const int* seqlens;      // [B] int32 on the device
+  long long kn_sb, kn_sl, kn_sh, vn_sb, vn_sl, vn_sh;
+  long long kc_sb, kc_sl, kc_sh, vc_sb, vc_sl, vc_sh;
+  int B, T, H, D, C;
+};
+void launch_kv_cache_append(const KvCacheAppendParams& p, cudaStream_t stream);
 
 struct FmhaBwdParams {
   FmhaFwdParams f;   // same inputs as forward (out/lse hold the forward results)

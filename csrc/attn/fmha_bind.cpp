@@ -297,6 +297,83 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   check_launch("fmha_decode");
   return out;
 }
+
+// A chunk of T >= 2 queries per sequence against a [B, C, H, D] key / value cache, in the KV-cache mode of the wgmma
+// forward (fmha_api.h).  With seqlens the T rows of k_new / v_new are first appended at rows seqlens[b] + i (a launch
+// of its own), and query i sees the keys j <= seqlens[b] + i; without seqlens every query sees all C rows.  max_len
+// is a host bound on seqlens, as in fmha_decode.  The bias is [1|B, H, T, Lb] with Lb % 8 == 0 (its TMA row stride).
+Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& seqlens,
+                        int64_t max_len, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
+                        const OptTensor& kpm, double scale) {
+  check_operand(q, "q", q.device(), k16Bit, any_shape(4), kAligned);
+  const int64_t B = q.size(0), T = q.size(1), H = q.size(2), D = q.size(3);
+  TORCH_CHECK(T >= 2, "fmha_kvcache_fwd takes chunks of T >= 2 queries (fmha_decode takes T = 1)");
+  TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
+  check_decode_operand(q, "q", q);
+  check_decode_operand(k_cache, "k_cache", q);
+  check_decode_operand(v_cache, "v_cache", q);
+  const int64_t C = k_cache.size(1);
+  TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
+  const bool append = has(k_new);
+  TORCH_CHECK(append == has(v_new), "k_new and v_new go together");
+  TORCH_CHECK(append == has(seqlens), "a chunk with seqlens appends k_new / v_new, and one without does not");
+  if (append) {
+    check_decode_operand(*k_new, "k_new", q, T);
+    check_decode_operand(*v_new, "v_new", q, T);
+  }
+  check_operand(seqlens, "seqlens", q.device(), {at::kInt}, {B});
+  TORCH_CHECK(max_len >= 0, "max_len must not be negative");
+  const int64_t bound = append ? max_len + T : C;   // visible keys of any batch
+  TORCH_CHECK(bound <= C, "max_len + T exceeds the cache capacity");
+  check_operand(bias, "bias", q.device(), {q.scalar_type()}, {kAnySize, H, T, kAnySize}, kVec);
+  if (has(bias)) {
+    TORCH_CHECK(bias->size(0) == 1 || bias->size(0) == B, "bias must be [1|B, H, T, Lb]");
+    TORCH_CHECK(bias->size(3) % 8 == 0, "bias columns Lb must be a multiple of 8 (the TMA row stride)");
+    TORCH_CHECK(bias->size(3) >= bound, "bias must have a column for every key that can be visible");
+  }
+  check_operand(kpm, "key_padding_mask", q.device(), {at::kBool}, {B, kAnySize});
+  TORCH_CHECK(!has(kpm) || kpm->size(1) >= bound, "key_padding_mask must have a column for every key that can be visible");
+  const c10::cuda::CUDAGuard guard(q.device());
+  ub::FmhaFwdParams p{};
+  // q / k / v as the forward takes them (K / V maps over the C cache rows); the bias has Lb columns, not C, so its
+  // map is made below
+  fill_common(p, q, k_cache, v_cache, std::nullopt, kpm, 0.0, scale, /*forward=*/true);
+  if (has(bias)) {
+    p.bias = bias->data_ptr();
+    p.bias_batch = (int)bias->size(0);
+    TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_bias, p.bias, p.is_bf16 != 0, p.bias_batch * p.H, p.Lq,
+                                             (int)bias->size(3)),
+                "cuTensorMapEncodeTiled failed for the bias");
+  }
+  p.kvcache = 1;
+  p.seqlens = has(seqlens) ? seqlens->data_ptr<int>() : nullptr;
+  p.kpm_cols = has(kpm) ? (int)kpm->size(1) : 0;
+  int64_t cap = C;
+  if (has(bias)) cap = std::min<int64_t>(cap, bias->size(3));
+  if (has(kpm)) cap = std::min<int64_t>(cap, kpm->size(1));
+  p.kv_cap = (int)cap;
+  Tensor out = torch::empty({B, T, H, D}, q.options());
+  p.out = out.data_ptr();
+  p.lse = nullptr;
+  if (append) {
+    ub::KvCacheAppendParams a{};
+    a.k_new = k_new->data_ptr();
+    a.v_new = v_new->data_ptr();
+    a.k_cache = k_cache.data_ptr();
+    a.v_cache = v_cache.data_ptr();
+    a.seqlens = p.seqlens;
+    a.kn_sb = k_new->stride(0); a.kn_sl = k_new->stride(1); a.kn_sh = k_new->stride(2);
+    a.vn_sb = v_new->stride(0); a.vn_sl = v_new->stride(1); a.vn_sh = v_new->stride(2);
+    a.kc_sb = p.k_sb; a.kc_sl = p.k_sl; a.kc_sh = p.k_sh;
+    a.vc_sb = p.v_sb; a.vc_sl = p.v_sl; a.vc_sh = p.v_sh;
+    a.B = p.B; a.T = p.Lq; a.H = p.H; a.D = p.D; a.C = p.Lk;
+    ub::launch_kv_cache_append(a, cur_stream());
+    check_launch("kv_cache_append");
+  }
+  ub::launch_fmha_fwd(p, cur_stream());
+  check_launch("fmha_kvcache_fwd");
+  return out;
+}
 }  // namespace
 
 void register_fmha(pybind11::module_& m) {
@@ -310,6 +387,12 @@ void register_fmha(pybind11::module_& m) {
   m.def("fmha_decode", &fmha_decode, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("seqlens"),
         py::arg("max_len"), py::arg("k_new"), py::arg("v_new"), py::arg("bias"), py::arg("key_padding_mask"),
         py::arg("scale"), py::arg("num_splits") = 0);
+  // its own submodule, _C.kvcache; tests/test_gpu_attention_kvcache_chunk.py runs the operand-rejection table of
+  // tests/test_gpu_bindings.py over it
+  auto kv = m.def_submodule("kvcache", "multi-token steps into a key / value cache");
+  kv.def("fmha_kvcache_fwd", &fmha_kvcache_fwd, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"),
+         py::arg("seqlens"), py::arg("max_len"), py::arg("k_new"), py::arg("v_new"), py::arg("bias"),
+         py::arg("key_padding_mask"), py::arg("scale"));
   m.def("fmha_decode_max_splits", [] { return (int64_t)ub::kDecodeMaxSplits; });
   m.def("fmha_decode_num_splits", [](int64_t B, int64_t H, int64_t len_bound) {
     return (int64_t)ub::fmha_decode_num_splits((int)B, (int)H, (int)len_bound,

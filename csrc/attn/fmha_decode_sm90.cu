@@ -271,7 +271,31 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_combine_kernel(const Fmh
   reinterpret_cast<T*>(p.out)[bh * p.D + d] = from_f32<T>(ls > 0.f ? o / ls : 0.f);
 }
 
+// Row i of k_new / v_new -> row p_b + i of the caches (fmha_api.h).  CTA (i, b) copies all H heads of K and of V,
+// one 16-byte vector per thread and step; a row at or past C is skipped.
+__global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCacheAppendParams p) {
+  const int i = blockIdx.x, b = blockIdx.y;
+  const int pos = min(max(p.seqlens[b], 0), p.C) + i;
+  if (pos >= p.C) return;
+  const int nch = p.D / 8, per = p.H * nch;   // 16-byte chunks of one row of one tensor
+  for (int x = threadIdx.x; x < 2 * per; x += kThreads) {
+    const bool is_v = x >= per;
+    const int h = (x % per) / nch, c = x % nch;
+    const uint16_t* src = reinterpret_cast<const uint16_t*>(is_v ? p.v_new : p.k_new) +
+                          (long long)b * (is_v ? p.vn_sb : p.kn_sb) + (long long)i * (is_v ? p.vn_sl : p.kn_sl) +
+                          (long long)h * (is_v ? p.vn_sh : p.kn_sh) + 8 * c;
+    uint16_t* dst = reinterpret_cast<uint16_t*>(is_v ? p.v_cache : p.k_cache) +
+                    (long long)b * (is_v ? p.vc_sb : p.kc_sb) + (long long)pos * (is_v ? p.vc_sl : p.kc_sl) +
+                    (long long)h * (is_v ? p.vc_sh : p.kc_sh) + 8 * c;
+    st_global_v4(dst, ld_global_v4(src));
+  }
+}
+
 }  // namespace
+
+void launch_kv_cache_append(const KvCacheAppendParams& p, cudaStream_t stream) {
+  kv_cache_append_kernel<<<dim3(p.T, p.B), kThreads, 0, stream>>>(p);
+}
 
 int fmha_decode_num_splits(int B, int H, int len_bound, int num_sms) {
   // As many splits as fit the num_sms * kDecodeCtasPerSm resident CTAs in one wave (a partial second wave would

@@ -112,9 +112,16 @@ UB_DEVICE void quad_transpose4(uint32_t (&w)[4], int c) {
 // of 64, kBlockN of 64), so only there do some elements get -inf, by index, in registers.  The skipped tiles would
 // have added exact zeros (alpha = ex2(0) = 1, l += 0, P = +0), so O, LSE and the keep words written are bitwise those
 // of the plain kernel given bias + the future mask.  The CTAs take the query tiles longest first.
-template <typename T, int DP, bool kLogits, bool kCausal>
+// kKVCache: a chunk of T queries against a [B, C, H, D] cache (fmha_api.h): query i of sequence b sees key j iff
+// j < n_b and j <= p_b + i.  p_b is read from the device and is not tile-aligned, so the tile loop (and the prefetch)
+// stops at the tile holding key min(n_b, p_b + q0 + 64) - 1, and every tile that reaches past key p_b + q0 (the band
+// may span two) sets the invisible elements to -inf by index.  Cache rows at or past n_b lie inside the tensor, so TMA
+// loads them and they may hold anything, NaN included: their scores are replaced (never added to), and their V rows
+// are zeroed in shared memory before P V (0 x NaN is NaN).  Only the last tile walked can hold such rows.  No dropout.
+template <typename T, int DP, bool kLogits, bool kCausal, bool kKVCache>
 __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
+  static_assert(!(kKVCache && (kLogits || kCausal)), "the KV-cache mode is neither causal nor logits mode");
   using C = FwdCfg<DP>;
   constexpr int kBlockN = C::kBlockN;
   constexpr int kWords = kBlockN / 32;   // keep-bit words per row of a key tile
@@ -124,15 +131,24 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   uint8_t* smem = smem_raw + (smem_base - raw_base);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, c = lane & 3;
-  const int q_tile = kCausal ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
+  const int q_tile = (kCausal || kKVCache) ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
   const int q0 = q_tile * kBlockM, h = blockIdx.y, b = blockIdx.z;
   const uint32_t bar0 = smem_base + C::kSmemBar;   // bar0 + 8 * stage: K / V / bias of a key tile (+ Q on the first)
   float* kadd = reinterpret_cast<float*>(smem + C::kSmemKAdd);
 
   const bool has_bias = p.bias != nullptr;
   const int n_key_tiles = (p.Lk + kBlockN - 1) / kBlockN;
+  // KV-cache mode: kv_p = p_b, kv_n = n_b, and kv_lim = the first key that some row of this query tile does not see
+  int kv_p = 0, kv_n = 0, kv_lim = 0;
+  if constexpr (kKVCache) {
+    kv_p = p.seqlens != nullptr ? min(max(p.seqlens[b], 0), p.Lk) : p.Lk;
+    kv_n = min(kv_p + p.Lq, p.kv_cap);
+    kv_lim = min(kv_n, kv_p + q0 + 1);
+  }
   // causal: key tiles 0 .. (q0 + 63) / kBlockN hold a key visible to one of the rows q0 .. q0 + 63
-  const int n_tiles = kCausal ? min(n_key_tiles, (q0 + kBlockM - 1) / kBlockN + 1) : n_key_tiles;
+  const int n_tiles = kCausal ? min(n_key_tiles, (q0 + kBlockM - 1) / kBlockN + 1)
+                      : kKVCache ? max(1, (min(kv_n, kv_p + q0 + kBlockM) + kBlockN - 1) / kBlockN)
+                                 : n_key_tiles;
   const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
   // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
   constexpr uint32_t kKVBytes = C::kKVStage, kBiasBytes = C::kBiasStage, kQBytes = C::kBoxes * C::kQBox;
@@ -161,8 +177,8 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 
   const int rl0 = warp * 16 + g, rl1 = rl0 + 8;   // my two rows of the tile
   const int row0 = q0 + rl0, row1 = q0 + rl1;
-  const uint8_t* kpm_row = p.kpm != nullptr ? p.kpm + (long long)b * p.Lk : nullptr;
-  const bool drop = p.p_drop > 0.f;
+  const uint8_t* kpm_row = p.kpm != nullptr ? p.kpm + (long long)b * (kKVCache ? p.kpm_cols : p.Lk) : nullptr;
+  const bool drop = !kKVCache && p.p_drop > 0.f;
   const uint32_t t14 = dropout_thresh14(p.p_drop);
   const uint32_t t14x2 = t14 | (t14 << 16);
   // the 1/(1-p) of the kept probabilities is applied once, to the normalised output row
@@ -188,7 +204,8 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     bool masked = false;
     if (tid < kBlockN) {
       const int key = key0 + tid;
-      masked = key >= p.Lk || (kpm_row != nullptr && kpm_row[key] != 0);
+      // KV-cache mode: kpm_cols >= kv_cap >= kv_n, so the key mask is read only below kv_n
+      masked = key >= (kKVCache ? kv_n : p.Lk) || (kpm_row != nullptr && kpm_row[key] != 0);
       kadd[st * kBlockN + tid] = masked ? -CUDART_INF_F : 0.f;
     }
     // barrier: every thread is done with tile j-1, so its stage may be refilled with tile j+1
@@ -196,6 +213,18 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     if (kLogits && tid == 0) bulk_wait_read();   // the logits store of tile j-1 has read the stage tile j+1 fills
     if (tid == 0 && j + 1 < n_tiles) load_tile(j + 1);
     mbar_wait(bar0 + 8u * st, (uint32_t)((j >> 1) & 1));
+    if constexpr (kKVCache) {
+      if (key0 + kBlockN > kv_n) {   // zero the V rows at or past n_b: whole 128-byte rows of every column box
+        const int r0 = max(kv_n - key0, 0), chunks = (kBlockN - r0) * 8;
+        uint8_t* sv = smem + C::kSmemV + st * C::kKVStage;
+        for (int x = tid; x < C::kBoxes * chunks; x += kFwdThreads) {
+          const int box = x / chunks, r = r0 + (x % chunks) / 8;
+          *reinterpret_cast<uint4*>(sv + box * C::kKVBox + r * 128 + (x % 8) * 16) = make_uint4(0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async_smem();   // the generic-proxy stores, before wgmma reads V
+        __syncthreads();
+      }
+    }
 
     // ---- S = Q K^T --------------------------------------------------------------------------------------
     float s[kBlockN / 2];
@@ -238,6 +267,16 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
           if (key + 1 > row0) s[4 * i + 1] = -CUDART_INF_F;
           if (key > row1) s[4 * i + 2] = -CUDART_INF_F;
           if (key + 1 > row1) s[4 * i + 3] = -CUDART_INF_F;
+        }
+      }
+      if constexpr (kKVCache) {   // assigned, not added: a stale score may be NaN
+        if (key0 + kBlockN > kv_lim) {
+          const int key = key0 + col;
+          const int lim0 = min(kv_n, kv_p + row0 + 1), lim1 = min(kv_n, kv_p + row1 + 1);
+          if (key >= lim0) s[4 * i + 0] = -CUDART_INF_F;
+          if (key + 1 >= lim0) s[4 * i + 1] = -CUDART_INF_F;
+          if (key >= lim1) s[4 * i + 2] = -CUDART_INF_F;
+          if (key + 1 >= lim1) s[4 * i + 3] = -CUDART_INF_F;
         }
       }
       if constexpr (kLogits) {   // the same swizzled positions as the bias elements above
@@ -364,14 +403,15 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 #pragma unroll
     for (int i = 0; i < DP / 8; ++i)
       if (8 * i < D) og[4 * i] = pack2<T>(o[4 * i + 0] * inv0, o[4 * i + 1] * inv0);
-    if (c == 0) p.lse[lin0] = l0 > 0.f ? m0 + __logf(l0) : -CUDART_INF_F;   // natural-log LSE of the logits
+    if (c == 0 && (!kKVCache || p.lse != nullptr))
+      p.lse[lin0] = l0 > 0.f ? m0 + __logf(l0) : -CUDART_INF_F;   // natural-log LSE of the logits
   }
   if (row1 < p.Lq) {
     uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row1) * p.H + h) * D + 2 * c);
 #pragma unroll
     for (int i = 0; i < DP / 8; ++i)
       if (8 * i < D) og[4 * i] = pack2<T>(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
-    if (c == 0) p.lse[lin1] = l1 > 0.f ? m1 + __logf(l1) : -CUDART_INF_F;
+    if (c == 0 && (!kKVCache || p.lse != nullptr)) p.lse[lin1] = l1 > 0.f ? m1 + __logf(l1) : -CUDART_INF_F;
   }
   if constexpr (kLogits) {
     if (tid == 0) bulk_wait_all();   // shared memory must outlive the last logits store's reads
@@ -386,20 +426,23 @@ void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
     kern<<<grid, kFwdThreads, smem_bytes, stream>>>(p);
   };
-  auto dispatch = [&](auto logits, auto causal) {
+  auto dispatch = [&](auto logits, auto causal, auto kvcache) {
     constexpr bool kLogits = decltype(logits)::value, kCausal = decltype(causal)::value;
+    constexpr bool kKV = decltype(kvcache)::value;
     if (p.D <= 64) {
-      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits, kCausal>, FwdCfg<64>::kSmemBytes);
-      else run(fmha_fwd_kernel<__half, 64, kLogits, kCausal>, FwdCfg<64>::kSmemBytes);
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits, kCausal, kKV>, FwdCfg<64>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 64, kLogits, kCausal, kKV>, FwdCfg<64>::kSmemBytes);
     } else {
-      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits, kCausal>, FwdCfg<128>::kSmemBytes);
-      else run(fmha_fwd_kernel<__half, 128, kLogits, kCausal>, FwdCfg<128>::kSmemBytes);
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits, kCausal, kKV>, FwdCfg<128>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 128, kLogits, kCausal, kKV>, FwdCfg<128>::kSmemBytes);
     }
   };
-  // causal + logits is refused by the binding (fmha_bind.cpp)
-  if (p.logits != nullptr) dispatch(std::true_type{}, std::false_type{});
-  else if (p.causal) dispatch(std::false_type{}, std::true_type{});
-  else dispatch(std::false_type{}, std::false_type{});
+  // causal + logits is refused by the binding (fmha_bind.cpp); the KV-cache mode sets neither
+  const std::false_type no;
+  if (p.kvcache) dispatch(no, no, std::true_type{});
+  else if (p.logits != nullptr) dispatch(std::true_type{}, no, no);
+  else if (p.causal) dispatch(no, std::true_type{}, no);
+  else dispatch(no, no, no);
 }
 
 }  // namespace ub

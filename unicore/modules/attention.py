@@ -19,7 +19,8 @@ to the kernel as a flag (no mask tensor); the materialised path adds the future 
 its logits are those of the same call with that mask in ``attn_bias``.
 
 ``DecoderCache`` holds what incremental decoding keeps between steps: per layer the self-attention keys and values
-``[B, C, H, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.
+``[B, C, H, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.  A step may
+add one token or a chunk of several per sequence, and ``rewind`` drops tokens again.
 """
 from typing import Optional
 
@@ -102,9 +103,9 @@ class SelfMultiheadAttention(nn.Module):
         ``need_probs=False`` returns ``probs = None``; with ``return_attn`` the fused kernel then also computes the
         logits ``[B*H, L, L]`` where it takes the shapes.  ``causal`` hides key j from query i when j > i (see the module
         docstring).  ``cache`` (a ``LayerKVCache`` of a ``DecoderCache``): on the prefill the keys and values of the L
-        positions are also stored in it; on a decoding step (``query [B, 1, E]``) the new token's key and value are
-        appended and its query attends to the cached keys (``ops.attention_with_kv_cache``), with ``attn_bias`` the
-        ``[B, H, 1, Lb]`` row of the new queries."""
+        positions are also stored in it; on a decoding step (``query [B, T, E]``, one token or a chunk) the new tokens'
+        keys and values are appended and their queries attend to the cached keys up to their own positions
+        (``ops.attention_with_kv_cache``), with ``attn_bias`` the ``[B, H, T, Lb]`` rows of the new queries."""
         bsz, tgt_len, embed_dim = query.size()
         if embed_dim != self.embed_dim:
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
@@ -172,8 +173,8 @@ class CrossMultiheadAttention(nn.Module):
         """Everything up to (not including) ``out_proj``.
 
         ``cache`` (a ``LayerKVCache``): the projected keys and values are computed once, on the prefill, and kept in
-        it; a decoding step (``query [B, 1, E]``, ``key`` / ``value`` unused) attends to them with
-        ``ops.attention_with_kv_cache``."""
+        it; a decoding step (``query [B, T, E]``, ``key`` / ``value`` unused) attends to them with
+        ``ops.attention_with_kv_cache``, ``attn_bias`` holding the rows of the T new queries."""
         bsz, tgt_len, embed_dim = query.size()
         if embed_dim != self.embed_dim:
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
@@ -274,3 +275,18 @@ class DecoderCache:
         self.seqlens = self.seqlens.index_select(0, index)
         for layer in self.layers:
             layer.reorder(index)
+
+    def rewind(self, n):
+        """Drop the last ``n`` tokens of every sequence (an int), or ``n[b]`` of sequence b (an integer ``[B]`` tensor
+        on the device), as speculative decoding does after verifying a chunk of draft tokens: ``seqlens -= n``, clamped
+        at 0, without a host synchronisation.  An int also lowers ``max_len``; a tensor leaves it, a valid bound.  The
+        rows past ``seqlens`` are never read, so nothing else is reset; rewinding every token empties the cache, and
+        the next call is a prefill again."""
+        if isinstance(n, torch.Tensor):
+            self.seqlens.sub_(n.to(device=self.seqlens.device, dtype=self.seqlens.dtype)).clamp_(min=0)
+            return
+        n = int(n)
+        if n < 0:
+            raise ValueError("rewind takes a count of tokens >= 0, not {}".format(n))
+        self.seqlens.sub_(n).clamp_(min=0)
+        self.max_len = max(self.max_len - n, 0)

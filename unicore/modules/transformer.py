@@ -476,11 +476,13 @@ class TransformerDecoder(nn.Module, _StackMixin):
         * the first call (the prefill) takes the prompts ``emb [B, L, E]``, right-padded as ``padding_mask`` says, runs
           exactly the path above and stores every layer's keys / values of the L positions and its projected encoder
           keys / values; the cache then holds the unpadded lengths;
-        * every later call (a step) takes one token per sequence, ``emb [B, 1, E]`` at position ``seqlens[b]``, and
-          returns ``[B, 1, E]``.  Its self-attention appends the token's key / value and attends to the cache; the
-          encoder attention uses the stored encoder keys / values (``encoder_out`` may be None) with
-          ``encoder_padding_mask``, and ``encoder_attn_mask``, if given, holds the rows of the new queries
-          ``[B*H, 1, S]``.  ``padding_mask`` and ``attn_mask`` are not supported on a step.
+        * every later call (a step) takes T tokens per sequence, ``emb [B, T, E]`` at positions ``seqlens[b] ..
+          seqlens[b] + T - 1`` (one token, or a chunk: a prompt continued, a long prompt fed in pieces, draft tokens to
+          verify), and returns ``[B, T, E]``.  Its self-attention appends the tokens' keys / values and each token
+          attends to the cache up to its own position; the encoder attention uses the stored encoder keys / values
+          (``encoder_out`` may be None) with ``encoder_padding_mask``, and ``encoder_attn_mask``, if given, holds the
+          rows of the new queries ``[B*H, T, S]``.  ``padding_mask`` and ``attn_mask`` are not supported on a step.
+          ``cache.rewind`` drops tokens again.
         """
         if cache is not None:
             return self._forward_cached(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
@@ -523,14 +525,24 @@ class TransformerDecoder(nn.Module, _StackMixin):
             rates += [layer.dropout, layer.attention_dropout, layer.activation_dropout]
         return self.training and any(r > 0 for r in rates)
 
-    def _step_rel_pos_bias(self, cache, like):
-        """``[B, H, 1, max_len + 1]``: the relative-position bias row of each sequence's new token, gathered on the
-        device at its position ``seqlens[b]`` (keys past it are not visible)."""
+    def _step_rel_pos_bias(self, cache, like, T=1):
+        """``[B, H, T, Lb]``: the relative-position bias rows of each sequence's T new tokens, gathered on the device at
+        their positions ``seqlens[b] + i`` (keys past them are not visible).  ``Lb`` is ``max_len + 1`` for one token and
+        ``max_len + T`` rounded up to 8 for a chunk (the row stride the chunk kernel reads); columns past the bucket
+        table are 0."""
         if self.rp_bucket.device != like.device:
             self.rp_bucket = self.rp_bucket.to(like.device)
-        idx = self.rp_bucket[cache.seqlens.long(), : cache.max_len + 1]   # [B, max_len + 1]
-        values = F.embedding(idx, self.relative_attention_bias.weight)   # [B, max_len + 1, H]
-        return values.permute(0, 2, 1).unsqueeze(2).to(like.dtype).contiguous()
+        cols = cache.max_len + T
+        if T > 1:
+            cols += -cols % 8
+        width = min(cols, self.max_seq_len)
+        pos = cache.seqlens.long()[:, None] + torch.arange(T, device=like.device)   # [B, T]
+        idx = self.rp_bucket[pos.clamp(max=self.max_seq_len - 1), :width]   # [B, T, width]
+        values = F.embedding(idx, self.relative_attention_bias.weight)   # [B, T, width, H]
+        bias = values.permute(0, 3, 1, 2)
+        if cols > width:
+            bias = F.pad(bias, (0, cols - width))
+        return bias.to(like.dtype).contiguous()
 
     def _forward_cached(self, emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask,
                         cache):
@@ -555,21 +567,21 @@ class TransformerDecoder(nn.Module, _StackMixin):
                 cache.seqlens.copy_(L - padding_mask.to(torch.int32).sum(1))
             cache.max_len = L
         else:
-            if emb.size(1) != 1:
-                raise ValueError("a decoding step takes one token per sequence: emb must be [B, 1, E]")
+            T = emb.size(1)
             if attn_mask is not None:
                 raise NotImplementedError("attn_mask is not supported on a decoding step")
             if padding_mask is not None:
                 raise NotImplementedError("padding_mask is not supported on a decoding step")
-            if cache.max_len + 1 > cache.capacity:
-                raise ValueError("the cache is full: capacity {}".format(cache.capacity))
+            if cache.max_len + T > cache.capacity:
+                raise ValueError("{} more tokens do not fit the cache: {} of capacity {} are in use".format(
+                    T, cache.max_len, cache.capacity))
             x = self._embed_prologue(emb, None)
-            attn_bias = self._step_rel_pos_bias(cache, x) if self.rel_pos else None
+            attn_bias = self._step_rel_pos_bias(cache, x, T) if self.rel_pos else None
             for layer, lc in zip(self.layers, cache.layers):
                 x = layer(x, encoder_out=encoder_out, attn_bias=attn_bias, encoder_padding_mask=encoder_padding_mask,
                           encoder_attn_bias=encoder_attn_mask, cache=lc)
-            cache.seqlens += 1
-            cache.max_len += 1
+            cache.seqlens += T
+            cache.max_len += T
         if self.final_layer_norm is not None:
             x = self.final_layer_norm(x)
         return x

@@ -24,9 +24,13 @@ bottom-right convention when ``Lq != Lk``).  It combines with the bias, the key 
 take it as a flag: no mask tensor is read, and the key tiles above the diagonal are never computed, in the forward or
 the backward pass.  ``causal=True`` with ``return_logits=True`` runs ``attention_reference``.
 
-``attention_with_kv_cache`` is the decoding step: one query per sequence against a ``[B, C, H, D]`` key / value cache,
-optionally appending the new token's key and value first.  It runs in ``csrc/attn/fmha_decode_sm90.cu`` (split-KV,
-fp32 on the CUDA cores) for every head dim the fused kernels take, and has no backward.
+``attention_with_kv_cache`` is the decoding step: T queries per sequence against a ``[B, C, H, D]`` key / value cache,
+optionally appending the new tokens' keys and values first.  One query (T = 1) runs in
+``csrc/attn/fmha_decode_sm90.cu`` (split-KV, fp32 on the CUDA cores).  A chunk (T > 1: a prompt continued after some
+decoding, a chunked prefill, the candidates of speculative decoding) runs in the KV-cache mode of the wgmma forward
+(``csrc/attn/fmha_fwd_sm90.cu``), after a small kernel that appends its rows: query ``i`` of sequence ``b`` sees the
+cache rows up to ``seqlens[b] + i``, so K and V are streamed once per 64-query tile instead of once per token.  Both
+take every head dim the fused kernels take and have no backward.
 """
 import math
 
@@ -221,9 +225,9 @@ def _check_no_grad(*tensors):
 
 
 def _visible_bound(C, max_len, append, bias, key_padding_mask):
-    """Host bound on the visible keys of any batch: ``max_len`` (+1 when appending), else ``C``; never more than the
-    columns of the bias and of the key mask (the kernel clamps to them as well)."""
-    bound = C if max_len is None else min(C, int(max_len) + (1 if append else 0))
+    """Host bound on the visible keys of any batch: ``max_len`` (+ the ``append`` new rows), else ``C``; never more
+    than the columns of the bias and of the key mask (the kernel clamps to them as well)."""
+    bound = C if max_len is None else min(C, int(max_len) + int(append))
     if bias is not None:
         bound = min(bound, bias.shape[-1])
     if key_padding_mask is not None:
@@ -235,45 +239,67 @@ def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len
                                       bias=None, key_padding_mask=None, scale=None):
     """Plain PyTorch implementation of ``attention_with_kv_cache`` (CPU path, fallback and test oracle).
 
-    Performs the append in place like the kernel: row ``seqlens[b]`` (clamped to ``C - 1``) of the caches becomes
-    ``k_new[b] / v_new[b]``.  Keys past the visible length are masked; a row with no visible unmasked key gives 0.
+    Performs the append in place like the kernels.  One query (T = 1): row ``seqlens[b]`` (clamped to ``C - 1``) of the
+    caches becomes ``k_new[b] / v_new[b]``.  A chunk (T > 1): rows ``p_b + i``, ``p_b = seqlens[b]`` clamped to
+    ``[0, C]``, become ``k_new[b, i] / v_new[b, i]``, rows at or past ``C`` are skipped, and query ``i`` sees key ``j``
+    only when ``j <= p_b + i``.  Keys past the visible length are masked; a row with no visible unmasked key gives 0.
     """
-    B, _, H, D = q.shape
+    B, T, H, D = q.shape
     C = k_cache.shape[1]
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     append = k_new is not None
-    if append:
-        if seqlens is None:
-            raise ValueError("appending needs seqlens (the row to write)")
+    if append and seqlens is None:
+        raise ValueError("appending needs seqlens (the row to write)")
+    if T > 1 and seqlens is not None and not append:
+        raise ValueError("a chunk of T > 1 queries with seqlens appends k_new / v_new")
+    future = None
+    if T == 1 and append:
         pos = seqlens.long().clamp(0, C - 1)
         rows = torch.arange(B, device=k_cache.device)
         k_cache[rows, pos] = k_new[:, 0].to(k_cache.dtype)
         v_cache[rows, pos] = v_new[:, 0].to(v_cache.dtype)
         n = pos + 1
+    elif append:
+        p = seqlens.long().to(k_cache.device).clamp(0, C)
+        pos = p[:, None] + torch.arange(T, device=k_cache.device)[None, :]   # [B, T]
+        rows = torch.arange(B, device=k_cache.device)
+        for i in range(T):   # one row per sequence at a time; a row at or past C keeps row C - 1 as it is
+            at, keep = pos[:, i].clamp(max=C - 1), (pos[:, i] >= C)[:, None, None]
+            k_cache[rows, at] = torch.where(keep, k_cache[rows, at], k_new[:, i].to(k_cache.dtype))
+            v_cache[rows, at] = torch.where(keep, v_cache[rows, at], v_new[:, i].to(v_cache.dtype))
+        n = (p + T).clamp(max=C)
+        future = pos.to(q.device)   # query i of batch b sees keys j <= p_b + i
     elif seqlens is not None:
         n = seqlens.long().clamp(0, C)
     else:
         n = torch.full((B,), C, dtype=torch.long, device=q.device)
-    K = _visible_bound(C, max_len if seqlens is not None else None, append, bias, key_padding_mask)
+    K = _visible_bound(C, max_len if seqlens is not None else None, T if append else 0, bias, key_padding_mask)
     k, v = k_cache[:, :K], v_cache[:, :K]
-    scores = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale   # [B, H, 1, K]
+    scores = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale   # [B, H, T, K]
     if bias is not None:
         scores = scores + bias[..., :K].to(scores.dtype)
-    hidden = torch.arange(K, device=q.device)[None, :] >= n.to(q.device)[:, None]   # [B, K]
+    keys = torch.arange(K, device=q.device)
+    hidden = keys[None, :] >= n.to(q.device)[:, None]   # [B, K]
     # rows past the visible length are never read by the kernel: whatever they hold (NaN included) must not matter
     v = v.masked_fill(hidden[:, :, None, None], 0)
     if key_padding_mask is not None:
         hidden = hidden | key_padding_mask[:, :K].to(torch.bool)
-    scores = scores.masked_fill(hidden[:, None, None, :], float("-inf"))
+    hidden = hidden[:, None, None, :]   # [B, 1, 1, K]
+    if future is not None:
+        hidden = hidden | (keys[None, None, :] > future[:, :, None])[:, None]   # [B, 1, T, K]
+    scores = scores.masked_fill(hidden, float("-inf"))
     probs = torch.nan_to_num(F.softmax(scores.float(), dim=-1), nan=0.0).to(q.dtype)   # all masked -> 0
     return torch.einsum("bhqk,bkhd->bqhd", probs, v)
 
 
 def _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask) -> bool:
+    """True when ``fmha_decode`` (T = 1) or ``kvcache.fmha_kvcache_fwd`` (T > 1) takes the operands."""
     if not use_native(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask) \
             or not hasattr(native(), "fmha_decode"):
         return False
-    if q.dim() != 4 or q.shape[1] != 1 or q.dtype not in (torch.float16, torch.bfloat16):
+    if q.dim() != 4 or q.shape[1] < 1 or q.dtype not in (torch.float16, torch.bfloat16):
+        return False
+    if q.shape[1] > 1 and not hasattr(native(), "kvcache"):
         return False
     if not fused_head_dim_supported(q.shape[-1]):
         return False
@@ -291,37 +317,63 @@ def _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padd
 
 def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_new=None, v_new=None, bias=None,
                             key_padding_mask=None, scale=None):
-    """One decoding step of attention against a key / value cache.
+    """Attention of T new queries per sequence against a key / value cache: one decoding step (T = 1) or a chunk.
 
-    q: ``[B, 1, H, D]``; k_cache / v_cache: ``[B, C, H, D]`` (strided views are fine, the last dim contiguous).
-    The visible keys of batch b are rows ``0 .. seqlens[b] - 1``, plus row ``seqlens[b]`` when appending; with
-    ``seqlens=None`` all C rows are (cross-attention).  ``k_new`` / ``v_new`` ``[B, 1, H, D]``: the new token's key
-    and value, written bitwise into row ``seqlens[b]`` of the caches before the attention (needs ``seqlens``).
-    ``max_len``: a host-side upper bound on ``seqlens`` (default: the most the capacity allows); the device lengths are
-    never read on the host, so a step does not synchronise.  bias: ``[1|B, H, 1, Lb]``, ``Lb`` covering the visible
-    keys (columns past them are ignored); key_padding_mask: bool ``[B, Lk]``, True = masked.  A row whose visible keys
-    are all masked gives 0.  Returns ``[B, 1, H, D]``.  No dropout and no backward."""
+    q: ``[B, T, H, D]``; k_cache / v_cache: ``[B, C, H, D]`` (strided views are fine, the last dim contiguous).
+    ``k_new`` / ``v_new`` ``[B, T, H, D]`` (needs ``seqlens``): the new tokens' keys and values, written bitwise into
+    rows ``seqlens[b] .. seqlens[b] + T - 1`` of the caches before the attention.  Query ``i`` of batch b then sees
+    rows ``0 .. seqlens[b] + i`` (the future mask of the whole sequence); with ``seqlens=None`` every query sees all C
+    rows (cross-attention).  At T = 1, ``seqlens`` without ``k_new`` shows rows ``0 .. seqlens[b] - 1``; a chunk with
+    ``seqlens`` must append.  ``max_len``: a host-side upper bound on ``seqlens`` (default: the most the capacity
+    allows); ``max_len + T > C`` raises, and the device lengths are never read on the host, so a step does not
+    synchronise.  bias: ``[1|B, H, T, Lb]``, row i for query i, ``Lb`` covering the visible keys (columns past them
+    are ignored); key_padding_mask: bool ``[B, Lk]``, True = masked.  A query whose visible keys are all masked gives
+    0.  Returns ``[B, T, H, D]``.  No dropout and no backward."""
     _check_no_grad(q, k_cache, v_cache, k_new, v_new, bias)
     append = k_new is not None
     if append != (v_new is not None):
         raise ValueError("k_new and v_new go together")
     if append and seqlens is None:
         raise ValueError("appending needs seqlens (the row to write)")
+    T = q.shape[1]
+    if T > 1 and seqlens is not None and not append:
+        raise ValueError("a chunk of T > 1 queries with seqlens appends k_new / v_new")
     C = k_cache.shape[1]
+    new_rows = T if append else 0
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
     if seqlens is not None and max_len is None:
-        max_len = C - (1 if append else 0)
-    if max_len is not None and int(max_len) + (1 if append else 0) > C:
-        raise ValueError("max_len {} {}exceeds the cache capacity {}".format(max_len, "+ 1 " if append else "", C))
+        max_len = C - new_rows
+    if max_len is not None and int(max_len) + new_rows > C:
+        raise ValueError("max_len {} {}exceeds the cache capacity {}".format(
+            max_len, "+ {} ".format(new_rows) if append else "", C))
     if not _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask):
         return attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
                                                  key_padding_mask, scale)
     if seqlens is not None and (seqlens.dtype != torch.int32 or not seqlens.is_contiguous()):
         seqlens = seqlens.to(torch.int32).contiguous()
-    if bias is not None and (bias.dtype != q.dtype or bias.stride(-1) != 1):
-        bias = bias.to(q.dtype).contiguous()
     if key_padding_mask is not None and (key_padding_mask.dtype != torch.bool or key_padding_mask.stride(-1) != 1):
         key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
-    return native().fmha_decode(q, k_cache, v_cache, seqlens, 0 if max_len is None else int(max_len), k_new, v_new,
-                                bias, key_padding_mask, float(scale))
+    max_len = 0 if max_len is None else int(max_len)
+    if T == 1:
+        if bias is not None and (bias.dtype != q.dtype or bias.stride(-1) != 1):
+            bias = bias.to(q.dtype).contiguous()
+        return native().fmha_decode(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias, key_padding_mask,
+                                    float(scale))
+    bound = C if seqlens is None else max_len + T
+    if bias is not None:
+        # the kernel reads the bias by TMA (rows of a multiple of 8 columns); the padding is -inf, so a bias narrower
+        # than the visible keys hides the keys past it, as the reference's clamp to its columns does
+        Lb = bias.shape[-1]
+        width = max(Lb, bound) + (-max(Lb, bound)) % 8
+        bias = bias.to(q.dtype).expand(bias.shape[0], q.shape[2], T, Lb)
+        if width != Lb:
+            bias = F.pad(bias, (0, width - Lb), value=float("-inf"))
+        bias = bias.contiguous()
+    if key_padding_mask is not None:
+        cols = key_padding_mask.shape[1]
+        if cols < bound:   # the same for a key mask narrower than the visible keys: the keys past it are masked
+            key_padding_mask = torch.cat([key_padding_mask, key_padding_mask.new_ones(q.shape[0], bound - cols)], 1)
+        key_padding_mask = key_padding_mask.contiguous()
+    return native().kvcache.fmha_kvcache_fwd(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
+                                             key_padding_mask, float(scale))
