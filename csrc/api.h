@@ -152,12 +152,26 @@ void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const fl
                                     bool deterministic = false);
 // ---- Gaussian radial basis of (mul[edge] * d + bias[edge]) (Uni-Mol pair features), csrc/fused/gaussian.cu ----------
 // y: [n, K] in `dtype` (fp16 / bf16), K a multiple of 8 with K / 8 a power of two <= 32
+
+// Launch plan of a grid-stride kernel: `grid` CTAs take `items_per_sweep` of its `items` work items per pass over the
+// grid, `sweeps` passes cover them all (the last one ragged unless items % items_per_sweep == 0).
+struct SweepPlan {
+  int grid;
+  long long items, items_per_sweep, sweeps;
+};
+
 // token-major [B, L, T, H, D] <-> T head-major [B, H, L, D] tensors (null head pointer = zeros when gathering);
 // slice 0 is multiplied by scale0 in either direction.  D * sizeof(elem) must be a multiple of 16.
+// The launcher runs head_permute_plan: an item is one 16-byte vector of one of a pair of neighbouring tokens (an odd
+// L leaves the second token of the last pair idle), 256 threads per CTA, at most 16 CTAs per SM.
+SweepPlan head_permute_plan(int B, int L, int T, int H, int D, int dtype);
 void launch_head_permute(void* token_major, void* const* head_major, int B, int L, int T, int H, int D, float scale0,
                          bool to_heads, int dtype, cudaStream_t stream);
 
 // head-major [B, H, M] <-> pair-major [B, M, H] for 16-bit elements (H % 8 == 0, M % 8 == 0)
+// The transpose and both tail kernels run pair_plan: an item is one 8 x 8 tile (8 heads x 8 pair rows), 256 threads
+// per CTA, at most 8 CTAs per SM.
+SweepPlan pair_plan(int B, int H, long long M);
 void launch_pair_transpose(const void* in, void* out, int B, int H, long long M, bool to_pair, cudaStream_t stream);
 // encoder tail of pair-bias models: pair = T(z) with -inf -> 0, delta = T(z - z0) with padded keys -> 0 (Lk % 8 == 0)
 void launch_pair_tail_fwd(const void* z, const void* z0, const unsigned char* key_pad, void* pair, void* delta, int B,
@@ -165,6 +179,13 @@ void launch_pair_tail_fwd(const void* z, const void* z0, const unsigned char* ke
 void launch_pair_tail_bwd(const void* d_pair, const void* d_delta, const void* z, const unsigned char* key_pad, void* dz,
                           void* dz0, int B, int H, int Lq, int Lk, int dtype, cudaStream_t stream);
 
+// Launch plan of the embedding-gradient kernels (at most 132 x 16 CTAs each): the scatter runs a warp per row of dy and
+// the finalize a warp per vocabulary row (8 per CTA); the sorted kernel runs a CTA per vocabulary row (grid 0: the
+// launcher launches nothing).
+struct EmbeddingPlan {
+  SweepPlan scatter, finalize, sorted;
+};
+EmbeddingPlan embedding_plan(long long rows, long long vocab);
 // Embedding gradient without a sort: grad[token[r], :] (+)= dy[r, :], fp32 accumulation in `scratch` [vocab, cols]
 // (persistent, all zero between calls) with `touched` [vocab] row flags; rows equal to padding_idx contribute nothing.
 // accumulate != 0: add to grad (the optimizer's arena view); else touched rows are overwritten (grad pre-zeroed).

@@ -312,6 +312,38 @@ pybind11::dict gbf_plan(int64_t n, int64_t K, int64_t E) {
   return d;
 }
 
+pybind11::dict sweep_dict(const ub::SweepPlan& p) {
+  pybind11::dict d;
+  d["grid"] = p.grid;
+  d["items"] = p.items;
+  d["items_per_sweep"] = p.items_per_sweep;
+  d["sweeps"] = p.sweeps;
+  return d;
+}
+
+pybind11::dict head_permute_plan(int64_t B, int64_t L, int64_t T, int64_t H, int64_t D, at::ScalarType dtype) {
+  const int64_t esz = c10::elementSize(dtype);
+  TORCH_CHECK(B >= 1 && L >= 1 && T >= 1 && T <= 4 && H >= 1 && D >= 1 && (D * esz) % 16 == 0,
+              "head_permute_plan needs positive sizes, 1 <= T <= 4 and a head_dim of whole 16-byte vectors");
+  return sweep_dict(ub::head_permute_plan((int)B, (int)L, (int)T, (int)H, (int)D, dtype_tag(dtype)));
+}
+
+pybind11::dict pair_plan(int64_t B, int64_t H, int64_t M) {
+  TORCH_CHECK(B >= 1 && H >= 8 && H % 8 == 0 && M >= 8 && M % 8 == 0,
+              "pair_plan needs B >= 1 and positive multiples of 8 for H and M");
+  return sweep_dict(ub::pair_plan((int)B, (int)H, M));
+}
+
+pybind11::dict embedding_plan(int64_t rows, int64_t vocab) {
+  TORCH_CHECK(rows >= 0 && vocab >= 1, "embedding_plan needs rows >= 0 and vocab >= 1");
+  const ub::EmbeddingPlan p = ub::embedding_plan(rows, vocab);
+  pybind11::dict d;
+  d["scatter"] = sweep_dict(p.scatter);
+  d["finalize"] = sweep_dict(p.finalize);
+  d["sorted"] = sweep_dict(p.sorted);
+  return d;
+}
+
 // ---------------------------------------------------------------------------------------------------
 // softmax + dropout
 // ---------------------------------------------------------------------------------------------------
@@ -474,7 +506,8 @@ Tensor column_sum(const Tensor& x, const OptTensor& sink) {
 }
 
 // grad[tokens[r], :] (+)= dy[r, :]  (csrc/fused/embedding.cu); scratch fp32 [V, D] and touched uint8 [V] are persistent,
-// zero between calls.  `grad` is either the parameter's arena view (accumulate) or a zero-filled tensor.
+// zero between calls.  `grad` is either the parameter's arena view (accumulate) or a zero-filled tensor.  dy and grad
+// are read as 16-byte vectors, scratch with float4 loads and red.global.add.v4.f32, so all three are kVec.
 void embedding_bwd(const Tensor& dy, const Tensor& tokens, int64_t padding_idx, Tensor scratch, Tensor touched, Tensor grad,
                    bool accumulate) {
   check_operand(dy, "dy", dy.device(), k16Bit, {}, kVec);
@@ -483,7 +516,7 @@ void embedding_bwd(const Tensor& dy, const Tensor& tokens, int64_t padding_idx, 
   const long long vocab = grad.size(0);
   TORCH_CHECK(cols > 0 && cols % 8 == 0 && dy.dim() >= 1 && dy.size(-1) == cols, "embedding_bwd: shape mismatch");
   check_operand(tokens, "tokens", dy.device(), {at::kLong}, {dy.numel() / cols}, kContig | kNumel);
-  check_operand(scratch, "scratch", dy.device(), {at::kFloat}, {vocab * cols}, kContig | kNumel);
+  check_operand(scratch, "scratch", dy.device(), {at::kFloat}, {vocab * cols}, kVec | kNumel);
   check_operand(touched, "touched", dy.device(), {at::kByte}, {vocab}, kContig | kNumel);
   const c10::cuda::CUDAGuard guard(dy.device());
   const int tag = dtype_tag(dy.scalar_type());
@@ -651,9 +684,10 @@ Tensor merge_heads(const std::vector<OptTensor>& heads, double scale0) {
 // ---------------------------------------------------------------------------------------------------
 // pair representation relayout
 // ---------------------------------------------------------------------------------------------------
-// Every pair operand is a 4-D fp16 / bf16 tensor read as 16-byte vectors; key_padding_mask is bool / uint8 [B, Lk].
+// Every pair operand is a 4-D fp16 / bf16 tensor read as 16-byte vectors; key_padding_mask is bool / uint8 [B, Lk],
+// read 8 flags at a time with 8-byte loads, so it is kVec too.
 static const unsigned char* key_pad_ptr(const OptTensor& key_pad, const Tensor& z, int64_t Lk) {
-  check_operand(key_pad, "key_padding_mask", z.device(), {at::kBool, at::kByte}, {z.size(0), Lk});
+  check_operand(key_pad, "key_padding_mask", z.device(), {at::kBool, at::kByte}, {z.size(0), Lk}, kVec);
   return static_cast<const unsigned char*>(opt_ptr(key_pad));
 }
 
@@ -787,6 +821,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         pybind11::arg("aligned") = true, pybind11::arg("kind") = "fwd");
   m.def("bias_gelu_plan", &bias_gelu_plan, pybind11::arg("rows"), pybind11::arg("cols"), pybind11::arg("kind"));
   m.def("gbf_plan", &gbf_plan, pybind11::arg("n"), pybind11::arg("K"), pybind11::arg("E"));
+  m.def("head_permute_plan", &head_permute_plan, pybind11::arg("B"), pybind11::arg("L"), pybind11::arg("T"),
+        pybind11::arg("H"), pybind11::arg("D"), pybind11::arg("dtype"));
+  m.def("pair_plan", &pair_plan, pybind11::arg("B"), pybind11::arg("H"), pybind11::arg("M"));
+  m.def("embedding_plan", &embedding_plan, pybind11::arg("rows"), pybind11::arg("vocab"));
   m.def("softmax_dropout_fwd", &softmax_dropout_fwd);
   m.def("softmax_dropout_bwd", &softmax_dropout_bwd);
   m.def("softmax_dropout_logits_fwd", &softmax_dropout_logits_fwd);

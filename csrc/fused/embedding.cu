@@ -150,13 +150,35 @@ __global__ void __launch_bounds__(kEmbDetThreads) embedding_sorted_kernel(const 
   }
 }
 
+constexpr long long kEmbGridCap = 132 * 16;
+
+// `items` units of work, `per_cta` of them per CTA, on at most kEmbGridCap CTAs
+SweepPlan emb_sweep(long long items, long long per_cta) {
+  SweepPlan p;
+  long long grid = (items + per_cta - 1) / per_cta;
+  if (grid > kEmbGridCap) grid = kEmbGridCap;
+  p.grid = (int)grid;
+  p.items = items;
+  p.items_per_sweep = grid * per_cta;
+  p.sweeps = grid > 0 ? (items + p.items_per_sweep - 1) / p.items_per_sweep : 0;
+  return p;
+}
+
 }  // namespace
+
+EmbeddingPlan embedding_plan(long long rows, long long vocab) {
+  EmbeddingPlan p;
+  p.scatter = emb_sweep(rows, kEmbThreads / 32);  // a warp per row
+  p.finalize = emb_sweep(vocab, kEmbThreads / 32);  // a warp per vocabulary row
+  p.sorted = emb_sweep(rows == 0 ? 0 : vocab, 1);  // a CTA per vocabulary row
+  return p;
+}
 
 void launch_embedding_bwd_sorted(const void* dy, const long long* sorted, const long long* perm, void* grad,
                                  long long rows, int cols, long long vocab, long long padding_idx, int accumulate,
                                  int dtype, cudaStream_t stream) {
   if (rows == 0 || vocab == 0) return;
-  const unsigned grid = (unsigned)(vocab < 132 * 16 ? vocab : 132 * 16);
+  const unsigned grid = (unsigned)embedding_plan(rows, vocab).sorted.grid;
   if (dtype == kBF16)
     embedding_sorted_kernel<__nv_bfloat16><<<grid, kEmbDetThreads, 0, stream>>>(
         reinterpret_cast<const __nv_bfloat16*>(dy), sorted, perm, reinterpret_cast<__nv_bfloat16*>(grad), rows, cols,
@@ -170,12 +192,8 @@ void launch_embedding_bwd_sorted(const void* dy, const long long* sorted, const 
 void launch_embedding_bwd(const void* dy, const long long* tokens, float* scratch, unsigned char* touched, void* grad,
                           long long rows, int cols, long long vocab, long long padding_idx, int accumulate, int dtype,
                           cudaStream_t stream) {
-  const int warps_per_block = kEmbThreads / 32;
-  long long b1 = (rows + warps_per_block - 1) / warps_per_block;
-  if (b1 > 132 * 16) b1 = 132 * 16;
-  long long b2 = (vocab + warps_per_block - 1) / warps_per_block;
-  if (b2 > 132 * 16) b2 = 132 * 16;
-  if (rows == 0) b1 = 0;
+  const EmbeddingPlan plan = embedding_plan(rows, vocab);
+  const long long b1 = plan.scatter.grid, b2 = plan.finalize.grid;
   if (dtype == kBF16) {
     if (b1 > 0)
       embedding_scatter_kernel<__nv_bfloat16><<<(unsigned)b1, kEmbThreads, 0, stream>>>(

@@ -228,15 +228,21 @@ static PairGeom make_pair_geom(int B, int H, int L, long long M) {
   return g;
 }
 
-static int pair_grid(const PairGeom& g) {
-  const long long total = (long long)g.B * g.HV * g.MV;
+SweepPlan pair_plan(int B, int H, long long M) {
+  SweepPlan p;
+  p.items = (long long)B * (H / 8) * (M / 8);
   int sms = 132, dev = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long blocks = (total + 255) / 256;
+  long long blocks = (p.items + 255) / 256;
   const long long cap = (long long)sms * 8;
-  return (int)(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
+  p.grid = (int)(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
+  p.items_per_sweep = (long long)p.grid * 256;
+  p.sweeps = (p.items + p.items_per_sweep - 1) / p.items_per_sweep;
+  return p;
 }
+
+static int pair_grid(const PairGeom& g) { return pair_plan(g.B, g.H, g.M).grid; }
 
 void launch_pair_transpose(const void* in, void* out, int B, int H, long long M, bool to_pair, cudaStream_t stream) {
   if (B <= 0 || H <= 0 || M <= 0) return;

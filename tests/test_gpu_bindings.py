@@ -142,7 +142,7 @@ CASES = {
     "bias_gelu_bwd": (lambda: [_r(4, 64), _r(4, 64), _r(64), _r(64)],
                       {1: ("x", NO_SMALL_V), 0: ("dy", VEC), 2: ("bias", VEC), 3: ("dbias_sink", CONTIG)}),
     "embedding_bwd": (_embedding, {0: ("dy", NO_SMALL_V), 5: ("grad", VEC), 1: ("tokens", CONTIG),
-                                   3: ("scratch", CONTIG), 4: ("touched", CONTIG)}),
+                                   3: ("scratch", VEC), 4: ("touched", CONTIG)}),
     "column_sum": (lambda: [_r(4, 64), _r(64)], {0: ("x", NO_SMALL_V), 1: ("sink", CONTIG)}),
     "bias_dropout_add_ln_fwd": (lambda: [_r(4, 64), _r(64), _r(4, 64), _r(64), _r(64), 0.1, 1e-5],
                                 {0: ("x", VEC), 1: ("bias", VEC), 2: ("residual", VEC), 3: ("gamma", VEC),
@@ -160,10 +160,10 @@ CASES = {
                                                                               (0, 0): ("heads", VEC)}),
     "pair_transpose": (lambda: [_r(1, 8, 8, 8), True], {0: ("input", VEC)}),
     "pair_tail_fwd": (lambda: [_r(1, 8, 8, 8), _r(1, 8, 8, 8), torch.zeros(1, 8, dtype=torch.bool, device="cuda")],
-                      {0: ("logits", VEC), 1: ("input bias", VEC), 2: ("key_padding_mask", CONTIG)}),
+                      {0: ("logits", VEC), 1: ("input bias", VEC), 2: ("key_padding_mask", VEC)}),
     "pair_tail_bwd": (lambda: [_r(1, 8, 8, 8), _r(1, 8, 8, 8), _r(1, 8, 8, 8),
                                torch.zeros(1, 8, dtype=torch.bool, device="cuda")],
-                      {2: ("logits", VEC), 0: ("d_pair", VEC), 1: ("d_delta", VEC), 3: ("key_padding_mask", CONTIG)}),
+                      {2: ("logits", VEC), 0: ("d_pair", VEC), 1: ("d_delta", VEC), 3: ("key_padding_mask", VEC)}),
     "gbf_fwd": (_gbf, {0: ("d", NO_SMALL_C), 1: ("edge", CONTIG), 2: ("mul_w", NO_SMALL_C), 3: ("bias_w", CONTIG),
                        4: ("means", NO_SMALL_C), 5: ("stds", CONTIG)}),
     "gbf_bwd": (lambda: _gbf(dy=True), {1: ("d", NO_SMALL_C), 0: ("dy", CONTIG), 2: ("edge", CONTIG),
@@ -196,9 +196,10 @@ CASES = {
 
 # callables without tensor operands: launch plans and queries, the symmetric-memory allocation, and the collectives
 # that take raw peer addresses only
-EXEMPT = {"norm_plan", "softmax_plan", "bias_gelu_plan", "gbf_plan", "fmha_decode_max_splits", "fmha_decode_num_splits",
-          "fmha_det_timeouts", "symm_allreduce", "symm_reduce_scatter", "symm_pick_algo", "symm_error_channel",
-          "symm_tail_max_blocks", "symm_mem_supported", "symm_multicast_supported", "SymmAllocation"}
+EXEMPT = {"norm_plan", "softmax_plan", "bias_gelu_plan", "gbf_plan", "head_permute_plan", "pair_plan", "embedding_plan",
+          "fmha_decode_max_splits", "fmha_decode_num_splits", "fmha_det_timeouts", "symm_allreduce", "symm_reduce_scatter",
+          "symm_pick_algo", "symm_error_channel", "symm_tail_max_blocks", "symm_mem_supported", "symm_multicast_supported",
+          "SymmAllocation"}
 
 
 def _call(name, args):
@@ -303,6 +304,20 @@ def test_fmha_backward_checks_lse_bits_and_dout():
         a[i] = bad
         with pytest.raises(RuntimeError, match=label):
             nat.fmha_bwd(*a)
+
+
+def test_layout_plans_reject_shapes_no_launcher_takes():
+    """The exempt launch-plan queries of the relayout and embedding kernels check their sizes as the bindings do."""
+    nat = _nat()
+    for args in ((0, 8, 3, 2, 8, F16), (2, 8, 5, 2, 8, F16), (2, 8, 3, 2, 4, F16), (2, 8, 3, 2, 6, F32)):
+        with pytest.raises(RuntimeError, match="head_permute_plan needs"):
+            nat.head_permute_plan(*args)
+    for args in ((0, 8, 64), (1, 12, 64), (1, 8, 60), (1, 8, 0)):
+        with pytest.raises(RuntimeError, match="pair_plan needs"):
+            nat.pair_plan(*args)
+    for args in ((-1, 10), (10, 0)):
+        with pytest.raises(RuntimeError, match="embedding_plan needs"):
+            nat.embedding_plan(*args)
 
 
 def test_zero_width_inputs_raise_instead_of_dividing_by_zero():

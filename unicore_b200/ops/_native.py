@@ -56,7 +56,8 @@ _LAUNCHES_PER_CALL = {
     # not kernels: allocation / capability queries
     "SymmAllocation": 0, "symm_error_channel": 0, "symm_mem_supported": 0, "symm_multicast_supported": 0,
     "symm_tail_max_blocks": 0, "symm_pick_algo": 0, "norm_v2_supported": 0,
-    "norm_plan": 0, "softmax_plan": 0, "bias_gelu_plan": 0, "gbf_plan": 0, "fmha_decode_max_splits": 0,
+    "norm_plan": 0, "softmax_plan": 0, "bias_gelu_plan": 0, "gbf_plan": 0, "head_permute_plan": 0, "pair_plan": 0,
+    "embedding_plan": 0, "fmha_decode_max_splits": 0,
     "fmha_decode_num_splits": 0,
 }
 _launch_count = 0

@@ -335,7 +335,10 @@ class _EmbeddingFn(torch.autograd.Function):
     def forward(ctx, tokens, weight, padding_idx):
         ctx.save_for_backward(tokens, weight)
         ctx.padding_idx = -1 if padding_idx is None else int(padding_idx)
-        ctx.w_sink = grad_sink.claim(weight, ctx.needs_input_grad[1])
+        # the kernels write the sink with 16-byte vectors; flat arenas pad parameters to 2 elements only, so an arena
+        # view may start 4-byte aligned: its gradient then goes through autograd (AccumulateGrad adds it to the view)
+        aligned = weight.grad is not None and weight.grad.data_ptr() % 16 == 0
+        ctx.w_sink = grad_sink.claim(weight, ctx.needs_input_grad[1] and aligned)
         return F.embedding(tokens, weight, padding_idx)
 
     @staticmethod
@@ -359,6 +362,8 @@ def embedding(tokens: torch.Tensor, weight: torch.Tensor, padding_idx: Optional[
     """``F.embedding`` whose backward is two kernels (fp32 ``red`` scatter + finalize, ``csrc/fused/embedding.cu``)
     instead of ATen's radix sort + segmented reduction (~30 launches per BERT-base step), writing into the
     gradient arena when the weight is claimed."""
+    if padding_idx is not None and padding_idx < 0:
+        padding_idx += weight.shape[0]  # F.embedding's convention: -1 is the last row (an index < -V stays invalid)
     if (
         use_native(weight) and torch.is_grad_enabled() and weight.requires_grad
         and weight.dtype in (torch.float16, torch.bfloat16) and weight.dim() == 2 and weight.shape[1] % 8 == 0

@@ -10,7 +10,7 @@ from typing import Optional, Sequence, Tuple
 
 import torch
 
-from ._native import native, use_native
+from ._native import aligned_param, native, use_native
 
 
 def _eligible(x: torch.Tensor, head_dim: int) -> bool:
@@ -48,8 +48,7 @@ class _SplitHeadsFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, *grads):
-        grads = [None if g is None else g.contiguous() for g in grads]
-        return native().merge_heads(grads, ctx.scale0), None, None, None
+        return native().merge_heads([aligned_param(g) for g in grads], ctx.scale0), None, None, None
 
 
 class _MergeHeadsFn(torch.autograd.Function):
@@ -62,7 +61,7 @@ class _MergeHeadsFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad):
-        parts = native().split_heads(grad.contiguous(), ctx.count, ctx.num_heads, ctx.scale0)
+        parts = native().split_heads(aligned_param(grad), ctx.count, ctx.num_heads, ctx.scale0)
         return (None,) + tuple(parts)
 
 
@@ -72,7 +71,9 @@ def split_heads(x: torch.Tensor, num_slices: int, num_heads: int, scale0: float 
         raise ValueError("expected [B, L, T*H*D], got {}".format(tuple(x.shape)))
     head_dim = x.shape[-1] // (num_slices * num_heads)
     if 1 <= num_slices <= 4 and _eligible(x, head_dim):
-        return _SplitHeadsFn.apply(x.contiguous(), num_slices, num_heads, float(scale0))
+        # the kernel moves 16-byte vectors: a view at an odd element offset is copied once (aligned_param), here and
+        # for every tensor below that reaches a binding
+        return _SplitHeadsFn.apply(aligned_param(x), num_slices, num_heads, float(scale0))
     return _split_reference(x.contiguous(), num_slices, num_heads, float(scale0))
 
 
@@ -82,7 +83,7 @@ def merge_heads(*heads: torch.Tensor, scale0: float = 1.0) -> torch.Tensor:
     if ref.dim() != 4:
         raise ValueError("expected [B, H, L, D], got {}".format(tuple(ref.shape)))
     if 1 <= len(heads) <= 4 and _eligible(ref, ref.shape[-1]):
-        return _MergeHeadsFn.apply(float(scale0), *[h.contiguous() for h in heads])
+        return _MergeHeadsFn.apply(float(scale0), *[aligned_param(h) for h in heads])
     return _merge_reference(list(heads), float(scale0))
 
 
@@ -108,20 +109,20 @@ class _PairTransposeFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad):
-        return native().pair_transpose(grad.contiguous(), not ctx.to_pair), None
+        return native().pair_transpose(aligned_param(grad), not ctx.to_pair), None
 
 
 def heads_to_pair(x: torch.Tensor) -> torch.Tensor:
     """``[B, H, Lq, Lk] -> [B, Lq, Lk, H]`` (contiguous) - register-tile transpose, see ``csrc/fused/pair_layout.cu``."""
     if x.dim() == 4 and _pair_eligible(x, x.shape[1], x.shape[2], x.shape[3], False):
-        return _PairTransposeFn.apply(x.contiguous(), True)
+        return _PairTransposeFn.apply(aligned_param(x), True)
     return x.permute(0, 2, 3, 1).contiguous()
 
 
 def pair_to_heads(x: torch.Tensor) -> torch.Tensor:
     """``[B, Lq, Lk, H] -> [B, H, Lq, Lk]`` (contiguous)."""
     if x.dim() == 4 and _pair_eligible(x, x.shape[3], x.shape[1], x.shape[2], False):
-        return _PairTransposeFn.apply(x.contiguous(), False)
+        return _PairTransposeFn.apply(aligned_param(x), False)
     return x.permute(0, 3, 1, 2).contiguous()
 
 
@@ -136,9 +137,7 @@ class _PairTailFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, d_pair, d_delta):
         z, key_pad = ctx.saved_tensors
-        dz, dz0 = native().pair_tail_bwd(
-            None if d_pair is None else d_pair.contiguous(), None if d_delta is None else d_delta.contiguous(), z, key_pad
-        )
+        dz, dz0 = native().pair_tail_bwd(aligned_param(d_pair), aligned_param(d_delta), z, key_pad)
         return dz, (dz0 if ctx.need_z0 else None), None
 
 
@@ -156,8 +155,8 @@ def pair_tail(logits: torch.Tensor, input_bias: torch.Tensor, key_padding_mask: 
     if key_padding_mask is not None:
         key_padding_mask = key_padding_mask.to(torch.bool)
     if _pair_eligible(logits, heads, lq, lk, True) and input_bias.dtype == logits.dtype:
-        pad = None if key_padding_mask is None else key_padding_mask.contiguous()
-        return _PairTailFn.apply(logits.contiguous(), input_bias.contiguous(), pad)
+        # the mask is read 8 flags at a time: it is copied like the logits when its view is not 16-byte aligned
+        return _PairTailFn.apply(aligned_param(logits), aligned_param(input_bias), aligned_param(key_padding_mask))
     delta = logits - input_bias
     if key_padding_mask is not None:
         delta = delta.masked_fill(key_padding_mask[:, None, None, :], 0)
