@@ -96,6 +96,10 @@ void launch_rmsnorm_fwd(const void* x, const void* gamma, void* y, float* rstd, 
 void launch_rmsnorm_bwd(const void* dy, const void* x, const float* rstd, const void* gamma, void* dx, void* dgamma,
                         float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate = 0,
                         bool deterministic = false);
+// out[cols] (16-bit `dtype`) = column sums of the fp32 partial rows part[parts][cols] (parts == 0: zeros), in the
+// summation order of the norm backward's parameter gradients; accumulate != 0 adds them to what out holds
+void launch_colsum_finalize(const float* part, int parts, int cols, void* out, int accumulate, int dtype,
+                            cudaStream_t stream);
 
 // ---- softmax + dropout ---------------------------------------------------------------------------------------
 // Launch plan of the softmax-dropout kernels (the launchers run exactly this plan).  `aligned`: every buffer of the
@@ -179,9 +183,9 @@ void launch_pair_tail_fwd(const void* z, const void* z0, const unsigned char* ke
 void launch_pair_tail_bwd(const void* d_pair, const void* d_delta, const void* z, const unsigned char* key_pad, void* dz,
                           void* dz0, int B, int H, int Lq, int Lk, int dtype, cudaStream_t stream);
 
-// Launch plan of the embedding-gradient kernels (at most 132 x 16 CTAs each): the scatter runs a warp per row of dy and
-// the finalize a warp per vocabulary row (8 per CTA); the sorted kernel runs a CTA per vocabulary row (grid 0: the
-// launcher launches nothing).
+// Launch plan of the embedding-gradient kernels (at most 16 CTAs per SM each): the scatter runs a warp per row of dy
+// and the finalize a warp per vocabulary row (8 per CTA); the sorted kernel runs a CTA per vocabulary row (grid 0:
+// the launcher launches nothing).
 struct EmbeddingPlan {
   SweepPlan scatter, finalize, sorted;
 };

@@ -32,8 +32,6 @@
 #include <cuda_fp16.h>
 #include <math_constants.h>
 
-#include <algorithm>
-
 #include "../common.cuh"
 #include "fmha_api.h"
 #include "wgmma.cuh"
@@ -65,27 +63,6 @@ struct BwdCfg {
 };
 static_assert(BwdCfg<64>::kOffStats == 81920 && BwdCfg<64>::kSmemBytes == 85024,
               "DP = 64 keeps the shared memory map of the 64-only kernel");
-
-template <typename T>
-UB_DEVICE uint32_t bwd_pack2(float a, float b);
-template <>
-UB_DEVICE uint32_t bwd_pack2<__half>(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-template <>
-UB_DEVICE uint32_t bwd_pack2<__nv_bfloat16>(float a, float b) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-template <typename T>
-UB_DEVICE float2 bwd_unpack2(uint32_t w) {
-  if constexpr (std::is_same<T, __half>::value) {
-    return __half22float2(*reinterpret_cast<const __half2*>(&w));
-  } else {
-    return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
-  }
-}
 
 // Column layout of the fp32 dQ tile in shared memory and of its accumulator rows in global memory (the bulk reduction
 // copies the tile linearly): the 8-column (32-byte) group of column `col` in row q is stored at group ^ (q & 7).  A
@@ -359,7 +336,7 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
       for (int r = 0; r < 4; ++r) {   // r: rows (key kl0 or kl1) x query half (16sb + 2c or 16sb + 8 + 2c)
         const int e = 8 * sb + 2 * r;
         const int ql = 16 * sb + 8 * (r >> 1) + 2 * c;
-        const float2 bb = has_bias ? bwd_unpack2<T>(bias_r[r]) : make_float2(0.f, 0.f);
+        const float2 bb = has_bias ? unpack2<T>(bias_r[r]) : make_float2(0.f, 0.f);
         const float ka = (r & 1) ? kadd1 : kadd0;
         const float2 l2 = *reinterpret_cast<const float2*>(lse2_s + ql);
         float ka0 = ka, ka1 = ka;
@@ -403,12 +380,12 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
         float ds0 = p0 * (dp[e] * (k0 ? keep_scale : 0.f) - dl.x);
         float ds1 = p1 * (dp[e + 1] * (k1 ? keep_scale : 0.f) - dl.y);
         if constexpr (kLogits) {
-          const float2 dz = bwd_unpack2<T>(dz_r[r]);
+          const float2 dz = unpack2<T>(dz_r[r]);
           ds0 += dz.x;
           ds1 += dz.y;
         }
-        pa[sb][r] = bwd_pack2<T>(k0 ? p0 : 0.f, k1 ? p1 : 0.f);   // keep_scale is applied to dV in the epilogue
-        da[sb][r] = bwd_pack2<T>(ds0, ds1);                         // the softmax scale to dQ / dK at read-out
+        pa[sb][r] = pack2<T>(k0 ? p0 : 0.f, k1 ? p1 : 0.f);   // keep_scale is applied to dV in the epilogue
+        da[sb][r] = pack2<T>(ds0, ds1);                         // the softmax scale to dQ / dK at read-out
       }
     }
 
@@ -489,8 +466,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     for (int n = 0; n < DP / 8; ++n) {
       if (8 * n >= p.D) continue;   // columns 8n + 2c, +1 exist iff 8n < D (D % 8 == 0)
       const int e = 4 * n + 2 * half;
-      *reinterpret_cast<uint32_t*>(dvg + 8 * n + 2 * c) = bwd_pack2<T>(dv[e] * keep_scale, dv[e + 1] * keep_scale);
-      *reinterpret_cast<uint32_t*>(dkg + 8 * n + 2 * c) = bwd_pack2<T>(dk[e] * p.scale, dk[e + 1] * p.scale);
+      *reinterpret_cast<uint32_t*>(dvg + 8 * n + 2 * c) = pack2<T>(dv[e] * keep_scale, dv[e + 1] * keep_scale);
+      *reinterpret_cast<uint32_t*>(dkg + 8 * n + 2 * c) = pack2<T>(dk[e] * p.scale, dk[e + 1] * p.scale);
     }
   }
 }
@@ -530,16 +507,6 @@ __global__ void __launch_bounds__(256) fmha_dbias_reduce_kernel(const T* __restr
   }
 }
 
-int device_sms() {
-  static int sms = [] {
-    int dev = 0, n = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    return n > 0 ? n : 132;
-  }();
-  return sms;
-}
-
 template <typename T, int DP>
 void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
   const FmhaFwdParams& p = bp.f;
@@ -562,19 +529,16 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
   } else if (bp.dlogits != nullptr) run(fmha_bwd_kernel<T, DP, true, false>, BwdCfg<DP, true>::kSmemBytes);
   else if (p.causal) run(fmha_bwd_kernel<T, DP, false, true>, BwdCfg<DP, false>::kSmemBytes);
   else run(fmha_bwd_kernel<T, DP, false, false>, BwdCfg<DP, false>::kSmemBytes);
-  const long long cap = (long long)device_sms() * 16;
   if (bp.ds_buf != nullptr && bp.dbias != bp.ds_buf) {
     const long long nv = (long long)p.H * p.Lq * p.Lk / 8;
-    const long long rb = std::min((nv + 255) / 256, cap);
     auto reduce = p.causal ? fmha_dbias_reduce_kernel<T, true> : fmha_dbias_reduce_kernel<T, false>;
-    reduce<<<(unsigned)rb, 256, 0, stream>>>(reinterpret_cast<const T*>(bp.ds_buf), reinterpret_cast<T*>(bp.dbias), p.B,
-                                             nv, p.Lq, p.Lk);
+    reduce<<<sweep_plan(nv, 256, 16).grid, 256, 0, stream>>>(reinterpret_cast<const T*>(bp.ds_buf),
+                                                            reinterpret_cast<T*>(bp.dbias), p.B, nv, p.Lq, p.Lk);
   }
   const long long nvec = nrows * (p.D / 8);
-  const long long blocks = std::min((nvec + 255) / 256, cap);
-  fmha_dq_convert_kernel<T><<<(unsigned)blocks, 256, 0, stream>>>(bp.dq_acc, reinterpret_cast<T*>(bp.dq), p.H, p.Lq,
-                                                                  n_qt * kBM, p.D, DP, nvec, p.scale, bp.dq_sb, bp.dq_sl,
-                                                                  bp.dq_sh);
+  fmha_dq_convert_kernel<T><<<sweep_plan(nvec, 256, 16).grid, 256, 0, stream>>>(
+      bp.dq_acc, reinterpret_cast<T*>(bp.dq), p.H, p.Lq, n_qt * kBM, p.D, DP, nvec, p.scale, bp.dq_sb, bp.dq_sl,
+      bp.dq_sh);
 }
 
 }  // namespace

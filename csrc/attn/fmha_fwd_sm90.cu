@@ -60,27 +60,6 @@ struct FwdCfg {
 };
 static_assert(FwdCfg<64>::kSmemBytes == 108608, "DP = 64 keeps the shared memory map of the 64-only kernel");
 
-template <typename T>
-UB_DEVICE uint32_t pack2(float a, float b);
-template <>
-UB_DEVICE uint32_t pack2<__half>(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-template <>
-UB_DEVICE uint32_t pack2<__nv_bfloat16>(float a, float b) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-template <typename T>
-UB_DEVICE float2 unpack2(uint32_t w) {
-  if constexpr (std::is_same<T, __half>::value) {
-    return __half22float2(*reinterpret_cast<const __half2*>(&w));
-  } else {
-    return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
-  }
-}
-
 // w[j] <- w[j ^ x] for x in 0..3 (per-thread), as two conditional swaps: 8 selects, no runtime-indexed array
 UB_DEVICE void xor_permute4(uint32_t (&w)[4], int x) {
   const bool s1 = (x & 1) != 0, s2 = (x & 2) != 0;

@@ -332,99 +332,63 @@ __global__ void softmax_dropout_bwd_scalar(const T* dy, T* dx, const T* probs, S
 }
 
 // ---- host ------------------------------------------------------------------------------------------------------
-static int sm_count2() {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
-  }
-  return sms;
-}
-
 static bool make_sm_geom(SmGeom& g, long long rows, int K, int epv, int& vpt) {
   g.rows = rows;
   g.K = K;
   if (K % epv != 0) return false;
   g.nvec = K / epv;
-  int p2 = 1;
-  while (p2 < g.nvec) p2 <<= 1;
-  if (g.nvec <= 128) {
-    g.tpr = p2 < 32 ? p2 : 32;
-  } else {
-    int need = (g.nvec + 3) / 4;
-    p2 = 1;
-    while (p2 < need) p2 <<= 1;
-    g.tpr = p2;
-  }
-  if (g.tpr > 256) return false;
-  vpt = (g.nvec + g.tpr - 1) / g.tpr;
-  return vpt <= 4;
+  return row_group_geom(g.nvec, g.tpr, vpt);
 }
-
-#define UB_SM_VPT(VPT_VALUE, ...)                              \
-  switch (VPT_VALUE) {                                         \
-    case 1: { constexpr int VPT = 1; __VA_ARGS__; break; }     \
-    case 2: { constexpr int VPT = 2; __VA_ARGS__; break; }     \
-    case 3: { constexpr int VPT = 3; __VA_ARGS__; break; }     \
-    case 4: { constexpr int VPT = 4; __VA_ARGS__; break; }     \
-    default: break;                                            \
-  }
 
 // The kernels are grid-stride loops over rows: launch exactly as many CTAs as fit on the machine at once.  (A fixed
 // "8 per SM" left the register-limited kernels with 1.6 waves: the second wave ran on 60 % of the SMs.)
 template <typename Kernel>
-static int resident_blocks(Kernel kernel) {
+static int resident_per_sm(Kernel kernel) {
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kSmThreads, 0) != cudaSuccess || per_sm < 1) per_sm = 2;
-  return per_sm * sm_count2();
+  return per_sm;
 }
 
 template <typename T, int VPT>
 static int resident_fwd() {
-  static const int n = resident_blocks(softmax_dropout_fwd_kernel<T, VPT>);
+  static const int n = resident_per_sm(softmax_dropout_fwd_kernel<T, VPT>);
   return n;
 }
 
 template <typename T, int VPT>
 static int resident_bwd() {
-  static const int n = resident_blocks(softmax_dropout_bwd_kernel<T, VPT>);
+  static const int n = resident_per_sm(softmax_dropout_bwd_kernel<T, VPT>);
   return n;
 }
 
 template <typename T>
 static SoftmaxPlan plan_sm(long long rows, int K, bool aligned, bool bwd, SmGeom& g) {
   SoftmaxPlan pl{};
+  SweepPlan s;
   int vpt = 0;
   if (make_sm_geom(g, rows, K, VecTraits<T>::kElems, vpt) && aligned) {
-    const int rows_per_cta = kSmThreads / g.tpr;
-    const long long need = (rows + rows_per_cta - 1) / rows_per_cta;
-    int resident = 0;
-    UB_SM_VPT(vpt, resident = bwd ? resident_bwd<T, VPT>() : resident_fwd<T, VPT>());
+    int per_sm = 0;
+    UB_DISPATCH_VPT(vpt, per_sm = bwd ? resident_bwd<T, VPT>() : resident_fwd<T, VPT>());
+    s = sweep_plan(rows, kSmThreads / g.tpr, per_sm);
     pl.vec = 1;
     pl.vpt = vpt;
     pl.tpr = g.tpr;
-    pl.grid = (int)(need < resident ? need : resident);
     pl.threads = kSmThreads;
-    pl.rows_per_sweep = (long long)pl.grid * rows_per_cta;
   } else {  // scalar kernels: 8 warps per CTA, one row per warp
-    const long long need = (rows + 7) / 8;
-    const long long cap = (long long)sm_count2() * 8;
+    s = sweep_plan(rows, 8, 8);
     pl.tpr = 32;
-    pl.grid = (int)(need < cap ? need : cap);
     pl.threads = 256;
-    pl.rows_per_sweep = (long long)pl.grid * 8;
   }
-  pl.sweeps = pl.rows_per_sweep > 0 ? (rows + pl.rows_per_sweep - 1) / pl.rows_per_sweep : 0;
+  pl.grid = s.grid;
+  pl.rows_per_sweep = s.items_per_sweep;
+  pl.sweeps = s.sweeps;
   return pl;
 }
 
 SoftmaxPlan softmax_plan(long long rows, int K, int dtype, bool aligned, bool bwd) {
   SmGeom g;
-  if (dtype == kF32) return plan_sm<float>(rows, K, aligned, bwd, g);
-  if (dtype == kF16) return plan_sm<__half>(rows, K, aligned, bwd, g);
-  return plan_sm<__nv_bfloat16>(rows, K, aligned, bwd, g);
+  UB_DISPATCH_FLOAT(dtype, return plan_sm<T>(rows, K, aligned, bwd, g));
+  return SoftmaxPlan{};
 }
 
 // 1 / P(keep) for the 14-bit threshold the kernels compare against (mirrors dropout_thresh14)
@@ -452,7 +416,7 @@ static void run_sm_fwd(void* x, void* out, const void* mask, const void* bias, l
   g.bias_rows = bias_rows > 0 ? bias_rows : 1;
   const float keep_scale = keep_scale_for(p);
   if (pl.vec) {
-    UB_SM_VPT(pl.vpt, {
+    UB_DISPATCH_VPT(pl.vpt, {
       softmax_dropout_fwd_kernel<T, VPT><<<pl.grid, kSmThreads, 0, stream>>>(
           (const T*)x, (T*)probs, (T*)out, (const T*)mask, (const T*)bias, g, p, keep_scale, seed, offset, (T*)logits, lse);
     });
@@ -472,7 +436,7 @@ static void run_sm_bwd(const void* dy, void* dx, const void* probs, long long ro
   g.bias_rows = 1;
   const float keep_scale = keep_scale_for(p);
   if (pl.vec) {
-    UB_SM_VPT(pl.vpt, {
+    UB_DISPATCH_VPT(pl.vpt, {
       softmax_dropout_bwd_kernel<T, VPT><<<pl.grid, kSmThreads, 0, stream>>>(
           (const T*)dy, (T*)dx, (const T*)probs, g, p, keep_scale, seed, offset, lse, (const T*)addend);
     });
@@ -487,21 +451,15 @@ void launch_softmax_dropout_fwd(void* x, void* out, const void* mask, const void
                                 unsigned long long offset, int dtype, cudaStream_t stream, void* logits, float* lse,
                                 void* probs) {
   if (rows <= 0 || K <= 0) return;
-  if (dtype == kF32)
-    run_sm_fwd<float>(x, out, mask, bias, rows, K, mask_div, bias_rows, p, seed, offset, logits, lse, stream, probs);
-  else if (dtype == kF16)
-    run_sm_fwd<__half>(x, out, mask, bias, rows, K, mask_div, bias_rows, p, seed, offset, logits, lse, stream, probs);
-  else
-    run_sm_fwd<__nv_bfloat16>(x, out, mask, bias, rows, K, mask_div, bias_rows, p, seed, offset, logits, lse, stream, probs);
+  UB_DISPATCH_FLOAT(dtype, run_sm_fwd<T>(x, out, mask, bias, rows, K, mask_div, bias_rows, p, seed, offset, logits, lse,
+                                         stream, probs));
 }
 
 void launch_softmax_dropout_bwd(const void* dy, void* dx, const void* probs, long long rows, int K, float p,
                                 unsigned long long seed, unsigned long long offset, int dtype, cudaStream_t stream,
                                 const float* lse, const void* addend) {
   if (rows <= 0 || K <= 0) return;
-  if (dtype == kF32) run_sm_bwd<float>(dy, dx, probs, rows, K, p, seed, offset, lse, addend, stream);
-  else if (dtype == kF16) run_sm_bwd<__half>(dy, dx, probs, rows, K, p, seed, offset, lse, addend, stream);
-  else run_sm_bwd<__nv_bfloat16>(dy, dx, probs, rows, K, p, seed, offset, lse, addend, stream);
+  UB_DISPATCH_FLOAT(dtype, run_sm_bwd<T>(dy, dx, probs, rows, K, p, seed, offset, lse, addend, stream));
 }
 
 }  // namespace ub

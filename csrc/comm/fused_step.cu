@@ -23,6 +23,7 @@
 //   P4  peer barrier: all parameter shards have landed everywhere; the next forward may start.
 //
 // Only CTA 0 talks to the peers; the CTAs of one GPU meet at a counter barrier in local memory (cooperative launch).
+#include "../optim/adam_math.cuh"
 #include "comm_device.cuh"
 
 namespace ub {
@@ -46,17 +47,6 @@ UB_DEVICE void grid_barrier(unsigned int* gs) {
     __threadfence();
   }
   __syncthreads();
-}
-
-UB_DEVICE void tail_adam_math(float& p, float& m, float& v, float g, const TailGroup& G) {
-  m = G.beta1 * m + (1.f - G.beta1) * g;
-  v = G.beta2 * v + (1.f - G.beta2) * g * g;
-  p = p * G.decay_mul - G.step_size * (m / (sqrtf(v) + G.eps));
-}
-UB_DEVICE uint32_t tail_bf16_sr(float x, uint32_t rnd16) {
-  uint32_t bits = __float_as_uint(x);
-  if ((bits & 0x7f800000u) != 0x7f800000u) bits += rnd16;  // inf / nan stay as they are
-  return bits >> 16;
 }
 
 // ---- P1: reduce-scatter of this rank's slice [lo_vec, hi_vec) (16-byte vectors) of a bucket ------------------------
@@ -142,7 +132,7 @@ UB_DEVICE void tail_adam_slice(const TailArgs& A, const TailGroup& G, const Tail
     unpack<float>(v0, v);
     unpack<float>(v1, v + 4);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) tail_adam_math(p[k], m[k], v[k], g[k] * gmul, G);
+    for (int k = 0; k < 8; ++k) adam_math(p[k], m[k], v[k], g[k] * gmul, G);
     st_global_v4(G.master + c, pack<float>(p));
     st_global_v4(G.master + c + 4, pack<float>(p + 4));
     st_global_v4(G.exp_avg + c, pack<float>(m));
@@ -154,7 +144,7 @@ UB_DEVICE void tail_adam_slice(const TailArgs& A, const TailGroup& G, const Tail
       unpack<float>(ld_global_v4(G.ema + i), e);
       unpack<float>(ld_global_v4(G.ema + i + 4), e + 4);
 #pragma unroll
-      for (int k = 0; k < 8; ++k) e[k] -= ema_w * (e[k] - p[k]);
+      for (int k = 0; k < 8; ++k) e[k] = ema_step(e[k], p[k], ema_w);
       st_global_v4(G.ema + i, pack<float>(e));
       st_global_v4(G.ema + i + 4, pack<float>(e + 4));
     }
@@ -163,8 +153,11 @@ UB_DEVICE void tail_adam_slice(const TailArgs& A, const TailGroup& G, const Tail
       const Philox4 r = philox4x32_10(A.seed, A.offset, (unsigned long long)i >> 3);
       const uint32_t rw[4] = {r.x, r.y, r.z, r.w};
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        o.w[k] = tail_bf16_sr(p[2 * k], rw[k] & 0xffffu) | (tail_bf16_sr(p[2 * k + 1], rw[k] >> 16) << 16);
+      for (int k = 0; k < 4; ++k) {
+        const uint32_t lo = bf16_sr_bits(p[2 * k], rw[k] & 0xffffu);
+        const uint32_t hi = bf16_sr_bits(p[2 * k + 1], rw[k] >> 16);
+        o.w[k] = lo | (hi << 16);
+      }
     } else {
       o = pack<T>(p);
     }
@@ -347,20 +340,8 @@ __global__ void __launch_bounds__(kMaxStats) stats_allreduce_kernel(CommPeers x,
 
 }  // namespace
 
-int fused_tail_max_blocks() {
-  static int blocks = 0;
-  if (blocks == 0) {
-    int dev = 0, sms = 0, per_sm = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fused_tail_kernel, kCommThreads, 0);
-    if (sms <= 0) sms = 132;
-    if (per_sm < 1) per_sm = 1;
-    blocks = sms;  // one CTA per SM: enough to saturate HBM and the links, always co-resident
-    (void)per_sm;
-  }
-  return blocks;
-}
+// one CTA per SM: enough to saturate HBM and the links, always co-resident
+int fused_tail_max_blocks() { return device_sm_count(); }
 
 void launch_fused_tail(const TailArgs& a, int blocks, cudaStream_t stream) {
   const int cap = fused_tail_max_blocks();

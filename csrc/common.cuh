@@ -3,11 +3,15 @@
 //   * warp / block reductions
 //   * counter-based Philox4x32-10 (no per-thread state, no curand_init)
 //   * dtype tags shared with the host binding (csrc/api.h)
+//   * host side: the SM count, grid-stride sweep plans, row-group geometry and dtype / VPT dispatch of the launchers
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <atomic>
+#include <type_traits>
 
 #include "api.h"
 
@@ -129,6 +133,28 @@ UB_DEVICE Vec16 pack<__nv_bfloat16>(const float* in) {
     v.w[i] = *reinterpret_cast<uint32_t*>(&h);
   }
   return v;
+}
+
+// one pair of 16-bit values <-> two fp32 (round to nearest)
+template <typename T>
+UB_DEVICE uint32_t pack2(float a, float b);
+template <>
+UB_DEVICE uint32_t pack2<__half>(float a, float b) {
+  __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+template <>
+UB_DEVICE uint32_t pack2<__nv_bfloat16>(float a, float b) {
+  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+template <typename T>
+UB_DEVICE float2 unpack2(uint32_t w) {
+  if constexpr (std::is_same<T, __half>::value) {
+    return __half22float2(*reinterpret_cast<const __half2*>(&w));
+  } else {
+    return make_float2(__uint_as_float(w << 16), __uint_as_float(w & 0xffff0000u));
+  }
 }
 
 // 14-bit dropout thresholds compared two at a time as fp16 bit patterns (HSET2): a random 16-bit
@@ -300,5 +326,71 @@ UB_DEVICE uint32_t dropout_thresh16(float p) {
   float t = p * 65536.f + 0.5f;
   return t >= 65535.f ? 65535u : (uint32_t)t;
 }
+
+// ------------------------------------------------------------------------------------------------
+// host: launch geometry and dispatch
+// ------------------------------------------------------------------------------------------------
+// Streaming multiprocessors of the current device, queried once per device ordinal (132, an H100 SXM, when the query
+// fails).
+inline int device_sm_count() {
+  constexpr int kMaxDevices = 64;
+  static std::atomic<int> cache[kMaxDevices];  // 0: not queried yet
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::atomic<int>* slot = dev >= 0 && dev < kMaxDevices ? &cache[dev] : nullptr;
+  int sms = slot != nullptr ? slot->load(std::memory_order_relaxed) : 0;
+  if (sms == 0) {
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    if (slot != nullptr) slot->store(sms, std::memory_order_relaxed);
+  }
+  return sms;
+}
+
+// Plan of a grid-stride kernel over `items` work items, `per_cta` of them per CTA and pass: as many CTAs as the items
+// need, at most `ctas_per_sm` per SM.  The grid is 0 exactly when there are no items.
+inline SweepPlan sweep_plan(long long items, long long per_cta, int ctas_per_sm) {
+  const long long need = (items + per_cta - 1) / per_cta, cap = (long long)device_sm_count() * ctas_per_sm;
+  SweepPlan p;
+  p.grid = (int)(need < cap ? need : cap);
+  p.items = items;
+  p.items_per_sweep = (long long)p.grid * per_cta;
+  p.sweeps = p.grid > 0 ? (items + p.items_per_sweep - 1) / p.items_per_sweep : 0;
+  return p;
+}
+
+// A row of `nvec` 16-byte vectors held in registers by a group of `tpr` threads (a power of two), `vpt` vectors each:
+// rows up to 128 vectors take a vector per thread on at most 32 threads, longer rows about four per thread on at most
+// 256.  False when that leaves more than 4 vectors per thread.
+inline bool row_group_geom(int nvec, int& tpr, int& vpt) {
+  const int want = nvec <= 128 ? nvec : (nvec + 3) / 4, max_tpr = nvec <= 128 ? 32 : 256;
+  tpr = 1;
+  while (tpr < want && tpr < max_tpr) tpr <<= 1;
+  vpt = (nvec + tpr - 1) / tpr;
+  return vpt <= 4;
+}
+
+// Host dispatch of a launcher body on a run-time value: the body is compiled once per case, with `T` the element type
+// of a dtype tag or `VPT` the vectors per thread of row_group_geom.  Other values run nothing.
+#define UB_DISPATCH_FLOAT(DTYPE_VALUE, ...)                               \
+  switch (DTYPE_VALUE) {                                                  \
+    case kF32: { using T = float; __VA_ARGS__; break; }                   \
+    case kF16: { using T = __half; __VA_ARGS__; break; }                  \
+    case kBF16: { using T = __nv_bfloat16; __VA_ARGS__; break; }          \
+    default: break;                                                       \
+  }
+#define UB_DISPATCH_16BIT(DTYPE_VALUE, ...)                               \
+  switch (DTYPE_VALUE) {                                                  \
+    case kF16: { using T = __half; __VA_ARGS__; break; }                  \
+    case kBF16: { using T = __nv_bfloat16; __VA_ARGS__; break; }          \
+    default: break;                                                       \
+  }
+#define UB_DISPATCH_VPT(VPT_VALUE, ...)                                   \
+  switch (VPT_VALUE) {                                                    \
+    case 1: { constexpr int VPT = 1; __VA_ARGS__; break; }                \
+    case 2: { constexpr int VPT = 2; __VA_ARGS__; break; }                \
+    case 3: { constexpr int VPT = 3; __VA_ARGS__; break; }                \
+    case 4: { constexpr int VPT = 4; __VA_ARGS__; break; }                \
+    default: break;                                                       \
+  }
 
 }  // namespace ub

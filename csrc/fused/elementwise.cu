@@ -11,17 +11,6 @@
 
 namespace ub {
 
-static int sm_count3() {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
-  }
-  return sms;
-}
-
 // ================================================================================================
 // bias + GELU
 //
@@ -151,32 +140,9 @@ __global__ void __launch_bounds__(256) bias_gelu_kernel(const T* __restrict__ dy
   }
 }
 
-// partial rows [parts][cols] fp32 -> column sums in T.  block = 32 columns x 32 row slices.
-template <typename T>
-__global__ void __launch_bounds__(1024) colsum_kernel(const float* __restrict__ part, int parts, int cols,
-                                                        T* __restrict__ out, int accumulate) {
-  __shared__ float red[32][33];
-  const int cx = threadIdx.x & 31, ry = threadIdx.x >> 5;
-  const int col = blockIdx.x * 32 + cx;
-  float a = 0.f;
-  if (col < cols) {
-#pragma unroll 4
-    for (int r = ry; r < parts; r += 32) a += part[(size_t)r * cols + col];
-  }
-  red[ry][cx] = a;
-  __syncthreads();
-  if (ry == 0 && col < cols) {
-    float s = 0.f;
-#pragma unroll
-    for (int r = 0; r < 32; ++r) s += red[r][cx];
-    if (accumulate) s += to_f32<T>(out[col]);  // straight into the optimizer's gradient arena
-    out[col] = from_f32<T>(s);
-  }
-}
-
 // Column sums of a [rows, cols] 16-bit matrix (bias gradient of a Linear layer: ATen runs a generic reduce at
 // ~2 TB/s for these shapes).  Same geometry as bias_gelu_kernel: a thread owns one 16-byte column vector, two row
-// lanes per CTA, kGeluUnroll rows in flight; fp32 partial rows, finished by colsum_kernel.
+// lanes per CTA, kGeluUnroll rows in flight; fp32 partial rows, finished by launch_colsum_finalize.
 template <typename T>
 __global__ void __launch_bounds__(256) column_sum_kernel(const T* __restrict__ x, float* __restrict__ part, int rows,
                                                            int nvec) {
@@ -229,7 +195,7 @@ ColumnPlan bias_gelu_plan(long long rows, int cols, bool fwd) {
   // The forward fits 5 CTAs per SM (48 registers): a grid of 16 CTAs per SM keeps the tail of the last wave short
   // (with 6, the 32 x 512 x 3072 fp16 forward ran 1.2 waves in 92 us, with 16 in 76 us: H100 80GB HBM3, 400 W limit).
   // The backward and the column sum keep 6 per SM: each slice adds a partial row to the final column pass.
-  long long slices = ((long long)sm_count3() * (fwd ? 16 : 6) + p.col_blocks - 1) / p.col_blocks;
+  long long slices = ((long long)device_sm_count() * (fwd ? 16 : 6) + p.col_blocks - 1) / p.col_blocks;
   const long long max_slices = (rows + 2 * kGeluUnroll - 1) / (2 * kGeluUnroll);
   if (slices > max_slices) slices = max_slices;
   p.slices = (int)(slices < 1 ? 1 : slices);
@@ -240,49 +206,37 @@ ColumnPlan bias_gelu_plan(long long rows, int cols, bool fwd) {
 
 int bias_gelu_parts(long long rows, int cols) { return bias_gelu_plan(rows, cols, false).slices; }
 
-template <typename T, bool kBwd>
-static void run_bias_gelu_t(const void* dy, const void* x, const void* bias, void* out, void* dbias, float* part,
-                            long long rows, int cols, cudaStream_t stream, int accumulate = 0) {
-  const ColumnPlan p = bias_gelu_plan(rows, cols, !kBwd);
-  dim3 grid(p.col_blocks, p.slices);
-  const bool want = kBwd && dbias != nullptr && part != nullptr;
-  bias_gelu_kernel<T, kBwd><<<grid, 256, 0, stream>>>((const T*)dy, (const T*)x, (const T*)bias, (T*)out,
-                                                      want ? part : nullptr, (int)rows, p.nvec);
-  if (want) colsum_kernel<T><<<(cols + 31) / 32, 1024, 0, stream>>>(part, p.slices, cols, (T*)dbias, accumulate);
-}
-
 // out[cols] = column sums of x[rows, cols]; part = float[bias_gelu_parts(rows, cols) * cols] scratch
 void launch_column_sum(const void* x, void* out, float* part, long long rows, int cols, int dtype, cudaStream_t stream,
                        int accumulate) {
-  if (rows <= 0 || cols <= 0) return;
+  if (cols <= 0) return;
   const ColumnPlan p = bias_gelu_plan(rows, cols, false);
-  const int nvec = p.nvec, slices = p.slices;
-  dim3 grid(p.col_blocks, slices);
-  if (dtype == kF16) {
-    column_sum_kernel<__half><<<grid, 256, 0, stream>>>((const __half*)x, part, (int)rows, nvec);
-    colsum_kernel<__half><<<(cols + 31) / 32, 1024, 0, stream>>>(part, slices, cols, (__half*)out, accumulate);
-  } else {
-    column_sum_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)x, part, (int)rows, nvec);
-    colsum_kernel<__nv_bfloat16><<<(cols + 31) / 32, 1024, 0, stream>>>(part, slices, cols, (__nv_bfloat16*)out, accumulate);
-  }
+  const int parts = rows > 0 ? p.slices : 0;  // no rows: zero sums
+  if (parts > 0)
+    UB_DISPATCH_16BIT(dtype, (column_sum_kernel<T><<<dim3(p.col_blocks, parts), 256, 0, stream>>>((const T*)x, part,
+                                                                                                (int)rows, p.nvec)));
+  launch_colsum_finalize(part, parts, cols, out, accumulate, dtype, stream);
 }
 
 void launch_bias_gelu_fwd(const void* x, const void* bias, void* y, long long rows, int cols, int dtype,
                           cudaStream_t stream) {
   if (rows <= 0 || cols <= 0) return;
-  if (dtype == kF16)
-    run_bias_gelu_t<__half, false>(nullptr, x, bias, y, nullptr, nullptr, rows, cols, stream);
-  else
-    run_bias_gelu_t<__nv_bfloat16, false>(nullptr, x, bias, y, nullptr, nullptr, rows, cols, stream);
+  const ColumnPlan p = bias_gelu_plan(rows, cols, true);
+  UB_DISPATCH_16BIT(dtype, (bias_gelu_kernel<T, false><<<dim3(p.col_blocks, p.slices), 256, 0, stream>>>(
+                               nullptr, (const T*)x, (const T*)bias, (T*)y, nullptr, (int)rows, p.nvec)));
 }
 // dbias (nullable): column sums of dx; part: float[bias_gelu_parts(rows, cols) * cols] scratch
 void launch_bias_gelu_bwd(const void* dy, const void* x, const void* bias, void* dx, void* dbias, float* part,
                           long long rows, int cols, int dtype, cudaStream_t stream, int accumulate) {
-  if (rows <= 0 || cols <= 0) return;
-  if (dtype == kF16)
-    run_bias_gelu_t<__half, true>(dy, x, bias, dx, dbias, part, rows, cols, stream, accumulate);
-  else
-    run_bias_gelu_t<__nv_bfloat16, true>(dy, x, bias, dx, dbias, part, rows, cols, stream, accumulate);
+  if (cols <= 0) return;
+  const ColumnPlan p = bias_gelu_plan(rows, cols, false);
+  const bool want = dbias != nullptr && part != nullptr;
+  const int parts = rows > 0 ? p.slices : 0;  // no rows: zero sums
+  if (parts > 0)
+    UB_DISPATCH_16BIT(dtype, (bias_gelu_kernel<T, true><<<dim3(p.col_blocks, parts), 256, 0, stream>>>(
+                                 (const T*)dy, (const T*)x, (const T*)bias, (T*)dx, want ? part : nullptr, (int)rows,
+                                 p.nvec)));
+  if (want) launch_colsum_finalize(part, parts, cols, dbias, accumulate, dtype, stream);
 }
 
 // ================================================================================================
@@ -427,31 +381,16 @@ __global__ void __launch_bounds__(kXentThreads) xent_bwd_kernel(const T* __restr
 void launch_softmax_xent_fwd(const void* logits, const long long* target, float* loss_rows, float* lse, int rows,
                              int cols, int stride, long long ignore_index, int dtype, cudaStream_t stream) {
   if (rows <= 0) return;
-  if (dtype == kF32)
-    xent_fwd_kernel<float><<<rows, kXentThreads, 0, stream>>>((const float*)logits, target, loss_rows, lse, cols,
-                                                              stride, ignore_index);
-  else if (dtype == kF16)
-    xent_fwd_kernel<__half><<<rows, kXentThreads, 0, stream>>>((const __half*)logits, target, loss_rows, lse, cols,
-                                                               stride, ignore_index);
-  else
-    xent_fwd_kernel<__nv_bfloat16><<<rows, kXentThreads, 0, stream>>>((const __nv_bfloat16*)logits, target, loss_rows,
-                                                                      lse, cols, stride, ignore_index);
+  UB_DISPATCH_FLOAT(dtype, (xent_fwd_kernel<T><<<rows, kXentThreads, 0, stream>>>(
+                               (const T*)logits, target, loss_rows, lse, cols, stride, ignore_index)));
 }
 
 void launch_softmax_xent_bwd(const void* logits, const long long* target, const float* lse, const float* dloss,
                              void* dlogits, int rows, int cols, int stride, long long ignore_index, int dtype,
                              cudaStream_t stream) {
   if (rows <= 0) return;
-  if (dtype == kF32)
-    xent_bwd_kernel<float><<<rows, kXentThreads, 0, stream>>>((const float*)logits, target, lse, dloss,
-                                                              (float*)dlogits, cols, stride, ignore_index);
-  else if (dtype == kF16)
-    xent_bwd_kernel<__half><<<rows, kXentThreads, 0, stream>>>((const __half*)logits, target, lse, dloss,
-                                                               (__half*)dlogits, cols, stride, ignore_index);
-  else
-    xent_bwd_kernel<__nv_bfloat16><<<rows, kXentThreads, 0, stream>>>((const __nv_bfloat16*)logits, target, lse,
-                                                                      dloss, (__nv_bfloat16*)dlogits, cols,
-                                                                      stride, ignore_index);
+  UB_DISPATCH_FLOAT(dtype, (xent_bwd_kernel<T><<<rows, kXentThreads, 0, stream>>>(
+                               (const T*)logits, target, lse, dloss, (T*)dlogits, cols, stride, ignore_index)));
 }
 
 }  // namespace ub

@@ -150,27 +150,13 @@ __global__ void __launch_bounds__(kEmbDetThreads) embedding_sorted_kernel(const 
   }
 }
 
-constexpr long long kEmbGridCap = 132 * 16;
-
-// `items` units of work, `per_cta` of them per CTA, on at most kEmbGridCap CTAs
-SweepPlan emb_sweep(long long items, long long per_cta) {
-  SweepPlan p;
-  long long grid = (items + per_cta - 1) / per_cta;
-  if (grid > kEmbGridCap) grid = kEmbGridCap;
-  p.grid = (int)grid;
-  p.items = items;
-  p.items_per_sweep = grid * per_cta;
-  p.sweeps = grid > 0 ? (items + p.items_per_sweep - 1) / p.items_per_sweep : 0;
-  return p;
-}
-
 }  // namespace
 
 EmbeddingPlan embedding_plan(long long rows, long long vocab) {
   EmbeddingPlan p;
-  p.scatter = emb_sweep(rows, kEmbThreads / 32);  // a warp per row
-  p.finalize = emb_sweep(vocab, kEmbThreads / 32);  // a warp per vocabulary row
-  p.sorted = emb_sweep(rows == 0 ? 0 : vocab, 1);  // a CTA per vocabulary row
+  p.scatter = sweep_plan(rows, kEmbThreads / 32, 16);  // a warp per row
+  p.finalize = sweep_plan(vocab, kEmbThreads / 32, 16);  // a warp per vocabulary row
+  p.sorted = sweep_plan(rows == 0 ? 0 : vocab, 1, 16);  // a CTA per vocabulary row
   return p;
 }
 
@@ -178,35 +164,22 @@ void launch_embedding_bwd_sorted(const void* dy, const long long* sorted, const 
                                  long long rows, int cols, long long vocab, long long padding_idx, int accumulate,
                                  int dtype, cudaStream_t stream) {
   if (rows == 0 || vocab == 0) return;
-  const unsigned grid = (unsigned)embedding_plan(rows, vocab).sorted.grid;
-  if (dtype == kBF16)
-    embedding_sorted_kernel<__nv_bfloat16><<<grid, kEmbDetThreads, 0, stream>>>(
-        reinterpret_cast<const __nv_bfloat16*>(dy), sorted, perm, reinterpret_cast<__nv_bfloat16*>(grad), rows, cols,
-        vocab, padding_idx, accumulate);
-  else
-    embedding_sorted_kernel<__half><<<grid, kEmbDetThreads, 0, stream>>>(reinterpret_cast<const __half*>(dy), sorted, perm,
-                                                                         reinterpret_cast<__half*>(grad), rows, cols,
-                                                                         vocab, padding_idx, accumulate);
+  const int grid = embedding_plan(rows, vocab).sorted.grid;
+  UB_DISPATCH_16BIT(dtype, (embedding_sorted_kernel<T><<<grid, kEmbDetThreads, 0, stream>>>(
+                               (const T*)dy, sorted, perm, (T*)grad, rows, cols, vocab, padding_idx, accumulate)));
 }
 
 void launch_embedding_bwd(const void* dy, const long long* tokens, float* scratch, unsigned char* touched, void* grad,
                           long long rows, int cols, long long vocab, long long padding_idx, int accumulate, int dtype,
                           cudaStream_t stream) {
   const EmbeddingPlan plan = embedding_plan(rows, vocab);
-  const long long b1 = plan.scatter.grid, b2 = plan.finalize.grid;
-  if (dtype == kBF16) {
-    if (b1 > 0)
-      embedding_scatter_kernel<__nv_bfloat16><<<(unsigned)b1, kEmbThreads, 0, stream>>>(
-          reinterpret_cast<const __nv_bfloat16*>(dy), tokens, scratch, touched, rows, cols, vocab, padding_idx);
-    embedding_finalize_kernel<__nv_bfloat16><<<(unsigned)b2, kEmbThreads, 0, stream>>>(
-        scratch, touched, reinterpret_cast<__nv_bfloat16*>(grad), vocab, cols, accumulate);
-  } else {
-    if (b1 > 0)
-      embedding_scatter_kernel<__half><<<(unsigned)b1, kEmbThreads, 0, stream>>>(
-          reinterpret_cast<const __half*>(dy), tokens, scratch, touched, rows, cols, vocab, padding_idx);
-    embedding_finalize_kernel<__half><<<(unsigned)b2, kEmbThreads, 0, stream>>>(scratch, touched, reinterpret_cast<__half*>(grad),
-                                                                               vocab, cols, accumulate);
-  }
+  UB_DISPATCH_16BIT(dtype, {
+    if (plan.scatter.grid > 0)
+      embedding_scatter_kernel<T><<<plan.scatter.grid, kEmbThreads, 0, stream>>>((const T*)dy, tokens, scratch, touched,
+                                                                                rows, cols, vocab, padding_idx);
+    embedding_finalize_kernel<T><<<plan.finalize.grid, kEmbThreads, 0, stream>>>(scratch, touched, (T*)grad, vocab,
+                                                                                 cols, accumulate);
+  });
 }
 
 }  // namespace ub

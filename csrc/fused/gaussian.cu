@@ -198,37 +198,29 @@ __global__ void __launch_bounds__(kGbfSumThreads) gbf_edge_sum_kernel(const floa
 }
 
 GbfPlan gbf_plan(long long n, int K, int E) {
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   GbfPlan p;
   p.kvec = K / 8;
   p.rows_per_cta = kGbfThreads / p.kvec;
-  const long long need = (n + p.rows_per_cta - 1) / p.rows_per_cta;
-  const long long cap = (long long)sms * 4;
-  p.grid = (int)(need < cap ? (need < 1 ? 1 : need) : cap);
-  p.rows_per_sweep = (long long)p.grid * p.rows_per_cta;
-  p.sweeps = (n + p.rows_per_sweep - 1) / p.rows_per_sweep;
+  const SweepPlan s = sweep_plan(n, p.rows_per_cta, 4);
+  p.grid = s.grid;
+  p.rows_per_sweep = s.items_per_sweep;
+  p.sweeps = s.sweeps;
   p.smem = (2 * E + 2 * K) * (int)sizeof(float);
   return p;
 }
 
 static int gbf_grid(long long n, int K) { return gbf_plan(n, K, 0).grid; }
 
+// (no rows: no partial rows, their column sums are zero)
 int gbf_parts(long long n, int K) { return gbf_grid(n, K); }
 
 void launch_gbf_fwd(const void* d, const long long* edge, const void* mul_w, const void* bias_w, const void* means,
                     const void* stds, void* y, long long n, int K, int dtype, cudaStream_t stream) {
   if (n <= 0) return;
   const int grid = gbf_grid(n, K);
-  if (dtype == kF16)
-    gbf_fwd_kernel<__half><<<grid, kGbfThreads, 0, stream>>>((const __half*)d, edge, (const __half*)mul_w,
-                                                             (const __half*)bias_w, (const __half*)means,
-                                                             (const __half*)stds, (__half*)y, n, K);
-  else
-    gbf_fwd_kernel<__nv_bfloat16><<<grid, kGbfThreads, 0, stream>>>(
-        (const __nv_bfloat16*)d, edge, (const __nv_bfloat16*)mul_w, (const __nv_bfloat16*)bias_w,
-        (const __nv_bfloat16*)means, (const __nv_bfloat16*)stds, (__nv_bfloat16*)y, n, K);
+  UB_DISPATCH_16BIT(dtype, (gbf_fwd_kernel<T><<<grid, kGbfThreads, 0, stream>>>(
+                               (const T*)d, edge, (const T*)mul_w, (const T*)bias_w, (const T*)means, (const T*)stds,
+                               (T*)y, n, K)));
 }
 
 void launch_gbf_bwd(const void* dy, const void* d, const long long* edge, const void* mul_w, const void* bias_w,
@@ -236,21 +228,13 @@ void launch_gbf_bwd(const void* dy, const void* d, const long long* edge, const 
                     cudaStream_t stream) {
   if (n <= 0) return;
   const GbfPlan plan = gbf_plan(n, K, E);
-  const int grid = plan.grid;
   const size_t smem = (size_t)plan.smem;
-  if (dtype == kF16) {
-    auto kern = gbf_bwd_kernel<__half>;
+  UB_DISPATCH_16BIT(dtype, {
+    auto kern = gbf_bwd_kernel<T>;
     if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, kGbfThreads, smem, stream>>>((const __half*)dy, (const __half*)d, edge, (const __half*)mul_w,
-                                              (const __half*)bias_w, (const __half*)means, (const __half*)stds, part,
-                                              hist, n, K, E);
-  } else {
-    auto kern = gbf_bwd_kernel<__nv_bfloat16>;
-    if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    kern<<<grid, kGbfThreads, smem, stream>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)d, edge,
-                                              (const __nv_bfloat16*)mul_w, (const __nv_bfloat16*)bias_w,
-                                              (const __nv_bfloat16*)means, (const __nv_bfloat16*)stds, part, hist, n, K, E);
-  }
+    kern<<<plan.grid, kGbfThreads, smem, stream>>>((const T*)dy, (const T*)d, edge, (const T*)mul_w, (const T*)bias_w,
+                                                   (const T*)means, (const T*)stds, part, hist, n, K, E);
+  });
 }
 
 void launch_gbf_bwd_det(const void* dy, const void* d, const long long* edge, const void* mul_w, const void* bias_w,
@@ -259,15 +243,10 @@ void launch_gbf_bwd_det(const void* dy, const void* d, const long long* edge, co
   if (n <= 0) return;
   const int grid = gbf_grid(n, K);
   const size_t smem = (size_t)kGbfThreads * 16 * sizeof(float);   // [rows_per_cta][2 * K] = 256 / (K / 8) * 2 * K
-  if (dtype == kF16)
-    gbf_bwd_kernel<__half, true><<<grid, kGbfThreads, smem, stream>>>(
-        (const __half*)dy, (const __half*)d, edge, (const __half*)mul_w, (const __half*)bias_w, (const __half*)means,
-        (const __half*)stds, part, rowg, n, K, E);
-  else
-    gbf_bwd_kernel<__nv_bfloat16, true><<<grid, kGbfThreads, smem, stream>>>(
-        (const __nv_bfloat16*)dy, (const __nv_bfloat16*)d, edge, (const __nv_bfloat16*)mul_w,
-        (const __nv_bfloat16*)bias_w, (const __nv_bfloat16*)means, (const __nv_bfloat16*)stds, part, rowg, n, K, E);
-  const int egrid = E < 132 * 8 ? E : 132 * 8;
+  UB_DISPATCH_16BIT(dtype, (gbf_bwd_kernel<T, true><<<grid, kGbfThreads, smem, stream>>>(
+                               (const T*)dy, (const T*)d, edge, (const T*)mul_w, (const T*)bias_w, (const T*)means,
+                               (const T*)stds, part, rowg, n, K, E)));
+  const int egrid = sweep_plan(E, 1, 8).grid;
   if (egrid > 0) gbf_edge_sum_kernel<<<egrid, kGbfSumThreads, 0, stream>>>(rowg, sorted, perm, hist, n, E);
 }
 

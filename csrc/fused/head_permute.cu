@@ -64,40 +64,20 @@ __global__ void __launch_bounds__(256) head_permute_kernel(void* token_major, He
 }
 
 SweepPlan head_permute_plan(int B, int L, int T, int H, int D, int dtype) {
-  SweepPlan p;
   const int dv = D / (dtype == kF32 ? 4 : 8);
-  p.items = (long long)B * T * ((L + 1) / 2) * H * 2 * dv;
-  int sms = 132;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long blocks = (p.items + 255) / 256;
-  const long long cap = (long long)sms * 16;
-  if (blocks > cap) blocks = cap;
-  p.grid = (int)blocks;
-  p.items_per_sweep = blocks * 256;
-  p.sweeps = blocks > 0 ? (p.items + p.items_per_sweep - 1) / p.items_per_sweep : 0;
-  return p;
+  return sweep_plan((long long)B * T * ((L + 1) / 2) * H * 2 * dv, 256, 16);
 }
 
-template <typename T>
-static void run_head_permute(void* token_major, const HeadPtrs& heads, int B, int L, int NT, int H, int DV, int grid,
-                             float scale0, bool to_heads, cudaStream_t stream) {
-  if (to_heads)
-    head_permute_kernel<T, true><<<grid, 256, 0, stream>>>(token_major, heads, B, L, NT, H, DV, scale0);
-  else
-    head_permute_kernel<T, false><<<grid, 256, 0, stream>>>(token_major, heads, B, L, NT, H, DV, scale0);
-}
-
-void launch_head_permute(void* token_major, void* const* head_major, int B, int L, int T, int H, int D, float scale0,
+void launch_head_permute(void* token_major, void* const* head_major, int B, int L, int NT, int H, int D, float scale0,
                          bool to_heads, int dtype, cudaStream_t stream) {
-  if (B <= 0 || L <= 0 || T <= 0 || H <= 0 || D <= 0) return;
+  if (B <= 0 || L <= 0 || NT <= 0 || H <= 0 || D <= 0) return;
   HeadPtrs heads;
-  for (int t = 0; t < 4; ++t) heads.p[t] = t < T ? head_major[t] : nullptr;
-  const int grid = head_permute_plan(B, L, T, H, D, dtype).grid;
-  if (dtype == kF32) run_head_permute<float>(token_major, heads, B, L, T, H, D / 4, grid, scale0, to_heads, stream);
-  else if (dtype == kF16) run_head_permute<__half>(token_major, heads, B, L, T, H, D / 8, grid, scale0, to_heads, stream);
-  else run_head_permute<__nv_bfloat16>(token_major, heads, B, L, T, H, D / 8, grid, scale0, to_heads, stream);
+  for (int t = 0; t < 4; ++t) heads.p[t] = t < NT ? head_major[t] : nullptr;
+  const int grid = head_permute_plan(B, L, NT, H, D, dtype).grid;
+  UB_DISPATCH_FLOAT(dtype, {
+    auto kern = to_heads ? head_permute_kernel<T, true> : head_permute_kernel<T, false>;
+    kern<<<grid, 256, 0, stream>>>(token_major, heads, B, L, NT, H, D / VecTraits<T>::kElems, scale0);
+  });
 }
 
 }  // namespace ub

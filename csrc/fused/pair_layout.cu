@@ -73,6 +73,10 @@ UB_DEVICE uint32_t as_word(T2 v) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// the packed pair type of a 16-bit element type
+template <typename T>
+using Pair2 = std::conditional_t<std::is_same<T, __half>::value, __half2, __nv_bfloat162>;
+
 template <typename T2>
 struct NegInf;
 template <>
@@ -228,19 +232,7 @@ static PairGeom make_pair_geom(int B, int H, int L, long long M) {
   return g;
 }
 
-SweepPlan pair_plan(int B, int H, long long M) {
-  SweepPlan p;
-  p.items = (long long)B * (H / 8) * (M / 8);
-  int sms = 132, dev = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  long long blocks = (p.items + 255) / 256;
-  const long long cap = (long long)sms * 8;
-  p.grid = (int)(blocks < cap ? (blocks > 0 ? blocks : 1) : cap);
-  p.items_per_sweep = (long long)p.grid * 256;
-  p.sweeps = (p.items + p.items_per_sweep - 1) / p.items_per_sweep;
-  return p;
-}
+SweepPlan pair_plan(int B, int H, long long M) { return sweep_plan((long long)B * (H / 8) * (M / 8), 256, 8); }
 
 static int pair_grid(const PairGeom& g) { return pair_plan(g.B, g.H, g.M).grid; }
 
@@ -255,18 +247,16 @@ void launch_pair_tail_fwd(const void* z, const void* z0, const unsigned char* ke
                           int H, int Lq, int Lk, int dtype, cudaStream_t stream) {
   if (B <= 0 || H <= 0 || Lq <= 0 || Lk <= 0) return;
   const PairGeom g = make_pair_geom(B, H, Lk, (long long)Lq * Lk);
-  if (dtype == kF16) pair_tail_fwd_kernel<__half2><<<pair_grid(g), 256, 0, stream>>>(z, z0, key_pad, pair, delta, g);
-  else pair_tail_fwd_kernel<__nv_bfloat162><<<pair_grid(g), 256, 0, stream>>>(z, z0, key_pad, pair, delta, g);
+  UB_DISPATCH_16BIT(dtype,
+                    (pair_tail_fwd_kernel<Pair2<T>><<<pair_grid(g), 256, 0, stream>>>(z, z0, key_pad, pair, delta, g)));
 }
 
 void launch_pair_tail_bwd(const void* d_pair, const void* d_delta, const void* z, const unsigned char* key_pad, void* dz,
                           void* dz0, int B, int H, int Lq, int Lk, int dtype, cudaStream_t stream) {
   if (B <= 0 || H <= 0 || Lq <= 0 || Lk <= 0) return;
   const PairGeom g = make_pair_geom(B, H, Lk, (long long)Lq * Lk);
-  if (dtype == kF16)
-    pair_tail_bwd_kernel<__half2><<<pair_grid(g), 256, 0, stream>>>(d_pair, d_delta, z, key_pad, dz, dz0, g);
-  else
-    pair_tail_bwd_kernel<__nv_bfloat162><<<pair_grid(g), 256, 0, stream>>>(d_pair, d_delta, z, key_pad, dz, dz0, g);
+  UB_DISPATCH_16BIT(dtype, (pair_tail_bwd_kernel<Pair2<T>><<<pair_grid(g), 256, 0, stream>>>(d_pair, d_delta, z,
+                                                                                            key_pad, dz, dz0, g)));
 }
 
 }  // namespace ub

@@ -1055,17 +1055,6 @@ static thread_local int g_acc_mask = 0;
 // in a fixed order
 static thread_local bool g_det = false;
 
-static int sm_count() {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
-  }
-  return sms;
-}
-
 static int pow2ceil(int v) {
   int p = 1;
   while (p < v) p <<= 1;
@@ -1122,7 +1111,7 @@ NormPlan norm_plan(int rows, int cols, int dtype, int kind) {
     const int warps = bwd ? kNormV3BwdWarps : kNormV3Warps;
     p.threads = warps * 32;
     p.tile_rows = (32 / p.lpr) * p.r;
-    cap = (long long)sm_count() * (bwd ? (p.vpl <= 1 ? 2 : 1) : (p.vpl <= 3 ? 3 : (p.vpl == 4 ? 2 : 1)));
+    cap = (long long)device_sm_count() * (bwd ? (p.vpl <= 1 ? 2 : 1) : (p.vpl <= 3 ? 3 : (p.vpl == 4 ? 2 : 1)));
     const long long need = ((long long)rows + warps * p.tile_rows - 1) / (warps * p.tile_rows);
     p.grid = (int)std::max(1ll, std::min(need, cap));
     p.units = (long long)p.grid * warps;
@@ -1135,19 +1124,17 @@ NormPlan norm_plan(int rows, int cols, int dtype, int kind) {
     p.threads = p.tpr * p.groups;
     p.tile_rows = p.groups * p.r;
     const long long need = ((long long)rows + p.tile_rows - 1) / p.tile_rows;
-    p.grid = (int)std::max(1ll, std::min(need, (long long)sm_count() * 2));
+    p.grid = (int)std::max(1ll, std::min(need, (long long)device_sm_count() * 2));
     p.units = p.grid;
   } else {
-    p.tpr = p.nvec <= 128 ? std::min(pow2ceil(p.nvec), 32) : std::min(pow2ceil((p.nvec + 3) / 4), kNormThreads);
-    p.vpt = (p.nvec + p.tpr - 1) / p.tpr;
-    if (p.vpt > 4) return NormPlan{};
+    if (!row_group_geom(p.nvec, p.tpr, p.vpt)) return NormPlan{};
     p.gen = 1;
     p.groups = kNormThreads / p.tpr;
     p.full = p.nvec == p.vpt * p.tpr;
     p.threads = kNormThreads;
     p.tile_rows = p.groups;
     const long long need = bwd ? ((long long)rows + 7) / 8 : ((long long)rows + p.tile_rows - 1) / p.tile_rows;
-    p.grid = (int)std::max(1ll, std::min(need, (long long)sm_count() * (bwd ? 2 : 8)));
+    p.grid = (int)std::max(1ll, std::min(need, (long long)device_sm_count() * (bwd ? 2 : 8)));
     p.units = p.grid;
   }
   const long long tiles = ((long long)rows + p.tile_rows - 1) / p.tile_rows;
@@ -1204,23 +1191,6 @@ static bool run_bwd_v3(const NormPlan& pl, const void* dy, const void* x, const 
   });
   return false;
 }
-
-#define UB_DISPATCH_VPT(VPT_VALUE, ...)                                   \
-  switch (VPT_VALUE) {                                                    \
-    case 1: { constexpr int VPT = 1; __VA_ARGS__; break; }                \
-    case 2: { constexpr int VPT = 2; __VA_ARGS__; break; }                \
-    case 3: { constexpr int VPT = 3; __VA_ARGS__; break; }                \
-    case 4: { constexpr int VPT = 4; __VA_ARGS__; break; }                \
-    default: break;                                                       \
-  }
-
-#define UB_DISPATCH_DTYPE(DTYPE_VALUE, ...)                               \
-  switch (DTYPE_VALUE) {                                                  \
-    case kF32: { using T = float; __VA_ARGS__; break; }                   \
-    case kF16: { using T = __half; __VA_ARGS__; break; }                  \
-    case kBF16: { using T = __nv_bfloat16; __VA_ARGS__; break; }          \
-    default: break;                                                       \
-  }
 
 template <typename T, bool kRMS, bool kFused>
 static void run_fwd(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd, int rows,
@@ -1284,9 +1254,15 @@ static void run_bwd(const void* dy, const void* x, const float* mean, const floa
   }
 }
 
+void launch_colsum_finalize(const float* part, int parts, int cols, void* out, int accumulate, int dtype,
+                            cudaStream_t stream) {
+  UB_DISPATCH_16BIT(dtype, (colsum_finalize_kernel<T><<<(cols + 31) / 32, 1024, 0, stream>>>(
+                               part, parts, cols, (T*)out, nullptr, nullptr, accumulate)));
+}
+
 void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd,
                           int rows, int cols, float eps, int dtype, cudaStream_t stream) {
-  UB_DISPATCH_DTYPE(dtype, (run_fwd<T, false, false>(x, gamma, beta, y, mean, rstd, rows, cols, eps, nullptr, nullptr,
+  UB_DISPATCH_FLOAT(dtype, (run_fwd<T, false, false>(x, gamma, beta, y, mean, rstd, rows, cols, eps, nullptr, nullptr,
                                                      nullptr, 0.f, 0, 0, stream)));
 }
 
@@ -1295,7 +1271,7 @@ void launch_layernorm_bwd(const void* dy, const void* x, const float* mean, cons
                           cudaStream_t stream, int accumulate, bool deterministic) {
   g_acc_mask = accumulate;
   g_det = deterministic;
-  UB_DISPATCH_DTYPE(dtype, (run_bwd<T, false, false>(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, nullptr, part, rows,
+  UB_DISPATCH_FLOAT(dtype, (run_bwd<T, false, false>(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, nullptr, part, rows,
                                                      cols, nullptr, 0.f, 0, 0, stream)));
   g_acc_mask = 0;
   g_det = false;
@@ -1303,7 +1279,7 @@ void launch_layernorm_bwd(const void* dy, const void* x, const float* mean, cons
 
 void launch_rmsnorm_fwd(const void* x, const void* gamma, void* y, float* rstd, int rows, int cols, float eps,
                         int dtype, cudaStream_t stream) {
-  UB_DISPATCH_DTYPE(dtype, (run_fwd<T, true, false>(x, gamma, nullptr, y, nullptr, rstd, rows, cols, eps, nullptr,
+  UB_DISPATCH_FLOAT(dtype, (run_fwd<T, true, false>(x, gamma, nullptr, y, nullptr, rstd, rows, cols, eps, nullptr,
                                                     nullptr, nullptr, 0.f, 0, 0, stream)));
 }
 
@@ -1311,7 +1287,7 @@ void launch_rmsnorm_bwd(const void* dy, const void* x, const float* rstd, const 
                         float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate, bool deterministic) {
   g_acc_mask = accumulate;
   g_det = deterministic;
-  UB_DISPATCH_DTYPE(dtype, (run_bwd<T, true, false>(dy, x, nullptr, rstd, gamma, dx, dgamma, nullptr, nullptr, part,
+  UB_DISPATCH_FLOAT(dtype, (run_bwd<T, true, false>(dy, x, nullptr, rstd, gamma, dx, dgamma, nullptr, nullptr, part,
                                                     rows, cols, nullptr, 0.f, 0, 0, stream)));
   g_acc_mask = 0;
   g_det = false;
@@ -1321,13 +1297,8 @@ void launch_bias_dropout_add_ln_fwd(const void* x, const void* bias, const void*
                                     const void* beta, void* y, void* summed, float* mean, float* rstd, int rows,
                                     int cols, float p, float eps, unsigned long long seed, unsigned long long offset,
                                     int dtype, cudaStream_t stream) {
-  if (dtype == kF16) {
-    run_fwd<__half, false, true>(x, gamma, beta, y, mean, rstd, rows, cols, eps, bias, residual, summed, p, seed,
-                                 offset, stream);
-  } else if (dtype == kBF16) {
-    run_fwd<__nv_bfloat16, false, true>(x, gamma, beta, y, mean, rstd, rows, cols, eps, bias, residual, summed, p,
-                                        seed, offset, stream);
-  }
+  UB_DISPATCH_16BIT(dtype, (run_fwd<T, false, true>(x, gamma, beta, y, mean, rstd, rows, cols, eps, bias, residual,
+                                                    summed, p, seed, offset, stream)));
 }
 
 void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const float* mean, const float* rstd,
@@ -1337,13 +1308,8 @@ void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const fl
   // dbias (optional, v2 geometries only): column sums of dx, produced by the same pass
   g_acc_mask = accumulate;
   g_det = deterministic;
-  if (dtype == kF16) {
-    run_bwd<__half, false, true>(dy, summed, mean, rstd, gamma, dsum, dgamma, dbeta, dbias, part, rows, cols, dx, p,
-                                 seed, offset, stream);
-  } else if (dtype == kBF16) {
-    run_bwd<__nv_bfloat16, false, true>(dy, summed, mean, rstd, gamma, dsum, dgamma, dbeta, dbias, part, rows, cols,
-                                        dx, p, seed, offset, stream);
-  }
+  UB_DISPATCH_16BIT(dtype, (run_bwd<T, false, true>(dy, summed, mean, rstd, gamma, dsum, dgamma, dbeta, dbias, part,
+                                                    rows, cols, dx, p, seed, offset, stream)));
   g_acc_mask = 0;
   g_det = false;
 }

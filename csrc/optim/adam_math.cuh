@@ -1,0 +1,31 @@
+// Element updates shared by the multi-tensor optimizer (multi_tensor.cu) and the fused optimizer tail
+// (comm/fused_step.cu): both must train bit for bit alike.
+#pragma once
+#include "../common.cuh"
+
+namespace ub {
+
+// Adam(W) on one element: m, v are the moments; `h` is an AdamHyper or any type with its fields (the fused tail reads
+// them from its parameter group in place).  step_size = lr * sqrt(1-b2^t)/(1-b1^t), decay_mul = 1 - step_size * wd.
+struct AdamHyper {
+  float beta1, beta2, eps, step_size, decay_mul;
+};
+template <typename Hyper>
+UB_DEVICE void adam_math(float& p, float& m, float& v, float g, const Hyper& h) {
+  m = h.beta1 * m + (1.f - h.beta1) * g;
+  v = h.beta2 * v + (1.f - h.beta2) * g * g;
+  p = p * h.decay_mul - h.step_size * (m / (sqrtf(v) + h.eps));
+}
+
+// bf16 bits of x stochastically rounded with 16 random bits
+UB_DEVICE uint16_t bf16_sr_bits(float x, uint32_t rnd16) {
+  uint32_t bits = __float_as_uint(x);
+  // leave inf/nan untouched; otherwise add 16 random low bits and truncate
+  if ((bits & 0x7f800000u) != 0x7f800000u) bits += rnd16;
+  return (uint16_t)(bits >> 16);
+}
+
+// exponential moving average of the parameter p, one_minus = 1 - decay
+UB_DEVICE float ema_step(float e, float p, float one_minus) { return e - one_minus * (e - p); }
+
+}  // namespace ub

@@ -12,6 +12,7 @@
 // g16 2B + p32 4B + m 4B + v 4B read, p32 4B + m 4B + v 4B + p16 2B + g16 2B (zero) write = 30 B.
 #include "../api.h"
 #include "../common.cuh"
+#include "adam_math.cuh"
 
 namespace ub {
 
@@ -78,17 +79,8 @@ static long long total_chunks(const Table& t) {
   for (int i = 0; i < t.count; ++i) n += (t.numel[i] + kChunk - 1) / kChunk;
   return n;
 }
-static int persistent_grid(long long chunks) {
-  static int sms = 0;
-  if (sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 132;
-  }
-  const long long cap = (long long)sms * 8;  // 8 CTAs of 256 threads per SM = full occupancy
-  return (int)(chunks < cap ? chunks : cap);
-}
+constexpr int kCtasPerSm = 8;  // 8 CTAs of 256 threads per SM = full occupancy
+static int persistent_grid(long long chunks) { return sweep_plan(chunks, 1, kCtasPerSm).grid; }
 
 // ================================================================================================
 // L2 norm
@@ -149,7 +141,7 @@ __global__ void __launch_bounds__(kThreads) l2norm_kernel(NormTensors t, long lo
   }
 }
 
-int l2norm_max_ctas() { return 132 * 8 * 2; }
+int l2norm_max_ctas() { return device_sm_count() * kCtasPerSm; }
 
 void launch_l2norm(const NormTensors& t, float* acc, float* partials, unsigned* counter, float* out, int finalize,
                    cudaStream_t stream) {
@@ -197,20 +189,6 @@ void launch_scale(const ScaleTensors& t, float scale, const float* scale_dev, cu
 // ================================================================================================
 // Adam
 // ================================================================================================
-UB_DEVICE void adam_math(float& p, float& m, float& v, float g, float b1, float b2, float eps, float step_size,
-                         float decay_mul) {
-  m = b1 * m + (1.f - b1) * g;
-  v = b2 * v + (1.f - b2) * g * g;
-  p = p * decay_mul - step_size * (m / (sqrtf(v) + eps));
-}
-
-UB_DEVICE uint16_t bf16_sr_bits(float x, uint32_t rnd16) {
-  uint32_t bits = __float_as_uint(x);
-  // leave inf/nan untouched; otherwise add 16 random low bits and truncate
-  if ((bits & 0x7f800000u) != 0x7f800000u) bits += rnd16;
-  return (uint16_t)(bits >> 16);
-}
-
 __global__ void __launch_bounds__(kThreads) adam_kernel(AdamTensors t, long long nchunks, AdamLaunch cfg) {
   // A non-finite (or zero) device divisor means "the gradients overflowed": the update skips itself -
   // parameters, moments and EMA stay untouched, only the gradient clearing happens - so the host does
@@ -232,7 +210,7 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(AdamTensors t, long long
     void* PH = t.p_half[ti];
     float* E = t.ema[ti];
     const int pdt = t.p_dtype[ti], gdt = t.g_dtype[ti], hdt = t.half_dtype[ti];
-    const float b1 = t.beta1[ti], b2 = t.beta2[ti], eps = t.eps[ti], ss = t.step_size[ti], dm = t.decay_mul[ti];
+    const AdamHyper h{t.beta1[ti], t.beta2[ti], t.eps[ti], t.step_size[ti], t.decay_mul[ti]};
     const bool sr = cfg.stochastic_rounding && PH != nullptr && hdt == kBF16;
     const bool vec_ok = aligned16(P) && aligned16(G) && aligned16(M) && aligned16(V) &&
                         (PH == nullptr || aligned16(PH)) && (E == nullptr || aligned16(E));
@@ -251,7 +229,7 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(AdamTensors t, long long
         load8(M, kF32, i, m);
         load8(V, kF32, i, v);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) adam_math(p[k], m[k], v[k], g[k] * gmul, b1, b2, eps, ss, dm);
+        for (int k = 0; k < 8; ++k) adam_math(p[k], m[k], v[k], g[k] * gmul, h);
         store8(P, pdt, i, p);
         store8(M, kF32, i, m);
         store8(V, kF32, i, v);
@@ -275,7 +253,7 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(AdamTensors t, long long
           float e[8];
           load8(E, kF32, i, e);
 #pragma unroll
-          for (int k = 0; k < 8; ++k) e[k] -= (1.f - cfg.ema_decay) * (e[k] - p[k]);
+          for (int k = 0; k < 8; ++k) e[k] = ema_step(e[k], p[k], 1.f - cfg.ema_decay);
           store8(E, kF32, i, e);
         }
         if (cfg.zero_grad) {
@@ -291,7 +269,7 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(AdamTensors t, long long
       }
       float p = load1(P, pdt, i), m = M[i], v = V[i];
       const float g = load1(G, gdt, i) * gmul;
-      adam_math(p, m, v, g, b1, b2, eps, ss, dm);
+      adam_math(p, m, v, g, h);
       store1(P, pdt, i, p);
       M[i] = m;
       V[i] = v;
@@ -307,7 +285,7 @@ __global__ void __launch_bounds__(kThreads) adam_kernel(AdamTensors t, long long
           store1(PH, hdt, i, p);
         }
       }
-      if (E != nullptr) E[i] -= (1.f - cfg.ema_decay) * (E[i] - p);
+      if (E != nullptr) E[i] = ema_step(E[i], p, 1.f - cfg.ema_decay);
       if (cfg.zero_grad) store1(G, gdt, i, 0.f);
     }
   }
@@ -365,11 +343,11 @@ __global__ void __launch_bounds__(kThreads) ema_kernel(float* ema, const float* 
     load8(ema, kF32, i, e);
     load8(p, kF32, i, w);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) e[k] -= one_minus * (e[k] - w[k]);
+    for (int k = 0; k < 8; ++k) e[k] = ema_step(e[k], w[k], one_minus);
     store8(ema, kF32, i, e);
   }
   for (long long i = vend + (long long)blockIdx.x * kThreads + threadIdx.x; i < n; i += (long long)gridDim.x * kThreads)
-    ema[i] -= one_minus * (ema[i] - p[i]);
+    ema[i] = ema_step(ema[i], p[i], one_minus);
 }
 
 void launch_ema(float* ema, const float* p, long long n, float decay, cudaStream_t stream) {

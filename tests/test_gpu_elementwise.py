@@ -52,6 +52,13 @@ def _assert_within(got, ref, bound, what):
             what, int(bad.sum()), i, got[tuple(i)].item(), ref[tuple(i)].item(), bound[tuple(i)].item(), worst))
 
 
+def _nan_blocks(shape, dtype=torch.float32, n=4):
+    """Leave `n` freed NaN blocks of `shape` in the caching allocator, so that an output or scratch buffer of that size
+    which no kernel writes reads as NaN rather than as zeros by luck."""
+    blocks = [torch.full(shape, math.nan, device="cuda", dtype=dtype) for _ in range(n)]
+    del blocks
+
+
 def _check_sum(got, ref, absum, comp_sum, dtype, chain, what, base=None):
     """A sum accumulated in fp32 and rounded once (onto `base` for a sink): the chain of additions behind it times
     the absolute sum, plus the per-term errors `comp_sum` of the fp32 terms."""
@@ -321,6 +328,37 @@ def test_linear_bias_gradient(dtype, shape):
     check_column_sum(b.grad, dy, dtype, column_chain(plan) + fold, extra_rel=UNIT[dtype] if fold > 1 else 0.0)
 
 
+@pytest.mark.parametrize("dtype", HALF)
+def test_column_sums_of_no_rows(dtype):
+    """Zero rows (a micro-batch without masked tokens): column_sum and bias_gelu_bwd return zero column sums and leave
+    a sink as it was, and ``ops.linear``'s backward gives a zero bias gradient."""
+    from unicore import ops
+
+    nat = _native()
+    cols = 768
+    zeros = torch.zeros(cols, device="cuda", dtype=dtype)
+    x = torch.empty(0, cols, device="cuda", dtype=dtype)
+    bias = torch.randn(cols, device="cuda").to(dtype)
+    _nan_blocks((cols,), dtype)
+    assert torch.equal(nat.column_sum(x, None), zeros)
+    _nan_blocks((cols,), dtype)
+    dx, db = nat.bias_gelu_bwd(x, x, bias, None)
+    assert dx.shape == x.shape and torch.equal(db, zeros)
+    sink = torch.randn(cols, device="cuda").to(dtype)
+    before = sink.clone()
+    assert nat.column_sum(x, sink).data_ptr() == sink.data_ptr() and torch.equal(sink, before)
+    nat.bias_gelu_bwd(x, x, bias, sink)
+    assert torch.equal(sink, before)
+    # 768 outputs take the column kernel; the bias is not claimed by a gradient arena
+    xr = x.clone().requires_grad_(True)
+    w = torch.randn(cols, cols, device="cuda").to(dtype).requires_grad_(True)
+    b = bias.clone().requires_grad_(True)
+    y = ops.linear(xr, w, b)
+    _nan_blocks((cols,), dtype)
+    y.backward(torch.empty_like(y))
+    assert torch.equal(b.grad, zeros)
+
+
 def test_column_dispatch_coverage():
     """The shapes above reach every (full / partial last column block) x (one slice / several) x (ragged or whole
     last sweep) case of the bias_gelu forward and backward / column_sum launch plans, and the long shapes loop several
@@ -583,6 +621,28 @@ def test_gaussian_basis_all_paths(dtype, K, E):
     for short in (1, 37):
         sub = [a[:short] if i in (0, 1, 6) else a for i, a in enumerate(args)]
         check_gbf(nat, *sub, dtype, det=False)
+
+
+@pytest.mark.parametrize("det", [False, True])
+def test_gaussian_basis_no_pairs(det):
+    """An empty distance tensor: every parameter gradient of ``ops.gaussian_basis`` is zero, in the default and in
+    deterministic mode."""
+    from unicore import ops
+
+    K, E, dtype = 128, 64, torch.float16
+    d, edge, mul, bias, means, stds, _ = _gbf_inputs(0, K, E, dtype, seed=11)
+    params = [t.clone().requires_grad_(True) for t in (mul, bias, means, stds)]
+    y = ops.gaussian_basis(d, edge, *params)
+    assert y.shape == (0, K)
+    prev = torch.are_deterministic_algorithms_enabled()
+    torch.use_deterministic_algorithms(det)
+    try:
+        _nan_blocks((1, 2 * K))  # the size of one CTA's partial (d mean, d std) row
+        y.backward(torch.empty_like(y))
+    finally:
+        torch.use_deterministic_algorithms(prev)
+    for p in params:
+        assert torch.equal(p.grad, torch.zeros_like(p)), p.grad
 
 
 def test_gaussian_dispatch_coverage():

@@ -486,7 +486,7 @@ def emb_multi(kind, vocab=None):
     """Rows (kind "rows") or a vocabulary (kind "vocab") for which the scatter or the finalize kernel runs two grid
     sweeps or more with a ragged last one."""
     nat = _native()
-    sweep = 132 * 16 * 8
+    sweep = _sms() * 16 * 8
     n = 2 * sweep + sweep // 2 + 1
     key = "scatter" if kind == "rows" else "finalize"
     plan = nat.embedding_plan(n, vocab or 1000) if kind == "rows" else nat.embedding_plan(1000, n)
@@ -688,11 +688,11 @@ def test_dispatch_coverage():
         cols, rows, vocab = emb_case(name)
         p = nat.embedding_plan(rows, vocab)
         for k in seen:
-            assert p[k]["grid"] == min(-(-p[k]["items"] // 8), 132 * 16), p
+            assert p[k]["grid"] == min(-(-p[k]["items"] // 8), sms * 16), p
             seen[k].add((p[k]["sweeps"] > 1, _ragged(p[k])))
     # one whole sweep, and several with a ragged last one, of both kernels
     assert seen["scatter"] >= {(False, False), (True, True)}, seen
     assert seen["finalize"] >= {(False, False), (True, True)}, seen
     p = nat.embedding_plan(14000, 30522)["sorted"]
-    assert p["grid"] == 132 * 16 and p["sweeps"] >= 2 and _ragged(p), p
+    assert p["grid"] == sms * 16 and p["sweeps"] >= 2 and _ragged(p), p
     assert nat.embedding_plan(0, 30522)["sorted"]["grid"] == 0  # no rows: nothing is launched
