@@ -122,7 +122,11 @@ struct FmhaDecodeParams {
   long long bias_sb, bias_sh, kpm_sb;
   int B, H, D, C;
   int bias_batch, bias_cols, kpm_cols;
-  int num_splits, chunk;   // split s takes keys [s * chunk, (s + 1) * chunk); the last one runs to n_b
+  // split s takes keys [s * chunk, (s + 1) * chunk); the last one runs to n_b.  chunk == 0 derives it per (b, h) from
+  // the device length: chunk_b = max(1, ceil(n_b / num_splits)), so that a host bound far above n_b (the capacity,
+  // in a captured CUDA graph) still spreads the n_b keys over every split.  Both give the same ranges when n_b equals
+  // the bound the host chunk was computed from.
+  int num_splits, chunk;
   int is_bf16;
   float scale;
 };

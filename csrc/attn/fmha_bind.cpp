@@ -211,10 +211,12 @@ void check_decode_operand(const Tensor& t, const char* name, const Tensor& q, in
 // One query row per (b, h) against a [B, C, H, D] key / value cache (fmha_api.h).  max_len is a host bound on
 // seqlens (the device values are never read here, so a decode step does not synchronise); with k_new / v_new the row
 // seqlens[b] is appended first and counts as visible, so up to max_len + 1 keys are.  num_splits = 0 picks the split
-// count from the shapes; any other value forces it.
+// count from the shapes; any other value forces it.  split_by_length: each (b, h) divides its own device length n_b
+// over the splits instead of the host bound (for a CUDA graph captured with the capacity as the bound, where the
+// true lengths are far below it); the split count still comes from the bound.
 Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& seqlens,
                    int64_t max_len, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
-                   const OptTensor& kpm, double scale, int64_t num_splits) {
+                   const OptTensor& kpm, double scale, int64_t num_splits, bool split_by_length) {
   check_operand(q, "q", q.device(), k16Bit, {kAnySize, 1, kAnySize, kAnySize}, kAligned);
   const int64_t B = q.size(0), H = q.size(2), D = q.size(3);
   TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
@@ -283,7 +285,7 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   TORCH_CHECK(num_splits >= 1 && num_splits <= ub::kDecodeMaxSplits,
               "num_splits must be 0 (heuristic) or 1 .. fmha_decode_max_splits()");
   p.num_splits = (int)num_splits;
-  p.chunk = (int)std::max<int64_t>(1, (bound + num_splits - 1) / num_splits);
+  p.chunk = split_by_length ? 0 : (int)std::max<int64_t>(1, (bound + num_splits - 1) / num_splits);
   Tensor out = torch::empty({p.B, 1, p.H, p.D}, q.options());
   p.out = out.data_ptr();
   Tensor work;
@@ -386,7 +388,7 @@ void register_fmha(pybind11::module_& m) {
         py::arg("need_dbias"), py::arg("packed_grad"), py::arg("dlogits") = py::none(), py::arg("causal") = false);
   m.def("fmha_decode", &fmha_decode, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("seqlens"),
         py::arg("max_len"), py::arg("k_new"), py::arg("v_new"), py::arg("bias"), py::arg("key_padding_mask"),
-        py::arg("scale"), py::arg("num_splits") = 0);
+        py::arg("scale"), py::arg("num_splits") = 0, py::arg("split_by_length") = false);
   // its own submodule, _C.kvcache; tests/test_gpu_attention_kvcache_chunk.py runs the operand-rejection table of
   // tests/test_gpu_bindings.py over it
   auto kv = m.def_submodule("kvcache", "multi-token steps into a key / value cache");

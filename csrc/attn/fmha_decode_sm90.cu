@@ -5,7 +5,8 @@
 // M = 1 leaves nothing for wgmma: each key is a dot product and an axpy, and a step has to stream K and V once at HBM
 // bandwidth.  So the kernel is a copy pipeline feeding the CUDA cores:
 //   * Split-KV: CTA (s, h, b) takes the contiguous key range [s * chunk, (s + 1) * chunk) of (b, h) (the last split
-//     runs to n_b).  With one split it writes O; otherwise it writes an fp32 partial (o[D] unnormalised, m, l) and
+//     runs to n_b); chunk comes from the host bound, or with p.chunk == 0 from n_b itself (a CUDA graph captured at
+//     the capacity).  With one split it writes O; otherwise it writes an fp32 partial (o[D] unnormalised, m, l) and
 //     fmha_decode_combine_kernel merges the splits in ascending order.  No atomics: for a given split count the
 //     result does not depend on the schedule.
 //   * Streaming: warp 0 requests the K and V rows of key tile t + kStages with one cp.async.bulk per row (rows are
@@ -73,8 +74,9 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeP
   const int len = p.seqlens != nullptr ? p.seqlens[b] : cap;
   const int pos = append ? clampi(len, 0, cap - 1) : -1;   // row of the new token
   const int n = append ? pos + 1 : clampi(len, 0, cap);
-  const int start = s * p.chunk;
-  const int end = s == p.num_splits - 1 ? n : min(start + p.chunk, n);
+  const int chunk = p.chunk > 0 ? p.chunk : max(1, (n + p.num_splits - 1) / p.num_splits);
+  const int start = s * chunk;
+  const int end = s == p.num_splits - 1 ? n : min(start + chunk, n);
 
   const T* kc = reinterpret_cast<const T*>(p.k_cache) + (long long)b * p.kc_sb + (long long)h * p.kc_sh;
   const T* vc = reinterpret_cast<const T*>(p.v_cache) + (long long)b * p.vc_sb + (long long)h * p.vc_sh;

@@ -215,6 +215,10 @@ class CrossMultiheadAttention(nn.Module):
         return self.out_proj(self.attend(query, key, value, key_padding_mask, attn_bias))
 
 
+def _same_layout(a: Tensor, b: Tensor) -> bool:
+    return a.shape == b.shape and a.dtype == b.dtype and a.device == b.device
+
+
 class LayerKVCache:
     """One decoder layer's share of a ``DecoderCache``: self-attention keys / values ``k``, ``v`` ``[B, C, H, D]`` and
     the projected encoder keys / values ``enc_k``, ``enc_v`` ``[B, S, H, D]`` (None until the prefill stores them)."""
@@ -244,12 +248,28 @@ class LayerKVCache:
             self.v[:, :v.size(1)].copy_(v)
 
     def store_encoder(self, k, v):
-        self.enc_k, self.enc_v = k.detach(), v.detach()
+        """Keep the prefill's projected encoder keys / values.  A later prefill of the same shape writes into the
+        tensors kept before, so that their addresses stay valid (a captured decoding step reads them)."""
+        if self.enc_k is not None and _same_layout(self.enc_k, k) and _same_layout(self.enc_v, v):
+            with torch.no_grad():
+                self.enc_k.copy_(k)
+                self.enc_v.copy_(v)
+        else:
+            self.enc_k, self.enc_v = k.detach(), v.detach()
 
     def reorder(self, index):
-        self.k, self.v = self.k.index_select(0, index), self.v.index_select(0, index)
-        if self.enc_k is not None:
-            self.enc_k, self.enc_v = self.enc_k.index_select(0, index), self.enc_v.index_select(0, index)
+        """In place when ``index`` keeps the batch size: only the rows below the host bound ``max_len`` can be read,
+        so only they are gathered (into a temporary) and written back.  A new batch size rebinds the buffers."""
+        n = self.owner.max_len
+        if index.numel() != self.k.size(0):
+            self.k, self.v = self.k.index_select(0, index), self.v.index_select(0, index)
+            if self.enc_k is not None:
+                self.enc_k, self.enc_v = self.enc_k.index_select(0, index), self.enc_v.index_select(0, index)
+            return
+        bufs = [self.k[:, :n], self.v[:, :n]] + ([self.enc_k, self.enc_v] if self.enc_k is not None else [])
+        with torch.no_grad():
+            for buf in bufs:
+                buf.copy_(buf.index_select(0, index))
 
 
 class DecoderCache:
@@ -271,10 +291,14 @@ class DecoderCache:
         ]
 
     def reorder(self, index):
-        """Select (and repeat) sequences of the batch along ``index`` in every buffer, as beam search does."""
-        self.seqlens = self.seqlens.index_select(0, index)
+        """Select (and repeat) sequences of the batch along ``index`` in every buffer, as beam search does.  With as
+        many entries as sequences it writes into the existing buffers (a captured decoding step keeps reading them)."""
         for layer in self.layers:
             layer.reorder(index)
+        if index.numel() == self.seqlens.numel():
+            self.seqlens.copy_(self.seqlens.index_select(0, index))
+        else:
+            self.seqlens = self.seqlens.index_select(0, index)
 
     def rewind(self, n):
         """Drop the last ``n`` tokens of every sequence (an int), or ``n[b]`` of sequence b (an integer ``[B]`` tensor

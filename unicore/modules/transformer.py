@@ -519,22 +519,25 @@ class TransformerDecoder(nn.Module, _StackMixin):
         return DecoderCache(len(self.layers), batch_size, capacity, heads, self.embed_dim // heads,
                             dtype or weight.dtype, device or weight.device)
 
-    def _dropout_active(self):
+    def _check_no_dropout(self):
         rates = [self.emb_dropout]
         for layer in self.layers:
             rates += [layer.dropout, layer.attention_dropout, layer.activation_dropout]
-        return self.training and any(r > 0 for r in rates)
+        if self.training and any(r > 0 for r in rates):
+            raise RuntimeError("incremental decoding runs without dropout: call eval() or set the dropout rates to 0")
 
-    def _step_rel_pos_bias(self, cache, like, T=1):
+    def _step_rel_pos_bias(self, cache, like, T=1, cols=None):
         """``[B, H, T, Lb]``: the relative-position bias rows of each sequence's T new tokens, gathered on the device at
-        their positions ``seqlens[b] + i`` (keys past them are not visible).  ``Lb`` is ``max_len + 1`` for one token and
-        ``max_len + T`` rounded up to 8 for a chunk (the row stride the chunk kernel reads); columns past the bucket
-        table are 0."""
+        their positions ``seqlens[b] + i`` (keys past them are not visible).  ``Lb`` is ``cols`` when given (a captured
+        step fixes it), else ``max_len + 1`` for one token and ``max_len + T`` rounded up to 8 for a chunk (the row
+        stride the chunk kernel reads); columns past the bucket table are 0.  A wider bias has the same first
+        columns."""
         if self.rp_bucket.device != like.device:
             self.rp_bucket = self.rp_bucket.to(like.device)
-        cols = cache.max_len + T
-        if T > 1:
-            cols += -cols % 8
+        if cols is None:
+            cols = cache.max_len + T
+            if T > 1:
+                cols += -cols % 8
         width = min(cols, self.max_seq_len)
         pos = cache.seqlens.long()[:, None] + torch.arange(T, device=like.device)   # [B, T]
         idx = self.rp_bucket[pos.clamp(max=self.max_seq_len - 1), :width]   # [B, T, width]
@@ -546,8 +549,7 @@ class TransformerDecoder(nn.Module, _StackMixin):
 
     def _forward_cached(self, emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask,
                         cache):
-        if self._dropout_active():
-            raise RuntimeError("incremental decoding runs without dropout: call eval() or set the dropout rates to 0")
+        self._check_no_dropout()
         if cache.max_len == 0:
             # prefill: the ordinary path, with every layer storing its keys / values on the way
             L = emb.size(1)
@@ -566,22 +568,147 @@ class TransformerDecoder(nn.Module, _StackMixin):
             else:
                 cache.seqlens.copy_(L - padding_mask.to(torch.int32).sum(1))
             cache.max_len = L
-        else:
-            T = emb.size(1)
-            if attn_mask is not None:
-                raise NotImplementedError("attn_mask is not supported on a decoding step")
-            if padding_mask is not None:
-                raise NotImplementedError("padding_mask is not supported on a decoding step")
-            if cache.max_len + T > cache.capacity:
-                raise ValueError("{} more tokens do not fit the cache: {} of capacity {} are in use".format(
-                    T, cache.max_len, cache.capacity))
-            x = self._embed_prologue(emb, None)
-            attn_bias = self._step_rel_pos_bias(cache, x, T) if self.rel_pos else None
-            for layer, lc in zip(self.layers, cache.layers):
-                x = layer(x, encoder_out=encoder_out, attn_bias=attn_bias, encoder_padding_mask=encoder_padding_mask,
-                          encoder_attn_bias=encoder_attn_mask, cache=lc)
-            cache.seqlens += T
-            cache.max_len += T
+            if self.final_layer_norm is not None:
+                x = self.final_layer_norm(x)
+            return x
+        T = emb.size(1)
+        if attn_mask is not None:
+            raise NotImplementedError("attn_mask is not supported on a decoding step")
+        if padding_mask is not None:
+            raise NotImplementedError("padding_mask is not supported on a decoding step")
+        _check_room(cache, T)
+        x = self._decode_step(emb, encoder_out, encoder_padding_mask, encoder_attn_mask, cache)
+        cache.max_len += T
+        return x
+
+    def _decode_step(self, emb, encoder_out, encoder_padding_mask, encoder_attn_mask, cache, bias_cols=None):
+        """A step of T tokens into a non-empty cache, final LayerNorm included: appends the tokens' keys / values,
+        attends and advances ``cache.seqlens`` by T on the device.  Every host-side shape follows ``cache.max_len``
+        (and ``bias_cols``), which the caller advances."""
+        T = emb.size(1)
+        x = self._embed_prologue(emb, None)
+        attn_bias = self._step_rel_pos_bias(cache, x, T, bias_cols) if self.rel_pos else None
+        for layer, lc in zip(self.layers, cache.layers):
+            x = layer(x, encoder_out=encoder_out, attn_bias=attn_bias, encoder_padding_mask=encoder_padding_mask,
+                      encoder_attn_bias=encoder_attn_mask, cache=lc)
+        cache.seqlens += T
         if self.final_layer_norm is not None:
             x = self.final_layer_norm(x)
         return x
+
+    def capture_step(self, cache, T=1, encoder_padding_mask=None, encoder_attn_mask=None):
+        """A decoding step of T tokens per sequence into ``cache`` as a CUDA graph: returns a ``CapturedDecoderStep``,
+        ``step(emb [B, T, E]) -> [B, T, E]``, which does what ``self(emb, encoder_padding_mask=...,
+        encoder_attn_mask=..., cache=cache)`` does on a step, with one graph launch instead of a chain of kernel
+        launches from Python.  Make it after the prefill (which stays eager: prompt lengths vary); it captures on its
+        first call.  Needs CUDA, the native kernels, a 16-bit cache and no active dropout."""
+        return CapturedDecoderStep(self, cache, T, encoder_padding_mask, encoder_attn_mask)
+
+
+def _check_room(cache, T):
+    if cache.max_len + T > cache.capacity:
+        raise ValueError("{} more tokens do not fit the cache: {} of capacity {} are in use".format(
+            T, cache.max_len, cache.capacity))
+
+
+def _static_copy(buf, src, dtype, device):
+    """``src`` written into the static buffer ``buf`` when the shapes match, else a copy of its own (whose new address
+    makes the next call capture again)."""
+    if src is None:
+        return buf
+    if buf is not None and buf.shape == src.shape:
+        return buf.copy_(src)
+    return src.to(device=device, dtype=dtype).clone(memory_format=torch.contiguous_format)
+
+
+class CapturedDecoderStep:
+    """A ``TransformerDecoder`` decoding step of T tokens per sequence captured in a CUDA graph
+    (``TransformerDecoder.capture_step``).
+
+    ``step(emb [B, T, E])`` copies ``emb`` into the graph's static input, replays the graph (append, attention, every
+    layer, ``seqlens += T``), advances ``cache.max_len`` by T on the host and returns the graph's static output
+    ``[B, T, E]``: the next call overwrites it, so clone what has to outlive it.  A step past the capacity raises
+    before the replay.  ``encoder_padding_mask`` / ``encoder_attn_mask`` given to a call replace those of the capture.
+
+    The graph is built for the largest host bound, ``max_len = capacity - T``: the relative-position bias has
+    ``capacity`` columns (rounded up to 8 for a chunk), and the one-token decode attention divides each sequence's
+    device length over its splits.  So the same graph serves every step until the cache is full, and between calls
+    ``cache.reorder``, ``cache.rewind`` (an int or a device tensor) and a new prefill of the same shapes need no new
+    capture: they write into the buffers the graph reads.  Before each replay the addresses and shapes of those
+    buffers are compared with the ones captured; when one differs (a prefill with another encoder length, a reorder
+    to another batch size, a mask of another shape) the step is captured again.  ``captures`` counts the captures."""
+
+    def __init__(self, model, cache, T=1, encoder_padding_mask=None, encoder_attn_mask=None):
+        k = cache.layers[0].k if cache.layers else None
+        if not torch.cuda.is_available() or k is None or not k.is_cuda:
+            raise RuntimeError("capture_step needs a CUDA device and a DecoderCache on it")
+        if not ops.USE_NATIVE or not model._fused_attention_capable(k):
+            raise RuntimeError("capture_step needs the native sm_90a kernels, an fp16 / bf16 cache and a head dim the "
+                               "fused attention kernels take")
+        model._check_no_dropout()
+        if cache.max_len == 0:
+            raise ValueError("capture_step comes after the prefill: the cache is empty")
+        if not 1 <= T < cache.capacity:
+            raise ValueError("a captured step takes 1 <= T < capacity ({}) tokens, not {}".format(cache.capacity, T))
+        self.model, self.cache, self.T = model, cache, T
+        self.captures = 0
+        self._graph = self._out = self._emb = self._key = None
+        self._enc_pad = _static_copy(None, encoder_padding_mask, torch.bool, k.device)
+        self._enc_bias = _static_copy(None, encoder_attn_mask, k.dtype, k.device)
+
+    def _buffers(self):
+        """Every tensor the graph reads or writes besides its own intermediates."""
+        bufs = [self.cache.seqlens, self._emb, self._enc_pad, self._enc_bias]
+        for lc in self.cache.layers:
+            bufs += [lc.k, lc.v, lc.enc_k, lc.enc_v]
+        return bufs
+
+    def _layout_key(self):
+        return tuple(None if t is None else (t.data_ptr(), tuple(t.shape), t.dtype) for t in self._buffers())
+
+    def _capture(self):
+        model, cache, T = self.model, self.cache, self.T
+        k = cache.layers[0].k
+        B, cap = k.size(0), cache.capacity
+        self._graph = self._out = None   # the old graph's memory pool goes back to the allocator
+        if self._emb is None or self._emb.size(0) != B:
+            self._emb = torch.zeros(B, T, model.embed_dim, dtype=k.dtype, device=k.device)
+        cols = cap + (-cap % 8 if T > 1 else 0)
+        args = (self._emb, None, self._enc_pad, self._enc_bias, cache, cols)
+        seqlens, max_len = cache.seqlens.clone(), cache.max_len
+        cache.max_len = cap - T   # the host bound every shape of the graph follows
+        try:
+            with torch.no_grad():
+                # the warm-up really runs (loads the modules, lets cuBLAS pick its kernels) on a side stream, as capture
+                # requires; it writes rows seqlens[b] .. seqlens[b] + T - 1 of the caches, which are not visible yet
+                side = torch.cuda.Stream(device=k.device)
+                side.wait_stream(torch.cuda.current_stream(k.device))
+                with torch.cuda.stream(side):
+                    model._decode_step(*args)
+                torch.cuda.current_stream(k.device).wait_stream(side)
+                cache.seqlens.copy_(seqlens)
+                graph = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(graph):
+                    out = model._decode_step(*args)
+        finally:
+            cache.seqlens.copy_(seqlens)
+            cache.max_len = max_len
+        self._graph, self._out = graph, out
+        self._key = self._layout_key()
+        self.captures += 1
+
+    def __call__(self, emb, encoder_padding_mask=None, encoder_attn_mask=None):
+        cache = self.cache
+        if cache.max_len == 0:
+            raise ValueError("the cache is empty: run the prefill first")
+        _check_room(cache, self.T)
+        self.model._check_no_dropout()
+        k = cache.layers[0].k
+        self._enc_pad = _static_copy(self._enc_pad, encoder_padding_mask, torch.bool, k.device)
+        self._enc_bias = _static_copy(self._enc_bias, encoder_attn_mask, k.dtype, k.device)
+        if self._graph is None or self._layout_key() != self._key:
+            self._capture()
+        self._emb.copy_(emb)
+        self._graph.replay()
+        cache.max_len += self.T
+        return self._out

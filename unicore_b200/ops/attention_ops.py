@@ -328,7 +328,8 @@ def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_n
     allows); ``max_len + T > C`` raises, and the device lengths are never read on the host, so a step does not
     synchronise.  bias: ``[1|B, H, T, Lb]``, row i for query i, ``Lb`` covering the visible keys (columns past them
     are ignored); key_padding_mask: bool ``[B, Lk]``, True = masked.  A query whose visible keys are all masked gives
-    0.  Returns ``[B, T, H, D]``.  No dropout and no backward."""
+    0.  Returns ``[B, T, H, D]``.  No dropout and no backward.  Under CUDA-graph capture (``max_len`` then a fixed
+    bound such as the capacity) a one-token step divides each sequence's device length over the split-KV splits."""
     _check_no_grad(q, k_cache, v_cache, k_new, v_new, bias)
     append = k_new is not None
     if append != (v_new is not None):
@@ -358,8 +359,10 @@ def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_n
     if T == 1:
         if bias is not None and (bias.dtype != q.dtype or bias.stride(-1) != 1):
             bias = bias.to(q.dtype).contiguous()
+        # A step captured in a CUDA graph runs with the capacity as its host bound, far above most true lengths: each
+        # (b, h) then spreads its own device length over the splits, not the bound (or most splits would be empty).
         return native().fmha_decode(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias, key_padding_mask,
-                                    float(scale))
+                                    float(scale), split_by_length=torch.cuda.is_current_stream_capturing())
     bound = C if seqlens is None else max_len + T
     if bias is not None:
         # the kernel reads the bias by TMA (rows of a multiple of 8 columns); the padding is -inf, so a bias narrower
