@@ -68,7 +68,8 @@ void launch_ema(float* ema, const float* p, long long n, float decay, cudaStream
 // Launch plan of the norm kernels for a [rows, cols] input: which kernel generation and template case runs, on what
 // grid, and how the rows are dealt out.  The launchers run exactly this plan.  Every kernel loops over tiles of
 // `tile_rows` consecutive rows; tile t goes to unit t % units (a unit is a warp for v3, a CTA for v2 and v1), so a
-// unit runs tiles_min or tiles_max tiles.
+// unit runs tiles_min or tiles_max tiles.  The generation changes only speed and summation order: the backward has
+// one contract (outputs, fixed-order sums, scratch layout, finisher) at every width.
 enum NormKind : int { kNormFwd = 0, kNormBwd = 1, kNormFusedFwd = 2 };  // the fused op's backward runs kNormBwd
 struct NormPlan {
   int gen;          // 3: one warp per row, 2: bulk-copy input ring, 1: rows in registers; 0: no kernel for this width
@@ -85,17 +86,16 @@ void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, vo
                           int rows, int cols, float eps, int dtype, cudaStream_t stream);
 // part: float[3 * norm_bwd_parts(...) * cols] scratch (per-CTA partial column sums); dgamma/dbeta in `dtype`
 int norm_bwd_parts(int rows, int cols, int dtype);
-bool norm_v2_supported(int cols, int dtype);  // geometries for which the fused op can also emit dbias
+// Every backward sums its parameter gradients in a fixed order (bitwise reproducible in both modes of
+// torch.use_deterministic_algorithms) and finishes them through colsum_finalize_kernel.
 // accumulate (bit 0: dgamma, bit 1: dbeta, bit 2: dbias): add to what the output already holds (gradient arena)
-// deterministic: the per-CTA column partials are combined in a fixed order on every launch path
 void launch_layernorm_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const void* gamma,
                           void* dx, void* dgamma, void* dbeta, float* part, int rows, int cols, int dtype,
-                          cudaStream_t stream, int accumulate = 0, bool deterministic = false);
+                          cudaStream_t stream, int accumulate = 0);
 void launch_rmsnorm_fwd(const void* x, const void* gamma, void* y, float* rstd, int rows, int cols, float eps,
                         int dtype, cudaStream_t stream);
 void launch_rmsnorm_bwd(const void* dy, const void* x, const float* rstd, const void* gamma, void* dx, void* dgamma,
-                        float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate = 0,
-                        bool deterministic = false);
+                        float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate = 0);
 // out[cols] (16-bit `dtype`) = column sums of the fp32 partial rows part[parts][cols] (parts == 0: zeros), in the
 // summation order of the norm backward's parameter gradients; accumulate != 0 adds them to what out holds
 void launch_colsum_finalize(const float* part, int parts, int cols, void* out, int accumulate, int dtype,
@@ -148,12 +148,12 @@ void launch_bias_dropout_add_ln_fwd(const void* x, const void* bias, const void*
                                     const void* beta, void* y, void* summed, float* mean, float* rstd, int rows,
                                     int cols, float p, float eps, unsigned long long seed, unsigned long long offset,
                                     int dtype, cudaStream_t stream);
-// dsum = dLN(dy); dx = dropout_mask * dsum / (1-p); dbias (nullable) = column sums of dx
+// dsum = dLN(dy); dx = dropout_mask * dsum / (1-p); dbias (nullable) = column sums of dx at every width: v3 / v2 sum
+// the fp32 values in the same pass, v1 sums the rounded dx with launch_column_sum afterwards (two more launches)
 void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const float* mean, const float* rstd,
                                     const void* gamma, void* dsum, void* dx, void* dgamma, void* dbeta,
                                     void* dbias, float* part, int rows, int cols, float p, unsigned long long seed,
-                                    unsigned long long offset, int dtype, cudaStream_t stream, int accumulate = 0,
-                                    bool deterministic = false);
+                                    unsigned long long offset, int dtype, cudaStream_t stream, int accumulate = 0);
 // ---- Gaussian radial basis of (mul[edge] * d + bias[edge]) (Uni-Mol pair features), csrc/fused/gaussian.cu ----------
 // y: [n, K] in `dtype` (fp16 / bf16), K a multiple of 8 with K / 8 a power of two <= 32
 

@@ -206,8 +206,7 @@ std::tuple<Tensor, Tensor, Tensor> layernorm_bwd(const Tensor& dy, const Tensor&
   Tensor part = torch::empty({3, ub::norm_bwd_parts(rows, cols, tag), cols}, x.options().dtype(at::kFloat));
   ub::launch_layernorm_bwd(dy.data_ptr(), x.data_ptr(), mean.data_ptr<float>(), rstd.data_ptr<float>(),
                            gamma.data_ptr(), dx.data_ptr(), dgamma.data_ptr(), dbeta.data_ptr(),
-                           part.data_ptr<float>(), rows, cols, tag, cur_stream(), acc,
-                           at::globalContext().deterministicAlgorithms());
+                           part.data_ptr<float>(), rows, cols, tag, cur_stream(), acc);
   check_launch("layernorm_bwd");
   return {dx, dgamma, dbeta};
 }
@@ -239,8 +238,7 @@ std::tuple<Tensor, Tensor> rmsnorm_bwd(const Tensor& dy, const Tensor& x, const 
   Tensor dgamma = grad_out(dgamma_sink, gamma, 0, acc);
   Tensor part = torch::empty({3, ub::norm_bwd_parts(rows, cols, tag), cols}, x.options().dtype(at::kFloat));
   ub::launch_rmsnorm_bwd(dy.data_ptr(), x.data_ptr(), rstd.data_ptr<float>(), gamma.data_ptr(), dx.data_ptr(),
-                         dgamma.data_ptr(), part.data_ptr<float>(), rows, cols, tag, cur_stream(), acc,
-                         at::globalContext().deterministicAlgorithms());
+                         dgamma.data_ptr(), part.data_ptr<float>(), rows, cols, tag, cur_stream(), acc);
   check_launch("rmsnorm_bwd");
   return {dx, dgamma};
 }
@@ -560,8 +558,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, int64_t, int64_t> bias_dropout_add_ln
   return {y, mean, rstd, summed, (int64_t)seed, (int64_t)offset};
 }
 
-// returns (dsum, dx, dgamma, dbeta, dbias); dbias is undefined unless `need_dbias` and the geometry allows
-// the in-kernel column sums (the caller then reduces dx itself)
+// returns (dsum, dx, dgamma, dbeta, dbias); dbias (column sums of dx) exactly when `need_dbias`
 std::tuple<Tensor, Tensor, Tensor, Tensor, OptTensor> bias_dropout_add_ln_bwd(const Tensor& dy, const Tensor& summed,
                                                                               const Tensor& mean, const Tensor& rstd,
                                                                               const Tensor& gamma, double p,
@@ -586,12 +583,12 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, OptTensor> bias_dropout_add_ln_bwd(co
   Tensor dgamma = grad_out(dgamma_sink, gamma, 0, acc), dbeta = grad_out(dbeta_sink, gamma, 1, acc);
   Tensor part = torch::empty({3, ub::norm_bwd_parts(rows, cols, tag), cols}, summed.options().dtype(at::kFloat));
   OptTensor dbias;
-  if (need_dbias && ub::norm_v2_supported(cols, tag)) dbias = grad_out(dbias_sink, gamma, 2, acc);
+  if (need_dbias) dbias = grad_out(dbias_sink, gamma, 2, acc);
   ub::launch_bias_dropout_add_ln_bwd(dy.data_ptr(), summed.data_ptr(), mean.data_ptr<float>(),
                                      rstd.data_ptr<float>(), gamma.data_ptr(), dsum.data_ptr(), dx.data_ptr(),
                                      dgamma.data_ptr(), dbeta.data_ptr(), has(dbias) ? dbias->data_ptr() : nullptr,
                                      part.data_ptr<float>(), rows, cols, (float)p, (uint64_t)seed, (uint64_t)offset,
-                                     tag, cur_stream(), acc, at::globalContext().deterministicAlgorithms());
+                                     tag, cur_stream(), acc);
   check_launch("bias_dropout_add_ln_bwd");
   return {dsum, dx, dgamma, dbeta, dbias};
 }

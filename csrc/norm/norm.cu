@@ -166,7 +166,7 @@ __global__ void __launch_bounds__(kNormThreads) norm_fwd_kernel(
 // ------------------------------------------------------------------------------------------------
 // backward: dx (+ optional dropout-masked copy for the fused op) and per-CTA dgamma/dbeta partials
 // ------------------------------------------------------------------------------------------------
-template <typename T, int VPT, bool kRMS, bool kFused, bool kDet = false>
+template <typename T, int VPT, bool kRMS, bool kFused>
 __global__ void __launch_bounds__(kNormThreads) norm_bwd_kernel(
     const T* __restrict__ dy, const T* __restrict__ x, const float* __restrict__ mean,
     const float* __restrict__ rstd, const T* __restrict__ gamma, T* __restrict__ dx, float* __restrict__ dgamma_part,
@@ -247,24 +247,19 @@ __global__ void __launch_bounds__(kNormThreads) norm_bwd_kernel(
     }
   }
 
-  // combine the row groups of this CTA, then publish one fp32 partial row per CTA.  kDet: group 0, 1, ... add in turn
-  // (each column belongs to one thread of a group), so the order is fixed; otherwise shared atomics in arrival order.
+  // combine the row groups of this CTA, then publish one fp32 partial row per CTA: group 0, 1, ... add in turn (each
+  // column belongs to one thread of a group), so the order is fixed
   __syncthreads();
-  for (int r = 0; r < (kDet ? rows_per_cta : 1); ++r) {
-    if (!kDet || grp == r) {
+  for (int r = 0; r < rows_per_cta; ++r) {
+    if (grp == r) {
 #pragma unroll
       for (int k = 0; k < VPT; ++k) {
         const int vi = j + k * tpr;
         if (vi < g.nvec) {
 #pragma unroll
           for (int e = 0; e < EPV; ++e) {
-            if constexpr (kDet) {
-              sm_acc[vi * EPV + e] += dg[k][e];
-              if (!kRMS) sm_acc[g.cols + vi * EPV + e] += db[k][e];
-            } else {
-              atomicAdd(&sm_acc[vi * EPV + e], dg[k][e]);
-              if (!kRMS) atomicAdd(&sm_acc[g.cols + vi * EPV + e], db[k][e]);
-            }
+            sm_acc[vi * EPV + e] += dg[k][e];
+            if (!kRMS) sm_acc[g.cols + vi * EPV + e] += db[k][e];
           }
         }
       }
@@ -274,41 +269,6 @@ __global__ void __launch_bounds__(kNormThreads) norm_bwd_kernel(
   for (int c = threadIdx.x; c < g.cols; c += kNormThreads) {
     dgamma_part[(size_t)blockIdx.x * g.cols + c] = sm_acc[c];
     if (!kRMS) dbeta_part[(size_t)blockIdx.x * g.cols + c] = sm_acc[g.cols + c];
-  }
-}
-
-// partial rows -> dgamma / dbeta. block = (32 columns, 8 row slices)
-template <typename T>
-__global__ void __launch_bounds__(256) norm_param_grad_kernel(const float* __restrict__ dg_part,
-                                                                const float* __restrict__ db_part, int parts,
-                                                                int cols, T* __restrict__ dgamma,
-                                                                T* __restrict__ dbeta, int acc_mask) {
-  __shared__ float red[2][8][33];
-  const int cx = threadIdx.x & 31, ry = threadIdx.x >> 5;
-  const int col = blockIdx.x * 32 + cx;
-  float a = 0.f, b = 0.f;
-  if (col < cols) {
-    for (int r = ry; r < parts; r += 8) {
-      a += dg_part[(size_t)r * cols + col];
-      if (db_part != nullptr) b += db_part[(size_t)r * cols + col];
-    }
-  }
-  red[0][ry][cx] = a;
-  red[1][ry][cx] = b;
-  __syncthreads();
-  if (ry == 0 && col < cols) {
-    float sa = 0.f, sb = 0.f;
-#pragma unroll
-    for (int r = 0; r < 8; ++r) {
-      sa += red[0][r][cx];
-      sb += red[1][r][cx];
-    }
-    if (acc_mask & 1) sa += to_f32<T>(dgamma[col]);
-    dgamma[col] = from_f32<T>(sa);
-    if (db_part != nullptr) {
-      if (acc_mask & 2) sb += to_f32<T>(dbeta[col]);
-      dbeta[col] = from_f32<T>(sb);
-    }
   }
 }
 
@@ -1049,12 +1009,6 @@ __global__ void __launch_bounds__(kNormV3BwdThreads, (VPL <= 1 ? 2 : 1)) norm_bw
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-// set by the launch_* entry points for the duration of one call (the host side of a stream is single-threaded)
-static thread_local int g_acc_mask = 0;
-// deterministic mode (torch.use_deterministic_algorithms), set the same way: the gen-1 backward combines its row groups
-// in a fixed order
-static thread_local bool g_det = false;
-
 static int pow2ceil(int v) {
   int p = 1;
   while (p < v) p <<= 1;
@@ -1144,9 +1098,11 @@ NormPlan norm_plan(int rows, int cols, int dtype, int kind) {
   return p;
 }
 
-bool norm_v2_supported(int cols, int dtype) { return norm_plan(1, cols, dtype, kNormBwd).gen >= 2; }
-
-int norm_bwd_parts(int rows, int cols, int dtype) { return norm_plan(rows, cols, dtype, kNormBwd).grid; }
+// At gen-1 widths the fused op's dbias is a launch_column_sum over the same scratch, so it has room for that too
+int norm_bwd_parts(int rows, int cols, int dtype) {
+  const NormPlan pl = norm_plan(rows, cols, dtype, kNormBwd);
+  return pl.gen == 1 ? std::max(pl.grid, (bias_gelu_parts(rows, cols) + 2) / 3) : pl.grid;
+}
 
 template <typename T, bool kRMS, bool kFused>
 static bool run_fwd_v3(const NormPlan& pl, const void* x, const void* gamma, const void* beta, void* y, float* mean,
@@ -1171,23 +1127,18 @@ static bool run_fwd_v3(const NormPlan& pl, const void* x, const void* gamma, con
 
 template <typename T, bool kRMS, bool kFused>
 static bool run_bwd_v3(const NormPlan& pl, const void* dy, const void* x, const float* mean, const float* rstd,
-                       const void* gamma, void* dx, void* dgamma, void* dbeta, void* dbias, float* part, int rows,
-                       int cols, void* dx_drop, float p, float keep_scale, unsigned long long seed,
-                       unsigned long long offset, cudaStream_t stream) {
+                       const void* gamma, void* dx, float* part, int rows, int cols, void* dx_drop, int want_dbias,
+                       float p, float keep_scale, unsigned long long seed, unsigned long long offset,
+                       cudaStream_t stream) {
   const NormGeom3 g{rows, cols, pl.nvec};
   const int vpl = pl.vpl, lpr = pl.lpr, grid = pl.grid;
   const size_t smem = (size_t)kNormV3BwdWarps * cols * sizeof(float);
-  auto finish = [&]() {
-    colsum_finalize_kernel<T><<<dim3((cols + 31) / 32, 3), 1024, 0, stream>>>(part, grid, cols, (T*)dgamma, (T*)dbeta,
-                                                                              (T*)dbias, g_acc_mask);
-  };
   UB_DISPATCH_V3({
     auto kern = pl.full ? norm_bwd_v3_kernel<T, VPL, LPR, R, (kPF && VPL <= 3), kRMS, kFused, true>
                         : norm_bwd_v3_kernel<T, VPL, LPR, R, (kPF && VPL <= 3), kRMS, kFused, false>;
     if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     kern<<<grid, kNormV3BwdThreads, smem, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx, part, g,
-                                                 (T*)dx_drop, dbias != nullptr ? 1 : 0, p, keep_scale, seed, offset);
-    finish();
+                                                 (T*)dx_drop, want_dbias, p, keep_scale, seed, offset);
   });
   return false;
 }
@@ -1217,15 +1168,19 @@ static void run_fwd(const void* x, const void* gamma, const void* beta, void* y,
   }
 }
 
+// Every generation leaves its fp32 partial rows in part[3][pl.grid][cols] and finishes through colsum_finalize_kernel.
+// dbias (fused op, nullable): v3 / v2 sum it in the same pass; the v1 kernel keeps no third accumulator (its dgamma /
+// dbeta registers already fill the thread), so its dbias is a column sum of dx_drop after the finish.
 template <typename T, bool kRMS, bool kFused>
 static void run_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const void* gamma, void* dx,
                     void* dgamma, void* dbeta, void* dbias, float* part, int rows, int cols, void* dx_drop, float p,
-                    unsigned long long seed, unsigned long long offset, cudaStream_t stream) {
+                    unsigned long long seed, unsigned long long offset, int acc_mask, cudaStream_t stream) {
   const float keep_scale = p > 0.f ? 1.f / (1.f - p) : 1.f;
   const NormPlan pl = norm_plan(rows, cols, dtype_of<T>(), kNormBwd);
+  if (pl.gen == 0) return;  // no kernel for this width (the bindings refuse it)
   if (pl.gen == 3) {
-    run_bwd_v3<T, kRMS, kFused>(pl, dy, x, mean, rstd, gamma, dx, dgamma, dbeta, dbias, part, rows, cols, dx_drop, p,
-                                keep_scale, seed, offset, stream);
+    run_bwd_v3<T, kRMS, kFused>(pl, dy, x, mean, rstd, gamma, dx, part, rows, cols, dx_drop, dbias != nullptr ? 1 : 0,
+                                p, keep_scale, seed, offset, stream);
   } else if (pl.gen == 2) {
     const NormGeom2 g2{rows, cols, pl.tpr, pl.nvec, pl.groups};
     const size_t smem2 = (((size_t)3 * cols * sizeof(float) + 127) & ~(size_t)127) +
@@ -1235,23 +1190,21 @@ static void run_bwd(const void* dy, const void* x, const float* mean, const floa
     kern<<<pl.grid, pl.threads, smem2, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx, part,
                                                   g2, (T*)dx_drop, dbias != nullptr ? 1 : 0, p, keep_scale, seed,
                                                   offset);
-    colsum_finalize_kernel<T><<<dim3((cols + 31) / 32, 3), 1024, 0, stream>>>(part, pl.grid, cols, (T*)dgamma,
-                                                                              (T*)dbeta, (T*)dbias, g_acc_mask);
-  } else if (pl.gen == 1) {
+  } else {
     const NormGeom g{rows, cols, pl.tpr, pl.nvec};
-    const int parts = pl.grid;
-    float* dg_part = part;
-    float* db_part = part + (size_t)parts * cols;
     const size_t smem = (size_t)(kRMS ? 1 : 2) * cols * sizeof(float);
     UB_DISPATCH_VPT(pl.vpt, {
-      auto kern = g_det ? norm_bwd_kernel<T, VPT, kRMS, kFused, true> : norm_bwd_kernel<T, VPT, kRMS, kFused>;
+      auto kern = norm_bwd_kernel<T, VPT, kRMS, kFused>;
       if (smem > 48 * 1024) cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      kern<<<parts, kNormThreads, smem, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx,
-                                                  dg_part, db_part, g, (T*)dx_drop, p, keep_scale, seed, offset);
+      kern<<<pl.grid, kNormThreads, smem, stream>>>((const T*)dy, (const T*)x, mean, rstd, (const T*)gamma, (T*)dx,
+                                                    part, part + (size_t)pl.grid * cols, g, (T*)dx_drop, p, keep_scale,
+                                                    seed, offset);
     });
-    norm_param_grad_kernel<T><<<(cols + 31) / 32, 256, 0, stream>>>(dg_part, kRMS ? nullptr : db_part, parts, cols,
-                                                                    (T*)dgamma, (T*)dbeta, g_acc_mask);
   }
+  colsum_finalize_kernel<T><<<dim3((cols + 31) / 32, 3), 1024, 0, stream>>>(
+      part, pl.grid, cols, (T*)dgamma, (T*)dbeta, pl.gen == 1 ? nullptr : (T*)dbias, acc_mask);
+  if (kFused && pl.gen == 1 && dbias != nullptr)
+    launch_column_sum(dx_drop, dbias, part, rows, cols, dtype_of<T>(), stream, (acc_mask >> 2) & 1);
 }
 
 void launch_colsum_finalize(const float* part, int parts, int cols, void* out, int accumulate, int dtype,
@@ -1268,13 +1221,9 @@ void launch_layernorm_fwd(const void* x, const void* gamma, const void* beta, vo
 
 void launch_layernorm_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const void* gamma,
                           void* dx, void* dgamma, void* dbeta, float* part, int rows, int cols, int dtype,
-                          cudaStream_t stream, int accumulate, bool deterministic) {
-  g_acc_mask = accumulate;
-  g_det = deterministic;
+                          cudaStream_t stream, int accumulate) {
   UB_DISPATCH_FLOAT(dtype, (run_bwd<T, false, false>(dy, x, mean, rstd, gamma, dx, dgamma, dbeta, nullptr, part, rows,
-                                                     cols, nullptr, 0.f, 0, 0, stream)));
-  g_acc_mask = 0;
-  g_det = false;
+                                                     cols, nullptr, 0.f, 0, 0, accumulate, stream)));
 }
 
 void launch_rmsnorm_fwd(const void* x, const void* gamma, void* y, float* rstd, int rows, int cols, float eps,
@@ -1284,13 +1233,9 @@ void launch_rmsnorm_fwd(const void* x, const void* gamma, void* y, float* rstd, 
 }
 
 void launch_rmsnorm_bwd(const void* dy, const void* x, const float* rstd, const void* gamma, void* dx, void* dgamma,
-                        float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate, bool deterministic) {
-  g_acc_mask = accumulate;
-  g_det = deterministic;
+                        float* part, int rows, int cols, int dtype, cudaStream_t stream, int accumulate) {
   UB_DISPATCH_FLOAT(dtype, (run_bwd<T, true, false>(dy, x, nullptr, rstd, gamma, dx, dgamma, nullptr, nullptr, part,
-                                                    rows, cols, nullptr, 0.f, 0, 0, stream)));
-  g_acc_mask = 0;
-  g_det = false;
+                                                    rows, cols, nullptr, 0.f, 0, 0, accumulate, stream)));
 }
 
 void launch_bias_dropout_add_ln_fwd(const void* x, const void* bias, const void* residual, const void* gamma,
@@ -1304,14 +1249,9 @@ void launch_bias_dropout_add_ln_fwd(const void* x, const void* bias, const void*
 void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const float* mean, const float* rstd,
                                     const void* gamma, void* dsum, void* dx, void* dgamma, void* dbeta,
                                     void* dbias, float* part, int rows, int cols, float p, unsigned long long seed,
-                                    unsigned long long offset, int dtype, cudaStream_t stream, int accumulate, bool deterministic) {
-  // dbias (optional, v2 geometries only): column sums of dx, produced by the same pass
-  g_acc_mask = accumulate;
-  g_det = deterministic;
+                                    unsigned long long offset, int dtype, cudaStream_t stream, int accumulate) {
   UB_DISPATCH_16BIT(dtype, (run_bwd<T, false, true>(dy, summed, mean, rstd, gamma, dsum, dgamma, dbeta, dbias, part,
-                                                    rows, cols, dx, p, seed, offset, stream)));
-  g_acc_mask = 0;
-  g_det = false;
+                                                    rows, cols, dx, p, seed, offset, accumulate, stream)));
 }
 
 }  // namespace ub

@@ -5,7 +5,8 @@ Checked, each with the switch on only around the kernel calls (warn-only, which 
   and dQ agrees with it up to the order of its fp32 sum; the gradients of one batch slice are bitwise those of a call
   on that slice alone (an entirely different schedule); no wait for a turn timed out;
 - embedding gradient: bitwise equal to a float32 host loop over the rows in ascending order;
-- Gaussian basis gradient and the gen-1 norm backward: repeated calls are bitwise equal;
+- Gaussian basis gradient and the gen-1 norm backward: repeated calls are bitwise equal; the norm backward's outputs
+  are bitwise those of the default mode;
 - end to end, in fresh interpreters: two ``unicore-train --deterministic`` BERT runs log the same losses and write
   bitwise identical checkpoints, and two Uni-Mol forward + backward passes leave bitwise identical gradients.
 """
@@ -212,9 +213,8 @@ def test_gen1_norm_backward_is_deterministic(dtype, rms):
     for other in runs[1:]:
         for a, c in zip(runs[0], other):
             assert torch.equal(a, c)
-    assert torch.equal(runs[0][0], ref[0])   # dx does not change with the mode
-    for a, r in zip(runs[0][1:], ref[1:]):   # dgamma / dbeta: the same fp32 terms in another order
-        torch.testing.assert_close(a.float(), r.float(), atol=2 * UNIT[dtype] * r.float().abs().max().item(), rtol=0)
+    for a, r in zip(runs[0], ref):   # the row groups add in turn in both modes
+        assert torch.equal(a, r)
 
 
 # ---- 5. end to end -------------------------------------------------------------------------------------------------

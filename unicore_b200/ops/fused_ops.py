@@ -171,10 +171,6 @@ class _BiasDropoutAddLNFn(torch.autograd.Function):
             dy2, summed, mean, rstd, ln_weight, ctx.p, ctx.rng[0], ctx.rng[1], ctx.has_bias,
             grad_sink.sink(g_sink), grad_sink.sink(be_sink), grad_sink.sink(b_sink),
         )
-        if ctx.has_bias and dbias is None:  # geometries without the in-kernel bias sum
-            dbias = dx.sum(dim=0)
-            if b_sink is not None:
-                b_sink.grad.add_(dbias)
         if g_sink is not None:
             grad_sink.done(g_sink)
             dgamma = None
