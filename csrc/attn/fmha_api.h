@@ -50,12 +50,17 @@ struct FmhaFwdParams {
   // [bias_batch * H, T, Lb], the key mask [B, kpm_cols] contiguous.  No dropout, no keep bits, lse may be null.
   const int* seqlens;
   int kvcache, kv_cap, kpm_cols;
+  // Grouped-query attention (appended so that no earlier field moves): k / v hold H / kv_group heads, and query head h
+  // reads key / value head h / kv_group (the order of repeat_interleave(kv_group, dim=2)).  1 = one per query head.
+  // Everything else - bias, key mask, keep bits, Philox counters, LSE, logits - stays per query head.
+  int kv_group;
 };
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
 
 // Copies the T new rows of k_new / v_new [B, T, H, D] into rows p_b + i of the [B, C, H, D] caches, p_b =
-// clamp(seqlens[b], 0, C), bitwise, with 16-byte vectors; rows at or past C are skipped.  It runs as a launch of its
-// own before the KV-cache forward, which reads those rows from every query tile of a (b, h).
+// clamp(seqlens[b], 0, C), bitwise, with 16-byte vectors; rows at or past C are skipped.  H is the caches' head count
+// (H_kv under grouped-query attention).  It runs as a launch of its own before the KV-cache forward, which reads those
+// rows from every query tile of a (b, h).
 struct KvCacheAppendParams {
   const void* k_new;       // [B, T, H, D] via strides (elements)
   const void* v_new;
@@ -129,6 +134,9 @@ struct FmhaDecodeParams {
   int num_splits, chunk;
   int is_bf16;
   float scale;
+  // query head h reads cache head h / kv_group (grouped-query attention; the caches and k_new / v_new hold
+  // H / kv_group heads); 1 = one cache head per query head
+  int kv_group;
 };
 constexpr int kDecodeCtasPerSm = 3;        // 72 KB of shared memory each
 constexpr int kDecodeMinSplitKeys = 256;   // the split heuristic makes no shorter split

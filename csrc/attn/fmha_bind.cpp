@@ -8,17 +8,19 @@
 namespace {
 using namespace ub_bind;
 
-// q / k / v [B, L, H, D] (heads contiguous, strides that are multiples of 8 elements), bias [1|B, H, Lq, Lk] and the
-// bool key_padding_mask [B, Lk]: what the TMA tile maps of fill_common need.
+// q [B, Lq, H, D] and k / v [B, Lk, H_kv, D] with H_kv dividing H (grouped-query attention; heads contiguous, strides
+// that are multiples of 8 elements), bias [1|B, H, Lq, Lk] and the bool key_padding_mask [B, Lk]: what the TMA tile
+// maps of fill_common need.
 void check_common(const Tensor& q, const Tensor& k, const Tensor& v, const OptTensor& bias, const OptTensor& kpm) {
   check_operand(q, "q", q.device(), k16Bit, any_shape(4), kAligned);
   check_operand(k, "k", q.device(), {q.scalar_type()}, any_shape(4), kAligned);
   check_operand(v, "v", q.device(), {q.scalar_type()}, any_shape(4), kAligned);
-  const int64_t B = q.size(0), Lq = q.size(1), H = q.size(2), D = q.size(3), Lk = k.size(1);
+  const int64_t B = q.size(0), Lq = q.size(1), H = q.size(2), D = q.size(3), Lk = k.size(1), H_kv = v.size(2);
   TORCH_CHECK(ub::fmha_head_dim_supported(D) && k.size(3) == D && v.size(3) == D,
               "head_dim must be the same for q/k/v and a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
-  TORCH_CHECK(k.size(0) == B && v.size(0) == B && k.size(2) == H && v.size(2) == H && v.size(1) == Lk,
-              "k / v must be [B, Lk, H, D] with the B, H and D of q");
+  TORCH_CHECK(k.size(0) == B && v.size(0) == B && k.size(2) == H_kv && v.size(1) == Lk,
+              "k / v must be [B, Lk, H_kv, D] with the B and D of q");
+  kv_group(H, H_kv, "v");
   TORCH_CHECK(Lq % 8 == 0 && Lk % 8 == 0, "sequence lengths must be multiples of 8");
   for (const Tensor* t : {&q, &k, &v}) {
     // TMA descriptors: heads must be contiguous (stride D) so that (head, 16-byte chunk) is one dimension
@@ -44,6 +46,8 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   p.H = (int)q.size(2);
   p.Lk = (int)k.size(1);
   p.D = (int)q.size(3);
+  p.kv_group = (int)(q.size(2) / v.size(2));
+  const int H_kv = (int)v.size(2);
   p.is_bf16 = q.scalar_type() == at::kBFloat16 ? 1 : 0;
   p.bias = has(bias) ? bias->data_ptr() : nullptr;
   p.bias_batch = has(bias) ? (int)bias->size(0) : 1;
@@ -59,8 +63,8 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   const int q_box_rows = forward ? ub::kFwdQBoxRows : ub::kBwdBoxRows;
   const int kv_box_rows = forward ? ub::fmha_fwd_kv_box_rows(p.D) : ub::kBwdBoxRows;
   bool ok = ub::make_head_tile_map_sw128(&p.sw_q, p.q, bf16, p.B, p.Lq, p.H, p.D, p.q_sb, p.q_sl, p.q_sh, q_box_rows);
-  ok = ok && ub::make_head_tile_map_sw128(&p.sw_k, p.k, bf16, p.B, p.Lk, p.H, p.D, p.k_sb, p.k_sl, p.k_sh, kv_box_rows);
-  ok = ok && ub::make_head_tile_map_sw128(&p.sw_v, p.v, bf16, p.B, p.Lk, p.H, p.D, p.v_sb, p.v_sl, p.v_sh, kv_box_rows);
+  ok = ok && ub::make_head_tile_map_sw128(&p.sw_k, p.k, bf16, p.B, p.Lk, H_kv, p.D, p.k_sb, p.k_sl, p.k_sh, kv_box_rows);
+  ok = ok && ub::make_head_tile_map_sw128(&p.sw_v, p.v, bf16, p.B, p.Lk, H_kv, p.D, p.v_sb, p.v_sl, p.v_sh, kv_box_rows);
   if (p.bias != nullptr) ok = ok && ub::make_bias_tile_map_sw128(&p.sw_bias, p.bias, bf16, p.bias_batch * p.H, p.Lq, p.Lk);
   TORCH_CHECK(ok, "cuTensorMapEncodeTiled failed for the attention operands");
 }
@@ -122,14 +126,15 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
                                                        const OptTensor& bias, const OptTensor& kpm, double p_drop,
                                                        double scale, const OptTensor& drop_bits, bool need_dbias,
                                                        bool packed_grad, const OptTensor& dlogits, bool causal) {
-  // packed_grad: q/k/v are slices [:, :, i] of one [B, L, 3, H, D] tensor; the gradients are then
-  // written straight into one packed [B, L, 3, H, D] tensor (returned three times as views), which
-  // spares autograd three zero-filled select-backward tensors and two full-size adds per layer.
+  // packed_grad: q/k/v are the head slices [0, H), [H, H + H_kv), [H + H_kv, H + 2 H_kv) of one [B, L, H + 2 H_kv, D]
+  // tensor (a contiguous [B, L, 3, H, D] tensor is that layout with H_kv = H); the gradients are then written straight
+  // into one packed tensor of that layout (returned three times as views), which spares autograd three zero-filled
+  // slice-backward tensors and two full-size adds per layer.  dK / dV are [B, Lk, H_kv, D]: the sum over each group.
   // dlogits: gradient of the logits output of fmha_fwd_logits, [B, H, Lq, Lk]; None means zero.
   // causal: the backward of fmha_fwd(..., causal=True); its keep bits cover only the key tiles that forward walked.
   TORCH_CHECK(!(causal && has(dlogits)), "fmha_bwd: causal attention has no logits output, so dlogits must be None");
   check_common(q, k, v, bias, kpm);
-  const int64_t B = q.size(0), Lq = q.size(1), H = q.size(2), Lk = k.size(1);
+  const int64_t B = q.size(0), Lq = q.size(1), H = q.size(2), Lk = k.size(1), H_kv = k.size(2);
   // dO is read through a TMA tile map, so it is kVec like dlogits
   check_operand(dout, "dout", q.device(), {q.scalar_type()}, q.sizes(), kVec);
   check_operand(out, "out", q.device(), {q.scalar_type()}, q.sizes());
@@ -161,14 +166,14 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   p.dq_turn = det ? reinterpret_cast<int*>(dq_acc.data_ptr<float>() + acc_floats) : nullptr;
   Tensor dq, dk, dv;
   if (packed_grad) {
-    Tensor dqkv = torch::empty({p.f.B, p.f.Lq, 3, p.f.H, D}, q.options());
-    dq = dqkv.select(2, 0);
-    dk = dqkv.select(2, 1);
-    dv = dqkv.select(2, 2);
+    Tensor dqkv = torch::empty({B, Lq, H + 2 * H_kv, D}, q.options());
+    dq = dqkv.narrow(2, 0, H);
+    dk = dqkv.narrow(2, H, H_kv);
+    dv = dqkv.narrow(2, H + H_kv, H_kv);
   } else {
-    dq = torch::empty({p.f.B, p.f.Lq, p.f.H, D}, q.options());
-    dk = torch::empty({p.f.B, p.f.Lk, p.f.H, D}, q.options());
-    dv = torch::empty({p.f.B, p.f.Lk, p.f.H, D}, q.options());
+    dq = torch::empty({B, Lq, H, D}, q.options());
+    dk = torch::empty({B, Lk, H_kv, D}, q.options());
+    dv = torch::empty({B, Lk, H_kv, D}, q.options());
   }
   p.dq_sb = dq.stride(0); p.dq_sl = dq.stride(1); p.dq_sh = dq.stride(2);
   p.dk_sb = dk.stride(0); p.dk_sl = dk.stride(1); p.dk_sh = dk.stride(2);
@@ -201,14 +206,22 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   return {dq, dk, dv, dbias};
 }
 
-// q / k_cache / v_cache / k_new / v_new: [B, L, H, D] with the B, H, D and dtype of q, read as 16-byte vectors
-void check_decode_operand(const Tensor& t, const char* name, const Tensor& q, int64_t L = kAnySize) {
-  check_operand(t, name, q.device(), {q.scalar_type()}, {q.size(0), L, q.size(2), q.size(3)}, kAligned);
+// q / k_cache / v_cache / k_new / v_new: [B, L, heads, D] with the B, D and dtype of q, read as 16-byte vectors
+void check_decode_operand(const Tensor& t, const char* name, const Tensor& q, int64_t L, int64_t heads) {
+  check_operand(t, name, q.device(), {q.scalar_type()}, {q.size(0), L, heads, q.size(3)}, kAligned);
   TORCH_CHECK(t.stride(3) == 1 && t.stride(0) % 8 == 0 && t.stride(1) % 8 == 0 && t.stride(2) % 8 == 0, name,
               " needs a contiguous last dim and strides that are multiples of 8 elements");
 }
 
-// One query row per (b, h) against a [B, C, H, D] key / value cache (fmha_api.h).  max_len is a host bound on
+// The value cache [B, C, H_kv, D] fixes the key / value head count H_kv, which must divide the H query heads of q
+// (grouped-query attention); k_cache, k_new and v_new are then checked against it.  Returns H_kv.
+int64_t check_cache_heads(const Tensor& q, const Tensor& v_cache) {
+  check_decode_operand(v_cache, "v_cache", q, kAnySize, kAnySize);
+  kv_group(q.size(2), v_cache.size(2), "v_cache");
+  return v_cache.size(2);
+}
+
+// One query row per (b, h) against a [B, C, H_kv, D] key / value cache (fmha_api.h).  max_len is a host bound on
 // seqlens (the device values are never read here, so a decode step does not synchronise); with k_new / v_new the row
 // seqlens[b] is appended first and counts as visible, so up to max_len + 1 keys are.  num_splits = 0 picks the split
 // count from the shapes; any other value forces it.  split_by_length: each (b, h) divides its own device length n_b
@@ -220,17 +233,17 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   check_operand(q, "q", q.device(), k16Bit, {kAnySize, 1, kAnySize, kAnySize}, kAligned);
   const int64_t B = q.size(0), H = q.size(2), D = q.size(3);
   TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
-  check_decode_operand(q, "q", q);
-  check_decode_operand(k_cache, "k_cache", q);
-  check_decode_operand(v_cache, "v_cache", q);
+  check_decode_operand(q, "q", q, kAnySize, H);
+  const int64_t H_kv = check_cache_heads(q, v_cache);
+  check_decode_operand(k_cache, "k_cache", q, kAnySize, H_kv);
   const int64_t C = k_cache.size(1);
   TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
   const bool append = has(k_new);
   TORCH_CHECK(append == has(v_new), "k_new and v_new go together");
   TORCH_CHECK(!append || has(seqlens), "appending needs seqlens (the row to write)");
   if (append) {
-    check_decode_operand(*k_new, "k_new", q, 1);
-    check_decode_operand(*v_new, "v_new", q, 1);
+    check_decode_operand(*k_new, "k_new", q, 1, H_kv);
+    check_decode_operand(*v_new, "v_new", q, 1, H_kv);
   }
   check_operand(seqlens, "seqlens", q.device(), {at::kInt}, {B});
   if (!has(seqlens)) max_len = C;
@@ -252,6 +265,7 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   p.H = (int)H;
   p.D = (int)D;
   p.C = (int)C;
+  p.kv_group = (int)(H / H_kv);
   p.is_bf16 = q.scalar_type() == at::kBFloat16 ? 1 : 0;
   p.scale = (float)scale;
   p.q = q.data_ptr();
@@ -311,17 +325,17 @@ Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   const int64_t B = q.size(0), T = q.size(1), H = q.size(2), D = q.size(3);
   TORCH_CHECK(T >= 2, "fmha_kvcache_fwd takes chunks of T >= 2 queries (fmha_decode takes T = 1)");
   TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
-  check_decode_operand(q, "q", q);
-  check_decode_operand(k_cache, "k_cache", q);
-  check_decode_operand(v_cache, "v_cache", q);
+  check_decode_operand(q, "q", q, kAnySize, H);
+  const int64_t H_kv = check_cache_heads(q, v_cache);
+  check_decode_operand(k_cache, "k_cache", q, kAnySize, H_kv);
   const int64_t C = k_cache.size(1);
   TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
   const bool append = has(k_new);
   TORCH_CHECK(append == has(v_new), "k_new and v_new go together");
   TORCH_CHECK(append == has(seqlens), "a chunk with seqlens appends k_new / v_new, and one without does not");
   if (append) {
-    check_decode_operand(*k_new, "k_new", q, T);
-    check_decode_operand(*v_new, "v_new", q, T);
+    check_decode_operand(*k_new, "k_new", q, T, H_kv);
+    check_decode_operand(*v_new, "v_new", q, T, H_kv);
   }
   check_operand(seqlens, "seqlens", q.device(), {at::kInt}, {B});
   TORCH_CHECK(max_len >= 0, "max_len must not be negative");
@@ -368,7 +382,7 @@ Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_
     a.vn_sb = v_new->stride(0); a.vn_sl = v_new->stride(1); a.vn_sh = v_new->stride(2);
     a.kc_sb = p.k_sb; a.kc_sl = p.k_sl; a.kc_sh = p.k_sh;
     a.vc_sb = p.v_sb; a.vc_sl = p.v_sl; a.vc_sh = p.v_sh;
-    a.B = p.B; a.T = p.Lq; a.H = p.H; a.D = p.D; a.C = p.Lk;
+    a.B = p.B; a.T = p.Lq; a.H = (int)H_kv; a.D = p.D; a.C = p.Lk;
     ub::launch_kv_cache_append(a, cur_stream());
     check_launch("kv_cache_append");
   }

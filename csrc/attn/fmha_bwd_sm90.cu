@@ -6,7 +6,8 @@
 //   Templated on the padded head width DP (64 or 128): Q / K / V / dO tiles are DP / 64 column boxes whose columns
 //   D..DP-1 the TMA unit zero-fills, so they add nothing to S, dP or the products, and the epilogues store columns
 //   below D only.
-//   grid = (64-key tiles, H, B); one CTA = one warpgroup owns K_j, V_j and walks the 64-row query tiles i.  The
+//   grid = (64-key tiles, H_kv, B); one CTA = one warpgroup owns K_j, V_j and walks the 64-row query tiles i (of
+//   every query head that shares that key / value head).  The
 //   products are computed transposed (keys are the M dimension), so that P^T and dS^T are accumulator tiles whose
 //   16-bit conversions are directly the register A operands of the dV / dK products:
 //     S^T  = K_j Q_i^T                      wgmma m64n64, both operands K-major from shared memory
@@ -165,20 +166,29 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
 // ---- main kernel ----------------------------------------------------------------------------------------------
 // kLogits: the forward also returned z, and dz (fmha_api.h) is added to dS before it is packed, so that the dK operand,
 // the dQ tile and the dBias store all carry dS_total = P o (drop(dP) - delta) + dz
-// kCausal: only queries >= key0 see the CTA's keys, so the query-tile loop starts at i0 = key0 / 64 (kBM == kBN: tile i0
-// is the diagonal one, where P = dS = 0 at key > query through an additive -inf, as the future mask gives).  Stages and
-// mbarrier phases count from i0.  A CTA with key0 >= Lq has no query tile: it loads nothing and stores dK = dV = 0.
-// dBias above the diagonal is exactly 0: with a per-batch bias (ds_buf == dbias) the CTA stores a zero tile for each
-// skipped query tile i < i0; with a shared bias the reduction kernel writes the zeros and never reads those tiles.
-// kDet (deterministic mode, bp.dq_turn set): the key tiles add their dQ shares into query tile i strictly in ascending
-// key-tile order j, so dQ_i = ((0 + dQ_i^0) + dQ_i^1) + ... whatever the schedule.  Before its reduction, thread 0 of
-// key tile j waits until the turn counter of (b, h, i) is j; after the reduction has completed it increments the
-// counter.  The chain has no gap: every key tile walks every query tile, and in causal mode key tile j starts at query
-// tile j, so the tiles that reach query tile i are exactly 0 .. min(i, n_kt - 1).  Forward progress: a CTA only ever
-// waits on the CTA of the same (b, h) with the next lower blockIdx.x, whose linear block index is lower, so the
-// hardware dispatched it before this one; by induction down to key tile 0, which never waits, the chain completes.
-// The wait is at the last point, with the dQ tile already staged, so a CTA does not hold up the chain while it
-// computes.  dK, dV and dS are computed exactly as in the default mode.
+// Grouped-query attention (p.kv_group = G > 1): the grid is (key tiles, H / G, B), and CTA (j, hk, b) walks the query
+// tiles of each of the G query heads h = hk * G .. hk * G + G - 1 that read its K_j / V_j, in one flat sequence of
+// steps t (head-major; stages and phase parities count over t).  dK_j and dV_j accumulate in registers over the whole
+// group and are stored once: no atomics, no per-query-head scratch, and the sum over the group has one fixed order in
+// both modes.  dQ, dS / dBias, the keep bits, LSE and delta stay per query head.  At G = 1 the steps are the query
+// tiles of the one head, in the order and with the operations of a plain per-head walk.
+// kCausal: only queries >= key0 see the CTA's keys, so each head's query-tile walk starts at i0 = key0 / 64 (kBM == kBN:
+// tile i0 is the diagonal one, where P = dS = 0 at key > query through an additive -inf, as the future mask gives).  A
+// CTA with key0 >= Lq has no query tile: it loads nothing and stores dK = dV = 0.  dBias above the diagonal is exactly
+// 0: with a per-batch bias (ds_buf == dbias) the CTA stores a zero tile for each skipped query tile i < i0 of each
+// head of its group; with a shared bias the reduction kernel writes the zeros and never reads those tiles.
+// kDet (deterministic mode, bp.dq_turn set): the key tiles add their dQ shares into query tile i of query head h
+// strictly in ascending key-tile order j, so dQ_i = ((0 + dQ_i^0) + dQ_i^1) + ... whatever the schedule.  Before its
+// reduction, thread 0 of key tile j waits until the turn counter of (b, h, i) is j; after the reduction has completed
+// it increments the counter.  The chain has no gap: every key tile walks every query tile of every head of its group,
+// and in causal mode key tile j starts each head at query tile j, so the tiles that reach (h, i) are exactly
+// 0 .. min(i, n_kt - 1), all of the same (b, hk = h / G).  Forward progress: a CTA only ever waits on the CTA of the
+// same (b, hk) with the next lower blockIdx.x, whose linear block index x + n_kt * (hk + H / G * b) is lower, so the
+// hardware dispatched it before this one.  That CTA walks the same (h, i) sequence and passes each turn when it
+// reaches it, waiting only on its own lower neighbour; by induction down to key tile 0, which never waits, every CTA
+// finishes its whole sequence, so every turn this CTA waits for arrives.  The wait is at the last point, with the dQ
+// tile already staged, so a CTA does not hold up the chain while it computes.  dK, dV and dS are computed exactly as
+// in the default mode.
 template <typename T, int DP, bool kLogits, bool kCausal, bool kDet = false>
 __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
@@ -192,7 +202,7 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   const FmhaFwdParams& p = bp.f;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, c = lane & 3;
-  const int key0 = blockIdx.x * kBN, h = blockIdx.y, b = blockIdx.z;
+  const int key0 = blockIdx.x * kBN, hk = blockIdx.y, b = blockIdx.z;
   const uint32_t bar_kv = smem_base + kOffBar, bar_in0 = smem_base + kOffBar + 8;   // + 8 * stage
   const bool has_bias = p.bias != nullptr;
   const bool drop = p.p_drop > 0.f && p.drop_bits != nullptr;
@@ -200,12 +210,15 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   const int Lq_pad = n_qtiles * kBM;
   // first query tile: causal CTAs skip the tiles whose queries all precede key0 (i0 == n_qtiles: none is left)
   const int i0 = kCausal ? min(key0 / kBM, n_qtiles) : 0;
-  const long long bh = (long long)b * p.H + h;
-  const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
+  // the group's query heads h0 .. h0 + G - 1 one after the other, each over its query tiles i0 .. n_qtiles - 1: step
+  // t = (h - h0) * (n_qtiles - i0) + (i - i0) of one flat sequence, whose index counts the stages and phase parities
+  const int h0 = hk * p.kv_group;
+  const int n_steps = p.kv_group * (n_qtiles - i0);
   const int words_per_row = (p.Lk + 31) / 32;
   // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
-  auto load_tile = [&](int i) {   // one thread: Q_i, dO_i (and the bias and dz tiles) -> stage (i - i0) & 1
-    const uint32_t st = (uint32_t)((i - i0) & 1), bar = bar_in0 + 8u * st;
+  auto load_tile = [&](int h, int i, int t) {   // one thread: Q_i, dO_i (and the bias and dz tiles) of head h
+    const uint32_t st = (uint32_t)(t & 1), bar = bar_in0 + 8u * st;
+    const int bh = b * p.H + h, bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
     mbar_expect_tx(bar, 2 * kTile + (has_bias ? 8192u : 0u) + (kLogits ? 8192u : 0u));
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
@@ -213,12 +226,14 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
       tma_load_4d(smem_base + kOffDO + st * kTile + x * 8192, &bp.sw_do, 64 * x, h, i * kBM, b, bar);
     }
     if (has_bias) tma_load_3d(smem_base + kOffDS + st * 8192, &p.sw_bias, key0, i * kBM, bias_nb, bar);
-    if constexpr (kLogits) tma_load_3d(smem_base + C::kOffDZ + st * 8192, &bp.sw_dz, key0, i * kBM, (int)bh, bar);
+    if constexpr (kLogits) tma_load_3d(smem_base + C::kOffDZ + st * 8192, &bp.sw_dz, key0, i * kBM, bh, bar);
   };
   // causal: the keep words (key0 >> 5) + {0, 1} are read for query tiles i >= key0 / 64 only; the causal forward of such
   // a tile walked the keys up to at least i * 64 + 63 >= key0 + 63, so it wrote both words of every row it read here
-  auto load_stats = [&](int i) {  // all threads: LSE (log2 units, +inf = row contributes nothing), delta, keep bits
-    uint8_t* s = smem + kOffStats + ((i - i0) & 1) * 1024;
+  // all threads: LSE (log2 units, +inf = row contributes nothing), delta, keep bits of query tile i of head h
+  auto load_stats = [&](int h, int i, int t) {
+    uint8_t* s = smem + kOffStats + (t & 1) * 1024;
+    const long long bh = (long long)b * p.H + h;
     const int q = i * kBM + (tid & 63);
     const bool ok = q < p.Lq;
     if (tid < 64) {
@@ -244,15 +259,15 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
       mbar_expect_tx(bar_kv, 2 * kTile);
 #pragma unroll
       for (int x = 0; x < C::kBoxes; ++x) {
-        tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, h, key0, b, bar_kv);
-        tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, h, key0, b, bar_kv);
+        tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, hk, key0, b, bar_kv);
+        tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, hk, key0, b, bar_kv);
       }
-      load_tile(i0);
+      load_tile(h0, i0, 0);
     }
   }
-  if (any_q) load_stats(i0);
+  if (any_q) load_stats(h0, i0, 0);
   // causal, per-batch dBias: the skipped tiles (i < i0, every key above every query) are zero.  The first 8 KB of the
-  // dQ staging tile are zeroed and stored over each of them; the first dQ tile is written after the bulk_wait_read of
+  // dQ staging tile are zeroed and stored over each of them, for each query head of the group; the first dQ tile is written after the bulk_wait_read of
   // the loop's first barrier (A), when the stores have read it.
   const bool zero_ds = kCausal && i0 > 0 && bp.ds_buf != nullptr && bp.ds_buf == bp.dbias;
   if (zero_ds) {
@@ -286,20 +301,28 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   }
   __syncthreads();   // barriers initialised, stats of tile i0 in shared memory
   if (zero_ds && tid == 0) {
-    for (int i = 0; i < i0; ++i) tma_store_3d(&bp.sw_ds, key0, i * kBM, (int)bh, smem_base + kOffDQ);
+    for (int h = h0; h < h0 + p.kv_group; ++h)
+      for (int i = 0; i < i0; ++i) tma_store_3d(&bp.sw_ds, key0, i * kBM, b * p.H + h, smem_base + kOffDQ);
     bulk_commit();
   }
   if (any_q) mbar_wait(bar_kv, 0);
 
-  for (int i = i0; i < n_qtiles; ++i) {
-    const uint32_t st = (uint32_t)((i - i0) & 1);
-    __syncthreads();   // (A) tile i-1 is finished by every thread: its stage, stats and dQ staging may be reused
-    if (tid == 0) {
-      bulk_wait_read();   // the dS store and the dQ reduction of tile i-1 have read shared memory
-      if (i + 1 < n_qtiles) load_tile(i + 1);
+  int h = h0, i = i0;   // query head and query tile of step t
+  for (int t = 0; t < n_steps; ++t) {
+    const uint32_t st = (uint32_t)(t & 1);
+    const long long bh = (long long)b * p.H + h;
+    int h_next = h, i_next = i + 1;   // step t + 1
+    if (i_next == n_qtiles) {
+      i_next = i0;
+      ++h_next;
     }
-    if (i + 1 < n_qtiles) load_stats(i + 1);
-    mbar_wait(bar_in0 + 8u * st, (uint32_t)(((i - i0) >> 1) & 1));
+    __syncthreads();   // (A) step t-1 is finished by every thread: its stage, stats and dQ staging may be reused
+    if (tid == 0) {
+      bulk_wait_read();   // the dS store and the dQ reduction of step t-1 have read shared memory
+      if (t + 1 < n_steps) load_tile(h_next, i_next, t + 1);
+    }
+    if (t + 1 < n_steps) load_stats(h_next, i_next, t + 1);
+    mbar_wait(bar_in0 + 8u * st, (uint32_t)((t >> 1) & 1));
 
     const uint32_t sQ = smem_base + kOffQ + st * kTile, sDO = smem_base + kOffDO + st * kTile;
     const uint32_t sDS = smem_base + kOffDS + st * 8192;
@@ -452,6 +475,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
         red_release_gpu_add(bp.dq_turn + bh * n_qtiles + i, 1);
       }
     }
+    h = h_next;
+    i = i_next;
   }
   if (tid == 0) bulk_wait_all();   // shared memory must outlive the last store's and reduction's reads
 
@@ -460,8 +485,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   for (int half = 0; half < 2; ++half) {
     const int key = half ? kr1 : kr0;
     if (key >= p.Lk) continue;
-    T* dvg = reinterpret_cast<T*>(bp.dv) + (long long)b * bp.dv_sb + (long long)key * bp.dv_sl + (long long)h * bp.dv_sh;
-    T* dkg = reinterpret_cast<T*>(bp.dk) + (long long)b * bp.dk_sb + (long long)key * bp.dk_sl + (long long)h * bp.dk_sh;
+    T* dvg = reinterpret_cast<T*>(bp.dv) + (long long)b * bp.dv_sb + (long long)key * bp.dv_sl + (long long)hk * bp.dv_sh;
+    T* dkg = reinterpret_cast<T*>(bp.dk) + (long long)b * bp.dk_sb + (long long)key * bp.dk_sl + (long long)hk * bp.dk_sh;
 #pragma unroll
     for (int n = 0; n < DP / 8; ++n) {
       if (8 * n >= p.D) continue;   // columns 8n + 2c, +1 exist iff 8n < D (D % 8 == 0)
@@ -516,7 +541,7 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
   cudaMemsetAsync(bp.dq_acc, 0, (size_t)p.B * p.H * n_qt * (kBM * DP * sizeof(float) + (det ? sizeof(int) : 0)), stream);
   fmha_delta_kernel<T><<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
       reinterpret_cast<const T*>(bp.dout), reinterpret_cast<const T*>(p.out), bp.delta, p.B, p.H, p.Lq, p.D);
-  dim3 grid((p.Lk + kBN - 1) / kBN, p.H, p.B);
+  dim3 grid((p.Lk + kBN - 1) / kBN, p.H / p.kv_group, p.B);
   auto run = [&](auto kern, uint32_t smem_bytes) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
     kern<<<grid, kBwdThreads, smem_bytes, stream>>>(bp);

@@ -4,6 +4,8 @@
 //
 // M = 1 leaves nothing for wgmma: each key is a dot product and an axpy, and a step has to stream K and V once at HBM
 // bandwidth.  So the kernel is a copy pipeline feeding the CUDA cores:
+//   * Grouped-query attention: query head h reads key / value head h / G (G = kv_group).  The grid stays (splits, H,
+//     B): placing the G CTAs that read the same rows next to each other (x = s * G + g) measured no faster on an H100.
 //   * Split-KV: CTA (s, h, b) takes the contiguous key range [s * chunk, (s + 1) * chunk) of (b, h) (the last split
 //     runs to n_b); chunk comes from the host bound, or with p.chunk == 0 from n_b itself (a CUDA graph captured at
 //     the capacity).  With one split it writes O; otherwise it writes an fp32 partial (o[D] unnormalised, m, l) and
@@ -17,10 +19,10 @@
 //     shuffles, then the online softmax with ex2 over the group's keys of the tile and P V into the lane's fp32
 //     chunks.  At the end the 16 group states are merged in shared memory in group order.
 //   * Append (k_new / v_new set): the new token's key and value are row pos = seqlens[b] of the caches, and that row
-//     is always the last visible key (n_b = pos + 1).  The CTA whose range holds pos bulk-copies that row into its
-//     stage straight from k_new / v_new (not from the cache) and stores it bitwise into the caches.  No other CTA
-//     reads row pos of (b, h) - every other key range ends before it - so the write needs no ordering against any
-//     read, and one launch both appends and attends.
+//     is always the last visible key (n_b = pos + 1).  The CTAs whose range holds pos bulk-copy that row into their
+//     stage straight from k_new / v_new (not from the cache), and the one of the first query head of the group stores
+//     it bitwise into the caches.  No CTA reads row pos of (b, h / G) from the caches - every other key range ends
+//     before it - so the write needs no ordering against any read, and one launch both appends and attends.
 //   * Bounds: n_b is clamped to the cache capacity C (and to the columns of the bias / key mask), pos to n_b - 1, for
 //     any device value of seqlens: no read or write outside the tensors.  A row whose visible keys are all masked
 //     gives O = 0.
@@ -62,7 +64,9 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeP
   using C = DecCfg<NC>;
   extern __shared__ __align__(16) unsigned char smem[];
   const int tid = threadIdx.x, lane = tid & 31, g = tid >> 3, j8 = tid & 7;
-  const int s = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  // query head h = hk * G + gq reads cache head hk (fmha_api.h)
+  const int G = p.kv_group, s = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int hk = h / G, gq = h % G;
   const int D = p.D, nch = D / 8;
   const uint32_t row_bytes = (uint32_t)D * 2;
 
@@ -78,11 +82,12 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeP
   const int start = s * chunk;
   const int end = s == p.num_splits - 1 ? n : min(start + chunk, n);
 
-  const T* kc = reinterpret_cast<const T*>(p.k_cache) + (long long)b * p.kc_sb + (long long)h * p.kc_sh;
-  const T* vc = reinterpret_cast<const T*>(p.v_cache) + (long long)b * p.vc_sb + (long long)h * p.vc_sh;
-  const T* kn = append ? reinterpret_cast<const T*>(p.k_new) + (long long)b * p.kn_sb + (long long)h * p.kn_sh : nullptr;
-  const T* vn = append ? reinterpret_cast<const T*>(p.v_new) + (long long)b * p.vn_sb + (long long)h * p.vn_sh : nullptr;
-  const bool owner = append && start <= pos && pos < end;
+  const T* kc = reinterpret_cast<const T*>(p.k_cache) + (long long)b * p.kc_sb + (long long)hk * p.kc_sh;
+  const T* vc = reinterpret_cast<const T*>(p.v_cache) + (long long)b * p.vc_sb + (long long)hk * p.vc_sh;
+  const T* kn = append ? reinterpret_cast<const T*>(p.k_new) + (long long)b * p.kn_sb + (long long)hk * p.kn_sh : nullptr;
+  const T* vn = append ? reinterpret_cast<const T*>(p.v_new) + (long long)b * p.vn_sb + (long long)hk * p.vn_sh : nullptr;
+  // one CTA of the group stores the new row; the other G - 1 take it from k_new / v_new into their stage only
+  const bool owner = append && gq == 0 && start <= pos && pos < end;
   if (owner && tid < 2 * nch) {
     // bitwise copy of the new row into the caches (see the append invariant above)
     const int c = tid % nch;
@@ -273,7 +278,7 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_combine_kernel(const Fmh
   reinterpret_cast<T*>(p.out)[bh * p.D + d] = from_f32<T>(ls > 0.f ? o / ls : 0.f);
 }
 
-// Row i of k_new / v_new -> row p_b + i of the caches (fmha_api.h).  CTA (i, b) copies all H heads of K and of V,
+// Row i of k_new / v_new -> row p_b + i of the caches (fmha_api.h).  CTA (i, b) copies all H cache heads of K and V,
 // one 16-byte vector per thread and step; a row at or past C is skipped.
 __global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCacheAppendParams p) {
   const int i = blockIdx.x, b = blockIdx.y;

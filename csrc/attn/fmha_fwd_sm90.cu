@@ -20,7 +20,8 @@
 //   4. O += P V_j            kBlockN/16 x wgmma m64n{DP}k16, A (P) from registers, V presented MN-major from its
 //                            row-major bytes (at DP = 128 the descriptor steps to the second box through its LBO)
 //   q/k/v are read through strides straight out of the packed in_proj output; O is written as [B, Lq, H, D] so
-//   that out_proj consumes it without a transpose.
+//   that out_proj consumes it without a transpose.  Grouped-query attention: the K / V maps span H / kv_group heads
+//   and the CTA of query head h loads head h / kv_group; its arithmetic is that of the same call on expanded K / V.
 // 106 KB (DP = 64) / 98 KB (DP = 128) of shared memory and <= 255 registers per thread: two CTAs (8 warps) per SM,
 // so one CTA's softmax overlaps the other's tensor-core work and copies.
 // Logits mode (template flag kLogits, p.logits set) also writes z = S*scale + bias + key mask as [B, H, Lq, Lk]: the
@@ -112,6 +113,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   const int g = lane >> 2, c = lane & 3;
   const int q_tile = (kCausal || kKVCache) ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
   const int q0 = q_tile * kBlockM, h = blockIdx.y, b = blockIdx.z;
+  const int hk = h / p.kv_group;   // key / value head of query head h (fmha_api.h)
   const uint32_t bar0 = smem_base + C::kSmemBar;   // bar0 + 8 * stage: K / V / bias of a key tile (+ Q on the first)
   float* kadd = reinterpret_cast<float*>(smem + C::kSmemKAdd);
 
@@ -137,8 +139,8 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
       if (j == 0) tma_load_4d(smem_base + C::kSmemQ + x * C::kQBox, &p.sw_q, 64 * x, h, q0, b, bar);
-      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, h, j * kBlockN, b, bar);
-      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, h, j * kBlockN, b, bar);
+      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, j * kBlockN, b, bar);
+      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, j * kBlockN, b, bar);
     }
     if (has_bias) {   // 64 rows x kBlockN keys = kBlockN / 64 boxes of 64 keys
 #pragma unroll

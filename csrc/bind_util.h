@@ -118,4 +118,12 @@ inline void check_operand(const OptTensor& t, const char* name, const c10::Devic
   if (has(t)) check_operand(*t, name, dev, dtypes, sizes, need);
 }
 
+// Grouped-query attention: the `kv_heads` key / value heads of operand `name` are shared by groups of G = heads /
+// kv_heads query heads, so kv_heads must divide the query head count.  Returns G.
+inline int kv_group(int64_t heads, int64_t kv_heads, const char* name) {
+  TORCH_CHECK(kv_heads >= 1 && heads % kv_heads == 0, name, " has ", kv_heads,
+              " key / value heads, which must divide the ", heads, " query heads");
+  return (int)(heads / kv_heads);
+}
+
 }  // namespace ub_bind

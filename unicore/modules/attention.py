@@ -18,8 +18,14 @@ dim, or on the CPU, the materialised path (bmm + ``softmax_dropout`` kernel) is 
 to the kernel as a flag (no mask tensor); the materialised path adds the future mask ``triu(-inf, 1)`` to the bias, so
 its logits are those of the same call with that mask in ``attn_bias``.
 
+``num_kv_heads`` (grouped-query attention): the keys and values have ``H_kv`` heads, each shared by ``H / H_kv``
+consecutive query heads (``repeat_interleave`` order).  ``None`` or ``num_heads`` keeps the parameters and checkpoints
+of plain multi-head attention; otherwise ``SelfMultiheadAttention.in_proj`` projects to ``(H + 2 * H_kv) * D`` (q, k, v
+head slices in that order) and ``CrossMultiheadAttention.k_proj`` / ``v_proj`` to ``H_kv * D``.  The fused kernels read
+the shared heads as they are; the materialised path expands them, and autograd sums the expanded gradients.
+
 ``DecoderCache`` holds what incremental decoding keeps between steps: per layer the self-attention keys and values
-``[B, C, H, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.  A step may
+``[B, C, H_kv, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.  A step may
 add one token or a chunk of several per sequence, and ``rewind`` drops tokens again.
 """
 from typing import Optional
@@ -83,17 +89,32 @@ def _materialised_attention(qh, kh, vh, key_padding_mask, attn_bias4, dropout, t
     return ops.merge_heads(out.view(bsz, heads, tgt_len, dim)), logits, probs
 
 
+def _kv_heads(num_heads, num_kv_heads):
+    """The key / value head count: ``num_heads`` for ``None``; it must divide ``num_heads``."""
+    if num_kv_heads is None:
+        return num_heads
+    if num_kv_heads < 1 or num_heads % num_kv_heads != 0:
+        raise ValueError("num_kv_heads {} must divide num_heads {}".format(num_kv_heads, num_heads))
+    return num_kv_heads
+
+
+def _expand_heads(x, groups):
+    """``[B, H_kv, L, D]`` -> ``[B, H_kv * groups, L, D]``, each head repeated for the query heads of its group."""
+    return x if groups == 1 else x.repeat_interleave(groups, dim=1)
+
+
 class SelfMultiheadAttention(nn.Module):
-    def __init__(self, embed_dim, num_heads, dropout=0.1, bias=True, scaling_factor=1):
+    def __init__(self, embed_dim, num_heads, dropout=0.1, bias=True, scaling_factor=1, num_kv_heads=None):
         super().__init__()
         self.embed_dim = embed_dim
         self.num_heads = num_heads
+        self.num_kv_heads = _kv_heads(num_heads, num_kv_heads)
         self.dropout = dropout
         self.head_dim = embed_dim // num_heads
         if self.head_dim * num_heads != embed_dim:
             raise ValueError("embed_dim must be divisible by num_heads")
         self.scaling = (self.head_dim * scaling_factor) ** -0.5
-        self.in_proj = nn.Linear(embed_dim, embed_dim * 3, bias=bias)
+        self.in_proj = nn.Linear(embed_dim, (num_heads + 2 * self.num_kv_heads) * self.head_dim, bias=bias)
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
 
     def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False, need_probs=True, causal=False,
@@ -112,8 +133,13 @@ class SelfMultiheadAttention(nn.Module):
         if key_padding_mask is not None and key_padding_mask.dim() == 0:
             key_padding_mask = None
         qkv = ops.linear(query, self.in_proj.weight, self.in_proj.bias)
-        qkv = qkv.view(bsz, tgt_len, 3, self.num_heads, self.head_dim)
-        q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]  # strided views [B, L, H, D]
+        H, H_kv = self.num_heads, self.num_kv_heads
+        if H_kv == H:
+            qkv = qkv.view(bsz, tgt_len, 3, H, self.head_dim)
+            q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]  # strided views [B, L, H, D]
+        else:   # head slices of [B, L, H + 2 H_kv, D]: q [B, L, H, D], k / v [B, L, H_kv, D]
+            qkv = qkv.view(bsz, tgt_len, H + 2 * H_kv, self.head_dim)
+            q, k, v = qkv[:, :, :H], qkv[:, :, H:H + H_kv], qkv[:, :, H + H_kv:]
         if cache is not None and cache.stepping:
             if return_attn:
                 raise ValueError("a decoding step does not return attention weights")
@@ -127,13 +153,18 @@ class SelfMultiheadAttention(nn.Module):
             res = ops.fused_attention_qkvpacked(
                 qkv, bias=bias4, key_padding_mask=key_padding_mask,
                 dropout_p=self.dropout, training=self.training, scale=self.scaling, return_logits=return_attn,
-                causal=causal,
+                causal=causal, num_kv_heads=None if H_kv == H else H_kv,
             )
             if not return_attn:
                 return res.reshape(bsz, tgt_len, embed_dim), None, None
             o, logits = res
             return o.reshape(bsz, tgt_len, embed_dim), logits.view(bsz * self.num_heads, tgt_len, tgt_len), None
-        qh, kh, vh = ops.split_heads(qkv.view(bsz, tgt_len, 3 * embed_dim), 3, self.num_heads, self.scaling)
+        if H_kv == H:
+            qh, kh, vh = ops.split_heads(qkv.view(bsz, tgt_len, 3 * embed_dim), 3, self.num_heads, self.scaling)
+        else:
+            qh = (q * self.scaling).transpose(1, 2).contiguous()
+            kh = _expand_heads(k.transpose(1, 2), H // H_kv).contiguous()
+            vh = _expand_heads(v.transpose(1, 2), H // H_kv).contiguous()
         if causal:
             bias4 = _add_future_mask(bias4, self.num_heads, tgt_len, qh)
         o, logits, probs = _materialised_attention(qh, kh, vh, key_padding_mask, bias4, self.dropout, self.training,
@@ -155,18 +186,20 @@ class SelfMultiheadAttention(nn.Module):
 
 
 class CrossMultiheadAttention(nn.Module):
-    def __init__(self, embed_dim, num_heads, dropout=0.1, bias=True, scaling_factor=1):
+    def __init__(self, embed_dim, num_heads, dropout=0.1, bias=True, scaling_factor=1, num_kv_heads=None):
         super().__init__()
         self.embed_dim = embed_dim
         self.num_heads = num_heads
+        self.num_kv_heads = _kv_heads(num_heads, num_kv_heads)
         self.dropout = dropout
         self.head_dim = embed_dim // num_heads
         if self.head_dim * num_heads != embed_dim:
             raise ValueError("embed_dim must be divisible by num_heads")
         self.scaling = (self.head_dim * scaling_factor) ** -0.5
+        kv_dim = self.num_kv_heads * self.head_dim
         self.q_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
-        self.k_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
-        self.v_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
+        self.k_proj = nn.Linear(embed_dim, kv_dim, bias=bias)
+        self.v_proj = nn.Linear(embed_dim, kv_dim, bias=bias)
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
 
     def attend(self, query, key, value, key_padding_mask=None, attn_bias=None, cache=None):
@@ -188,8 +221,9 @@ class CrossMultiheadAttention(nn.Module):
                                             key_padding_mask=key_padding_mask, scale=self.scaling)
             return o.reshape(bsz, tgt_len, embed_dim)
         src_len = key.size(1)
-        k = self.k_proj(key).view(bsz, src_len, self.num_heads, self.head_dim)
-        v = self.v_proj(value).view(bsz, src_len, self.num_heads, self.head_dim)
+        H_kv = self.num_kv_heads
+        k = self.k_proj(key).view(bsz, src_len, H_kv, self.head_dim)
+        v = self.v_proj(value).view(bsz, src_len, H_kv, self.head_dim)
         if cache is not None:
             cache.store_encoder(k, v)
         bias4 = _bias_as_4d(attn_bias, bsz, self.num_heads, tgt_len, src_len)
@@ -199,8 +233,10 @@ class CrossMultiheadAttention(nn.Module):
                 dropout_p=self.dropout, training=self.training, scale=self.scaling,
             ).reshape(bsz, tgt_len, embed_dim)
         (qh,) = ops.split_heads(q.view(bsz, tgt_len, embed_dim), 1, self.num_heads, self.scaling)
-        (kh,) = ops.split_heads(k.view(bsz, src_len, embed_dim), 1, self.num_heads)
-        (vh,) = ops.split_heads(v.view(bsz, src_len, embed_dim), 1, self.num_heads)
+        (kh,) = ops.split_heads(k.view(bsz, src_len, H_kv * self.head_dim), 1, H_kv)
+        (vh,) = ops.split_heads(v.view(bsz, src_len, H_kv * self.head_dim), 1, H_kv)
+        kh = _expand_heads(kh, self.num_heads // H_kv).contiguous()
+        vh = _expand_heads(vh, self.num_heads // H_kv).contiguous()
         o, _, _ = _materialised_attention(qh, kh, vh, key_padding_mask, bias4, self.dropout, self.training, False)
         return o
 
@@ -220,8 +256,9 @@ def _same_layout(a: Tensor, b: Tensor) -> bool:
 
 
 class LayerKVCache:
-    """One decoder layer's share of a ``DecoderCache``: self-attention keys / values ``k``, ``v`` ``[B, C, H, D]`` and
-    the projected encoder keys / values ``enc_k``, ``enc_v`` ``[B, S, H, D]`` (None until the prefill stores them)."""
+    """One decoder layer's share of a ``DecoderCache``: self-attention keys / values ``k``, ``v`` ``[B, C, H_kv, D]``
+    and the projected encoder keys / values ``enc_k``, ``enc_v`` ``[B, S, H_kv, D]`` (None until the prefill stores
+    them)."""
 
     def __init__(self, owner, k, v):
         self.owner = owner
@@ -277,7 +314,8 @@ class DecoderCache:
 
     ``layers``: one ``LayerKVCache`` per layer.  ``seqlens``: int32 ``[B]`` on the device, the tokens decoded so far per
     sequence (the position of the next one).  ``max_len``: a host-side upper bound on ``seqlens`` (0 = empty cache), so
-    that no step has to read the device lengths.  ``capacity``: rows of the self-attention buffers."""
+    that no step has to read the device lengths.  ``capacity``: rows of the self-attention buffers.  ``heads``: the
+    key / value heads of the layers (``H_kv`` under grouped-query attention)."""
 
     def __init__(self, num_layers, batch_size, capacity, heads, head_dim, dtype, device):
         self.capacity = capacity

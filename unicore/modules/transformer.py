@@ -16,6 +16,9 @@ fused attention kernel is usable; otherwise the reference's merged-mask formulat
 The auto-regressive decoder's future mask is not a tensor either on that path: its layers run self-attention with
 ``causal=True``, and the kernels skip the key tiles above the diagonal.  On the CPU, in fp32 or at a head dim the
 kernels do not take, the future mask is added into the bias as in the reference.
+``attention_kv_heads`` (default ``None``: one key / value head per query head) makes every attention of the stack
+grouped-query attention with that many key / value heads (``unicore/modules/attention.py``); the decoder's cache then
+holds ``H_kv`` heads per layer.
 """
 import math
 from typing import Optional
@@ -161,6 +164,7 @@ class TransformerEncoderLayer(nn.Module, _BlockMixin):
         activation_dropout: float = 0.0,
         activation_fn: str = "gelu",
         post_ln=False,
+        attention_kv_heads: Optional[int] = None,
     ) -> None:
         super().__init__()
         self.embed_dim = embed_dim
@@ -170,7 +174,8 @@ class TransformerEncoderLayer(nn.Module, _BlockMixin):
         self.activation_dropout = activation_dropout
         self.activation_fn = utils.get_activation_fn(activation_fn)
         self._gelu = activation_fn == "gelu"
-        self.self_attn = SelfMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout)
+        self.self_attn = SelfMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout,
+                                                num_kv_heads=attention_kv_heads)
         self.self_attn_layer_norm = LayerNorm(self.embed_dim)
         self.fc1 = nn.Linear(self.embed_dim, ffn_embed_dim)
         self.fc2 = nn.Linear(ffn_embed_dim, self.embed_dim)
@@ -209,6 +214,7 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
         activation_dropout: float = 0.0,
         activation_fn: str = "gelu",
         post_ln=False,
+        attention_kv_heads: Optional[int] = None,
     ) -> None:
         super().__init__()
         self.embed_dim = embed_dim
@@ -218,9 +224,11 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
         self.activation_dropout = activation_dropout
         self.activation_fn = utils.get_activation_fn(activation_fn)
         self._gelu = activation_fn == "gelu"
-        self.self_attn = SelfMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout)
+        self.self_attn = SelfMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout,
+                                                num_kv_heads=attention_kv_heads)
         self.self_attn_layer_norm = LayerNorm(self.embed_dim)
-        self.encoder_attn = CrossMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout)
+        self.encoder_attn = CrossMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout,
+                                                    num_kv_heads=attention_kv_heads)
         self.encoder_attn_layer_norm = LayerNorm(self.embed_dim)
         self.fc1 = nn.Linear(self.embed_dim, ffn_embed_dim)
         self.fc2 = nn.Linear(ffn_embed_dim, self.embed_dim)
@@ -360,6 +368,7 @@ class TransformerEncoder(nn.Module, _StackMixin):
         rel_pos_bins: int = 32,
         max_rel_pos: int = 128,
         post_ln: bool = False,
+        attention_kv_heads: Optional[int] = None,
     ) -> None:
         super().__init__()
         self.emb_dropout = emb_dropout
@@ -379,6 +388,7 @@ class TransformerEncoder(nn.Module, _StackMixin):
                     activation_dropout=activation_dropout,
                     activation_fn=activation_fn,
                     post_ln=post_ln,
+                    attention_kv_heads=attention_kv_heads,
                 )
                 for _ in range(encoder_layers)
             ]
@@ -418,12 +428,14 @@ class TransformerDecoder(nn.Module, _StackMixin):
         max_rel_pos: int = 128,
         post_ln: bool = False,
         auto_regressive: bool = True,
+        attention_kv_heads: Optional[int] = None,
     ) -> None:
         super().__init__()
         self.emb_dropout = emb_dropout
         self.max_seq_len = max_seq_len
         self.embed_dim = embed_dim
         self.attention_heads = attention_heads
+        self.attention_kv_heads = attention_kv_heads
         self.emb_layer_norm = LayerNorm(self.embed_dim)
         self.auto_regressive = auto_regressive
         self._future_mask = bulid_future_mask(self.max_seq_len) if auto_regressive else None
@@ -439,6 +451,7 @@ class TransformerDecoder(nn.Module, _StackMixin):
                     activation_dropout=activation_dropout,
                     activation_fn=activation_fn,
                     post_ln=post_ln,
+                    attention_kv_heads=attention_kv_heads,
                 )
                 for _ in range(decoder_layers)
             ]
@@ -516,7 +529,8 @@ class TransformerDecoder(nn.Module, _StackMixin):
             raise ValueError("capacity {} exceeds max_seq_len {}".format(capacity, self.max_seq_len))
         weight = self.emb_layer_norm.weight
         heads = self.attention_heads
-        return DecoderCache(len(self.layers), batch_size, capacity, heads, self.embed_dim // heads,
+        kv_heads = self.attention_kv_heads or heads   # grouped-query attention caches H_kv heads
+        return DecoderCache(len(self.layers), batch_size, capacity, kv_heads, self.embed_dim // heads,
                             dtype or weight.dtype, device or weight.device)
 
     def _check_no_dropout(self):

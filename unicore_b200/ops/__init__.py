@@ -8,6 +8,7 @@ from .attention_ops import (  # noqa: F401
     fused_attention_qkvpacked,
     fused_attention_supported,
     fused_head_dim_supported,
+    kv_group,
 )
 from .fused_ops import (  # noqa: F401
     bias_dropout_add_layer_norm,

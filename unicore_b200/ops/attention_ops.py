@@ -31,6 +31,13 @@ decoding, a chunked prefill, the candidates of speculative decoding) runs in the
 (``csrc/attn/fmha_fwd_sm90.cu``), after a small kernel that appends its rows: query ``i`` of sequence ``b`` sees the
 cache rows up to ``seqlens[b] + i``, so K and V are streamed once per 64-query tile instead of once per token.  Both
 take every head dim the fused kernels take and have no backward.
+
+Grouped-query attention: every op takes k / v (and the caches) with ``H_kv`` heads where ``H_kv`` divides the ``H``
+query heads.  Query head ``h`` reads key / value head ``h // G``, ``G = H // H_kv`` - the order of
+``k.repeat_interleave(G, dim=2)`` - and everything else (bias, key mask, dropout, logits, causal) stays per query head,
+so the result is that of the same call on K / V expanded that way.  ``G`` comes from the shapes; a head count that
+does not divide raises ``ValueError``.  The kernels read each key / value head once per query head that shares it and
+never expand it; the backward pass sums dK / dV over each group on chip.  Multi-query attention is ``H_kv = 1``.
 """
 import math
 
@@ -47,16 +54,37 @@ def fused_head_dim_supported(head_dim: int) -> bool:
     return 8 <= head_dim <= FUSED_MAX_HEAD_DIM and head_dim % 8 == 0
 
 
+def kv_group(q_heads, k, v=None):
+    """``G = q_heads // H_kv``: the query heads that share each of the ``H_kv`` key / value heads of ``k`` (and ``v``,
+    which must have as many).  Raises ``ValueError`` when ``H_kv`` does not divide ``q_heads``."""
+    kv_heads = k.shape[2]
+    if v is not None and v.shape[2] != kv_heads:
+        raise ValueError("k and v must have the same number of heads, not {} and {}".format(kv_heads, v.shape[2]))
+    if kv_heads < 1 or q_heads % kv_heads != 0:
+        raise ValueError("{} key / value heads do not divide {} query heads".format(kv_heads, q_heads))
+    return q_heads // kv_heads
+
+
+def _expand_kv(q_heads, k, v):
+    """k / v with one head per query head: ``repeat_interleave(G, dim=2)`` (unchanged when G = 1)."""
+    G = kv_group(q_heads, k, v)
+    if G == 1:
+        return k, v
+    return k.repeat_interleave(G, dim=2), v.repeat_interleave(G, dim=2)
+
+
 def attention_reference(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
                         return_logits=False, causal=False):
     """Plain PyTorch implementation with the same signature (fallback + test oracle).
 
-    q: [B, Lq, H, D], k/v: [B, Lk, H, D]; bias broadcastable to [B, H, Lq, Lk];
+    q: [B, Lq, H, D], k/v: [B, Lk, H_kv, D] (H_kv dividing H, expanded by ``repeat_interleave``); bias broadcastable
+    to [B, H, Lq, Lk];
     key_padding_mask: [B, Lk] bool (True = masked); ``causal`` masks key j > query i. Returns [B, Lq, H, D], or with
     ``return_logits`` ``(out, z)`` with ``z [B, H, Lq, Lk]`` built with additive ``-inf`` masks (its gradient reaches
     masked keys).
     """
     B, Lq, H, D = q.shape
+    k, v = _expand_kv(H, k, v)
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     scores = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale
     if bias is not None:
@@ -124,30 +152,47 @@ class _FusedAttentionFn(torch.autograd.Function):
         return dq, dk, dv, dbias, None, None, None, None, None, None
 
 
+def _split_packed(qkv, num_kv_heads):
+    """q, k, v views of a packed projection: ``[B, L, 3, H, D]``, or ``[B, L, H + 2 * H_kv, D]`` with
+    ``num_kv_heads = H_kv`` (heads ``[0, H)``, ``[H, H + H_kv)`` and ``[H + H_kv, H + 2 * H_kv)``)."""
+    if qkv.dim() == 5:
+        return qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+    if num_kv_heads is None:
+        raise ValueError("a [B, L, H + 2 * H_kv, D] projection needs num_kv_heads")
+    H = qkv.shape[2] - 2 * num_kv_heads
+    if H < 1 or num_kv_heads < 1 or H % num_kv_heads != 0:
+        raise ValueError("{} key / value heads do not divide the {} query heads of a packed projection of {} heads"
+                         .format(num_kv_heads, H, qkv.shape[2]))
+    return qkv[:, :, :H], qkv[:, :, H:H + num_kv_heads], qkv[:, :, H + num_kv_heads:]
+
+
 class _FusedAttentionPackedFn(torch.autograd.Function):
-    """Self-attention on a packed ``[B, L, 3, H, D]`` projection: q/k/v are strided slices on the way
-    in, and the backward kernels write dq/dk/dv directly into ONE packed gradient tensor."""
+    """Self-attention on a packed projection (``_split_packed``): q/k/v are strided slices on the way in, and the
+    backward kernels write dq/dk/dv directly into ONE packed gradient tensor."""
 
     @staticmethod
-    def forward(ctx, qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits=False, causal=False):
-        q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+    def forward(ctx, qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits=False, causal=False,
+                num_kv_heads=None):
+        q, k, v = _split_packed(qkv, num_kv_heads)
         out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits,
                                       causal)
+        ctx.num_kv_heads = num_kv_heads
         ctx.save_for_backward(qkv, out, lse, bias, key_padding_mask, bits)
         return (out, logits) if return_logits else out
 
     @staticmethod
     def backward(ctx, dout, dlogits=None):
         qkv, out, lse, bias, kpm, bits = ctx.saved_tensors
-        q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+        q, k, v = _split_packed(qkv, ctx.num_kv_heads)
         dout, dlogits = _bwd_grads(out, dout, dlogits)
         dq, _dk, _dv, dbias = native().fmha_bwd(
             dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, True, dlogits, causal=ctx.causal
         )
-        dqkv = dq._base  # the packed [B, L, 3, H, D] tensor the three gradients are views of
+        # the packed [B, L, H + 2 * H_kv, D] tensor the three gradients are views of, in the layout of qkv
+        dqkv = dq._base.view(qkv.shape)
         if dbias is not None and dbias.dtype != bias.dtype:
             dbias = dbias.to(bias.dtype)
-        return dqkv, dbias, None, None, None, None, None, None
+        return dqkv, dbias, None, None, None, None, None, None, None
 
 
 def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool:
@@ -156,6 +201,8 @@ def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool
     if key_padding_mask is not None and key_padding_mask.dtype != torch.bool:
         return False
     if q.dim() != 4 or k.dim() != 4 or v.dim() != 4:
+        return False
+    if k.shape[2] != v.shape[2] or k.shape[2] < 1 or q.shape[2] % k.shape[2] != 0:
         return False
     head_dim = q.shape[-1]
     if not fused_head_dim_supported(head_dim) or k.shape[-1] != head_dim or v.shape[-1] != head_dim:
@@ -185,8 +232,10 @@ def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, tr
                     return_logits=False, causal=False):
     """Dispatch to the wgmma kernel when shapes/dtypes allow, else to the PyTorch reference.
 
-    Returns ``[B, Lq, H, D]``, or ``(out, z [B, H, Lq, Lk])`` with ``return_logits`` (see the module docstring).
-    ``causal`` masks key j > query i; with ``return_logits`` it runs the reference."""
+    q: ``[B, Lq, H, D]``, k / v: ``[B, Lk, H_kv, D]`` with ``H_kv`` dividing ``H`` (grouped-query attention, see the
+    module docstring).  Returns ``[B, Lq, H, D]``, or ``(out, z [B, H, Lq, Lk])`` with ``return_logits``.  ``causal``
+    masks key j > query i; with ``return_logits`` it runs the reference."""
+    kv_group(q.shape[2], k, v)
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
     if not (causal and return_logits) and fused_attention_supported(q, k, v, bias, key_padding_mask):
@@ -201,10 +250,11 @@ def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, tr
 
 
 def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
-                              return_logits=False, causal=False):
-    """Self-attention on the packed in_proj output ``qkv [B, L, 3, H, D]`` (returns ``[B, L, H, D]``, or
-    ``(out, z [B, H, L, L])`` with ``return_logits``); ``causal`` as in ``fused_attention``."""
-    q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]
+                              return_logits=False, causal=False, num_kv_heads=None):
+    """Self-attention on the packed in_proj output ``qkv [B, L, 3, H, D]``, or with grouped-query attention
+    ``qkv [B, L, H + 2 * H_kv, D]`` (q, k, v the head slices in that order) and ``num_kv_heads = H_kv``.  Returns
+    ``[B, L, H, D]``, or ``(out, z [B, H, L, L])`` with ``return_logits``; ``causal`` as in ``fused_attention``."""
+    q, k, v = _split_packed(qkv, num_kv_heads)
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
     if not (causal and return_logits) and qkv.is_contiguous() and fused_attention_supported(q, k, v, bias,
@@ -214,7 +264,7 @@ def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0
         if key_padding_mask is not None:
             key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
         return _FusedAttentionPackedFn.apply(qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits,
-                                             causal)
+                                             causal, num_kv_heads)
     return fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal)
 
 
@@ -245,6 +295,7 @@ def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len
     only when ``j <= p_b + i``.  Keys past the visible length are masked; a row with no visible unmasked key gives 0.
     """
     B, T, H, D = q.shape
+    kv_group(H, k_cache, v_cache)
     C = k_cache.shape[1]
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
     append = k_new is not None
@@ -274,7 +325,7 @@ def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len
     else:
         n = torch.full((B,), C, dtype=torch.long, device=q.device)
     K = _visible_bound(C, max_len if seqlens is not None else None, T if append else 0, bias, key_padding_mask)
-    k, v = k_cache[:, :K], v_cache[:, :K]
+    k, v = _expand_kv(H, k_cache[:, :K], v_cache[:, :K])
     scores = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale   # [B, H, T, K]
     if bias is not None:
         scores = scores + bias[..., :K].to(scores.dtype)
@@ -319,8 +370,8 @@ def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_n
                             key_padding_mask=None, scale=None):
     """Attention of T new queries per sequence against a key / value cache: one decoding step (T = 1) or a chunk.
 
-    q: ``[B, T, H, D]``; k_cache / v_cache: ``[B, C, H, D]`` (strided views are fine, the last dim contiguous).
-    ``k_new`` / ``v_new`` ``[B, T, H, D]`` (needs ``seqlens``): the new tokens' keys and values, written bitwise into
+    q: ``[B, T, H, D]``; k_cache / v_cache: ``[B, C, H_kv, D]`` with ``H_kv`` dividing ``H`` (strided views are fine,
+    the last dim contiguous).  ``k_new`` / ``v_new`` ``[B, T, H_kv, D]`` (needs ``seqlens``): the new tokens' keys and values, written bitwise into
     rows ``seqlens[b] .. seqlens[b] + T - 1`` of the caches before the attention.  Query ``i`` of batch b then sees
     rows ``0 .. seqlens[b] + i`` (the future mask of the whole sequence); with ``seqlens=None`` every query sees all C
     rows (cross-attention).  At T = 1, ``seqlens`` without ``k_new`` shows rows ``0 .. seqlens[b] - 1``; a chunk with
@@ -331,11 +382,14 @@ def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_n
     0.  Returns ``[B, T, H, D]``.  No dropout and no backward.  Under CUDA-graph capture (``max_len`` then a fixed
     bound such as the capacity) a one-token step divides each sequence's device length over the split-KV splits."""
     _check_no_grad(q, k_cache, v_cache, k_new, v_new, bias)
+    kv_group(q.shape[2], k_cache, v_cache)
     append = k_new is not None
     if append != (v_new is not None):
         raise ValueError("k_new and v_new go together")
     if append and seqlens is None:
         raise ValueError("appending needs seqlens (the row to write)")
+    if append and (k_new.shape[2] != k_cache.shape[2] or v_new.shape[2] != k_cache.shape[2]):
+        raise ValueError("k_new / v_new must have the {} heads of the caches".format(k_cache.shape[2]))
     T = q.shape[1]
     if T > 1 and seqlens is not None and not append:
         raise ValueError("a chunk of T > 1 queries with seqlens appends k_new / v_new")
