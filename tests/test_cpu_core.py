@@ -311,6 +311,22 @@ def test_softmax_dropout_fallback_and_modules():
     assert "emb_layer_norm.weight" in keys and "layers.1.final_layer_norm.bias" in keys
 
 
+@pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
+def test_softmax_cross_entropy_fallback_keeps_at_least_fp32(dtype):
+    """The fallback reduces fp32 logits in fp32 and fp64 logits (a float64 reference model) in fp64."""
+    from unicore import ops
+
+    torch.manual_seed(0)
+    logits = (torch.randn(16, 50, dtype=torch.float64) * 4).to(dtype)
+    target = torch.randint(0, 50, (16,))
+    target[3] = 0
+    loss = ops.softmax_cross_entropy(logits, target, ignore_index=0)
+    keep = target != 0
+    want = -torch.log_softmax(logits.double(), -1)[keep, target[keep]].sum()
+    assert loss.dtype == dtype
+    assert abs(loss.item() - want.item()) <= (1e-12 if dtype == torch.float64 else 1e-5) * want.item()
+
+
 def test_bert_parameter_count_and_names():
     import bert  # noqa: F401
     from unicore.tasks.synthetic import build_synthetic_dictionary

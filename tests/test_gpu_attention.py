@@ -233,10 +233,11 @@ def test_self_attention_module_matches_materialised_path():
     assert probs.shape == (24, 128, 128)
 
 
-@pytest.mark.parametrize("post_ln", [False])
+@pytest.mark.parametrize("post_ln", [False, True])
 def test_encoder_layer_matches_fp32_formulation(post_ln):
-    """Whole pre-LN layer (wgmma attention, bias-GELU, column-sum bias gradients) against the plain fp32
-    formulation of the same layer, forward and all gradients (dropout off)."""
+    """Whole pre-LN or post-LN layer (wgmma attention, bias-GELU, column-sum bias gradients, and on the post-LN path
+    the fused bias + dropout + residual + LayerNorm) against the plain fp32 formulation of the same layer, forward
+    and all gradients (dropout off)."""
     import copy
 
     import torch.nn.functional as F

@@ -370,7 +370,8 @@ def embedding(tokens: torch.Tensor, weight: torch.Tensor, padding_idx: Optional[
 
 
 def softmax_cross_entropy(logits: torch.Tensor, target: torch.Tensor, ignore_index: int = -100) -> torch.Tensor:
-    """``nll_loss(log_softmax(logits, fp32), target, reduction='sum', ignore_index=...)``."""
+    """``nll_loss(log_softmax(logits, fp32), target, reduction='sum', ignore_index=...)``; fp64 logits are reduced in
+    fp64."""
     if (
         use_native(logits, target)
         and logits.dim() == 2
@@ -384,8 +385,10 @@ def softmax_cross_entropy(logits: torch.Tensor, target: torch.Tensor, ignore_ind
         if base is not None:
             return _SoftmaxXentFn.apply(base, target.contiguous(), ignore_index, logits.shape[1])
         return _SoftmaxXentFn.apply(logits.contiguous(), target.contiguous(), ignore_index, 0)
+    # fp32 math for 16-bit and fp32 logits; fp64 logits (a float64 reference model) stay in fp64
     return F.nll_loss(
-        F.log_softmax(logits, dim=-1, dtype=torch.float32), target, ignore_index=ignore_index, reduction="sum"
+        F.log_softmax(logits, dim=-1, dtype=torch.promote_types(logits.dtype, torch.float32)), target,
+        ignore_index=ignore_index, reduction="sum"
     )
 
 
