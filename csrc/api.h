@@ -172,6 +172,23 @@ SweepPlan head_permute_plan(int B, int L, int T, int H, int D, int dtype);
 void launch_head_permute(void* token_major, void* const* head_major, int B, int L, int T, int H, int D, float scale0,
                          bool to_heads, int dtype, cudaStream_t stream);
 
+// Rotary position embeddings (rotate-half form), csrc/fused/rotary.cu.  x [B, L, N, D] 16-bit with a contiguous last dim,
+// head stride D and token / batch strides sl / sb (elements); out a new contiguous [B, L, N, D].  Heads 0 .. rotated_heads-1
+// are rotated on their first rd columns at positions l + offsets[b] (offsets: nullable int32 [B], read on the device),
+// everything else is copied bitwise; `inverse` rotates by -theta (the backward).  2 <= rd <= min(D, 512), rd even.
+// The launcher runs rotary_plan: an item is a tile of tile_tokens tokens, 256 threads per CTA, at most 8 CTAs per SM,
+// `smem` bytes of dynamic shared memory (the tile's cos / sin).  vec: the 16-byte path (8 pairs per thread), taken when
+// `aligned` (x 16-byte aligned, sb and sl multiples of 8) and rd / 2 and D are multiples of 8; else one pair per thread.
+struct RotaryPlan {
+  SweepPlan sweep;
+  bool vec;
+  int tile_tokens, smem;
+};
+RotaryPlan rotary_plan(int B, int L, int N, int D, int rd, int dtype, bool aligned);
+void launch_rotary(const void* x, void* out, const float* inv_freq, const int* offsets, long long sb, long long sl,
+                   int B, int L, int N, int D, int rd, int rotated_heads, bool aligned, bool inverse, int dtype,
+                   cudaStream_t stream);
+
 // head-major [B, H, M] <-> pair-major [B, M, H] for 16-bit elements (H % 8 == 0, M % 8 == 0)
 // The transpose and both tail kernels run pair_plan: an item is one 8 x 8 tile (8 heads x 8 pair rows), 256 threads
 // per CTA, at most 8 CTAs per SM.

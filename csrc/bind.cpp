@@ -679,6 +679,48 @@ Tensor merge_heads(const std::vector<OptTensor>& heads, double scale0) {
 }
 
 // ---------------------------------------------------------------------------------------------------
+// rotary position embeddings
+// ---------------------------------------------------------------------------------------------------
+constexpr int64_t kRotaryMaxDim = 512;   // the cos / sin tile of 8 tokens stays within 16 KB of shared memory
+
+pybind11::dict rotary_plan(int64_t B, int64_t L, int64_t N, int64_t D, int64_t rd, at::ScalarType dtype, bool aligned) {
+  TORCH_CHECK(B >= 1 && L >= 1 && N >= 1 && rd >= 2 && rd % 2 == 0 && rd <= D && rd <= kRotaryMaxDim &&
+                  (dtype == at::kHalf || dtype == at::kBFloat16),
+              "rotary_plan needs positive sizes, an even 2 <= rotary_dim <= min(head_dim, 512) and fp16 / bf16");
+  const ub::RotaryPlan p = ub::rotary_plan((int)B, (int)L, (int)N, (int)D, (int)rd, dtype_tag(dtype), aligned);
+  pybind11::dict d = sweep_dict(p.sweep);
+  d["vec"] = p.vec;
+  d["tile_tokens"] = p.tile_tokens;
+  d["smem"] = p.smem;
+  return d;
+}
+
+// x: [B, L, N, D] with a contiguous last dim and head stride D -> a new contiguous [B, L, N, D], heads 0 ..
+// rotated_heads-1 rotated on their first 2 * inv_freq.numel() columns (the inverse rotation when `inverse`)
+Tensor rotary_embedding(const Tensor& x, const Tensor& inv_freq, int64_t rotated_heads, const OptTensor& position_offsets,
+                        bool inverse) {
+  check_operand(x, "x", x.device(), k16Bit, any_shape(4), 0);
+  const int64_t B = x.size(0), L = x.size(1), N = x.size(2), D = x.size(3);
+  TORCH_CHECK(x.stride(3) == 1 && (N == 1 || x.stride(2) == D), "x must have a contiguous last dim and head stride D");
+  check_operand(inv_freq, "inv_freq", x.device(), {at::kFloat}, any_shape(1));
+  const int64_t rd = 2 * inv_freq.size(0);
+  TORCH_CHECK(rd >= 2 && rd <= D && rd <= kRotaryMaxDim, "inv_freq must have 1 .. min(head_dim, 512) / 2 entries, not ",
+              inv_freq.size(0));
+  TORCH_CHECK(rotated_heads >= 0 && rotated_heads <= N, "rotated_heads must be in [0, ", N, "], not ", rotated_heads);
+  check_operand(position_offsets, "position_offsets", x.device(), {at::kInt}, {B});
+  const c10::cuda::CUDAGuard guard(x.device());
+  Tensor out = torch::empty({B, L, N, D}, x.options());
+  if (out.numel() == 0) return out;
+  const bool aligned = aligned16(x.data_ptr()) && x.stride(0) % 8 == 0 && x.stride(1) % 8 == 0;
+  ub::launch_rotary(x.data_ptr(), out.data_ptr(), inv_freq.data_ptr<float>(),
+                    has(position_offsets) ? position_offsets->data_ptr<int>() : nullptr, x.stride(0), x.stride(1),
+                    (int)B, (int)L, (int)N, (int)D, (int)rd, (int)rotated_heads, aligned, inverse,
+                    dtype_tag(x.scalar_type()), cur_stream());
+  check_launch("rotary_embedding");
+  return out;
+}
+
+// ---------------------------------------------------------------------------------------------------
 // pair representation relayout
 // ---------------------------------------------------------------------------------------------------
 // Every pair operand is a 4-D fp16 / bf16 tensor read as 16-byte vectors; key_padding_mask is bool / uint8 [B, Lk],
@@ -845,6 +887,13 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("pair_tail_bwd", &pair_tail_bwd);
   m.def("gbf_fwd", &gbf_fwd);
   m.def("gbf_bwd", &gbf_bwd);
+  // its own submodule, _C.rotary, as _C.kvcache; tests/test_gpu_rotary.py runs the operand-rejection table of
+  // tests/test_gpu_bindings.py over it
+  auto rot = m.def_submodule("rotary", "rotary position embeddings");
+  rot.def("rotary_embedding", &rotary_embedding, pybind11::arg("x"), pybind11::arg("inv_freq"),
+          pybind11::arg("rotated_heads"), pybind11::arg("position_offsets"), pybind11::arg("inverse") = false);
+  rot.def("rotary_plan", &rotary_plan, pybind11::arg("B"), pybind11::arg("L"), pybind11::arg("N"), pybind11::arg("D"),
+          pybind11::arg("rd"), pybind11::arg("dtype"), pybind11::arg("aligned") = true);
   register_fmha(m);
   register_comm(m);
   register_symm_mem(m);

@@ -24,6 +24,14 @@ of plain multi-head attention; otherwise ``SelfMultiheadAttention.in_proj`` proj
 head slices in that order) and ``CrossMultiheadAttention.k_proj`` / ``v_proj`` to ``H_kv * D``.  The fused kernels read
 the shared heads as they are; the materialised path expands them, and autograd sums the expanded gradients.
 
+``rotary_dim`` (rotary position embeddings, ``ops.rotary_embedding``): ``SelfMultiheadAttention`` rotates the first
+``rotary_dim`` columns of every query and key head right after ``in_proj`` (rotate-half form, frequencies
+``1 / rotary_base ** (2i / rotary_dim)``), before anything reads the projection: the fused and materialised attention,
+the prefill's ``store_prefix`` (the cache holds rotated keys) and a step's ``k_new``.  Positions are ``0 .. L-1`` on a
+whole sequence or a prefill, ``seqlens[b] + i`` on a decoding step, read on the device.  ``None`` (the default) rotates
+nothing; the frequencies are a non-persistent buffer, so ``state_dict`` keys are the same either way.  Cross-attention is
+never rotated.
+
 ``DecoderCache`` holds what incremental decoding keeps between steps: per layer the self-attention keys and values
 ``[B, C, H_kv, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.  A step may
 add one token or a chunk of several per sequence, and ``rewind`` drops tokens again.
@@ -98,13 +106,23 @@ def _kv_heads(num_heads, num_kv_heads):
     return num_kv_heads
 
 
+def _rotary_dim(rotary_dim, head_dim):
+    """``rotary_dim`` checked: ``None`` (no rotation) or an even count of columns in ``[2, head_dim]``."""
+    if rotary_dim is None:
+        return None
+    if int(rotary_dim) != rotary_dim or rotary_dim % 2 != 0 or not 2 <= rotary_dim <= head_dim:
+        raise ValueError("rotary_dim {} must be even and in [2, head_dim = {}]".format(rotary_dim, head_dim))
+    return int(rotary_dim)
+
+
 def _expand_heads(x, groups):
     """``[B, H_kv, L, D]`` -> ``[B, H_kv * groups, L, D]``, each head repeated for the query heads of its group."""
     return x if groups == 1 else x.repeat_interleave(groups, dim=1)
 
 
 class SelfMultiheadAttention(nn.Module):
-    def __init__(self, embed_dim, num_heads, dropout=0.1, bias=True, scaling_factor=1, num_kv_heads=None):
+    def __init__(self, embed_dim, num_heads, dropout=0.1, bias=True, scaling_factor=1, num_kv_heads=None,
+                 rotary_dim=None, rotary_base=10000.0):
         super().__init__()
         self.embed_dim = embed_dim
         self.num_heads = num_heads
@@ -116,6 +134,17 @@ class SelfMultiheadAttention(nn.Module):
         self.scaling = (self.head_dim * scaling_factor) ** -0.5
         self.in_proj = nn.Linear(embed_dim, (num_heads + 2 * self.num_kv_heads) * self.head_dim, bias=bias)
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
+        self.rotary_dim = _rotary_dim(rotary_dim, self.head_dim)
+        self.rotary_base = rotary_base
+        if self.rotary_dim is not None:
+            self.register_buffer("inv_freq", ops.rotary_inv_freq(self.rotary_dim, rotary_base), persistent=False)
+
+    def _apply(self, fn, *args, **kwargs):
+        # .half() / .to(dtype) cast floating buffers too; the frequencies stay the fp32 values they were built as
+        super()._apply(fn, *args, **kwargs)
+        if self.rotary_dim is not None and self.inv_freq.dtype != torch.float32:
+            self.inv_freq = ops.rotary_inv_freq(self.rotary_dim, self.rotary_base).to(self.inv_freq.device)
+        return self
 
     def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False, need_probs=True, causal=False,
                cache=None):
@@ -134,6 +163,11 @@ class SelfMultiheadAttention(nn.Module):
             key_padding_mask = None
         qkv = ops.linear(query, self.in_proj.weight, self.in_proj.bias)
         H, H_kv = self.num_heads, self.num_kv_heads
+        if self.rotary_dim is not None:
+            # q and k are the leading H + H_kv heads of the projection in both packed layouts
+            offsets = cache.seqlens if cache is not None and cache.stepping else None
+            qkv = ops.rotary_embedding(qkv.view(bsz, tgt_len, H + 2 * H_kv, self.head_dim), self.inv_freq, H + H_kv,
+                                       offsets)
         if H_kv == H:
             qkv = qkv.view(bsz, tgt_len, 3, H, self.head_dim)
             q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]  # strided views [B, L, H, D]

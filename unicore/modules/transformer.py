@@ -19,6 +19,10 @@ kernels do not take, the future mask is added into the bias as in the reference.
 ``attention_kv_heads`` (default ``None``: one key / value head per query head) makes every attention of the stack
 grouped-query attention with that many key / value heads (``unicore/modules/attention.py``); the decoder's cache then
 holds ``H_kv`` heads per layer.
+``rotary_dim`` / ``rotary_base`` (default ``None``: off) give every layer's self-attention rotary position embeddings
+(``SelfMultiheadAttention``); they are independent of ``rel_pos``, and with ``rel_pos=False`` no attention of the stack
+has a bias.  A decoding step rotates its tokens at the cache lengths ``seqlens``, which ``_decode_step`` advances only
+after every layer, so all layers see the same positions.
 """
 import math
 from typing import Optional
@@ -165,6 +169,8 @@ class TransformerEncoderLayer(nn.Module, _BlockMixin):
         activation_fn: str = "gelu",
         post_ln=False,
         attention_kv_heads: Optional[int] = None,
+        rotary_dim: Optional[int] = None,
+        rotary_base: float = 10000.0,
     ) -> None:
         super().__init__()
         self.embed_dim = embed_dim
@@ -175,7 +181,8 @@ class TransformerEncoderLayer(nn.Module, _BlockMixin):
         self.activation_fn = utils.get_activation_fn(activation_fn)
         self._gelu = activation_fn == "gelu"
         self.self_attn = SelfMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout,
-                                                num_kv_heads=attention_kv_heads)
+                                                num_kv_heads=attention_kv_heads, rotary_dim=rotary_dim,
+                                                rotary_base=rotary_base)
         self.self_attn_layer_norm = LayerNorm(self.embed_dim)
         self.fc1 = nn.Linear(self.embed_dim, ffn_embed_dim)
         self.fc2 = nn.Linear(ffn_embed_dim, self.embed_dim)
@@ -215,6 +222,8 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
         activation_fn: str = "gelu",
         post_ln=False,
         attention_kv_heads: Optional[int] = None,
+        rotary_dim: Optional[int] = None,
+        rotary_base: float = 10000.0,
     ) -> None:
         super().__init__()
         self.embed_dim = embed_dim
@@ -225,7 +234,8 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
         self.activation_fn = utils.get_activation_fn(activation_fn)
         self._gelu = activation_fn == "gelu"
         self.self_attn = SelfMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout,
-                                                num_kv_heads=attention_kv_heads)
+                                                num_kv_heads=attention_kv_heads, rotary_dim=rotary_dim,
+                                                rotary_base=rotary_base)
         self.self_attn_layer_norm = LayerNorm(self.embed_dim)
         self.encoder_attn = CrossMultiheadAttention(self.embed_dim, attention_heads, dropout=attention_dropout,
                                                     num_kv_heads=attention_kv_heads)
@@ -369,6 +379,8 @@ class TransformerEncoder(nn.Module, _StackMixin):
         max_rel_pos: int = 128,
         post_ln: bool = False,
         attention_kv_heads: Optional[int] = None,
+        rotary_dim: Optional[int] = None,
+        rotary_base: float = 10000.0,
     ) -> None:
         super().__init__()
         self.emb_dropout = emb_dropout
@@ -389,6 +401,8 @@ class TransformerEncoder(nn.Module, _StackMixin):
                     activation_fn=activation_fn,
                     post_ln=post_ln,
                     attention_kv_heads=attention_kv_heads,
+                    rotary_dim=rotary_dim,
+                    rotary_base=rotary_base,
                 )
                 for _ in range(encoder_layers)
             ]
@@ -429,6 +443,8 @@ class TransformerDecoder(nn.Module, _StackMixin):
         post_ln: bool = False,
         auto_regressive: bool = True,
         attention_kv_heads: Optional[int] = None,
+        rotary_dim: Optional[int] = None,
+        rotary_base: float = 10000.0,
     ) -> None:
         super().__init__()
         self.emb_dropout = emb_dropout
@@ -452,6 +468,8 @@ class TransformerDecoder(nn.Module, _StackMixin):
                     activation_fn=activation_fn,
                     post_ln=post_ln,
                     attention_kv_heads=attention_kv_heads,
+                    rotary_dim=rotary_dim,
+                    rotary_base=rotary_base,
                 )
                 for _ in range(decoder_layers)
             ]

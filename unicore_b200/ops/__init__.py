@@ -29,4 +29,5 @@ from .optim_ops import (  # noqa: F401
     multi_tensor_scale_,
 )
 from .layout_ops import heads_to_pair, merge_heads, pair_tail, pair_to_heads, split_heads  # noqa: F401
+from .rotary_ops import rotary_embedding, rotary_embedding_reference, rotary_inv_freq  # noqa: F401
 from .softmax_ops import softmax_dropout, softmax_dropout_with_logits  # noqa: F401

@@ -11,6 +11,7 @@ The extension is built in-tree (``python setup.py build_ext --inplace`` or
 import importlib
 import logging
 import os
+import types
 
 import torch
 
@@ -59,7 +60,7 @@ _LAUNCHES_PER_CALL = {
     "symm_tail_max_blocks": 0, "symm_pick_algo": 0,
     "norm_plan": 0, "softmax_plan": 0, "bias_gelu_plan": 0, "gbf_plan": 0, "head_permute_plan": 0, "pair_plan": 0,
     "embedding_plan": 0, "fmha_decode_max_splits": 0,
-    "fmha_decode_num_splits": 0,
+    "fmha_decode_num_splits": 0, "rotary_plan": 0,
 }
 _launch_count = 0
 
@@ -75,6 +76,9 @@ class _CountingProxy:
         fn = self._cache.get(name)
         if fn is None:
             target = getattr(self._mod, name)
+            if isinstance(target, types.ModuleType):  # a submodule (_C.kvcache, _C.rotary): count its calls too
+                fn = self._cache[name] = _CountingProxy(target)
+                return fn
             if not callable(target):  # module constants (SYMM_MAX_PEERS, ...)
                 return target
             n = _LAUNCHES_PER_CALL.get(name, 1)
