@@ -317,7 +317,7 @@ def _decoder_pair(dtype):
 
 
 @pytest.mark.parametrize("dtype", DTYPES, ids=DT_IDS)
-def test_decoder_matches_fp32_merged_mask_path(dtype):
+def test_decoder_matches_fp32_materialised_path(dtype):
     ref, model = _decoder_pair(dtype)
     B, L, Le = 2, 136, 72
     g = torch.Generator(device="cuda").manual_seed(4)
@@ -369,19 +369,24 @@ def test_decoder_self_attention_calls_are_causal(monkeypatch):
             return getattr(real, name)
 
         def fmha_fwd(self, q, k, v, bias, kpm, p, scale, causal=False):
-            calls.append((q.shape[1], k.shape[1], causal, bias))
+            calls.append((q.shape[1], k.shape[1], causal, bias, kpm))
             return real.fmha_fwd(q, k, v, bias, kpm, p, scale, causal=causal)
 
     monkeypatch.setattr(attention_ops, "native", lambda: Spy())
     B, L, Le = 2, 136, 72
+    H = model.attention_heads
     emb = torch.randn(B, L, 768, device="cuda").half()
     enc = torch.randn(B, Le, 768, device="cuda").half()
     pad = torch.zeros(B, L, dtype=torch.bool, device="cuda")
     pad[1, L - 24:] = True
-    model(emb, encoder_out=enc, padding_mask=pad).float().sum().backward()
-    self_calls = [c for c in calls if c[1] == L]
-    cross_calls = [c for c in calls if c[1] == Le]
-    assert len(self_calls) == len(model.layers) and len(cross_calls) == len(model.layers)
-    for _, _, causal, bias in self_calls:
-        assert causal and bias is not None and not bool(torch.isinf(bias).any())
-    assert not any(c[2] for c in cross_calls)
+    # with an attn_mask as well, the padding still reaches the kernel as the [B, L] key mask, not as -inf in the bias
+    for attn_mask in (None, torch.randn(B * H, L, L, device="cuda").half()):
+        calls.clear()
+        model(emb, encoder_out=enc, padding_mask=pad, attn_mask=attn_mask).float().sum().backward()
+        self_calls = [c for c in calls if c[1] == L]
+        cross_calls = [c for c in calls if c[1] == Le]
+        assert len(self_calls) == len(model.layers) and len(cross_calls) == len(model.layers)
+        for _, _, causal, bias, kpm in self_calls:
+            assert causal and bias is not None and not bool(torch.isinf(bias).any())
+            assert kpm is not None and torch.equal(kpm, pad)
+        assert not any(c[2] for c in cross_calls)

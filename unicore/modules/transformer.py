@@ -10,12 +10,12 @@ GPU execution plan for one layer (post-LN shown; pre-LN analogous):
   in_proj GEMM -> fused wgmma attention (bias tile + key padding + dropout inside) ->
   out_proj GEMM -> ONE kernel: bias + dropout + residual + LayerNorm ->
   fc1 GEMM -> ONE kernel: bias + GELU -> fc2 GEMM -> ONE kernel: bias + dropout + residual + LN.
-The relative-position bias stays ``[1, H, L, L]`` (never repeated over the batch) and the key
-padding mask stays ``[B, L]`` (never merged into a ``[B*H, L, L]`` tensor of ``-inf``) whenever the
-fused attention kernel is usable; otherwise the reference's merged-mask formulation is used.
-The auto-regressive decoder's future mask is not a tensor either on that path: its layers run self-attention with
-``causal=True``, and the kernels skip the key tiles above the diagonal.  On the CPU, in fp32 or at a head dim the
-kernels do not take, the future mask is added into the bias as in the reference.
+The stacks hand every layer its masks in one form, whichever path the attention takes: the relative-position bias
+as ``[1, H, L, L]`` (never repeated over the batch), plus a user ``attn_mask`` as ``[B, H, L, L]``, and the key padding
+mask as ``[B, L]`` (never merged into the bias as ``-inf``).  The auto-regressive decoder's future mask is not a tensor
+at all: its layers run self-attention with ``causal=True``.  The attention module alone chooses between the fused
+kernels and the materialised path, and both take this form; the reference's merged ``[B*H, L, L]`` mask gives the same
+result.
 ``attention_kv_heads`` (default ``None``: one key / value head per query head) makes every attention of the stack
 grouped-query attention with that many key / value heads (``unicore/modules/attention.py``); the decoder's cache then
 holds ``H_kv`` heads per layer.
@@ -277,12 +277,6 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
 # stacks
 # ------------------------------------------------------------------------------------------------
 class _StackMixin:
-    def _fused_attention_capable(self, x):
-        """True when the layers' attention runs in the fused kernels: CUDA input, native kernels, 16-bit dtype and a
-        head dim the kernels take."""
-        return x.is_cuda and ops.USE_NATIVE and x.dtype in (torch.float16, torch.bfloat16) \
-            and ops.fused_head_dim_supported(self.embed_dim // self.attention_heads)
-
     def _init_rel_pos(self, rel_pos, rel_pos_bins, max_rel_pos):
         self.rel_pos = rel_pos
         if not rel_pos:
@@ -328,37 +322,18 @@ class _StackMixin:
             x = x * (1 - padding_mask.unsqueeze(-1).type_as(x))
         return x
 
-    def _compose_bias(self, x, attn_mask, padding_mask, future_mask=None):
-        """Combine user mask, rel-pos bias, causal mask and key padding into what layers receive.
+    def _compose_bias(self, x, attn_mask, padding_mask):
+        """What the layers receive: ``(attn_bias, key_padding_mask)``.
 
-        Returns ``(attn_bias, key_padding_mask)``.  Fast form: bias ``[1, H, L, L]`` + separate
-        padding mask (consumed by the fused attention kernel).  Reference form: everything merged
-        into ``[B*H, L, L]`` with ``-inf`` at padded keys.
-        """
+        ``attn_bias`` is None, the relative-position bias ``[1, H, L, L]``, or ``attn_mask`` (the reference's
+        ``[B*H, L, L]``, or ``[B, L, L]`` for every head) viewed as ``[B, H, L, L]`` plus that bias.  The key padding mask
+        ``[B, L]`` is passed on as it is."""
         bsz, seq_len = x.size(0), x.size(1)
-        heads = self.attention_heads
-        rel = self.get_rel_pos_bias(x) if self.rel_pos else None  # [H, L, L]
-        if attn_mask is None:
-            bias = rel.unsqueeze(0) if rel is not None else None  # [1, H, L, L]
-            if future_mask is not None:
-                fm = future_mask[:seq_len, :seq_len]
-                bias = fm.view(1, 1, seq_len, seq_len).expand(1, heads, seq_len, seq_len) if bias is None else bias + fm
-            if bias is None or self._fused_attention_capable(x) or padding_mask is None:
-                return bias, padding_mask
-            merged = bias.expand(bsz, heads, seq_len, seq_len).clone()
-        else:
-            merged = attn_mask.view(bsz, -1, seq_len, seq_len)
-            if rel is not None:
-                merged = merged + rel.unsqueeze(0)
-            if future_mask is not None:
-                merged = merged + future_mask[:seq_len, :seq_len]
-            if padding_mask is None:
-                return merged.reshape(-1, seq_len, seq_len), None
-            if merged.shape[1] != heads:
-                merged = merged.expand(bsz, heads, seq_len, seq_len)
-            merged = merged.clone() if merged.data_ptr() == attn_mask.data_ptr() else merged
-        merged = merged.masked_fill(padding_mask.unsqueeze(1).unsqueeze(2).to(torch.bool), float("-inf"))
-        return merged.reshape(-1, seq_len, seq_len), None
+        bias = self.get_rel_pos_bias(x).unsqueeze(0) if self.rel_pos else None  # [1, H, L, L]
+        if attn_mask is not None:
+            mask = attn_mask.view(bsz, -1, seq_len, seq_len).expand(bsz, self.attention_heads, seq_len, seq_len)
+            bias = mask if bias is None else mask + bias
+        return bias, padding_mask
 
 
 class TransformerEncoder(nn.Module, _StackMixin):
@@ -454,7 +429,6 @@ class TransformerDecoder(nn.Module, _StackMixin):
         self.attention_kv_heads = attention_kv_heads
         self.emb_layer_norm = LayerNorm(self.embed_dim)
         self.auto_regressive = auto_regressive
-        self._future_mask = bulid_future_mask(self.max_seq_len) if auto_regressive else None
         self.final_layer_norm = None if post_ln else LayerNorm(self.embed_dim)
         self.layers = nn.ModuleList(
             [
@@ -476,20 +450,13 @@ class TransformerDecoder(nn.Module, _StackMixin):
         )
         self._init_rel_pos(rel_pos, rel_pos_bins, max_rel_pos)
 
-    def _future(self, x):
-        if not self.auto_regressive:
-            return None
-        if self._future_mask.device != x.device or self._future_mask.dtype != x.dtype:
-            self._future_mask = self._future_mask.to(device=x.device, dtype=x.dtype)
-        return self._future_mask
-
     def get_future_mask(self, x, attn_mask):
         """Reference-format helper: returns ``[B*H, L, L]`` mask including the causal part."""
         if not self.auto_regressive:
             return attn_mask
-        fm = self._future(x)[: x.size(1), : x.size(1)]
+        fm = bulid_future_mask(x.size(1)).to(x)
         if attn_mask is None:
-            return fm.contiguous().unsqueeze(0).repeat(x.size(0) * self.attention_heads, 1, 1)
+            return fm.unsqueeze(0).repeat(x.size(0) * self.attention_heads, 1, 1)
         return attn_mask + fm
 
     def forward(
@@ -518,21 +485,19 @@ class TransformerDecoder(nn.Module, _StackMixin):
         if cache is not None:
             return self._forward_cached(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
                                         encoder_attn_mask, cache)
+        return self._forward_prefix(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask)
+
+    def _forward_prefix(self, emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask,
+                        cache=None):
+        """The whole sequence in one pass, final LayerNorm included; with a ``cache`` (the prefill) every layer also
+        stores its keys / values in it."""
         x = self._embed_prologue(emb, padding_mask)
-        # on the fused path the kernels apply the future mask themselves (causal=True); it joins no bias tensor
-        causal = self.auto_regressive and self._fused_attention_capable(x)
-        future_mask = None if causal else self._future(x)
-        attn_bias, key_padding = self._compose_bias(x, attn_mask, padding_mask, future_mask=future_mask)
-        for layer in self.layers:
-            x = layer(
-                x,
-                encoder_out=encoder_out,
-                padding_mask=key_padding,
-                attn_bias=attn_bias,
-                encoder_padding_mask=encoder_padding_mask,
-                encoder_attn_bias=encoder_attn_mask,
-                causal=causal,
-            )
+        attn_bias, key_padding = self._compose_bias(x, attn_mask, padding_mask)
+        layer_caches = cache.layers if cache is not None else [None] * len(self.layers)
+        for layer, lc in zip(self.layers, layer_caches):
+            x = layer(x, encoder_out=encoder_out, padding_mask=key_padding, attn_bias=attn_bias,
+                      encoder_padding_mask=encoder_padding_mask, encoder_attn_bias=encoder_attn_mask,
+                      causal=self.auto_regressive, cache=lc)
         if self.final_layer_norm is not None:
             x = self.final_layer_norm(x)
         return x
@@ -540,7 +505,7 @@ class TransformerDecoder(nn.Module, _StackMixin):
     # ---- incremental decoding ------------------------------------------------------------------------------------
     def new_cache(self, batch_size, capacity, dtype=None, device=None) -> DecoderCache:
         """An empty ``DecoderCache`` for ``batch_size`` sequences of up to ``capacity`` tokens (prompt included).
-        ``capacity <= max_seq_len``: the relative-position table and the future mask end there."""
+        ``capacity <= max_seq_len``: the relative-position table ends there."""
         if not self.auto_regressive:
             raise ValueError("incremental decoding needs an auto-regressive decoder")
         if capacity > self.max_seq_len:
@@ -587,21 +552,13 @@ class TransformerDecoder(nn.Module, _StackMixin):
             L = emb.size(1)
             if L > cache.capacity:
                 raise ValueError("the prompt ({} tokens) exceeds the cache capacity {}".format(L, cache.capacity))
-            x = self._embed_prologue(emb, padding_mask)
-            causal = self.auto_regressive and self._fused_attention_capable(x)
-            future_mask = None if causal else self._future(x)
-            attn_bias, key_padding = self._compose_bias(x, attn_mask, padding_mask, future_mask=future_mask)
-            for layer, lc in zip(self.layers, cache.layers):
-                x = layer(x, encoder_out=encoder_out, padding_mask=key_padding, attn_bias=attn_bias,
-                          encoder_padding_mask=encoder_padding_mask, encoder_attn_bias=encoder_attn_mask,
-                          causal=causal, cache=lc)
+            x = self._forward_prefix(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
+                                     encoder_attn_mask, cache)
             if padding_mask is None:
                 cache.seqlens.fill_(L)
             else:
                 cache.seqlens.copy_(L - padding_mask.to(torch.int32).sum(1))
             cache.max_len = L
-            if self.final_layer_norm is not None:
-                x = self.final_layer_norm(x)
             return x
         T = emb.size(1)
         if attn_mask is not None:
@@ -674,7 +631,8 @@ class CapturedDecoderStep:
         k = cache.layers[0].k if cache.layers else None
         if not torch.cuda.is_available() or k is None or not k.is_cuda:
             raise RuntimeError("capture_step needs a CUDA device and a DecoderCache on it")
-        if not ops.USE_NATIVE or not model._fused_attention_capable(k):
+        if not ops.USE_NATIVE or k.dtype not in (torch.float16, torch.bfloat16) \
+                or not ops.fused_head_dim_supported(k.size(-1)):
             raise RuntimeError("capture_step needs the native sm_90a kernels, an fp16 / bf16 cache and a head dim the "
                                "fused attention kernels take")
         model._check_no_dropout()

@@ -6,9 +6,9 @@ distance 128), post-LN by default, LM head (dense -> act -> LayerNorm -> tied pr
 evaluated only at masked positions; parameter names are identical, so checkpoints interchange.
 Architectures: bert/bert_base 12L-768-3072-12H, bert_large 24L-1024-4096-16H, xlm 16L-1280-5120-16H.
 
-GPU notes: the padding mask is handed to the fused attention kernel as ``[B, L]`` (no host sync to
-test whether the batch has padding when the fused path is active, no ``[B*H, L, L]`` ``-inf``
-tensor); the LM-head activation uses the fused bias+GELU kernel.
+GPU notes: the padding mask goes to the encoder as ``[B, L]`` on every path (no host sync to test
+whether the batch has padding: an all-False mask gives the same result as none, and no ``[B*H, L, L]``
+``-inf`` tensor); the LM-head activation uses the fused bias+GELU kernel.
 """
 import logging
 
@@ -94,22 +94,12 @@ class BertModel(BaseUnicoreModel):
     def build_model(cls, args, task):
         return cls(args, task.dictionary)
 
-    def _padding_mask(self, src_tokens, embedded):
-        mask = src_tokens.eq(self.padding_idx)
-        head_dim = self.args.encoder_embed_dim // self.args.encoder_attention_heads
-        fused = ops.use_native(embedded) and embedded.dtype in (torch.float16, torch.bfloat16) \
-            and ops.fused_head_dim_supported(head_dim)
-        if fused:
-            return mask  # consumed inside the attention kernel: no reason to sync on mask.any()
-        return mask if bool(mask.any()) else None
-
     def forward(self, src_tokens, masked_tokens=None, features_only=False, classification_head_name=None, **kwargs):
         if classification_head_name is not None:
             features_only = True
         x = ops.embedding(src_tokens, self.embed_tokens.weight, self.embed_tokens.padding_idx)   # sort-free backward
         x = x + self.embed_positions.weight[: src_tokens.size(1), :]
-        padding_mask = self._padding_mask(src_tokens, x)
-        x = self.sentence_encoder(x, padding_mask=padding_mask)
+        x = self.sentence_encoder(x, padding_mask=src_tokens.eq(self.padding_idx))
         if not features_only:
             x = self.lm_head(x, masked_tokens)
         if classification_head_name is not None:
