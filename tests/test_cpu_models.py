@@ -192,6 +192,54 @@ def test_unimol_plugin_trains_on_cpu():
             assert torch.equal(u, v)
 
 
+def _unimol_task(plugin):
+    importlib.import_module(plugin)
+    name = {"unimol": ("synthetic_unimol", "unimol", "unimol_base"),
+            "unimol_portable": ("synthetic_unimol_portable", "unimol_portable", "unimol_portable_base")}[plugin]
+    args = options.parse_args_and_arch(options.get_training_parser(), input_args=[
+        "--task", name[0], "--loss", name[1], "--arch", name[2], "--encoder-layers", "2", "--encoder-embed-dim", "32",
+        "--encoder-ffn-embed-dim", "64", "--encoder-attention-heads", "4", "--gaussian-kernels", "16",
+        "--synthetic-num-samples", "16", "--synthetic-min-atoms", "6", "--synthetic-max-atoms", "14", "--seed", "7",
+        "--dropout", "0.0", "--emb-dropout", "0.0", "--attention-dropout", "0.0", "--activation-dropout", "0.0",
+        "--cpu", "--distributed-world-size", "1",
+    ])
+    task = tasks.setup_task(args)
+    return task, task.build_model(args), task.build_loss(args)
+
+
+def test_unimol_matches_the_portable_plugin():
+    """``UniMolModel`` + ``UniMolLoss`` and the portable plug-in (``examples/unimol_portable``, the reference's
+    formulation: ``-inf`` written into the padded key columns of the pair bias up front, no fused tail) have the same
+    parameters, and with the same weights and batch the same five loss terms and gradients, up to fp32 rounding.  The
+    GPU test of the model against float64 uses the plug-in as its reference."""
+    torch.manual_seed(5)
+    task, model, loss = _unimol_task("unimol")
+    _, ref, ref_loss = _unimol_task("unimol_portable")
+    with torch.no_grad():   # an atom representation longer than sqrt(E) + 1: the x-norm term and its gradient are not 0
+        model.encoder.emb_layer_norm.weight.fill_(1.5)
+    ref.load_state_dict(model.state_dict(), strict=True)
+    task.load_dataset("train")
+    ds = task.dataset("train")
+    batch = ds.collater([ds[i] for i in range(4)])
+    assert batch["net_input"]["src_tokens"].eq(task.dictionary.pad()).any(), "the batch must have padded atoms"
+    model.train()
+    ref.train()
+    value, _, log = loss(model, batch)
+    value.backward()
+    ref_value, _, ref_log = ref_loss(ref, batch)
+    ref_value.backward()
+    for key in ("loss", "masked_token_loss", "masked_coord_loss", "masked_dist_loss", "x_norm_loss",
+                "delta_pair_repr_norm_loss"):
+        assert float(ref_log[key]) != 0, key
+        assert abs(float(log[key]) - float(ref_log[key])) <= 1e-6 * abs(float(ref_log[key])), key
+    ref_params = dict(ref.named_parameters())
+    assert set(ref_params) == {n for n, _ in model.named_parameters()}
+    for name, p in model.named_parameters():
+        g, r = p.grad, ref_params[name].grad
+        assert g is not None and r is not None, name
+        assert (g - r).abs().max() <= 1e-5 * r.abs().max(), name
+
+
 def test_nan_detector_names_the_first_bad_module(caplog):
     from unicore.nan_detector import NanDetector
 
