@@ -42,6 +42,7 @@ import torch
 from torch import Tensor, nn
 
 from unicore import ops
+from unicore_b200.ops.attention_ops import _fused_attention, _split_packed
 
 
 def _bias_as_4d(attn_bias: Optional[Tensor], bsz: int, heads: int, tgt: int, src: int) -> Optional[Tensor]:
@@ -161,19 +162,13 @@ class SelfMultiheadAttention(nn.Module):
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
         if key_padding_mask is not None and key_padding_mask.dim() == 0:
             key_padding_mask = None
-        qkv = ops.linear(query, self.in_proj.weight, self.in_proj.bias)
         H, H_kv = self.num_heads, self.num_kv_heads
+        qkv = ops.linear(query, self.in_proj.weight, self.in_proj.bias).view(bsz, tgt_len, H + 2 * H_kv, self.head_dim)
         if self.rotary_dim is not None:
-            # q and k are the leading H + H_kv heads of the projection in both packed layouts
+            # q and k are the leading H + H_kv heads of the projection
             offsets = cache.seqlens if cache is not None and cache.stepping else None
-            qkv = ops.rotary_embedding(qkv.view(bsz, tgt_len, H + 2 * H_kv, self.head_dim), self.inv_freq, H + H_kv,
-                                       offsets)
-        if H_kv == H:
-            qkv = qkv.view(bsz, tgt_len, 3, H, self.head_dim)
-            q, k, v = qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2]  # strided views [B, L, H, D]
-        else:   # head slices of [B, L, H + 2 H_kv, D]: q [B, L, H, D], k / v [B, L, H_kv, D]
-            qkv = qkv.view(bsz, tgt_len, H + 2 * H_kv, self.head_dim)
-            q, k, v = qkv[:, :, :H], qkv[:, :, H:H + H_kv], qkv[:, :, H + H_kv:]
+            qkv = ops.rotary_embedding(qkv, self.inv_freq, H + H_kv, offsets)
+        q, k, v = _split_packed(qkv, H_kv)   # strided views: q [B, L, H, D], k / v [B, L, H_kv, D]
         if cache is not None and cache.stepping:
             if return_attn:
                 raise ValueError("a decoding step does not return attention weights")
@@ -184,11 +179,8 @@ class SelfMultiheadAttention(nn.Module):
             cache.store_prefix(k, v)
         bias4 = _bias_as_4d(attn_bias, bsz, self.num_heads, tgt_len, tgt_len)
         if (not return_attn or not need_probs) and ops.fused_attention_supported(q, k, v, bias4, key_padding_mask):
-            res = ops.fused_attention_qkvpacked(
-                qkv, bias=bias4, key_padding_mask=key_padding_mask,
-                dropout_p=self.dropout, training=self.training, scale=self.scaling, return_logits=return_attn,
-                causal=causal, num_kv_heads=None if H_kv == H else H_kv,
-            )
+            res = _fused_attention(q, k, v, bias4, key_padding_mask, self.dropout, self.training, self.scaling,
+                                   return_attn, causal, qkv, supported=True)
             if not return_attn:
                 return res.reshape(bsz, tgt_len, embed_dim), None, None
             o, logits = res
@@ -262,10 +254,8 @@ class CrossMultiheadAttention(nn.Module):
             cache.store_encoder(k, v)
         bias4 = _bias_as_4d(attn_bias, bsz, self.num_heads, tgt_len, src_len)
         if ops.fused_attention_supported(q, k, v, bias4, key_padding_mask):
-            return ops.fused_attention(
-                q, k, v, bias=bias4, key_padding_mask=key_padding_mask,
-                dropout_p=self.dropout, training=self.training, scale=self.scaling,
-            ).reshape(bsz, tgt_len, embed_dim)
+            return _fused_attention(q, k, v, bias4, key_padding_mask, self.dropout, self.training, self.scaling,
+                                    False, False, supported=True).reshape(bsz, tgt_len, embed_dim)
         (qh,) = ops.split_heads(q.view(bsz, tgt_len, embed_dim), 1, self.num_heads, self.scaling)
         (kh,) = ops.split_heads(k.view(bsz, src_len, H_kv * self.head_dim), 1, H_kv)
         (vh,) = ops.split_heads(v.view(bsz, src_len, H_kv * self.head_dim), 1, H_kv)

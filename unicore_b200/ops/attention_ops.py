@@ -108,50 +108,6 @@ def attention_reference(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0
     return (out, scores) if return_logits else out
 
 
-def _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal):
-    """Shared forward of the two Functions: runs the kernel, records what the backward needs, returns
-    ``(out, lse, bits, logits)`` (logits None without ``return_logits``; never both logits and ``causal``)."""
-    p = float(dropout_p) if training else 0.0
-    logits = None
-    if return_logits:
-        out, lse, bits, logits = native().fmha_fwd_logits(q, k, v, bias, key_padding_mask, p, float(scale))
-        # a logits gradient that autograd never produced stays None (= zero) instead of a zero-filled [B, H, Lq, Lk]
-        ctx.set_materialize_grads(False)
-    else:
-        out, lse, bits = native().fmha_fwd(q, k, v, bias, key_padding_mask, p, float(scale), causal=causal)
-    ctx.p = p
-    ctx.causal = causal
-    ctx.scale = float(scale)
-    ctx.need_dbias = bias is not None and bias.requires_grad
-    return out, lse, bits, logits
-
-
-def _bwd_grads(out, dout, dlogits):
-    """(dout, dlogits) for the kernel; a missing gradient is zero, and a missing dlogits runs the plain backward."""
-    dout = torch.zeros_like(out) if dout is None else dout.contiguous()
-    return dout, (None if dlogits is None else dlogits.contiguous())
-
-
-class _FusedAttentionFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits=False, causal=False):
-        out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits,
-                                      causal)
-        ctx.save_for_backward(q, k, v, out, lse, bias, key_padding_mask, bits)
-        return (out, logits) if return_logits else out
-
-    @staticmethod
-    def backward(ctx, dout, dlogits=None):
-        q, k, v, out, lse, bias, kpm, bits = ctx.saved_tensors
-        dout, dlogits = _bwd_grads(out, dout, dlogits)
-        dq, dk, dv, dbias = native().fmha_bwd(
-            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, False, dlogits, causal=ctx.causal
-        )
-        if dbias is not None and dbias.dtype != bias.dtype:
-            dbias = dbias.to(bias.dtype)
-        return dq, dk, dv, dbias, None, None, None, None, None, None
-
-
 def _split_packed(qkv, num_kv_heads):
     """q, k, v views of a packed projection: ``[B, L, 3, H, D]``, or ``[B, L, H + 2 * H_kv, D]`` with
     ``num_kv_heads = H_kv`` (heads ``[0, H)``, ``[H, H + H_kv)`` and ``[H + H_kv, H + 2 * H_kv)``)."""
@@ -166,33 +122,63 @@ def _split_packed(qkv, num_kv_heads):
     return qkv[:, :, :H], qkv[:, :, H:H + num_kv_heads], qkv[:, :, H + num_kv_heads:]
 
 
-class _FusedAttentionPackedFn(torch.autograd.Function):
-    """Self-attention on a packed projection (``_split_packed``): q/k/v are strided slices on the way in, and the
-    backward kernels write dq/dk/dv directly into ONE packed gradient tensor."""
+class _FusedAttentionFn(torch.autograd.Function):
+    """The fused kernels' forward and backward.  ``qkv``: None, or the contiguous packed projection that q, k and v
+    are (detached) views of; the backward kernel then writes dq, dk and dv straight into one gradient of its layout,
+    which spares autograd three zero-filled slice gradients and their sum."""
 
     @staticmethod
-    def forward(ctx, qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits=False, causal=False,
-                num_kv_heads=None):
-        q, k, v = _split_packed(qkv, num_kv_heads)
-        out, lse, bits, logits = _fwd(ctx, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits,
-                                      causal)
-        ctx.num_kv_heads = num_kv_heads
-        ctx.save_for_backward(qkv, out, lse, bias, key_padding_mask, bits)
+    def forward(ctx, qkv, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal):
+        p = float(dropout_p) if training else 0.0
+        logits = None
+        if return_logits:
+            out, lse, bits, logits = native().fmha_fwd_logits(q, k, v, bias, key_padding_mask, p, float(scale))
+            # a logits gradient that autograd never produced stays None (= zero) instead of a zero-filled [B, H, Lq, Lk]
+            ctx.set_materialize_grads(False)
+        else:
+            out, lse, bits = native().fmha_fwd(q, k, v, bias, key_padding_mask, p, float(scale), causal=causal)
+        ctx.p = p
+        ctx.causal = causal
+        ctx.scale = float(scale)
+        ctx.need_dbias = bias is not None and bias.requires_grad
+        ctx.packed_shape = None if qkv is None else qkv.shape
+        ctx.save_for_backward(q, k, v, out, lse, bias, key_padding_mask, bits)
         return (out, logits) if return_logits else out
 
     @staticmethod
     def backward(ctx, dout, dlogits=None):
-        qkv, out, lse, bias, kpm, bits = ctx.saved_tensors
-        q, k, v = _split_packed(qkv, ctx.num_kv_heads)
-        dout, dlogits = _bwd_grads(out, dout, dlogits)
-        dq, _dk, _dv, dbias = native().fmha_bwd(
-            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, True, dlogits, causal=ctx.causal
+        q, k, v, out, lse, bias, kpm, bits = ctx.saved_tensors
+        # a missing gradient is zero, and a missing dlogits runs the plain backward
+        dout = torch.zeros_like(out) if dout is None else dout.contiguous()
+        dlogits = None if dlogits is None else dlogits.contiguous()
+        packed = ctx.packed_shape is not None
+        dq, dk, dv, dbias = native().fmha_bwd(
+            dout, q, k, v, out, lse, bias, kpm, ctx.p, ctx.scale, bits, ctx.need_dbias, packed, dlogits,
+            causal=ctx.causal
         )
-        # the packed [B, L, H + 2 * H_kv, D] tensor the three gradients are views of, in the layout of qkv
-        dqkv = dq._base.view(qkv.shape)
         if dbias is not None and dbias.dtype != bias.dtype:
             dbias = dbias.to(bias.dtype)
-        return dqkv, dbias, None, None, None, None, None, None, None
+        if packed:   # the [B, L, H + 2 * H_kv, D] tensor the three gradients are views of, in the layout of qkv
+            dqkv, dq, dk, dv = dq._base.view(ctx.packed_shape), None, None, None
+        else:
+            dqkv = None
+        return dqkv, dq, dk, dv, dbias, None, None, None, None, None, None
+
+
+def _kernel_tensors(q, *tensors) -> bool:
+    """The kernels' rule for q and the key / value tensors that go with it (None entries are skipped): 4-d, fp16 or
+    bf16 and all of the dtype of q, one head dim that ``fused_head_dim_supported`` takes, 16-byte aligned, strides
+    that are multiples of 8 elements and a contiguous last dim."""
+    if q.dtype not in (torch.float16, torch.bfloat16) or not fused_head_dim_supported(q.shape[-1]):
+        return False
+    for t in (q,) + tensors:
+        if t is None:
+            continue
+        if t.dim() != 4 or t.dtype != q.dtype or t.shape[-1] != q.shape[-1] or t.stride(-1) != 1:
+            return False
+        if t.data_ptr() % 16 != 0 or any(s % 8 != 0 for s in t.stride()[:3]):
+            return False
+    return True
 
 
 def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool:
@@ -200,19 +186,12 @@ def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool
         return False
     if key_padding_mask is not None and key_padding_mask.dtype != torch.bool:
         return False
-    if q.dim() != 4 or k.dim() != 4 or v.dim() != 4:
+    if not _kernel_tensors(q, k, v):
+        return False
+    # the TMA maps take (head, 16-byte chunk) as one dimension: the heads of each tensor are contiguous
+    if any(t.stride(2) != q.shape[-1] for t in (q, k, v)):
         return False
     if k.shape[2] != v.shape[2] or k.shape[2] < 1 or q.shape[2] % k.shape[2] != 0:
-        return False
-    head_dim = q.shape[-1]
-    if not fused_head_dim_supported(head_dim) or k.shape[-1] != head_dim or v.shape[-1] != head_dim:
-        return False
-    for t in (q, k, v):
-        if t.data_ptr() % 16 != 0 or any(s % 8 != 0 for s in t.stride()[:3]) or t.stride(2) != head_dim:
-            return False
-    if q.dtype not in (torch.float16, torch.bfloat16) or k.dtype != q.dtype or v.dtype != q.dtype:
-        return False
-    if q.stride(-1) != 1 or k.stride(-1) != 1 or v.stride(-1) != 1:
         return False
     if q.shape[1] % 8 != 0 or k.shape[1] % 8 != 0:
         return False
@@ -228,6 +207,32 @@ def fused_attention_supported(q, k, v, bias=None, key_padding_mask=None) -> bool
     return True
 
 
+def _fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal, qkv=None,
+                     supported=None):
+    """``fused_attention`` on q / k / v, which are the views of ``qkv`` (``_split_packed``) when it is given: a
+    contiguous ``qkv`` then gets one packed gradient.  ``supported``: the answer of ``fused_attention_supported`` for
+    these operands when the caller has it already (None: ask)."""
+    if scale is None:
+        scale = 1.0 / math.sqrt(q.shape[-1])
+    if causal and return_logits:   # the kernels do not return the logits of causal attention
+        supported = False
+    elif supported is None:
+        supported = fused_attention_supported(q, k, v, bias, key_padding_mask)
+    if not supported:
+        return attention_reference(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal)
+    if bias is not None:
+        # the kernel stages the bias tile next to P in shared memory in the compute dtype
+        bias = bias.to(q.dtype).contiguous()
+    if key_padding_mask is not None:
+        key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
+    if qkv is not None and qkv.is_contiguous():
+        q, k, v = q.detach(), k.detach(), v.detach()   # autograd sees qkv alone
+    else:
+        qkv = None
+    return _FusedAttentionFn.apply(qkv, q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits,
+                                   causal)
+
+
 def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
                     return_logits=False, causal=False):
     """Dispatch to the wgmma kernel when shapes/dtypes allow, else to the PyTorch reference.
@@ -236,17 +241,7 @@ def fused_attention(q, k, v, bias=None, key_padding_mask=None, dropout_p=0.0, tr
     module docstring).  Returns ``[B, Lq, H, D]``, or ``(out, z [B, H, Lq, Lk])`` with ``return_logits``.  ``causal``
     masks key j > query i; with ``return_logits`` it runs the reference."""
     kv_group(q.shape[2], k, v)
-    if scale is None:
-        scale = 1.0 / math.sqrt(q.shape[-1])
-    if not (causal and return_logits) and fused_attention_supported(q, k, v, bias, key_padding_mask):
-        if bias is not None:
-            # the kernel stages the bias tile next to P in shared memory in the compute dtype
-            bias = bias.to(q.dtype).contiguous()
-        if key_padding_mask is not None:
-            key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
-        return _FusedAttentionFn.apply(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits,
-                                       causal)
-    return attention_reference(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal)
+    return _fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal)
 
 
 def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0.0, training=True, scale=None,
@@ -255,17 +250,7 @@ def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0
     ``qkv [B, L, H + 2 * H_kv, D]`` (q, k, v the head slices in that order) and ``num_kv_heads = H_kv``.  Returns
     ``[B, L, H, D]``, or ``(out, z [B, H, L, L])`` with ``return_logits``; ``causal`` as in ``fused_attention``."""
     q, k, v = _split_packed(qkv, num_kv_heads)
-    if scale is None:
-        scale = 1.0 / math.sqrt(q.shape[-1])
-    if not (causal and return_logits) and qkv.is_contiguous() and fused_attention_supported(q, k, v, bias,
-                                                                                            key_padding_mask):
-        if bias is not None:
-            bias = bias.to(q.dtype).contiguous()
-        if key_padding_mask is not None:
-            key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
-        return _FusedAttentionPackedFn.apply(qkv, bias, key_padding_mask, dropout_p, training, scale, return_logits,
-                                             causal, num_kv_heads)
-    return fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal)
+    return _fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal, qkv)
 
 
 def _check_no_grad(*tensors):
@@ -274,15 +259,29 @@ def _check_no_grad(*tensors):
                            "torch.inference_mode(), or detach the inputs")
 
 
-def _visible_bound(C, max_len, append, bias, key_padding_mask):
-    """Host bound on the visible keys of any batch: ``max_len`` (+ the ``append`` new rows), else ``C``; never more
-    than the columns of the bias and of the key mask (the kernel clamps to them as well)."""
-    bound = C if max_len is None else min(C, int(max_len) + int(append))
-    if bias is not None:
-        bound = min(bound, bias.shape[-1])
-    if key_padding_mask is not None:
-        bound = min(bound, key_padding_mask.shape[-1])
-    return bound
+def _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new):
+    """The arguments of ``attention_with_kv_cache`` checked, as ``(T, append, max_len, bound)``: ``max_len`` the host
+    bound on ``seqlens`` (by default the most the capacity allows; None without ``seqlens`` unless given) and
+    ``bound`` the keys any query can see, ``max_len`` plus the appended rows, else the capacity C."""
+    kv_group(q.shape[2], k_cache, v_cache)
+    append = k_new is not None
+    if append != (v_new is not None):
+        raise ValueError("k_new and v_new go together")
+    if append and seqlens is None:
+        raise ValueError("appending needs seqlens (the row to write)")
+    if append and (k_new.shape[2] != k_cache.shape[2] or v_new.shape[2] != k_cache.shape[2]):
+        raise ValueError("k_new / v_new must have the {} heads of the caches".format(k_cache.shape[2]))
+    T = q.shape[1]
+    if T > 1 and seqlens is not None and not append:
+        raise ValueError("a chunk of T > 1 queries with seqlens appends k_new / v_new")
+    C = k_cache.shape[1]
+    new_rows = T if append else 0
+    if seqlens is not None and max_len is None:
+        max_len = C - new_rows
+    if max_len is not None and int(max_len) + new_rows > C:
+        raise ValueError("max_len {} {}exceeds the cache capacity {}".format(
+            max_len, "+ {} ".format(new_rows) if append else "", C))
+    return T, append, max_len, C if seqlens is None else int(max_len) + new_rows
 
 
 def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len=None, k_new=None, v_new=None,
@@ -294,15 +293,10 @@ def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len
     ``[0, C]``, become ``k_new[b, i] / v_new[b, i]``, rows at or past ``C`` are skipped, and query ``i`` sees key ``j``
     only when ``j <= p_b + i``.  Keys past the visible length are masked; a row with no visible unmasked key gives 0.
     """
-    B, T, H, D = q.shape
-    kv_group(H, k_cache, v_cache)
+    T, append, _, K = _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new)
+    B, _, H, D = q.shape
     C = k_cache.shape[1]
     scale = scale if scale is not None else 1.0 / math.sqrt(D)
-    append = k_new is not None
-    if append and seqlens is None:
-        raise ValueError("appending needs seqlens (the row to write)")
-    if T > 1 and seqlens is not None and not append:
-        raise ValueError("a chunk of T > 1 queries with seqlens appends k_new / v_new")
     future = None
     if T == 1 and append:
         pos = seqlens.long().clamp(0, C - 1)
@@ -324,7 +318,11 @@ def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len
         n = seqlens.long().clamp(0, C)
     else:
         n = torch.full((B,), C, dtype=torch.long, device=q.device)
-    K = _visible_bound(C, max_len if seqlens is not None else None, T if append else 0, bias, key_padding_mask)
+    # the keys past the columns of the bias or of the key mask are hidden
+    if bias is not None:
+        K = min(K, bias.shape[-1])
+    if key_padding_mask is not None:
+        K = min(K, key_padding_mask.shape[-1])
     k, v = _expand_kv(H, k_cache[:, :K], v_cache[:, :K])
     scores = torch.einsum("bqhd,bkhd->bhqk", q, k) * scale   # [B, H, T, K]
     if bias is not None:
@@ -348,22 +346,43 @@ def _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padd
     if not use_native(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask) \
             or not hasattr(native(), "fmha_decode"):
         return False
-    if q.dim() != 4 or q.shape[1] < 1 or q.dtype not in (torch.float16, torch.bfloat16):
+    if q.dim() != 4 or q.shape[1] < 1 or (q.shape[1] > 1 and not hasattr(native(), "kvcache")):
         return False
-    if q.shape[1] > 1 and not hasattr(native(), "kvcache"):
+    if not _kernel_tensors(q, k_cache, v_cache, k_new, v_new):
         return False
-    if not fused_head_dim_supported(q.shape[-1]):
-        return False
-    for t in (q, k_cache, v_cache, k_new, v_new):
-        if t is None:
-            continue
-        if t.dim() != 4 or t.dtype != q.dtype or t.shape[-1] != q.shape[-1] or t.stride(-1) != 1:
-            return False
-        if t.data_ptr() % 16 != 0 or any(s % 8 != 0 for s in t.stride()[:3]):
-            return False
     if bias is not None and bias.stride(-1) != 1 and bias.shape[-1] > 1:
         return False
     return True
+
+
+def _native_cache_operands(q, seqlens, bias, key_padding_mask, bound):
+    """``seqlens``, the bias and the key mask as ``fmha_decode`` (T = 1) and ``fmha_kvcache_fwd`` (T > 1) take them:
+    int32 lengths, a bool key mask and a bias in the dtype of q, each with a contiguous last dim.  A bias or key mask
+    narrower than the ``bound`` visible keys is widened with -inf / True, which hides the keys past it as the
+    reference's clamp to its columns does.  Operands that are already so are passed on as they are."""
+    T = q.shape[1]
+    if seqlens is not None and (seqlens.dtype != torch.int32 or not seqlens.is_contiguous()):
+        seqlens = seqlens.to(torch.int32).contiguous()
+    if bias is not None:
+        Lb = bias.shape[-1]
+        width = max(Lb, bound)
+        bias = bias.to(q.dtype)
+        if T > 1:   # read by TMA: a row for every query head, of a multiple of 8 columns
+            bias = bias.expand(bias.shape[0], q.shape[2], T, Lb)
+            width += -width % 8
+        if width != Lb:
+            bias = F.pad(bias, (0, width - Lb), value=float("-inf"))
+        if T > 1 or bias.stride(-1) != 1:
+            bias = bias.contiguous()
+    if key_padding_mask is not None:
+        if key_padding_mask.dtype != torch.bool or key_padding_mask.stride(-1) != 1:
+            key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
+        cols = key_padding_mask.shape[1]
+        if cols < bound:
+            key_padding_mask = torch.cat([key_padding_mask, key_padding_mask.new_ones(q.shape[0], bound - cols)], 1)
+        if T > 1:
+            key_padding_mask = key_padding_mask.contiguous()
+    return seqlens, bias, key_padding_mask
 
 
 def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_new=None, v_new=None, bias=None,
@@ -378,59 +397,23 @@ def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_n
     ``seqlens`` must append.  ``max_len``: a host-side upper bound on ``seqlens`` (default: the most the capacity
     allows); ``max_len + T > C`` raises, and the device lengths are never read on the host, so a step does not
     synchronise.  bias: ``[1|B, H, T, Lb]``, row i for query i, ``Lb`` covering the visible keys (columns past them
-    are ignored); key_padding_mask: bool ``[B, Lk]``, True = masked.  A query whose visible keys are all masked gives
-    0.  Returns ``[B, T, H, D]``.  No dropout and no backward.  Under CUDA-graph capture (``max_len`` then a fixed
-    bound such as the capacity) a one-token step divides each sequence's device length over the split-KV splits."""
+    are ignored); key_padding_mask: bool ``[B, Lk]``, True = masked; a narrower bias or key mask hides the keys past
+    its columns.  A query whose visible keys are all masked gives 0.  Returns ``[B, T, H, D]``.  No dropout and no
+    backward.  Under CUDA-graph capture (``max_len`` then a fixed bound such as the capacity) a one-token step divides
+    each sequence's device length over the split-KV splits."""
     _check_no_grad(q, k_cache, v_cache, k_new, v_new, bias)
-    kv_group(q.shape[2], k_cache, v_cache)
-    append = k_new is not None
-    if append != (v_new is not None):
-        raise ValueError("k_new and v_new go together")
-    if append and seqlens is None:
-        raise ValueError("appending needs seqlens (the row to write)")
-    if append and (k_new.shape[2] != k_cache.shape[2] or v_new.shape[2] != k_cache.shape[2]):
-        raise ValueError("k_new / v_new must have the {} heads of the caches".format(k_cache.shape[2]))
-    T = q.shape[1]
-    if T > 1 and seqlens is not None and not append:
-        raise ValueError("a chunk of T > 1 queries with seqlens appends k_new / v_new")
-    C = k_cache.shape[1]
-    new_rows = T if append else 0
+    T, _, max_len, bound = _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new)
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
-    if seqlens is not None and max_len is None:
-        max_len = C - new_rows
-    if max_len is not None and int(max_len) + new_rows > C:
-        raise ValueError("max_len {} {}exceeds the cache capacity {}".format(
-            max_len, "+ {} ".format(new_rows) if append else "", C))
     if not _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask):
         return attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
                                                  key_padding_mask, scale)
-    if seqlens is not None and (seqlens.dtype != torch.int32 or not seqlens.is_contiguous()):
-        seqlens = seqlens.to(torch.int32).contiguous()
-    if key_padding_mask is not None and (key_padding_mask.dtype != torch.bool or key_padding_mask.stride(-1) != 1):
-        key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
+    seqlens, bias, key_padding_mask = _native_cache_operands(q, seqlens, bias, key_padding_mask, bound)
     max_len = 0 if max_len is None else int(max_len)
     if T == 1:
-        if bias is not None and (bias.dtype != q.dtype or bias.stride(-1) != 1):
-            bias = bias.to(q.dtype).contiguous()
         # A step captured in a CUDA graph runs with the capacity as its host bound, far above most true lengths: each
         # (b, h) then spreads its own device length over the splits, not the bound (or most splits would be empty).
         return native().fmha_decode(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias, key_padding_mask,
                                     float(scale), split_by_length=torch.cuda.is_current_stream_capturing())
-    bound = C if seqlens is None else max_len + T
-    if bias is not None:
-        # the kernel reads the bias by TMA (rows of a multiple of 8 columns); the padding is -inf, so a bias narrower
-        # than the visible keys hides the keys past it, as the reference's clamp to its columns does
-        Lb = bias.shape[-1]
-        width = max(Lb, bound) + (-max(Lb, bound)) % 8
-        bias = bias.to(q.dtype).expand(bias.shape[0], q.shape[2], T, Lb)
-        if width != Lb:
-            bias = F.pad(bias, (0, width - Lb), value=float("-inf"))
-        bias = bias.contiguous()
-    if key_padding_mask is not None:
-        cols = key_padding_mask.shape[1]
-        if cols < bound:   # the same for a key mask narrower than the visible keys: the keys past it are masked
-            key_padding_mask = torch.cat([key_padding_mask, key_padding_mask.new_ones(q.shape[0], bound - cols)], 1)
-        key_padding_mask = key_padding_mask.contiguous()
     return native().kvcache.fmha_kvcache_fwd(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
                                              key_padding_mask, float(scale))
