@@ -54,8 +54,30 @@ struct FmhaFwdParams {
   // reads key / value head h / kv_group (the order of repeat_interleave(kv_group, dim=2)).  1 = one per query head.
   // Everything else - bias, key mask, keep bits, Philox counters, LSE, logits - stays per query head.
   int kv_group;
+  // Varlen mode (fmha_varlen_fwd / fmha_varlen_bwd; appended so that no earlier field moves): the B sequences are
+  // packed back to back.  q is [N, H, D], k / v [N, H_kv, D] (strided views with B = 1 in the TMA maps, L = N), and
+  // sequence b holds rows s_b .. s_b + n_b - 1 with s_b = clamp(cu_seqlens[b], 0, N) and
+  // n_b = clamp(cu_seqlens[b + 1] - cu_seqlens[b], 0, min(Lq, N - s_b)); Lq = Lk = max_seqlen.  O [N, H, D] (and dO) are
+  // packed too.  Everything per (b, h, row) keeps the padded layout of B sequences of Lq rows: LSE, keep bits, Philox
+  // counters, delta, the dQ accumulator and turn counters, the bias [1|B, H, Lq, Lk] (sequence b reads its top-left
+  // n_b x n_b block) and dS / dBias.  Query i of sequence b sees keys j < n_b (and j <= i when causal): the result at
+  // every row i < n_b is that of the padded call with key_padding_mask = (j >= n_b).  kpm must be null; no logits.
+  const int* cu_seqlens;   // [B + 1] int32 on the device
+  int varlen, packed_rows; // packed_rows = N
 };
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
+
+#ifdef __CUDACC__
+// Varlen mode: {s_b, n_b} of sequence b (L = max_seqlen, N = packed rows), clamped as documented above, so that no
+// value of cu_seqlens makes a kernel reach outside a tensor
+__device__ __forceinline__ int2 fmha_varlen_seq(const int* cu_seqlens, int b, int L, int N) {
+  const long long c0 = cu_seqlens[b], c1 = cu_seqlens[b + 1];
+  const long long s = c0 < 0 ? 0 : (c0 > N ? N : c0);
+  const long long cap = (long long)L < N - s ? (long long)L : N - s;
+  const long long n = c1 - c0;
+  return make_int2((int)s, (int)(n < 0 ? 0 : (n > cap ? cap : n)));
+}
+#endif
 
 // Copies the T new rows of k_new / v_new [B, T, H, D] into rows p_b + i of the [B, C, H, D] caches, p_b =
 // clamp(seqlens[b], 0, C), bitwise, with 16-byte vectors; rows at or past C are skipped.  H is the caches' head count

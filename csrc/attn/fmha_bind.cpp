@@ -390,6 +390,146 @@ Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   check_launch("fmha_kvcache_fwd");
   return out;
 }
+// ---- varlen: packed sequences described by cu_seqlens (fmha_api.h) ------------------------------------------------
+// q [N, H, D], k / v [N, H_kv, D] (head slices of one projection are fine), cu_seqlens int32 [B + 1] on the device,
+// max_seqlen a host bound on the lengths (a multiple of 8: the row stride of the bias, LSE, keep-bit and dS maps), bias
+// [1|B, H, max_seqlen, max_seqlen].  No key padding mask: the lengths take its place.  Returns B.
+int64_t check_varlen(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& cu_seqlens, int64_t max_seqlen,
+                     const OptTensor& bias) {
+  check_operand(q, "q", q.device(), k16Bit, any_shape(3), kAligned);
+  check_operand(k, "k", q.device(), {q.scalar_type()}, any_shape(3), kAligned);
+  check_operand(v, "v", q.device(), {q.scalar_type()}, any_shape(3), kAligned);
+  const int64_t N = q.size(0), H = q.size(1), D = q.size(2), H_kv = v.size(1);
+  TORCH_CHECK(ub::fmha_head_dim_supported(D) && k.size(2) == D && v.size(2) == D,
+              "head_dim must be the same for q/k/v and a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
+  TORCH_CHECK(N >= 1 && k.size(0) == N && v.size(0) == N && k.size(1) == H_kv,
+              "k / v must be [N, H_kv, D] with the N >= 1 packed rows and the D of q");
+  kv_group(H, H_kv, "v");
+  for (const Tensor* t : {&q, &k, &v}) {
+    TORCH_CHECK(t->stride(2) == 1 && t->stride(1) == D, "q/k/v head stride must be head_dim");
+    TORCH_CHECK(t->stride(0) % 8 == 0, "q/k/v row strides must be multiples of 8 elements");
+  }
+  check_operand(cu_seqlens, "cu_seqlens", q.device(), {at::kInt}, {kAnySize});
+  const int64_t B = cu_seqlens.size(0) - 1;
+  TORCH_CHECK(B >= 1, "cu_seqlens must have B + 1 >= 2 entries");
+  TORCH_CHECK(max_seqlen >= 1 && max_seqlen % 8 == 0, "max_seqlen must be a positive multiple of 8");
+  check_operand(bias, "bias", q.device(), {q.scalar_type()}, {kAnySize, H, max_seqlen, max_seqlen}, kVec);
+  TORCH_CHECK(!has(bias) || bias->size(0) == 1 || bias->size(0) == B, "bias must be [1|B, H, max_seqlen, max_seqlen]");
+  return B;
+}
+
+// The parameters of a varlen call: q / k / v maps over the N packed rows (B = 1), everything else at B x max_seqlen
+void fill_varlen(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& cu_seqlens,
+                 int64_t B, int64_t max_seqlen, const OptTensor& bias, double p_drop, double scale, bool causal,
+                 bool forward) {
+  fill_common(p, q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), std::nullopt, std::nullopt, p_drop, scale, forward);
+  p.B = (int)B;
+  p.Lq = p.Lk = (int)max_seqlen;
+  p.causal = causal ? 1 : 0;
+  p.varlen = 1;
+  p.cu_seqlens = cu_seqlens.data_ptr<int>();
+  p.packed_rows = (int)q.size(0);
+  if (has(bias)) {
+    p.bias = bias->data_ptr();
+    p.bias_batch = (int)bias->size(0);
+    TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_bias, p.bias, p.is_bf16 != 0, p.bias_batch * p.H, p.Lq, p.Lk),
+                "cuTensorMapEncodeTiled failed for the bias");
+  }
+}
+
+// (out [N, H, D], lse [B, H, max_seqlen], keep bits [B, H, max_seqlen, ceil(max_seqlen / 32)] or None); rows of LSE
+// and of the keep bits past each sequence's length are not written
+std::tuple<Tensor, Tensor, OptTensor> fmha_varlen_fwd(const Tensor& q, const Tensor& k, const Tensor& v,
+                                                      const Tensor& cu_seqlens, int64_t max_seqlen, const OptTensor& bias,
+                                                      double p_drop, double scale, bool causal) {
+  const int64_t B = check_varlen(q, k, v, cu_seqlens, max_seqlen, bias);
+  const c10::cuda::CUDAGuard guard(q.device());
+  ub::FmhaFwdParams p{};
+  fill_varlen(p, q, k, v, cu_seqlens, B, max_seqlen, bias, p_drop, scale, causal, /*forward=*/true);
+  Tensor out = torch::empty({q.size(0), p.H, p.D}, q.options());
+  Tensor lse = torch::empty({p.B, p.H, p.Lq}, q.options().dtype(at::kFloat));
+  p.out = out.data_ptr();
+  p.lse = lse.data_ptr<float>();
+  p.seed = p.offset = 0;
+  OptTensor bits;
+  if (p_drop > 0.0) {
+    std::tie(p.seed, p.offset) = philox_reserve(4);
+    bits = torch::empty({p.B, p.H, p.Lq, (p.Lk + 31) / 32}, q.options().dtype(at::kInt));
+    p.drop_bits = reinterpret_cast<uint32_t*>(bits->data_ptr());
+  }
+  ub::launch_fmha_fwd(p, cur_stream());
+  check_launch("fmha_varlen_fwd");
+  return {out, lse, bits};
+}
+
+// packed_grad: q / k / v are the head slices of one [N, H + 2 H_kv, D] projection, and the gradients are written into
+// one tensor of that layout (returned three times as views), as fmha_bwd does for [B, L, H + 2 H_kv, D].  dBias is 0
+// outside every sequence's block.
+std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_varlen_bwd(const Tensor& dout, const Tensor& q, const Tensor& k,
+                                                              const Tensor& v, const Tensor& out, const Tensor& lse,
+                                                              const Tensor& cu_seqlens, int64_t max_seqlen,
+                                                              const OptTensor& bias, double p_drop, double scale,
+                                                              const OptTensor& drop_bits, bool need_dbias,
+                                                              bool packed_grad, bool causal) {
+  const int64_t B = check_varlen(q, k, v, cu_seqlens, max_seqlen, bias);
+  const int64_t N = q.size(0), H = q.size(1), D = q.size(2), H_kv = k.size(1), L = max_seqlen;
+  check_operand(dout, "dout", q.device(), {q.scalar_type()}, q.sizes(), kVec);
+  check_operand(out, "out", q.device(), {q.scalar_type()}, q.sizes());
+  check_operand(lse, "lse", q.device(), {at::kFloat}, {B, H, L});
+  TORCH_CHECK(p_drop <= 0.0 || has(drop_bits), "dropout bits missing");
+  if (p_drop > 0.0) check_operand(drop_bits, "drop_bits", q.device(), {at::kInt}, {B, H, L, (L + 31) / 32});
+  const c10::cuda::CUDAGuard guard(q.device());
+  ub::FmhaBwdParams p{};
+  fill_varlen(p.f, q, k, v, cu_seqlens, B, max_seqlen, bias, p_drop, scale, causal, /*forward=*/false);
+  p.f.out = out.data_ptr();
+  p.f.lse = lse.data_ptr<float>();
+  if (p_drop > 0.0) p.f.drop_bits = reinterpret_cast<uint32_t*>(drop_bits->data_ptr());
+  p.dout = dout.data_ptr();
+  TORCH_CHECK(ub::make_head_tile_map_sw128(&p.sw_do, p.dout, p.f.is_bf16 != 0, 1, (int)N, (int)H, (int)D, N * H * D,
+                                           H * D, D, ub::kBwdBoxRows),
+              "cuTensorMapEncodeTiled failed for dO");
+  Tensor delta = torch::empty({B, H, L}, q.options().dtype(at::kFloat));
+  const bool det = at::globalContext().deterministicAlgorithms();
+  const int64_t n_qt = (L + 63) / 64;
+  const int64_t acc_floats = B * H * n_qt * 64 * ub::fmha_padded_head_dim((int)D);
+  Tensor dq_acc = torch::empty({acc_floats + (det ? B * H * n_qt : 0)}, q.options().dtype(at::kFloat));
+  p.dq_turn = det ? reinterpret_cast<int*>(dq_acc.data_ptr<float>() + acc_floats) : nullptr;
+  Tensor dq, dk, dv;
+  if (packed_grad) {
+    Tensor dqkv = torch::empty({N, H + 2 * H_kv, D}, q.options());
+    dq = dqkv.narrow(1, 0, H);
+    dk = dqkv.narrow(1, H, H_kv);
+    dv = dqkv.narrow(1, H + H_kv, H_kv);
+  } else {
+    dq = torch::empty({N, H, D}, q.options());
+    dk = torch::empty({N, H_kv, D}, q.options());
+    dv = torch::empty({N, H_kv, D}, q.options());
+  }
+  // the kernels address row r of sequence b as row s_b + r through the row stride; the batch stride is unused
+  p.dq_sb = p.dk_sb = p.dv_sb = 0;
+  p.dq_sl = dq.stride(0); p.dq_sh = dq.stride(1);
+  p.dk_sl = dk.stride(0); p.dk_sh = dk.stride(1);
+  p.dv_sl = dv.stride(0); p.dv_sh = dv.stride(1);
+  OptTensor dbias;
+  Tensor ds_buf;
+  if (need_dbias && p.f.bias != nullptr) {
+    // zeroed by the launcher: the kernels store the tiles inside each sequence's block only
+    ds_buf = torch::empty({B, H, L, L}, q.options());
+    p.ds_buf = ds_buf.data_ptr();
+    dbias = (p.f.bias_batch == B) ? ds_buf : torch::empty({p.f.bias_batch, H, L, L}, q.options());
+    p.dbias = dbias->data_ptr();
+    TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_ds, p.ds_buf, p.f.is_bf16 != 0, (int)(B * H), (int)L, (int)L),
+                "cuTensorMapEncodeTiled failed for the dS scratch tensor");
+  }
+  p.delta = delta.data_ptr<float>();
+  p.dq_acc = dq_acc.data_ptr<float>();
+  p.dq = dq.data_ptr();
+  p.dk = dk.data_ptr();
+  p.dv = dv.data_ptr();
+  ub::launch_fmha_bwd(p, cur_stream());
+  check_launch("fmha_varlen_bwd");
+  return {dq, dk, dv, dbias};
+}
 }  // namespace
 
 void register_fmha(pybind11::module_& m) {
@@ -409,6 +549,14 @@ void register_fmha(pybind11::module_& m) {
   kv.def("fmha_kvcache_fwd", &fmha_kvcache_fwd, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"),
          py::arg("seqlens"), py::arg("max_len"), py::arg("k_new"), py::arg("v_new"), py::arg("bias"),
          py::arg("key_padding_mask"), py::arg("scale"));
+  // packed variable-length sequences: its own submodule, _C.varlen
+  auto vl = m.def_submodule("varlen", "packed variable-length sequences described by cu_seqlens");
+  vl.def("fmha_varlen_fwd", &fmha_varlen_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("cu_seqlens"),
+         py::arg("max_seqlen"), py::arg("bias"), py::arg("p_drop"), py::arg("scale"), py::arg("causal") = false);
+  vl.def("fmha_varlen_bwd", &fmha_varlen_bwd, py::arg("dout"), py::arg("q"), py::arg("k"), py::arg("v"),
+         py::arg("out"), py::arg("lse"), py::arg("cu_seqlens"), py::arg("max_seqlen"), py::arg("bias"),
+         py::arg("p_drop"), py::arg("scale"), py::arg("drop_bits"), py::arg("need_dbias"), py::arg("packed_grad"),
+         py::arg("causal") = false);
   m.def("fmha_decode_max_splits", [] { return (int64_t)ub::kDecodeMaxSplits; });
   m.def("fmha_decode_num_splits", [](int64_t B, int64_t H, int64_t len_bound) {
     return (int64_t)ub::fmha_decode_num_splits((int)B, (int)H, (int)len_bound,

@@ -111,20 +111,33 @@ UB_DEVICE void det_wait_turn(const int* counter, int turn) {
 }
 
 // ---- pre-pass: delta[b,h,q] = sum_d dO * O -----------------------------------------------------------------
-template <typename T>
+// kVarlen: rows (b, q, h) of the padded enumeration read packed row s_b + q, and rows q >= n_b get delta = 0
+template <typename T, bool kVarlen = false>
 __global__ void __launch_bounds__(256) fmha_delta_kernel(const T* __restrict__ dout, const T* __restrict__ out,
-                                                           float* __restrict__ delta, int B, int H, int Lq, int D) {
+                                                           float* __restrict__ delta, int B, int H, int Lq, int D,
+                                                           const int* __restrict__ cu_seqlens, int N) {
   // 8 threads per (b, q, h) row of D elements; thread `part` sums the 8-element chunks part, part + 8
   const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long rowi = gid >> 3;
   const int part = (int)(gid & 7);
   const long long nrows = (long long)B * Lq * H;
   float acc = 0.f;
-  if (rowi < nrows) {
+  long long src = rowi;   // the [rows, D] row of dO and O
+  bool live = rowi < nrows;
+  if constexpr (kVarlen) {
+    if (live) {
+      const long long bq = rowi / H;
+      const int2 sn = fmha_varlen_seq(cu_seqlens, (int)(bq / Lq), Lq, N);
+      const int q = (int)(bq % Lq);
+      live = q < sn.y;
+      src = ((long long)sn.x + q) * H + rowi % H;
+    }
+  }
+  if (live) {
     for (int ch = part; ch < D / 8; ch += 8) {
       float a[8], o[8];
-      unpack<T>(ld_global_nc_v4(dout + rowi * D + ch * 8), a);
-      unpack<T>(ld_global_nc_v4(out + rowi * D + ch * 8), o);
+      unpack<T>(ld_global_nc_v4(dout + src * D + ch * 8), a);
+      unpack<T>(ld_global_nc_v4(out + src * D + ch * 8), o);
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc += a[e] * o[e];
     }
@@ -141,10 +154,12 @@ __global__ void __launch_bounds__(256) fmha_delta_kernel(const T* __restrict__ d
 }
 
 // ---- post-pass: dq = scale * fp32 accumulator, written through (batch, seq, head) strides -------------------------
-template <typename T>
+// kVarlen: row (b, h, q) goes to packed row s_b + q (sb unused); rows q >= n_b are not stored
+template <typename T, bool kVarlen = false>
 __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __restrict__ acc, T* __restrict__ out, int H,
                                                                 int Lq, int Lq_pad, int D, int DP, long long nvec, float scale,
-                                                                long long sb, long long sl, long long sh) {
+                                                                long long sb, long long sl, long long sh,
+                                                                const int* __restrict__ cu_seqlens, int N) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   const int groups = D / 8;   // the accumulator rows are DP wide; columns D..DP-1 are not stored
   for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < nvec; v += stride) {
@@ -155,11 +170,17 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
     const long long bh = row / Lq;
     const int h = (int)(bh % H);
     const long long b = bh / H;
+    long long dst_row = b * sb + (long long)q * sl;
+    if constexpr (kVarlen) {
+      const int2 sn = fmha_varlen_seq(cu_seqlens, (int)b, Lq, N);
+      if (q >= sn.y) continue;
+      dst_row = ((long long)sn.x + q) * sl;
+    }
     const float4* src = reinterpret_cast<const float4*>(acc + ((bh * Lq_pad + q) * DP + dq_swz_col(q, part * 8)));
     const float4 x0 = src[0], x1 = src[1];
     const float x[8] = {x0.x * scale, x0.y * scale, x0.z * scale, x0.w * scale,
                         x1.x * scale, x1.y * scale, x1.z * scale, x1.w * scale};
-    st_global_v4(out + b * sb + (long long)q * sl + (long long)h * sh + part * 8, pack<T>(x));
+    st_global_v4(out + dst_row + (long long)h * sh + part * 8, pack<T>(x));
   }
 }
 
@@ -189,9 +210,17 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
 // finishes its whole sequence, so every turn this CTA waits for arrives.  The wait is at the last point, with the dQ
 // tile already staged, so a CTA does not hold up the chain while it computes.  dK, dV and dS are computed exactly as
 // in the default mode.
-template <typename T, int DP, bool kLogits, bool kCausal, bool kDet = false>
+// kVarlen: packed sequences (fmha_api.h).  Key tile j of sequence b exists iff key0 < n_b (the others exit at once), and
+// it walks the query tiles below n_b only, so the turn chain of a query tile is the key tiles 0 .. below n_b, with no
+// gap.  Rows at or past n_b (rows of the next sequence) and keys at or past n_b get P = 0 and dS = 0 by selection, and
+// only keys below n_b store dK / dV.  The padded call with key_padding_mask = (j >= n_b) and dO = 0 at the pad rows
+// adds exact zeros for everything skipped, so dK and dV are bitwise its results, and dQ / dS too in deterministic mode.
+// The dS tiles no CTA stores are zeroed by the launcher (a memset of ds_buf), so dBias is exactly 0 outside every
+// sequence's n_b x n_b block.
+template <typename T, int DP, bool kLogits, bool kCausal, bool kDet = false, bool kVarlen = false>
 __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
+  static_assert(!(kLogits && kVarlen), "the varlen mode has no logits");
   using C = BwdCfg<DP, kLogits>;
   constexpr uint32_t kOffK = C::kOffK, kOffV = C::kOffV, kOffQ = C::kOffQ, kOffDO = C::kOffDO, kOffDS = C::kOffDS,
                      kOffDQ = C::kOffDQ, kOffStats = C::kOffStats, kOffBar = C::kOffBar, kTile = C::kTile;
@@ -203,17 +232,26 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, c = lane & 3;
   const int key0 = blockIdx.x * kBN, hk = blockIdx.y, b = blockIdx.z;
+  int vl_s = 0, vl_n = 0;   // varlen: the sequence's first packed row and its length
+  if constexpr (kVarlen) {
+    const int2 sn = fmha_varlen_seq(p.cu_seqlens, b, p.Lq, p.packed_rows);
+    vl_s = sn.x;
+    vl_n = sn.y;
+    if (key0 >= vl_n) return;
+  }
+  const int tb = kVarlen ? 0 : b;   // batch coordinate of the q / k / v / dO maps
   const uint32_t bar_kv = smem_base + kOffBar, bar_in0 = smem_base + kOffBar + 8;   // + 8 * stage
   const bool has_bias = p.bias != nullptr;
   const bool drop = p.p_drop > 0.f && p.drop_bits != nullptr;
   const int n_qtiles = (p.Lq + kBM - 1) / kBM;
   const int Lq_pad = n_qtiles * kBM;
-  // first query tile: causal CTAs skip the tiles whose queries all precede key0 (i0 == n_qtiles: none is left)
-  const int i0 = kCausal ? min(key0 / kBM, n_qtiles) : 0;
+  const int n_qwalk = kVarlen ? (vl_n + kBM - 1) / kBM : n_qtiles;   // query tiles walked
+  // first query tile: causal CTAs skip the tiles whose queries all precede key0 (i0 == n_qwalk: none is left)
+  const int i0 = kCausal ? min(key0 / kBM, n_qwalk) : 0;
   // the group's query heads h0 .. h0 + G - 1 one after the other, each over its query tiles i0 .. n_qtiles - 1: step
   // t = (h - h0) * (n_qtiles - i0) + (i - i0) of one flat sequence, whose index counts the stages and phase parities
   const int h0 = hk * p.kv_group;
-  const int n_steps = p.kv_group * (n_qtiles - i0);
+  const int n_steps = p.kv_group * (n_qwalk - i0);
   const int words_per_row = (p.Lk + 31) / 32;
   // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
   auto load_tile = [&](int h, int i, int t) {   // one thread: Q_i, dO_i (and the bias and dz tiles) of head h
@@ -222,8 +260,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     mbar_expect_tx(bar, 2 * kTile + (has_bias ? 8192u : 0u) + (kLogits ? 8192u : 0u));
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
-      tma_load_4d(smem_base + kOffQ + st * kTile + x * 8192, &p.sw_q, 64 * x, h, i * kBM, b, bar);
-      tma_load_4d(smem_base + kOffDO + st * kTile + x * 8192, &bp.sw_do, 64 * x, h, i * kBM, b, bar);
+      tma_load_4d(smem_base + kOffQ + st * kTile + x * 8192, &p.sw_q, 64 * x, h, vl_s + i * kBM, tb, bar);
+      tma_load_4d(smem_base + kOffDO + st * kTile + x * 8192, &bp.sw_do, 64 * x, h, vl_s + i * kBM, tb, bar);
     }
     if (has_bias) tma_load_3d(smem_base + kOffDS + st * 8192, &p.sw_bias, key0, i * kBM, bias_nb, bar);
     if constexpr (kLogits) tma_load_3d(smem_base + C::kOffDZ + st * 8192, &bp.sw_dz, key0, i * kBM, bh, bar);
@@ -235,7 +273,7 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     uint8_t* s = smem + kOffStats + (t & 1) * 1024;
     const long long bh = (long long)b * p.H + h;
     const int q = i * kBM + (tid & 63);
-    const bool ok = q < p.Lq;
+    const bool ok = q < (kVarlen ? vl_n : p.Lq);
     if (tid < 64) {
       const float lse = ok ? p.lse[bh * p.Lq + q] : -CUDART_INF_F;
       reinterpret_cast<float*>(s)[tid] = lse == -CUDART_INF_F ? CUDART_INF_F : lse * 1.4426950408889634f;
@@ -245,11 +283,11 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     if (drop) {   // bits[w][q]: word w of the tile's two for query q, so that queries q, q + 1 are one 8-byte load
       const int qb = i * kBM + (tid >> 1), wi = (key0 >> 5) + (tid & 1);
       reinterpret_cast<uint32_t*>(s + 512)[(tid & 1) * 64 + (tid >> 1)] =
-          (qb < p.Lq && wi < words_per_row) ? p.drop_bits[(bh * p.Lq + qb) * words_per_row + wi] : 0xffffffffu;
+          (qb < (kVarlen ? vl_n : p.Lq) && wi < words_per_row) ? p.drop_bits[(bh * p.Lq + qb) * words_per_row + wi] : 0xffffffffu;
     }
   };
 
-  const bool any_q = !kCausal || i0 < n_qtiles;   // a copy must not outlive the CTA: no query tile, no load
+  const bool any_q = !kCausal || i0 < n_qwalk;   // a copy must not outlive the CTA: no query tile, no load
   if (tid == 0) {
     mbar_init(bar_kv, 1);
     mbar_init(bar_in0, 1);
@@ -259,8 +297,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
       mbar_expect_tx(bar_kv, 2 * kTile);
 #pragma unroll
       for (int x = 0; x < C::kBoxes; ++x) {
-        tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, hk, key0, b, bar_kv);
-        tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, hk, key0, b, bar_kv);
+        tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, hk, vl_s + key0, tb, bar_kv);
+        tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, hk, vl_s + key0, tb, bar_kv);
       }
       load_tile(h0, i0, 0);
     }
@@ -269,7 +307,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   // causal, per-batch dBias: the skipped tiles (i < i0, every key above every query) are zero.  The first 8 KB of the
   // dQ staging tile are zeroed and stored over each of them, for each query head of the group; the first dQ tile is written after the bulk_wait_read of
   // the loop's first barrier (A), when the stores have read it.
-  const bool zero_ds = kCausal && i0 > 0 && bp.ds_buf != nullptr && bp.ds_buf == bp.dbias;
+  // (varlen: the launcher has zeroed ds_buf)
+  const bool zero_ds = kCausal && !kVarlen && i0 > 0 && bp.ds_buf != nullptr && bp.ds_buf == bp.dbias;
   if (zero_ds) {
     uint4* zt = reinterpret_cast<uint4*>(smem + kOffDQ);
 #pragma unroll
@@ -280,8 +319,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   // my two keys (accumulator rows) and their additive masks
   const int kl0 = warp * 16 + g, kl1 = kl0 + 8;
   const int kr0 = key0 + kl0, kr1 = key0 + kl1;
-  const float kadd0 = (kr0 >= p.Lk || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr0] != 0)) ? -CUDART_INF_F : 0.f;
-  const float kadd1 = (kr1 >= p.Lk || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr1] != 0)) ? -CUDART_INF_F : 0.f;
+  const float kadd0 = (kr0 >= (kVarlen ? vl_n : p.Lk) || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr0] != 0)) ? -CUDART_INF_F : 0.f;
+  const float kadd1 = (kr1 >= (kVarlen ? vl_n : p.Lk) || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr1] != 0)) ? -CUDART_INF_F : 0.f;
   // keep-bit positions of my keys inside their 32-key word (word (warp >> 1) of the tile's two)
   const int kk0 = 16 * (warp & 1) + g, kk1 = kk0 + 8;
   const int bit0 = (kk0 & 1) * 16 + (kk0 >> 1), bit1 = (kk1 & 1) * 16 + (kk1 >> 1);
@@ -312,7 +351,7 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     const uint32_t st = (uint32_t)(t & 1);
     const long long bh = (long long)b * p.H + h;
     int h_next = h, i_next = i + 1;   // step t + 1
-    if (i_next == n_qtiles) {
+    if (i_next == n_qwalk) {
       i_next = i0;
       ++h_next;
     }
@@ -373,6 +412,11 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
         const float x0 = fmaf(s[e], p.scale, bb.x + ka0), x1 = fmaf(s[e + 1], p.scale, bb.y + ka1);
         s[e] = ex2_approx(fmaf(x0, kLog2e, -l2.x));
         s[e + 1] = ex2_approx(fmaf(x1, kLog2e, -l2.y));
+        if constexpr (kVarlen) {   // rows and keys of the next sequence: selected, whatever their bias or data hold
+          const int q = i * kBM + ql, kl = (r & 1) ? kl1 : kl0;
+          if (key0 + kl >= vl_n || q >= vl_n) s[e] = 0.f;
+          if (key0 + kl >= vl_n || q + 1 >= vl_n) s[e + 1] = 0.f;
+        }
       }
     }
 
@@ -402,6 +446,10 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
         const float p0 = s[e], p1 = s[e + 1];
         float ds0 = p0 * (dp[e] * (k0 ? keep_scale : 0.f) - dl.x);
         float ds1 = p1 * (dp[e + 1] * (k1 ? keep_scale : 0.f) - dl.y);
+        if constexpr (kVarlen) {   // P = 0 there; dP of the next sequence's dO may not be finite
+          if (p0 == 0.f) ds0 = 0.f;
+          if (p1 == 0.f) ds1 = 0.f;
+        }
         if constexpr (kLogits) {
           const float2 dz = unpack2<T>(dz_r[r]);
           ds0 += dz.x;
@@ -484,9 +532,11 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
     const int key = half ? kr1 : kr0;
-    if (key >= p.Lk) continue;
-    T* dvg = reinterpret_cast<T*>(bp.dv) + (long long)b * bp.dv_sb + (long long)key * bp.dv_sl + (long long)hk * bp.dv_sh;
-    T* dkg = reinterpret_cast<T*>(bp.dk) + (long long)b * bp.dk_sb + (long long)key * bp.dk_sl + (long long)hk * bp.dk_sh;
+    if (key >= (kVarlen ? vl_n : p.Lk)) continue;
+    // padded: (b, key); varlen: packed row s_b + key
+    const long long row = kVarlen ? (long long)vl_s + key : (long long)key;
+    T* dvg = reinterpret_cast<T*>(bp.dv) + (long long)tb * bp.dv_sb + row * bp.dv_sl + (long long)hk * bp.dv_sh;
+    T* dkg = reinterpret_cast<T*>(bp.dk) + (long long)tb * bp.dk_sb + row * bp.dk_sl + (long long)hk * bp.dk_sh;
 #pragma unroll
     for (int n = 0; n < DP / 8; ++n) {
       if (8 * n >= p.D) continue;   // columns 8n + 2c, +1 exist iff 8n < D (D % 8 == 0)
@@ -539,15 +589,26 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
   const int n_qt = (p.Lq + kBM - 1) / kBM;
   const bool det = bp.dq_turn != nullptr;   // the turn counters follow dq_acc: one memset zeroes both
   cudaMemsetAsync(bp.dq_acc, 0, (size_t)p.B * p.H * n_qt * (kBM * DP * sizeof(float) + (det ? sizeof(int) : 0)), stream);
-  fmha_delta_kernel<T><<<(unsigned)((nrows * 8 + 255) / 256), 256, 0, stream>>>(
-      reinterpret_cast<const T*>(bp.dout), reinterpret_cast<const T*>(p.out), bp.delta, p.B, p.H, p.Lq, p.D);
+  const bool varlen = p.varlen != 0;
+  // varlen: the dS tiles outside each sequence's block are never stored; zeroed here, they give dBias = 0 there
+  if (varlen && bp.ds_buf != nullptr)
+    cudaMemsetAsync(bp.ds_buf, 0, (size_t)p.B * p.H * p.Lq * p.Lk * sizeof(T), stream);
+  const unsigned delta_grid = (unsigned)((nrows * 8 + 255) / 256);
+  (varlen ? fmha_delta_kernel<T, true> : fmha_delta_kernel<T, false>)<<<delta_grid, 256, 0, stream>>>(
+      reinterpret_cast<const T*>(bp.dout), reinterpret_cast<const T*>(p.out), bp.delta, p.B, p.H, p.Lq, p.D, p.cu_seqlens, p.packed_rows);
   dim3 grid((p.Lk + kBN - 1) / kBN, p.H / p.kv_group, p.B);
   auto run = [&](auto kern, uint32_t smem_bytes) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
     kern<<<grid, kBwdThreads, smem_bytes, stream>>>(bp);
   };
-  // causal + logits is refused by the binding (fmha_bind.cpp)
-  if (det) {
+  // causal + logits is refused by the binding (fmha_bind.cpp); the varlen bindings have no logits
+  if (varlen) {
+    if (det) {
+      if (p.causal) run(fmha_bwd_kernel<T, DP, false, true, true, true>, BwdCfg<DP, false>::kSmemBytes);
+      else run(fmha_bwd_kernel<T, DP, false, false, true, true>, BwdCfg<DP, false>::kSmemBytes);
+    } else if (p.causal) run(fmha_bwd_kernel<T, DP, false, true, false, true>, BwdCfg<DP, false>::kSmemBytes);
+    else run(fmha_bwd_kernel<T, DP, false, false, false, true>, BwdCfg<DP, false>::kSmemBytes);
+  } else if (det) {
     if (bp.dlogits != nullptr) run(fmha_bwd_kernel<T, DP, true, false, true>, BwdCfg<DP, true>::kSmemBytes);
     else if (p.causal) run(fmha_bwd_kernel<T, DP, false, true, true>, BwdCfg<DP, false>::kSmemBytes);
     else run(fmha_bwd_kernel<T, DP, false, false, true>, BwdCfg<DP, false>::kSmemBytes);
@@ -561,9 +622,10 @@ void run_bwd(const FmhaBwdParams& bp, cudaStream_t stream) {
                                                             reinterpret_cast<T*>(bp.dbias), p.B, nv, p.Lq, p.Lk);
   }
   const long long nvec = nrows * (p.D / 8);
-  fmha_dq_convert_kernel<T><<<sweep_plan(nvec, 256, 16).grid, 256, 0, stream>>>(
+  (varlen ? fmha_dq_convert_kernel<T, true> : fmha_dq_convert_kernel<T, false>)<<<sweep_plan(nvec, 256, 16).grid, 256, 0,
+                                                                                  stream>>>(
       bp.dq_acc, reinterpret_cast<T*>(bp.dq), p.H, p.Lq, n_qt * kBM, p.D, DP, nvec, p.scale, bp.dq_sb, bp.dq_sl,
-      bp.dq_sh);
+      bp.dq_sh, p.cu_seqlens, p.packed_rows);
 }
 
 }  // namespace

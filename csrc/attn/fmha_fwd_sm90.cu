@@ -98,10 +98,17 @@ UB_DEVICE void quad_transpose4(uint32_t (&w)[4], int c) {
 // may span two) sets the invisible elements to -inf by index.  Cache rows at or past n_b lie inside the tensor, so TMA
 // loads them and they may hold anything, NaN included: their scores are replaced (never added to), and their V rows
 // are zeroed in shared memory before P V (0 x NaN is NaN).  Only the last tile walked can hold such rows.  No dropout.
-template <typename T, int DP, bool kLogits, bool kCausal, bool kKVCache>
+// kVarlen: packed sequences (fmha_api.h).  The CTA of (query tile, h, b) reads rows s_b + q0 .. of the packed q / k / v
+// through B = 1 maps and exits when q0 >= n_b.  Its tile loop (and the prefetch) stops at the tile holding key n_b - 1;
+// the padded call would walk the later tiles as wholly masked ones, which add exact zeros (see kCausal), so O, LSE and
+// the keep words at rows below n_b are bitwise those of that call.  In the last tile the keys at or past n_b (rows of
+// the next sequence, or TMA zero fill past N) get -inf by assignment and their V rows are zeroed, as in the KV-cache
+// mode.  Only rows below n_b are stored.  Causal composes (its diagonal is per sequence); logits mode does not.
+template <typename T, int DP, bool kLogits, bool kCausal, bool kKVCache, bool kVarlen = false>
 __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
   static_assert(!(kKVCache && (kLogits || kCausal)), "the KV-cache mode is neither causal nor logits mode");
+  static_assert(!(kVarlen && (kLogits || kKVCache)), "the varlen mode is neither logits nor KV-cache mode");
   using C = FwdCfg<DP>;
   constexpr int kBlockN = C::kBlockN;
   constexpr int kWords = kBlockN / 32;   // keep-bit words per row of a key tile
@@ -114,6 +121,16 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   const int q_tile = (kCausal || kKVCache) ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
   const int q0 = q_tile * kBlockM, h = blockIdx.y, b = blockIdx.z;
   const int hk = h / p.kv_group;   // key / value head of query head h (fmha_api.h)
+  // varlen: the sequence's first packed row and length; its rows are addressed as batch 0 of the B = 1 maps
+  int vl_s = 0, vl_n = 0;
+  if constexpr (kVarlen) {
+    const int2 sn = fmha_varlen_seq(p.cu_seqlens, b, p.Lq, p.packed_rows);
+    vl_s = sn.x;
+    vl_n = sn.y;
+    if (q0 >= vl_n) return;
+  }
+  const int tb = kVarlen ? 0 : b;   // batch coordinate of the q / k / v maps
+  const int row_lim = kVarlen ? vl_n : p.Lq;   // rows stored
   const uint32_t bar0 = smem_base + C::kSmemBar;   // bar0 + 8 * stage: K / V / bias of a key tile (+ Q on the first)
   float* kadd = reinterpret_cast<float*>(smem + C::kSmemKAdd);
 
@@ -127,9 +144,10 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     kv_lim = min(kv_n, kv_p + q0 + 1);
   }
   // causal: key tiles 0 .. (q0 + 63) / kBlockN hold a key visible to one of the rows q0 .. q0 + 63
-  const int n_tiles = kCausal ? min(n_key_tiles, (q0 + kBlockM - 1) / kBlockN + 1)
+  const int n_key_walk = kVarlen ? (vl_n + kBlockN - 1) / kBlockN : n_key_tiles;
+  const int n_tiles = kCausal ? min(n_key_walk, (q0 + kBlockM - 1) / kBlockN + 1)
                       : kKVCache ? max(1, (min(kv_n, kv_p + q0 + kBlockM) + kBlockN - 1) / kBlockN)
-                                 : n_key_tiles;
+                                 : n_key_walk;
   const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
   // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
   constexpr uint32_t kKVBytes = C::kKVStage, kBiasBytes = C::kBiasStage, kQBytes = C::kBoxes * C::kQBox;
@@ -138,9 +156,11 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     mbar_expect_tx(bar, 2 * kKVBytes + (has_bias ? kBiasBytes : 0u) + (j == 0 ? kQBytes : 0u));
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
-      if (j == 0) tma_load_4d(smem_base + C::kSmemQ + x * C::kQBox, &p.sw_q, 64 * x, h, q0, b, bar);
-      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, j * kBlockN, b, bar);
-      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, j * kBlockN, b, bar);
+      if (j == 0) tma_load_4d(smem_base + C::kSmemQ + x * C::kQBox, &p.sw_q, 64 * x, h, vl_s + q0, tb, bar);
+      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, vl_s + j * kBlockN, tb,
+                  bar);
+      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, vl_s + j * kBlockN, tb,
+                  bar);
     }
     if (has_bias) {   // 64 rows x kBlockN keys = kBlockN / 64 boxes of 64 keys
 #pragma unroll
@@ -165,7 +185,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   // the 1/(1-p) of the kept probabilities is applied once, to the normalised output row
   const float keep_scale = drop ? dropout_keep_scale14(t14) : 1.f;
   const unsigned long long bh = (unsigned long long)b * p.H + h;
-  const unsigned long long lin0 = bh * p.Lq + (row0 < p.Lq ? row0 : 0), lin1 = bh * p.Lq + (row1 < p.Lq ? row1 : 0);
+  const unsigned long long lin0 = bh * p.Lq + (row0 < row_lim ? row0 : 0), lin1 = bh * p.Lq + (row1 < row_lim ? row1 : 0);
   const int words_per_row = (p.Lk + 31) / 32;
   // Philox counter of element (lin, key) is (lin * Lk + key) >> 3, one call per (row, 8 keys).  For each pair of 8-key
   // groups (i, i + 1) the quad needs four calls - rows rl0 / rl1 x groups i / i + 1 - and thread c computes call c:
@@ -186,7 +206,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     if (tid < kBlockN) {
       const int key = key0 + tid;
       // KV-cache mode: kpm_cols >= kv_cap >= kv_n, so the key mask is read only below kv_n
-      masked = key >= (kKVCache ? kv_n : p.Lk) || (kpm_row != nullptr && kpm_row[key] != 0);
+      masked = key >= (kKVCache ? kv_n : kVarlen ? vl_n : p.Lk) || (kpm_row != nullptr && kpm_row[key] != 0);
       kadd[st * kBlockN + tid] = masked ? -CUDART_INF_F : 0.f;
     }
     // barrier: every thread is done with tile j-1, so its stage may be refilled with tile j+1
@@ -194,9 +214,10 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     if (kLogits && tid == 0) bulk_wait_read();   // the logits store of tile j-1 has read the stage tile j+1 fills
     if (tid == 0 && j + 1 < n_tiles) load_tile(j + 1);
     mbar_wait(bar0 + 8u * st, (uint32_t)((j >> 1) & 1));
-    if constexpr (kKVCache) {
-      if (key0 + kBlockN > kv_n) {   // zero the V rows at or past n_b: whole 128-byte rows of every column box
-        const int r0 = max(kv_n - key0, 0), chunks = (kBlockN - r0) * 8;
+    if constexpr (kKVCache || kVarlen) {
+      const int v_lim = kKVCache ? kv_n : vl_n;
+      if (key0 + kBlockN > v_lim) {   // zero the V rows at or past n_b: whole 128-byte rows of every column box
+        const int r0 = max(v_lim - key0, 0), chunks = (kBlockN - r0) * 8;
         uint8_t* sv = smem + C::kSmemV + st * C::kKVStage;
         for (int x = tid; x < C::kBoxes * chunks; x += kFwdThreads) {
           const int box = x / chunks, r = r0 + (x % chunks) / 8;
@@ -258,6 +279,13 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
           if (key + 1 >= lim0) s[4 * i + 1] = -CUDART_INF_F;
           if (key >= lim1) s[4 * i + 2] = -CUDART_INF_F;
           if (key + 1 >= lim1) s[4 * i + 3] = -CUDART_INF_F;
+        }
+      }
+      if constexpr (kVarlen) {   // the last tile: keys of the next sequence, assigned (their bias is not this one's)
+        if (key0 + kBlockN > vl_n) {
+          const int key = key0 + col;
+          if (key >= vl_n) s[4 * i + 0] = s[4 * i + 2] = -CUDART_INF_F;
+          if (key + 1 >= vl_n) s[4 * i + 1] = s[4 * i + 3] = -CUDART_INF_F;
         }
       }
       if constexpr (kLogits) {   // the same swizzled positions as the bias elements above
@@ -342,8 +370,8 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
       }
       if (c < kWords && key0 + 32 * c < p.Lk) {
         const int wi = (key0 >> 5) + c;
-        if (row0 < p.Lq) p.drop_bits[lin0 * words_per_row + wi] = w0;
-        if (row1 < p.Lq) p.drop_bits[lin1 * words_per_row + wi] = w1;
+        if (row0 < row_lim) p.drop_bits[lin0 * words_per_row + wi] = w0;
+        if (row1 < row_lim) p.drop_bits[lin1 * words_per_row + wi] = w1;
       }
     }
 
@@ -379,16 +407,18 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   const float inv0 = l0 > 0.f ? keep_scale / l0 : 0.f, inv1 = l1 > 0.f ? keep_scale / l1 : 0.f;
   T* out = reinterpret_cast<T*>(p.out);
   const int D = p.D;   // columns 8i + 2c, +1 exist iff 8i < D (D % 8 == 0)
-  if (row0 < p.Lq) {
-    uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row0) * p.H + h) * D + 2 * c);
+  // padded: row (b, i) of [B, Lq, H, D]; varlen: packed row s_b + i of [N, H, D]
+  const long long orow0 = kVarlen ? (long long)vl_s : (long long)b * p.Lq;
+  if (row0 < row_lim) {
+    uint32_t* og = reinterpret_cast<uint32_t*>(out + ((orow0 + row0) * p.H + h) * D + 2 * c);
 #pragma unroll
     for (int i = 0; i < DP / 8; ++i)
       if (8 * i < D) og[4 * i] = pack2<T>(o[4 * i + 0] * inv0, o[4 * i + 1] * inv0);
     if (c == 0 && (!kKVCache || p.lse != nullptr))
       p.lse[lin0] = l0 > 0.f ? m0 + __logf(l0) : -CUDART_INF_F;   // natural-log LSE of the logits
   }
-  if (row1 < p.Lq) {
-    uint32_t* og = reinterpret_cast<uint32_t*>(out + (((long long)b * p.Lq + row1) * p.H + h) * D + 2 * c);
+  if (row1 < row_lim) {
+    uint32_t* og = reinterpret_cast<uint32_t*>(out + ((orow0 + row1) * p.H + h) * D + 2 * c);
 #pragma unroll
     for (int i = 0; i < DP / 8; ++i)
       if (8 * i < D) og[4 * i] = pack2<T>(o[4 * i + 2] * inv1, o[4 * i + 3] * inv1);
@@ -407,23 +437,28 @@ void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
     kern<<<grid, kFwdThreads, smem_bytes, stream>>>(p);
   };
-  auto dispatch = [&](auto logits, auto causal, auto kvcache) {
+  auto dispatch = [&](auto logits, auto causal, auto kvcache, auto varlen) {
     constexpr bool kLogits = decltype(logits)::value, kCausal = decltype(causal)::value;
-    constexpr bool kKV = decltype(kvcache)::value;
+    constexpr bool kKV = decltype(kvcache)::value, kVL = decltype(varlen)::value;
     if (p.D <= 64) {
-      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits, kCausal, kKV>, FwdCfg<64>::kSmemBytes);
-      else run(fmha_fwd_kernel<__half, 64, kLogits, kCausal, kKV>, FwdCfg<64>::kSmemBytes);
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits, kCausal, kKV, kVL>, FwdCfg<64>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 64, kLogits, kCausal, kKV, kVL>, FwdCfg<64>::kSmemBytes);
     } else {
-      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits, kCausal, kKV>, FwdCfg<128>::kSmemBytes);
-      else run(fmha_fwd_kernel<__half, 128, kLogits, kCausal, kKV>, FwdCfg<128>::kSmemBytes);
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits, kCausal, kKV, kVL>, FwdCfg<128>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 128, kLogits, kCausal, kKV, kVL>, FwdCfg<128>::kSmemBytes);
     }
   };
-  // causal + logits is refused by the binding (fmha_bind.cpp); the KV-cache mode sets neither
+  // causal + logits is refused by the binding (fmha_bind.cpp); the KV-cache mode sets neither, and the varlen
+  // bindings never set logits
   const std::false_type no;
-  if (p.kvcache) dispatch(no, no, std::true_type{});
-  else if (p.logits != nullptr) dispatch(std::true_type{}, no, no);
-  else if (p.causal) dispatch(no, std::true_type{}, no);
-  else dispatch(no, no, no);
+  const std::true_type yes;
+  if (p.varlen) {
+    if (p.causal) dispatch(no, yes, no, yes);
+    else dispatch(no, no, no, yes);
+  } else if (p.kvcache) dispatch(no, no, yes, no);
+  else if (p.logits != nullptr) dispatch(yes, no, no, no);
+  else if (p.causal) dispatch(no, yes, no, no);
+  else dispatch(no, no, no, no);
 }
 
 }  // namespace ub

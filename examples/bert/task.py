@@ -9,6 +9,11 @@ The pipeline is a chain of lazy dataset views, each adding one thing:
     records -> WordPiece ids (truncated to --max-seq-len) -> (masked input, targets at the masked positions)
             -> right-padded batches {"net_input": {"src_tokens"}, "target"} -> one fixed random order
 
+``--pack-sequences`` collates the same sentences back to back instead of right-padding them: ``src_tokens`` and
+``target`` are ``[N]`` (N the real tokens of the batch), and ``net_input`` also holds ``cu_seqlens`` and
+``max_seqlen`` (``PackedSequenceDataset``), so that no kernel of the model runs on pad rows.  The model follows the
+form of the batch it is given; checkpoints are the same either way.
+
 Masking follows BERT: ``--mask-prob`` of the positions are selected; of those ``--random-token-prob`` become a random
 token, ``--leave-unmasked-prob`` stay as they are, the rest become ``[MASK]``; the draw is a function of (seed, epoch,
 index), i.e. reproducible and different every epoch.
@@ -38,6 +43,8 @@ class BertTask(UnicoreTask):
                              help="probability that a masked token is unmasked")
         masking.add_argument("--random-token-prob", type=float, default=0.1,
                              help="probability of replacing a token with a random token")
+        parser.add_argument("--pack-sequences", action="store_true", default=False,
+                            help="batch the sentences back to back with cu_seqlens instead of right-padding them")
 
     @classmethod
     def setup_task(cls, args, **kwargs):
@@ -64,10 +71,13 @@ class BertTask(UnicoreTask):
             mask_prob=a.mask_prob, leave_unmasked_prob=a.leave_unmasked_prob, random_token_prob=a.random_token_prob,
         )
 
-        def padded(ds):
-            return D.RightPadDataset(ds, pad_idx=vocab.pad())
-
-        batch_layout = D.NestedDictionaryDataset({"net_input": {"src_tokens": padded(noisy)}, "target": padded(targets)})
+        if getattr(a, "pack_sequences", False):
+            layout = {"net_input": D.PackedSequenceDataset(noisy, tokens_key="src_tokens"),
+                      "target": D.PackedSequenceDataset(targets)}
+        else:
+            layout = {"net_input": {"src_tokens": D.RightPadDataset(noisy, pad_idx=vocab.pad())},
+                      "target": D.RightPadDataset(targets, pad_idx=vocab.pad())}
+        batch_layout = D.NestedDictionaryDataset(layout)
         with D.data_utils.numpy_seed(a.seed):
             fixed_order = np.random.permutation(len(noisy))
         self.datasets[split] = D.SortDataset(batch_layout, sort_order=[fixed_order])

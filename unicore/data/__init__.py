@@ -31,6 +31,7 @@ from .wrappers import (
     NestedDictionaryDataset,
     NumelDataset,
     NumSamplesDataset,
+    PackedSequenceDataset,
     PadDataset,
     PrependTokenDataset,
     RawArrayDataset,
@@ -46,7 +47,7 @@ __all__ = [
     "UnicoreDataset", "BaseWrapperDataset", "EpochListening", "Dictionary", "data_utils", "iterators",
     "AppendTokenDataset", "PrependTokenDataset", "TokenizeDataset", "BertTokenizeDataset",
     "MaskTokensDataset", "NestedDictionaryDataset", "NumelDataset", "NumSamplesDataset",
-    "LeftPadDataset", "PadDataset", "RightPadDataset", "RightPadDataset2D", "LRUCacheDataset",
+    "LeftPadDataset", "PadDataset", "PackedSequenceDataset", "RightPadDataset", "RightPadDataset2D", "LRUCacheDataset",
     "RawLabelDataset", "RawArrayDataset", "RawNumpyDataset", "LMDBDataset", "SortDataset",
     "EpochShuffleDataset", "FromNumpyDataset", "CountingIterator", "EpochBatchIterator",
     "GroupedIterator", "ShardedIterator", "BufferedIterator", "DevicePrefetcher",

@@ -159,6 +159,32 @@ class RightPadDataset(PadDataset):
         super().__init__(dataset, pad_idx, left_pad=False)
 
 
+class PackedSequenceDataset(BaseWrapperDataset):
+    """Collate 1-D items back to back, without padding: ``[N]`` with N the total length.  With ``tokens_key`` the
+    batch is ``{tokens_key: [N], "cu_seqlens": int32 [B + 1] (the cumulative lengths), "max_seqlen": int}``, the
+    ``net_input`` of a model that runs packed sequences; ``max_seqlen`` is the longest length rounded up to a
+    multiple of 8, the width ``RightPadDataset`` pads the same batch to.  Without it the batch is the ``[N]`` tensor
+    alone (the targets that go with such an input).  Every value is known on the host at collate time."""
+
+    pad_to_multiple = 8
+
+    def __init__(self, dataset, tokens_key=None):
+        super().__init__(dataset)
+        self.tokens_key = tokens_key
+
+    def collater(self, samples):
+        tokens = torch.cat(list(samples))
+        if self.tokens_key is None:
+            return tokens
+        lens = torch.tensor([0] + [len(s) for s in samples], dtype=torch.int64)
+        longest = int(lens.max())
+        return {
+            self.tokens_key: tokens,
+            "cu_seqlens": lens.cumsum(0).to(torch.int32),
+            "max_seqlen": longest + (-longest % self.pad_to_multiple),
+        }
+
+
 class RightPadDataset2D(BaseWrapperDataset):
     """Collate square pair tensors into ``[B, T, T]`` (``pad_dataset.py:32-38``)."""
 

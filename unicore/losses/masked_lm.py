@@ -5,6 +5,11 @@ the device-resident number of masked tokens.
 GPU path: log-softmax + NLL over the ``[n_masked, vocab]`` logits is one fused kernel
 (``unicore.ops.softmax_cross_entropy``) that never materialises fp32 log-probabilities, and the masked positions are
 resolved without a host stall (``utils.request_mask_index``).
+
+Logged per batch: ``bsz`` (sentences), ``sample_size`` (masked tokens) and ``seq_len`` (token slots of the padded
+batch, ``bsz * width``).  A packed batch (``target [N]``, ``cu_seqlens`` / ``max_seqlen`` in ``net_input``) logs the
+values of the padded batch of the same sentences: ``bsz = cu_seqlens.numel() - 1`` (a shape, not a device read) and
+``seq_len = bsz * max_seqlen``, ``max_seqlen`` being the width the padded batch has.
 """
 import math
 
@@ -32,7 +37,11 @@ class MaskedLMLoss(UnicoreLoss):
         logits = model(**sample["net_input"], masked_tokens=masked_tokens)
         wanted = target.reshape(-1).index_select(0, utils.mask_to_index(masked_tokens))
         loss = ops.softmax_cross_entropy(logits, wanted, ignore_index=self.padding_idx)
-        rows, width = target.size(0), target.size(1)
+        net_input = sample["net_input"]
+        if net_input.get("cu_seqlens") is not None:
+            rows, width = net_input["cu_seqlens"].numel() - 1, int(net_input["max_seqlen"])
+        else:
+            rows, width = target.size(0), target.size(1)
         return loss, sample_size, {"loss": loss.data, "bsz": rows, "sample_size": sample_size, "seq_len": rows * width}
 
     @staticmethod

@@ -32,6 +32,13 @@ whole sequence or a prefill, ``seqlens[b] + i`` on a decoding step, read on the 
 nothing; the frequencies are a non-persistent buffer, so ``state_dict`` keys are the same either way.  Cross-attention is
 never rotated.
 
+``cu_seqlens`` / ``max_seqlen`` on ``SelfMultiheadAttention``: the input is B sequences packed back to back, ``[N, E]``
+with sequence ``b`` on rows ``cu_seqlens[b] .. cu_seqlens[b + 1] - 1`` (int ``[B + 1]`` on the device) and
+``max_seqlen`` a host bound on the lengths; the output is packed too.  No row is padding, so the projections do no work
+on pad rows, and the attention runs in the varlen mode of the fused kernels (``ops.fused_attention_varlen``; the
+varlen reference elsewhere).  ``attn_bias`` is ``[1|B, H, max_seqlen, max_seqlen]`` (each sequence reads its top-left
+block); rotary positions restart at 0 in every sequence.  No key padding mask, logits, probabilities or cache.
+
 ``DecoderCache`` holds what incremental decoding keeps between steps: per layer the self-attention keys and values
 ``[B, C, H_kv, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.  A step may
 add one token or a chunk of several per sequence, and ``rewind`` drops tokens again.
@@ -42,7 +49,7 @@ import torch
 from torch import Tensor, nn
 
 from unicore import ops
-from unicore_b200.ops.attention_ops import _fused_attention, _split_packed
+from unicore_b200.ops.attention_ops import _fused_attention, _fused_attention_varlen, _split_packed
 
 
 def _bias_as_4d(attn_bias: Optional[Tensor], bsz: int, heads: int, tgt: int, src: int) -> Optional[Tensor]:
@@ -148,7 +155,7 @@ class SelfMultiheadAttention(nn.Module):
         return self
 
     def attend(self, query, key_padding_mask=None, attn_bias=None, return_attn=False, need_probs=True, causal=False,
-               cache=None):
+               cache=None, cu_seqlens=None, max_seqlen=None):
         """Everything up to (not including) ``out_proj``: returns ``(o [B, L, E], logits, probs)``.
 
         ``need_probs=False`` returns ``probs = None``; with ``return_attn`` the fused kernel then also computes the
@@ -156,7 +163,12 @@ class SelfMultiheadAttention(nn.Module):
         docstring).  ``cache`` (a ``LayerKVCache`` of a ``DecoderCache``): on the prefill the keys and values of the L
         positions are also stored in it; on a decoding step (``query [B, T, E]``, one token or a chunk) the new tokens'
         keys and values are appended and their queries attend to the cached keys up to their own positions
-        (``ops.attention_with_kv_cache``), with ``attn_bias`` the ``[B, H, T, Lb]`` rows of the new queries."""
+        (``ops.attention_with_kv_cache``), with ``attn_bias`` the ``[B, H, T, Lb]`` rows of the new queries.
+        ``cu_seqlens`` / ``max_seqlen``: packed sequences, ``query [N, E]`` -> ``o [N, E]`` (see the module
+        docstring)."""
+        if cu_seqlens is not None:
+            return self._attend_packed(query, key_padding_mask, attn_bias, return_attn, causal, cache, cu_seqlens,
+                                       max_seqlen)
         bsz, tgt_len, embed_dim = query.size()
         if embed_dim != self.embed_dim:
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
@@ -197,6 +209,29 @@ class SelfMultiheadAttention(nn.Module):
                                                    return_attn)
         return o, logits, (probs if need_probs else None)
 
+    def _attend_packed(self, query, key_padding_mask, attn_bias, return_attn, causal, cache, cu_seqlens, max_seqlen):
+        if return_attn:
+            raise ValueError("packed sequences (cu_seqlens) do not return attention weights")
+        if key_padding_mask is not None or cache is not None:
+            raise ValueError("packed sequences (cu_seqlens) take neither a key padding mask nor a cache")
+        if max_seqlen is None:
+            raise ValueError("cu_seqlens needs max_seqlen, a host bound on the lengths")
+        total, embed_dim = query.size()
+        if embed_dim != self.embed_dim:
+            raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
+        H, H_kv, D = self.num_heads, self.num_kv_heads, self.head_dim
+        qkv = ops.linear(query, self.in_proj.weight, self.in_proj.bias).view(total, H + 2 * H_kv, D)
+        if self.rotary_dim is not None:
+            # one token per row of the rotary op, at its position inside its sequence
+            pos = ops.varlen_positions(cu_seqlens, total)
+            qkv = ops.rotary_embedding(qkv.view(total, 1, H + 2 * H_kv, D), self.inv_freq, H + H_kv, pos)
+            qkv = qkv.view(total, H + 2 * H_kv, D)
+        q, k, v = (t[:, 0] for t in _split_packed(qkv[:, None], H_kv))
+        bias4 = _bias_as_4d(attn_bias, cu_seqlens.numel() - 1, H, max_seqlen, max_seqlen)
+        o = _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias4, self.dropout, self.training, self.scaling,
+                                    causal, qkv)
+        return o.reshape(total, embed_dim), None, None
+
     def forward(
         self,
         query,
@@ -205,8 +240,11 @@ class SelfMultiheadAttention(nn.Module):
         return_attn: bool = False,
         need_probs: bool = True,
         causal: bool = False,
+        cu_seqlens: Optional[Tensor] = None,
+        max_seqlen: Optional[int] = None,
     ) -> Tensor:
-        o, logits, probs = self.attend(query, key_padding_mask, attn_bias, return_attn, need_probs, causal)
+        o, logits, probs = self.attend(query, key_padding_mask, attn_bias, return_attn, need_probs, causal,
+                                       cu_seqlens=cu_seqlens, max_seqlen=max_seqlen)
         o = self.out_proj(o)
         return (o, logits, probs) if return_attn else o
 

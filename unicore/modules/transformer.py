@@ -23,6 +23,10 @@ holds ``H_kv`` heads per layer.
 (``SelfMultiheadAttention``); they are independent of ``rel_pos``, and with ``rel_pos=False`` no attention of the stack
 has a bias.  A decoding step rotates its tokens at the cache lengths ``seqlens``, which ``_decode_step`` advances only
 after every layer, so all layers see the same positions.
+``TransformerEncoder`` and its layers also take packed sequences: ``emb [N, E]`` with ``cu_seqlens`` (int ``[B + 1]`` on
+the device) and ``max_seqlen`` (a host bound on the lengths) instead of a padded batch and its padding mask.  Every
+token-wise kernel then runs on the N real tokens only, the relative-position bias is built at ``max_seqlen``, and the
+attention runs in the varlen mode of the fused kernels; the output is packed ``[N, E]``.
 """
 import math
 from typing import Optional
@@ -112,11 +116,15 @@ class _BlockMixin:
         need_probs = kw.pop("need_probs", True)
         causal = kw.pop("causal", False)
         cache = kw.pop("cache", None)
+        # packed sequences: passed on only when given, so that attend keeps its padded-batch signature otherwise
+        packed = {} if kw.get("cu_seqlens") is None else {"cu_seqlens": kw["cu_seqlens"], "max_seqlen": kw["max_seqlen"]}
+        kw.pop("cu_seqlens", None)
+        kw.pop("max_seqlen", None)
         h = attn_in if self.post_ln else norm(attn_in)
         extra = None
         if isinstance(attn_module, SelfMultiheadAttention):
             o, logits, probs = attn_module.attend(h, kw.get("key_padding_mask"), kw.get("attn_bias"), return_attn,
-                                                  need_probs, causal, cache=cache)
+                                                  need_probs, causal, cache=cache, **packed)
             if return_attn:
                 extra = (logits, probs)
         else:
@@ -196,12 +204,16 @@ class TransformerEncoderLayer(nn.Module, _BlockMixin):
         padding_mask: Optional[torch.Tensor] = None,
         return_attn: bool = False,
         need_probs: bool = True,
+        cu_seqlens: Optional[torch.Tensor] = None,
+        max_seqlen: Optional[int] = None,
     ) -> torch.Tensor:
         """With ``return_attn`` returns ``(x, logits, probs)``; ``need_probs=False`` makes ``probs`` None and lets the
-        fused attention kernel produce the logits."""
+        fused attention kernel produce the logits.  ``cu_seqlens`` / ``max_seqlen``: ``x`` is packed ``[N, E]`` (see
+        the module docstring)."""
         x, extra = self._attn_residual(
             self.self_attn, self.self_attn_layer_norm, x, x,
             key_padding_mask=padding_mask, attn_bias=attn_bias, return_attn=return_attn, need_probs=need_probs,
+            cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
         )
         x = self._ffn_residual(x)
         if not return_attn:
@@ -288,11 +300,11 @@ class _StackMixin:
         self.relative_attention_bias = nn.Embedding(rel_pos_bins, self.attention_heads)
         self.rp_bucket = _build_rp_bucket(self.max_seq_len, rel_pos_bins, max_rel_pos)
 
-    def get_rel_pos_bias(self, x):
-        """``[H, L, L]`` bias from the bucket table (positions assumed ordered)."""
+    def get_rel_pos_bias(self, x, seq_len=None):
+        """``[H, L, L]`` bias from the bucket table (positions assumed ordered), ``L = seq_len`` or ``x.size(1)``."""
         if self.rp_bucket.device != x.device:
             self.rp_bucket = self.rp_bucket.to(x.device)
-        seq_len = x.size(1)
+        seq_len = x.size(1) if seq_len is None else int(seq_len)
         weight = self.relative_attention_bias.weight
         one_hot_bytes = self.rel_pos_bins * seq_len * seq_len * 2
         if weight.is_cuda and weight.dtype in (torch.float16, torch.bfloat16) and one_hot_bytes <= (64 << 20):
@@ -322,14 +334,15 @@ class _StackMixin:
             x = x * (1 - padding_mask.unsqueeze(-1).type_as(x))
         return x
 
-    def _compose_bias(self, x, attn_mask, padding_mask):
+    def _compose_bias(self, x, attn_mask, padding_mask, bsz=None, seq_len=None):
         """What the layers receive: ``(attn_bias, key_padding_mask)``.
 
         ``attn_bias`` is None, the relative-position bias ``[1, H, L, L]``, or ``attn_mask`` (the reference's
         ``[B*H, L, L]``, or ``[B, L, L]`` for every head) viewed as ``[B, H, L, L]`` plus that bias.  The key padding mask
-        ``[B, L]`` is passed on as it is."""
-        bsz, seq_len = x.size(0), x.size(1)
-        bias = self.get_rel_pos_bias(x).unsqueeze(0) if self.rel_pos else None  # [1, H, L, L]
+        ``[B, L]`` is passed on as it is.  ``bsz`` / ``seq_len``: B and L of packed sequences (default: ``x [B, L, E]``)."""
+        bsz = x.size(0) if bsz is None else bsz
+        seq_len = x.size(1) if seq_len is None else seq_len
+        bias = self.get_rel_pos_bias(x, seq_len).unsqueeze(0) if self.rel_pos else None  # [1, H, L, L]
         if attn_mask is not None:
             mask = attn_mask.view(bsz, -1, seq_len, seq_len).expand(bsz, self.attention_heads, seq_len, seq_len)
             bias = mask if bias is None else mask + bias
@@ -389,7 +402,26 @@ class TransformerEncoder(nn.Module, _StackMixin):
         emb: torch.Tensor,
         attn_mask: Optional[torch.Tensor] = None,
         padding_mask: Optional[torch.Tensor] = None,
+        cu_seqlens: Optional[torch.Tensor] = None,
+        max_seqlen: Optional[int] = None,
     ) -> torch.Tensor:
+        """``emb [B, L, E]`` (right-padded as ``padding_mask`` says), or packed ``emb [N, E]`` with ``cu_seqlens`` and
+        ``max_seqlen``; ``attn_mask`` is then ``[B*H | B, max_seqlen, max_seqlen]``.  Returns the input's layout.
+        Without ``attn_mask``, ``max_seqlen`` is rounded up to a multiple of 8 (the row width of the kernels' bias and
+        side tensors), which changes no result; an ``attn_mask`` whose width is not a multiple of 8 makes the attention
+        take the materialised varlen reference, as a padded batch of that width does."""
+        if cu_seqlens is not None:
+            if padding_mask is not None:
+                raise ValueError("packed sequences (cu_seqlens) have no padding_mask")
+            if max_seqlen is None:
+                raise ValueError("cu_seqlens needs max_seqlen, a host bound on the lengths")
+            x = self._embed_prologue(emb, None)   # no pad rows to zero
+            if attn_mask is None:
+                max_seqlen = int(max_seqlen) + (-int(max_seqlen) % 8)
+            attn_bias, _ = self._compose_bias(x, attn_mask, None, cu_seqlens.numel() - 1, max_seqlen)
+            for layer in self.layers:
+                x = layer(x, attn_bias=attn_bias, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen)
+            return x if self.final_layer_norm is None else self.final_layer_norm(x)
         x = self._embed_prologue(emb, padding_mask)
         attn_bias, key_padding = self._compose_bias(x, attn_mask, padding_mask)
         for layer in self.layers:

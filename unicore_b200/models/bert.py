@@ -9,6 +9,10 @@ Architectures: bert/bert_base 12L-768-3072-12H, bert_large 24L-1024-4096-16H, xl
 GPU notes: the padding mask goes to the encoder as ``[B, L]`` on every path (no host sync to test
 whether the batch has padding: an all-False mask gives the same result as none, and no ``[B*H, L, L]``
 ``-inf`` tensor); the LM-head activation uses the fused bias+GELU kernel.
+
+Packed batches (``--pack-sequences``): ``src_tokens [N]`` with ``cu_seqlens`` / ``max_seqlen`` in ``net_input``.  Each
+token's position inside its sentence comes from ``cu_seqlens`` on the device, the encoder runs packed (no pad rows),
+and the LM head selects the masked tokens of the flat ``[N]`` mask as it does for a padded batch.
 """
 import logging
 
@@ -94,12 +98,20 @@ class BertModel(BaseUnicoreModel):
     def build_model(cls, args, task):
         return cls(args, task.dictionary)
 
-    def forward(self, src_tokens, masked_tokens=None, features_only=False, classification_head_name=None, **kwargs):
+    def forward(self, src_tokens, masked_tokens=None, features_only=False, classification_head_name=None,
+                cu_seqlens=None, max_seqlen=None, **kwargs):
         if classification_head_name is not None:
             features_only = True
         x = ops.embedding(src_tokens, self.embed_tokens.weight, self.embed_tokens.padding_idx)   # sort-free backward
-        x = x + self.embed_positions.weight[: src_tokens.size(1), :]
-        x = self.sentence_encoder(x, padding_mask=src_tokens.eq(self.padding_idx))
+        if cu_seqlens is not None:   # packed sentences [N]
+            if classification_head_name is not None:
+                raise ValueError("the classification heads take padded batches")
+            pos = ops.varlen_positions(cu_seqlens, src_tokens.size(0))
+            x = x + self.embed_positions.weight.index_select(0, pos)
+            x = self.sentence_encoder(x, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen)
+        else:
+            x = x + self.embed_positions.weight[: src_tokens.size(1), :]
+            x = self.sentence_encoder(x, padding_mask=src_tokens.eq(self.padding_idx))
         if not features_only:
             x = self.lm_head(x, masked_tokens)
         if classification_head_name is not None:

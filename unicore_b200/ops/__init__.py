@@ -2,13 +2,18 @@
 from ._native import HAS_CUDA_EXT, USE_NATIVE, native, use_native  # noqa: F401
 from .attention_ops import (  # noqa: F401
     attention_reference,
+    attention_varlen_reference,
     attention_with_kv_cache,
     attention_with_kv_cache_reference,
     fused_attention,
     fused_attention_qkvpacked,
     fused_attention_supported,
+    fused_attention_varlen,
+    fused_attention_varlen_qkvpacked,
+    fused_attention_varlen_supported,
     fused_head_dim_supported,
     kv_group,
+    varlen_positions,
 )
 from .fused_ops import (  # noqa: F401
     bias_dropout_add_layer_norm,

@@ -253,6 +253,163 @@ def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0
     return _fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal, qkv)
 
 
+def varlen_positions(cu_seqlens, total):
+    """int32 ``[total]``: the position of each packed row inside its sequence (``cu_seqlens [B + 1]``), computed on
+    the device, so that no length is read on the host."""
+    cu = cu_seqlens.to(torch.long)
+    rows = torch.arange(total, device=cu.device)
+    seq = torch.searchsorted(cu[1:], rows, right=True).clamp(max=cu.numel() - 1)
+    return (rows - cu[seq]).to(torch.int32)
+
+
+def _varlen_index(cu_seqlens, max_seqlen, total):
+    """``(rows [B, L], valid [B, L])``: the packed row of position ``i`` of sequence ``b`` and whether it exists, with
+    the kernels' clamps: ``s_b = clamp(cu[b], 0, N)``, ``n_b = clamp(cu[b + 1] - cu[b], 0, min(L, N - s_b))``."""
+    cu = cu_seqlens.to(torch.long)
+    start = cu[:-1].clamp(0, total)
+    n = torch.minimum((cu[1:] - cu[:-1]).clamp(min=0), (total - start).clamp(max=max_seqlen))
+    pos = torch.arange(max_seqlen, device=cu.device)
+    valid = pos[None, :] < n[:, None]
+    rows = torch.where(valid, start[:, None] + pos[None, :], torch.zeros_like(valid, dtype=torch.long))
+    return rows, valid
+
+
+def attention_varlen_reference(q, k, v, cu_seqlens, max_seqlen, bias=None, dropout_p=0.0, training=True, scale=None,
+                               causal=False):
+    """Plain PyTorch implementation of ``fused_attention_varlen`` (CPU path, fallback and test oracle): the packed
+    rows are scattered to ``[B, max_seqlen]``, ``attention_reference`` runs with the length mask (key ``j`` of
+    sequence ``b`` hidden when ``j >= n_b``), and the real rows are gathered back.  Packed rows that belong to no
+    sequence give 0.  Differentiable in q, k, v and the bias.  Without a bias ``max_seqlen`` is rounded up to a multiple
+    of 8, as on the kernel path, so that both clamp a length to the same bound."""
+    N, H, D = q.shape
+    L = _varlen_max_seqlen(max_seqlen, bias)
+    rows, valid = _varlen_index(cu_seqlens.to(q.device), L, N)
+    B = rows.shape[0]
+
+    def scatter(x):
+        return torch.where(valid[:, :, None, None], x[rows], torch.zeros((), dtype=x.dtype, device=x.device))
+
+    # the length mask as an additive bias; the rows past n_b see every key, so that they stay finite (they are dropped)
+    hide = (torch.arange(L, device=q.device)[None, None, :] >= valid.sum(1)[:, None, None]) & valid[:, :, None]
+    mask = torch.zeros(B, 1, L, L, dtype=q.dtype, device=q.device).masked_fill(hide[:, None], float("-inf"))
+    bias = mask if bias is None else bias.to(q.dtype) + mask
+    out = attention_reference(scatter(q), scatter(k), scatter(v), bias, None, dropout_p, training, scale,
+                              causal=causal)
+    # gather back: the rows of no sequence (and the positions past n_b) write into a dropped row N
+    dest = torch.where(valid, rows, torch.full_like(rows, N)).reshape(-1)
+    packed = torch.zeros(N + 1, H, D, dtype=out.dtype, device=out.device).index_put((dest,), out.reshape(-1, H, D))
+    return packed[:N]
+
+
+class _FusedVarlenAttentionFn(torch.autograd.Function):
+    """The varlen kernels' forward and backward (``_C.varlen``), shaped as ``_FusedAttentionFn``: ``qkv`` None or
+    the contiguous ``[N, H + 2 * H_kv, D]`` projection that q, k and v are (detached) views of, which then gets one
+    packed gradient."""
+
+    @staticmethod
+    def forward(ctx, qkv, q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal):
+        p = float(dropout_p) if training else 0.0
+        out, lse, bits = native().varlen.fmha_varlen_fwd(q, k, v, cu_seqlens, max_seqlen, bias, p, float(scale),
+                                                         causal=causal)
+        ctx.p = p
+        ctx.causal = causal
+        ctx.scale = float(scale)
+        ctx.max_seqlen = max_seqlen
+        ctx.need_dbias = bias is not None and bias.requires_grad
+        ctx.packed_shape = None if qkv is None else qkv.shape
+        ctx.save_for_backward(q, k, v, out, lse, cu_seqlens, bias, bits)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        q, k, v, out, lse, cu_seqlens, bias, bits = ctx.saved_tensors
+        packed = ctx.packed_shape is not None
+        dq, dk, dv, dbias = native().varlen.fmha_varlen_bwd(
+            dout.contiguous(), q, k, v, out, lse, cu_seqlens, ctx.max_seqlen, bias, ctx.p, ctx.scale, bits,
+            ctx.need_dbias, packed, causal=ctx.causal
+        )
+        if dbias is not None and dbias.dtype != bias.dtype:
+            dbias = dbias.to(bias.dtype)
+        if packed:   # the [N, H + 2 * H_kv, D] tensor the three gradients are views of
+            dqkv, dq, dk, dv = dq._base.view(ctx.packed_shape), None, None, None
+        else:
+            dqkv = None
+        return dqkv, dq, dk, dv, None, None, dbias, None, None, None, None
+
+
+def _varlen_max_seqlen(max_seqlen, bias):
+    """The kernels' ``max_seqlen``: a multiple of 8.  Without a bias it is rounded up (the padded side layout is
+    internal and the lengths stay below it); with one it must be the bias's own size."""
+    L = int(max_seqlen)
+    return L if bias is not None else L + (-L % 8)
+
+
+def fused_attention_varlen_supported(q, k, v, cu_seqlens, max_seqlen, bias=None) -> bool:
+    if not use_native(q, k, v, cu_seqlens, bias) or not hasattr(native(), "varlen"):
+        return False
+    if q.dim() != 3 or k.dim() != 3 or v.dim() != 3 or q.shape[0] < 1 or cu_seqlens.dim() != 1 \
+            or cu_seqlens.numel() < 2:
+        return False
+    if k.shape[0] != q.shape[0] or v.shape[0] != q.shape[0]:
+        return False
+    if not _kernel_tensors(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0)):
+        return False
+    if any(t.stride(1) != q.shape[-1] for t in (q, k, v)):
+        return False
+    if k.shape[1] != v.shape[1] or k.shape[1] < 1 or q.shape[1] % k.shape[1] != 0:
+        return False
+    L = _varlen_max_seqlen(max_seqlen, bias)
+    if L < 1 or L % 8 != 0:
+        return False
+    if bias is not None:
+        if bias.dim() != 4 or bias.shape[0] not in (1, cu_seqlens.numel() - 1) or bias.shape[1] != q.shape[1]:
+            return False
+        if bias.shape[2] != L or bias.shape[3] != L or bias.dtype not in (q.dtype, torch.float32):
+            return False
+    return True
+
+
+def _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal, qkv=None):
+    """``fused_attention_varlen`` on q / k / v, which are the views of ``qkv`` when it is given: a contiguous ``qkv``
+    then gets one packed gradient."""
+    if scale is None:
+        scale = 1.0 / math.sqrt(q.shape[-1])
+    if not fused_attention_varlen_supported(q, k, v, cu_seqlens, max_seqlen, bias):
+        return attention_varlen_reference(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal)
+    L = _varlen_max_seqlen(max_seqlen, bias)
+    cu_seqlens = cu_seqlens.to(torch.int32).contiguous()
+    if bias is not None:
+        bias = bias.to(q.dtype).contiguous()
+    if qkv is not None and qkv.is_contiguous():
+        q, k, v = q.detach(), k.detach(), v.detach()   # autograd sees qkv alone
+    else:
+        qkv = None
+    return _FusedVarlenAttentionFn.apply(qkv, q, k, v, cu_seqlens, L, bias, dropout_p, training, scale, causal)
+
+
+def fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias=None, dropout_p=0.0, training=True, scale=None,
+                           causal=False):
+    """Attention over packed variable-length sequences (no padding): q ``[N, H, D]``, k / v ``[N, H_kv, D]`` with
+    ``H_kv`` dividing ``H``, the B sequences back to back; sequence ``b`` holds rows ``cu_seqlens[b] ..
+    cu_seqlens[b + 1] - 1`` (int ``[B + 1]`` on the device, never read on the host).  ``max_seqlen``: a host bound
+    on the lengths; without a bias it is rounded up to a multiple of 8.  ``bias``: ``[1|B, H, max_seqlen,
+    max_seqlen]``, sequence b reading its top-left block; the kernels take it when ``max_seqlen`` is a multiple of 8
+    (the rule of the padded call), other widths run ``attention_varlen_reference``.
+    ``causal`` masks key j > query i within each sequence.  Returns ``[N, H, D]``: at every real row the result of
+    the padded call with ``key_padding_mask = (j >= len_b)``.  Lengths are clamped to ``[0, max_seqlen]`` and the
+    starts to ``[0, N]``."""
+    kv_group(q.shape[1], k.unsqueeze(0), v.unsqueeze(0))
+    return _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal)
+
+
+def fused_attention_varlen_qkvpacked(qkv, cu_seqlens, max_seqlen, bias=None, dropout_p=0.0, training=True,
+                                     scale=None, causal=False, num_kv_heads=None):
+    """``fused_attention_varlen`` on the packed projection ``qkv [N, 3, H, D]``, or ``[N, H + 2 * H_kv, D]`` with
+    ``num_kv_heads = H_kv``; a contiguous ``qkv`` gets one gradient tensor."""
+    q, k, v = (t[:, 0] for t in _split_packed(qkv[:, None], num_kv_heads))
+    return _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal, qkv)
+
+
 def _check_no_grad(*tensors):
     if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors):
         raise RuntimeError("attention_with_kv_cache has no backward: call it under torch.no_grad() or "
