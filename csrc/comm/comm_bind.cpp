@@ -93,7 +93,7 @@ void symm_fused_tail(const std::vector<int64_t>& xchg_ptrs, const std::vector<in
                      const std::vector<at::Tensor>& exp_avg, const std::vector<at::Tensor>& exp_avg_sq,
                      const std::vector<std::optional<at::Tensor>>& ema, const std::vector<int64_t>& numel,
                      const std::vector<int64_t>& dtypes, const std::vector<std::vector<double>>& hyper,
-                     const at::Tensor& ranges, int64_t pending_mask, at::Tensor bucket_sq, at::Tensor block_sq,
+                     const at::Tensor& ranges, uint64_t pending_mask, at::Tensor bucket_sq, at::Tensor block_sq,
                      at::Tensor grid_sync, const std::optional<at::Tensor>& stats_src,
                      const std::optional<at::Tensor>& stats_dst, int64_t parity, int64_t denom_index, double factor,
                      double max_norm, double clip_eps, double rs_scale, double ema_decay, bool stochastic_rounding,
@@ -167,7 +167,7 @@ void symm_fused_tail(const std::vector<int64_t>& xchg_ptrs, const std::vector<in
   a.ngroups = ng;
   a.nranges = nr;
   a.ranges = reinterpret_cast<const ub::TailRange*>(ranges.data_ptr<int64_t>());
-  a.pending_mask = (unsigned long long)pending_mask;
+  a.pending_mask = pending_mask;
   a.bucket_sq = bucket_sq.data_ptr<float>();
   a.block_sq = block_sq.data_ptr<float>();
   a.grid_sync = reinterpret_cast<unsigned int*>(grid_sync.data_ptr<int>());
