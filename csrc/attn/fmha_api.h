@@ -57,13 +57,24 @@ struct FmhaFwdParams {
   // Varlen mode (fmha_varlen_fwd / fmha_varlen_bwd; appended so that no earlier field moves): the B sequences are
   // packed back to back.  q is [N, H, D], k / v [N, H_kv, D] (strided views with B = 1 in the TMA maps, L = N), and
   // sequence b holds rows s_b .. s_b + n_b - 1 with s_b = clamp(cu_seqlens[b], 0, N) and
-  // n_b = clamp(cu_seqlens[b + 1] - cu_seqlens[b], 0, min(Lq, N - s_b)); Lq = Lk = max_seqlen.  O [N, H, D] (and dO) are
+  // n_b = clamp(cu_seqlens[b + 1] - cu_seqlens[b], 0, min(Lq, N - s_b)); Lq = Lk = max_seqlen (self-attention; the
+  // key description below generalises this to separate key sequences).  O [N, H, D] (and dO) are
   // packed too.  Everything per (b, h, row) keeps the padded layout of B sequences of Lq rows: LSE, keep bits, Philox
   // counters, delta, the dQ accumulator and turn counters, the bias [1|B, H, Lq, Lk] (sequence b reads its top-left
   // n_b x n_b block) and dS / dBias.  Query i of sequence b sees keys j < n_b (and j <= i when causal): the result at
   // every row i < n_b is that of the padded call with key_padding_mask = (j >= n_b).  kpm must be null; no logits.
   const int* cu_seqlens;   // [B + 1] int32 on the device
   int varlen, packed_rows; // packed_rows = N
+  // Varlen keys (appended so that no earlier field moves): every varlen call reads its key ranges from these.  k / v
+  // are [N_k, H_kv, D] and sequence b's keys are rows s_k + 0 .. s_k + n_k - 1 with {s_k, n_k} =
+  // fmha_varlen_seq(cu_seqlens_k, b, Lk, N_k), while its queries keep {s_q, n_q} from cu_seqlens, Lq and N_q; Lq =
+  // max_seqlen and Lk = max_seqlen_k may differ (cross-attention).  Self-attention sets cu_seqlens_k = cu_seqlens and
+  // packed_rows_k = packed_rows.  Query i < n_q of sequence b sees keys j < n_k, reads bias[b', h, i, j] of its top-left
+  // n_q x n_k block, and gets the result of the padded call with key_padding_mask = (j >= n_k).  A sequence with
+  // n_k = 0 < n_q follows the kernels' fully-masked contract: O = 0, LSE = -inf, dQ = 0 and no gradient elsewhere.
+  // Causal is defined only for cu_seqlens_k == cu_seqlens (the bindings refuse it otherwise).
+  const int* cu_seqlens_k;   // [B + 1] int32 on the device
+  int packed_rows_k;         // N_k
 };
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
 

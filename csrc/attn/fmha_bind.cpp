@@ -391,19 +391,25 @@ Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   return out;
 }
 // ---- varlen: packed sequences described by cu_seqlens (fmha_api.h) ------------------------------------------------
-// q [N, H, D], k / v [N, H_kv, D] (head slices of one projection are fine), cu_seqlens int32 [B + 1] on the device,
-// max_seqlen a host bound on the lengths (a multiple of 8: the row stride of the bias, LSE, keep-bit and dS maps), bias
-// [1|B, H, max_seqlen, max_seqlen].  No key padding mask: the lengths take its place.  Returns B.
-int64_t check_varlen(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& cu_seqlens, int64_t max_seqlen,
-                     const OptTensor& bias) {
+// q [N_q, H, D], k / v [N_k, H_kv, D] (head slices of one projection are fine), cu_seqlens int32 [B + 1] on the
+// device, max_seqlen a host bound on the query lengths (a multiple of 8: the row stride of the bias, LSE, keep-bit and
+// dS maps), bias [1|B, H, max_seqlen, max_seqlen_k].  cu_seqlens_k (int32 [B + 1] on the device, the same B) describes
+// separate key sequences, and max_seqlen_k bounds their lengths (0: max_seqlen); without it the keys are the queries'
+// own rows (N_k == N_q).  No key padding mask: the lengths take its place.  Causal needs the queries' own keys.
+// Returns {B, max_seqlen_k}.
+std::pair<int64_t, int64_t> check_varlen(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& cu_seqlens,
+                                         int64_t max_seqlen, const OptTensor& bias, const OptTensor& cu_seqlens_k,
+                                         int64_t max_seqlen_k, bool causal) {
   check_operand(q, "q", q.device(), k16Bit, any_shape(3), kAligned);
   check_operand(k, "k", q.device(), {q.scalar_type()}, any_shape(3), kAligned);
   check_operand(v, "v", q.device(), {q.scalar_type()}, any_shape(3), kAligned);
-  const int64_t N = q.size(0), H = q.size(1), D = q.size(2), H_kv = v.size(1);
+  const int64_t N = q.size(0), H = q.size(1), D = q.size(2), H_kv = v.size(1), N_k = k.size(0);
   TORCH_CHECK(ub::fmha_head_dim_supported(D) && k.size(2) == D && v.size(2) == D,
               "head_dim must be the same for q/k/v and a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
-  TORCH_CHECK(N >= 1 && k.size(0) == N && v.size(0) == N && k.size(1) == H_kv,
-              "k / v must be [N, H_kv, D] with the N >= 1 packed rows and the D of q");
+  TORCH_CHECK(N >= 1 && N_k >= 1 && v.size(0) == N_k && k.size(1) == H_kv,
+              "k / v must be [N_k, H_kv, D] with N_k >= 1 packed rows each and the D of q");
+  TORCH_CHECK(has(cu_seqlens_k) || N_k == N,
+              "k / v must be [N, H_kv, D] with the N packed rows of q when cu_seqlens_k is not given");
   kv_group(H, H_kv, "v");
   for (const Tensor* t : {&q, &k, &v}) {
     TORCH_CHECK(t->stride(2) == 1 && t->stride(1) == D, "q/k/v head stride must be head_dim");
@@ -412,23 +418,34 @@ int64_t check_varlen(const Tensor& q, const Tensor& k, const Tensor& v, const Te
   check_operand(cu_seqlens, "cu_seqlens", q.device(), {at::kInt}, {kAnySize});
   const int64_t B = cu_seqlens.size(0) - 1;
   TORCH_CHECK(B >= 1, "cu_seqlens must have B + 1 >= 2 entries");
+  check_operand(cu_seqlens_k, "cu_seqlens_k", q.device(), {at::kInt}, {B + 1});
+  TORCH_CHECK(!(causal && has(cu_seqlens_k)), "causal attention is not defined with separate key sequences "
+              "(cu_seqlens_k)");
   TORCH_CHECK(max_seqlen >= 1 && max_seqlen % 8 == 0, "max_seqlen must be a positive multiple of 8");
-  check_operand(bias, "bias", q.device(), {q.scalar_type()}, {kAnySize, H, max_seqlen, max_seqlen}, kVec);
-  TORCH_CHECK(!has(bias) || bias->size(0) == 1 || bias->size(0) == B, "bias must be [1|B, H, max_seqlen, max_seqlen]");
-  return B;
+  const int64_t Lk = max_seqlen_k == 0 ? max_seqlen : max_seqlen_k;
+  TORCH_CHECK(Lk >= 1 && Lk % 8 == 0, "max_seqlen_k must be 0 or a positive multiple of 8");
+  TORCH_CHECK(has(cu_seqlens_k) || Lk == max_seqlen, "max_seqlen_k other than max_seqlen needs cu_seqlens_k");
+  check_operand(bias, "bias", q.device(), {q.scalar_type()}, {kAnySize, H, max_seqlen, Lk}, kVec);
+  TORCH_CHECK(!has(bias) || bias->size(0) == 1 || bias->size(0) == B,
+              "bias must be [1|B, H, max_seqlen, max_seqlen_k]");
+  return {B, Lk};
 }
 
-// The parameters of a varlen call: q / k / v maps over the N packed rows (B = 1), everything else at B x max_seqlen
+// The parameters of a varlen call: q / k / v maps over the N_q / N_k packed rows (B = 1), everything else at
+// B x max_seqlen (x max_seqlen_k); the key description is the query one when cu_seqlens_k is not given
 void fill_varlen(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& cu_seqlens,
-                 int64_t B, int64_t max_seqlen, const OptTensor& bias, double p_drop, double scale, bool causal,
-                 bool forward) {
+                 int64_t B, int64_t max_seqlen, const OptTensor& cu_seqlens_k, int64_t max_seqlen_k,
+                 const OptTensor& bias, double p_drop, double scale, bool causal, bool forward) {
   fill_common(p, q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), std::nullopt, std::nullopt, p_drop, scale, forward);
   p.B = (int)B;
-  p.Lq = p.Lk = (int)max_seqlen;
+  p.Lq = (int)max_seqlen;
+  p.Lk = (int)max_seqlen_k;
   p.causal = causal ? 1 : 0;
   p.varlen = 1;
   p.cu_seqlens = cu_seqlens.data_ptr<int>();
   p.packed_rows = (int)q.size(0);
+  p.cu_seqlens_k = has(cu_seqlens_k) ? cu_seqlens_k->data_ptr<int>() : p.cu_seqlens;
+  p.packed_rows_k = (int)k.size(0);
   if (has(bias)) {
     p.bias = bias->data_ptr();
     p.bias_batch = (int)bias->size(0);
@@ -437,15 +454,16 @@ void fill_varlen(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   }
 }
 
-// (out [N, H, D], lse [B, H, max_seqlen], keep bits [B, H, max_seqlen, ceil(max_seqlen / 32)] or None); rows of LSE
-// and of the keep bits past each sequence's length are not written
+// (out [N_q, H, D], lse [B, H, max_seqlen], keep bits [B, H, max_seqlen, ceil(max_seqlen_k / 32)] or None); rows of
+// LSE and of the keep bits past each sequence's query length are not written
 std::tuple<Tensor, Tensor, OptTensor> fmha_varlen_fwd(const Tensor& q, const Tensor& k, const Tensor& v,
                                                       const Tensor& cu_seqlens, int64_t max_seqlen, const OptTensor& bias,
-                                                      double p_drop, double scale, bool causal) {
-  const int64_t B = check_varlen(q, k, v, cu_seqlens, max_seqlen, bias);
+                                                      double p_drop, double scale, bool causal,
+                                                      const OptTensor& cu_seqlens_k, int64_t max_seqlen_k) {
+  const auto [B, Lk] = check_varlen(q, k, v, cu_seqlens, max_seqlen, bias, cu_seqlens_k, max_seqlen_k, causal);
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaFwdParams p{};
-  fill_varlen(p, q, k, v, cu_seqlens, B, max_seqlen, bias, p_drop, scale, causal, /*forward=*/true);
+  fill_varlen(p, q, k, v, cu_seqlens, B, max_seqlen, cu_seqlens_k, Lk, bias, p_drop, scale, causal, /*forward=*/true);
   Tensor out = torch::empty({q.size(0), p.H, p.D}, q.options());
   Tensor lse = torch::empty({p.B, p.H, p.Lq}, q.options().dtype(at::kFloat));
   p.out = out.data_ptr();
@@ -463,24 +481,27 @@ std::tuple<Tensor, Tensor, OptTensor> fmha_varlen_fwd(const Tensor& q, const Ten
 }
 
 // packed_grad: q / k / v are the head slices of one [N, H + 2 H_kv, D] projection, and the gradients are written into
-// one tensor of that layout (returned three times as views), as fmha_bwd does for [B, L, H + 2 H_kv, D].  dBias is 0
-// outside every sequence's block.
+// one tensor of that layout (returned three times as views), as fmha_bwd does for [B, L, H + 2 H_kv, D]; self-attention
+// only.  dK / dV are [N_k, H_kv, D].  dBias is 0 outside every sequence's n_q x n_k block.
 std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_varlen_bwd(const Tensor& dout, const Tensor& q, const Tensor& k,
                                                               const Tensor& v, const Tensor& out, const Tensor& lse,
                                                               const Tensor& cu_seqlens, int64_t max_seqlen,
                                                               const OptTensor& bias, double p_drop, double scale,
                                                               const OptTensor& drop_bits, bool need_dbias,
-                                                              bool packed_grad, bool causal) {
-  const int64_t B = check_varlen(q, k, v, cu_seqlens, max_seqlen, bias);
-  const int64_t N = q.size(0), H = q.size(1), D = q.size(2), H_kv = k.size(1), L = max_seqlen;
+                                                              bool packed_grad, bool causal,
+                                                              const OptTensor& cu_seqlens_k, int64_t max_seqlen_k) {
+  const auto [B, Lk] = check_varlen(q, k, v, cu_seqlens, max_seqlen, bias, cu_seqlens_k, max_seqlen_k, causal);
+  const int64_t N = q.size(0), H = q.size(1), D = q.size(2), N_k = k.size(0), H_kv = k.size(1), L = max_seqlen;
   check_operand(dout, "dout", q.device(), {q.scalar_type()}, q.sizes(), kVec);
   check_operand(out, "out", q.device(), {q.scalar_type()}, q.sizes());
   check_operand(lse, "lse", q.device(), {at::kFloat}, {B, H, L});
   TORCH_CHECK(p_drop <= 0.0 || has(drop_bits), "dropout bits missing");
-  if (p_drop > 0.0) check_operand(drop_bits, "drop_bits", q.device(), {at::kInt}, {B, H, L, (L + 31) / 32});
+  if (p_drop > 0.0) check_operand(drop_bits, "drop_bits", q.device(), {at::kInt}, {B, H, L, (Lk + 31) / 32});
+  TORCH_CHECK(!(packed_grad && has(cu_seqlens_k)), "packed gradients need self-attention (no cu_seqlens_k)");
   const c10::cuda::CUDAGuard guard(q.device());
   ub::FmhaBwdParams p{};
-  fill_varlen(p.f, q, k, v, cu_seqlens, B, max_seqlen, bias, p_drop, scale, causal, /*forward=*/false);
+  fill_varlen(p.f, q, k, v, cu_seqlens, B, max_seqlen, cu_seqlens_k, Lk, bias, p_drop, scale, causal,
+              /*forward=*/false);
   p.f.out = out.data_ptr();
   p.f.lse = lse.data_ptr<float>();
   if (p_drop > 0.0) p.f.drop_bits = reinterpret_cast<uint32_t*>(drop_bits->data_ptr());
@@ -502,8 +523,8 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_varlen_bwd(const Tensor& dout
     dv = dqkv.narrow(1, H + H_kv, H_kv);
   } else {
     dq = torch::empty({N, H, D}, q.options());
-    dk = torch::empty({N, H_kv, D}, q.options());
-    dv = torch::empty({N, H_kv, D}, q.options());
+    dk = torch::empty({N_k, H_kv, D}, q.options());
+    dv = torch::empty({N_k, H_kv, D}, q.options());
   }
   // the kernels address row r of sequence b as row s_b + r through the row stride; the batch stride is unused
   p.dq_sb = p.dk_sb = p.dv_sb = 0;
@@ -514,11 +535,11 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_varlen_bwd(const Tensor& dout
   Tensor ds_buf;
   if (need_dbias && p.f.bias != nullptr) {
     // zeroed by the launcher: the kernels store the tiles inside each sequence's block only
-    ds_buf = torch::empty({B, H, L, L}, q.options());
+    ds_buf = torch::empty({B, H, L, Lk}, q.options());
     p.ds_buf = ds_buf.data_ptr();
-    dbias = (p.f.bias_batch == B) ? ds_buf : torch::empty({p.f.bias_batch, H, L, L}, q.options());
+    dbias = (p.f.bias_batch == B) ? ds_buf : torch::empty({p.f.bias_batch, H, L, Lk}, q.options());
     p.dbias = dbias->data_ptr();
-    TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_ds, p.ds_buf, p.f.is_bf16 != 0, (int)(B * H), (int)L, (int)L),
+    TORCH_CHECK(ub::make_bias_tile_map_sw128(&p.sw_ds, p.ds_buf, p.f.is_bf16 != 0, (int)(B * H), (int)L, (int)Lk),
                 "cuTensorMapEncodeTiled failed for the dS scratch tensor");
   }
   p.delta = delta.data_ptr<float>();
@@ -552,11 +573,12 @@ void register_fmha(pybind11::module_& m) {
   // packed variable-length sequences: its own submodule, _C.varlen
   auto vl = m.def_submodule("varlen", "packed variable-length sequences described by cu_seqlens");
   vl.def("fmha_varlen_fwd", &fmha_varlen_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("cu_seqlens"),
-         py::arg("max_seqlen"), py::arg("bias"), py::arg("p_drop"), py::arg("scale"), py::arg("causal") = false);
+         py::arg("max_seqlen"), py::arg("bias"), py::arg("p_drop"), py::arg("scale"), py::arg("causal") = false,
+         py::arg("cu_seqlens_k") = py::none(), py::arg("max_seqlen_k") = 0);
   vl.def("fmha_varlen_bwd", &fmha_varlen_bwd, py::arg("dout"), py::arg("q"), py::arg("k"), py::arg("v"),
          py::arg("out"), py::arg("lse"), py::arg("cu_seqlens"), py::arg("max_seqlen"), py::arg("bias"),
          py::arg("p_drop"), py::arg("scale"), py::arg("drop_bits"), py::arg("need_dbias"), py::arg("packed_grad"),
-         py::arg("causal") = false);
+         py::arg("causal") = false, py::arg("cu_seqlens_k") = py::none(), py::arg("max_seqlen_k") = 0);
   m.def("fmha_decode_max_splits", [] { return (int64_t)ub::kDecodeMaxSplits; });
   m.def("fmha_decode_num_splits", [](int64_t B, int64_t H, int64_t len_bound) {
     return (int64_t)ub::fmha_decode_num_splits((int)B, (int)H, (int)len_bound,

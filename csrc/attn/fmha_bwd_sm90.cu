@@ -210,13 +210,15 @@ __global__ void __launch_bounds__(256) fmha_dq_convert_kernel(const float* __res
 // finishes its whole sequence, so every turn this CTA waits for arrives.  The wait is at the last point, with the dQ
 // tile already staged, so a CTA does not hold up the chain while it computes.  dK, dV and dS are computed exactly as
 // in the default mode.
-// kVarlen: packed sequences (fmha_api.h).  Key tile j of sequence b exists iff key0 < n_b (the others exit at once), and
-// it walks the query tiles below n_b only, so the turn chain of a query tile is the key tiles 0 .. below n_b, with no
-// gap.  Rows at or past n_b (rows of the next sequence) and keys at or past n_b get P = 0 and dS = 0 by selection, and
-// only keys below n_b store dK / dV.  The padded call with key_padding_mask = (j >= n_b) and dO = 0 at the pad rows
-// adds exact zeros for everything skipped, so dK and dV are bitwise its results, and dQ / dS too in deterministic mode.
-// The dS tiles no CTA stores are zeroed by the launcher (a memset of ds_buf), so dBias is exactly 0 outside every
-// sequence's n_b x n_b block.
+// kVarlen: packed sequences (fmha_api.h), n_q queries from packed row s_q and n_k keys from packed key row s_k.  Key
+// tile j of sequence b exists iff key0 < n_k (the others exit at once), loads K / V at s_k + key0 and walks the query
+// tiles below n_q only (Q and dO at s_q + 64 i), so the turn chain of a query tile is the key tiles 0 .. below n_k, with
+// no gap; a sequence with n_k = 0 has no key CTA, so nothing waits on its query tiles and their dQ stays 0.  A key tile
+// of a sequence with n_q = 0 loads nothing and stores dK = dV = 0.  Rows at or past n_q (rows of the next sequence) and
+// keys at or past n_k get P = 0 and dS = 0 by selection, and only keys below n_k store dK / dV, at packed key rows.  The
+// padded call with key_padding_mask = (j >= n_k) and dO = 0 at the pad rows adds exact zeros for everything skipped, so
+// dK and dV are bitwise its results, and dQ / dS too in deterministic mode.  The dS tiles no CTA stores are zeroed by
+// the launcher (a memset of ds_buf), so dBias is exactly 0 outside every sequence's n_q x n_k block.
 template <typename T, int DP, bool kLogits, bool kCausal, bool kDet = false, bool kVarlen = false>
 __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel(const __grid_constant__ FmhaBwdParams bp) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
@@ -232,12 +234,16 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, c = lane & 3;
   const int key0 = blockIdx.x * kBN, hk = blockIdx.y, b = blockIdx.z;
-  int vl_s = 0, vl_n = 0;   // varlen: the sequence's first packed row and its length
+  // varlen: the sequence's first packed query row and query count, and its first packed key row and key count
+  int vl_s = 0, vl_n = 0, vk_s = 0, vk_n = 0;
   if constexpr (kVarlen) {
+    const int2 sk = fmha_varlen_seq(p.cu_seqlens_k, b, p.Lk, p.packed_rows_k);
+    vk_s = sk.x;
+    vk_n = sk.y;
+    if (key0 >= vk_n) return;
     const int2 sn = fmha_varlen_seq(p.cu_seqlens, b, p.Lq, p.packed_rows);
     vl_s = sn.x;
     vl_n = sn.y;
-    if (key0 >= vl_n) return;
   }
   const int tb = kVarlen ? 0 : b;   // batch coordinate of the q / k / v / dO maps
   const uint32_t bar_kv = smem_base + kOffBar, bar_in0 = smem_base + kOffBar + 8;   // + 8 * stage
@@ -287,7 +293,9 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
     }
   };
 
-  const bool any_q = !kCausal || i0 < n_qwalk;   // a copy must not outlive the CTA: no query tile, no load
+  // a copy must not outlive the CTA: no query tile (causal above the diagonal, or a varlen sequence without queries),
+  // no load; the CTA then stores dK = dV = 0
+  const bool any_q = !(kCausal || kVarlen) || i0 < n_qwalk;
   if (tid == 0) {
     mbar_init(bar_kv, 1);
     mbar_init(bar_in0, 1);
@@ -297,8 +305,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
       mbar_expect_tx(bar_kv, 2 * kTile);
 #pragma unroll
       for (int x = 0; x < C::kBoxes; ++x) {
-        tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, hk, vl_s + key0, tb, bar_kv);
-        tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, hk, vl_s + key0, tb, bar_kv);
+        tma_load_4d(smem_base + kOffK + x * 8192, &p.sw_k, 64 * x, hk, vk_s + key0, tb, bar_kv);
+        tma_load_4d(smem_base + kOffV + x * 8192, &p.sw_v, 64 * x, hk, vk_s + key0, tb, bar_kv);
       }
       load_tile(h0, i0, 0);
     }
@@ -319,8 +327,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
   // my two keys (accumulator rows) and their additive masks
   const int kl0 = warp * 16 + g, kl1 = kl0 + 8;
   const int kr0 = key0 + kl0, kr1 = key0 + kl1;
-  const float kadd0 = (kr0 >= (kVarlen ? vl_n : p.Lk) || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr0] != 0)) ? -CUDART_INF_F : 0.f;
-  const float kadd1 = (kr1 >= (kVarlen ? vl_n : p.Lk) || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr1] != 0)) ? -CUDART_INF_F : 0.f;
+  const float kadd0 = (kr0 >= (kVarlen ? vk_n : p.Lk) || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr0] != 0)) ? -CUDART_INF_F : 0.f;
+  const float kadd1 = (kr1 >= (kVarlen ? vk_n : p.Lk) || (p.kpm != nullptr && p.kpm[(long long)b * p.Lk + kr1] != 0)) ? -CUDART_INF_F : 0.f;
   // keep-bit positions of my keys inside their 32-key word (word (warp >> 1) of the tile's two)
   const int kk0 = 16 * (warp & 1) + g, kk1 = kk0 + 8;
   const int bit0 = (kk0 & 1) * 16 + (kk0 >> 1), bit1 = (kk1 & 1) * 16 + (kk1 >> 1);
@@ -414,8 +422,8 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
         s[e + 1] = ex2_approx(fmaf(x1, kLog2e, -l2.y));
         if constexpr (kVarlen) {   // rows and keys of the next sequence: selected, whatever their bias or data hold
           const int q = i * kBM + ql, kl = (r & 1) ? kl1 : kl0;
-          if (key0 + kl >= vl_n || q >= vl_n) s[e] = 0.f;
-          if (key0 + kl >= vl_n || q + 1 >= vl_n) s[e + 1] = 0.f;
+          if (key0 + kl >= vk_n || q >= vl_n) s[e] = 0.f;
+          if (key0 + kl >= vk_n || q + 1 >= vl_n) s[e + 1] = 0.f;
         }
       }
     }
@@ -532,9 +540,9 @@ __global__ void __launch_bounds__(kBwdThreads, DP == 64 ? 2 : 1) fmha_bwd_kernel
 #pragma unroll
   for (int half = 0; half < 2; ++half) {
     const int key = half ? kr1 : kr0;
-    if (key >= (kVarlen ? vl_n : p.Lk)) continue;
-    // padded: (b, key); varlen: packed row s_b + key
-    const long long row = kVarlen ? (long long)vl_s + key : (long long)key;
+    if (key >= (kVarlen ? vk_n : p.Lk)) continue;
+    // padded: (b, key); varlen: packed key row s_k + key
+    const long long row = kVarlen ? (long long)vk_s + key : (long long)key;
     T* dvg = reinterpret_cast<T*>(bp.dv) + (long long)tb * bp.dv_sb + row * bp.dv_sl + (long long)hk * bp.dv_sh;
     T* dkg = reinterpret_cast<T*>(bp.dk) + (long long)tb * bp.dk_sb + row * bp.dk_sl + (long long)hk * bp.dk_sh;
 #pragma unroll

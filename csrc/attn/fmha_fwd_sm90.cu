@@ -98,12 +98,14 @@ UB_DEVICE void quad_transpose4(uint32_t (&w)[4], int c) {
 // may span two) sets the invisible elements to -inf by index.  Cache rows at or past n_b lie inside the tensor, so TMA
 // loads them and they may hold anything, NaN included: their scores are replaced (never added to), and their V rows
 // are zeroed in shared memory before P V (0 x NaN is NaN).  Only the last tile walked can hold such rows.  No dropout.
-// kVarlen: packed sequences (fmha_api.h).  The CTA of (query tile, h, b) reads rows s_b + q0 .. of the packed q / k / v
-// through B = 1 maps and exits when q0 >= n_b.  Its tile loop (and the prefetch) stops at the tile holding key n_b - 1;
-// the padded call would walk the later tiles as wholly masked ones, which add exact zeros (see kCausal), so O, LSE and
-// the keep words at rows below n_b are bitwise those of that call.  In the last tile the keys at or past n_b (rows of
-// the next sequence, or TMA zero fill past N) get -inf by assignment and their V rows are zeroed, as in the KV-cache
-// mode.  Only rows below n_b are stored.  Causal composes (its diagonal is per sequence); logits mode does not.
+// kVarlen: packed sequences (fmha_api.h).  The CTA of (query tile, h, b) reads query rows s_q + q0 .. of the packed q
+// and key rows s_k + j * kBlockN .. of the packed k / v through B = 1 maps, and exits when q0 >= n_q.  Its tile loop
+// (and the prefetch) stops at the tile holding key n_k - 1; the padded call would walk the later tiles as wholly masked
+// ones, which add exact zeros (see kCausal), so O, LSE and the keep words at rows below n_q are bitwise those of that
+// call.  In the last tile the keys at or past n_k (rows of the next sequence, or TMA zero fill past N_k) get -inf by
+// assignment and their V rows are zeroed, as in the KV-cache mode.  A sequence with n_k = 0 walks tile 0 wholly masked
+// (Q arrives with the first tile), so its rows get O = 0 and LSE = -inf.  Only rows below n_q are stored.  Causal
+// composes (its diagonal is per sequence, with the keys the queries' own rows); logits mode does not.
 template <typename T, int DP, bool kLogits, bool kCausal, bool kKVCache, bool kVarlen = false>
 __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
@@ -121,13 +123,17 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   const int q_tile = (kCausal || kKVCache) ? (int)(gridDim.x - 1 - blockIdx.x) : (int)blockIdx.x;
   const int q0 = q_tile * kBlockM, h = blockIdx.y, b = blockIdx.z;
   const int hk = h / p.kv_group;   // key / value head of query head h (fmha_api.h)
-  // varlen: the sequence's first packed row and length; its rows are addressed as batch 0 of the B = 1 maps
-  int vl_s = 0, vl_n = 0;
+  // varlen: the sequence's first packed query row and query count, and its first packed key row and key count; its
+  // rows are addressed as batch 0 of the B = 1 maps
+  int vl_s = 0, vl_n = 0, vk_s = 0, vk_n = 0;
   if constexpr (kVarlen) {
     const int2 sn = fmha_varlen_seq(p.cu_seqlens, b, p.Lq, p.packed_rows);
     vl_s = sn.x;
     vl_n = sn.y;
     if (q0 >= vl_n) return;
+    const int2 sk = fmha_varlen_seq(p.cu_seqlens_k, b, p.Lk, p.packed_rows_k);
+    vk_s = sk.x;
+    vk_n = sk.y;
   }
   const int tb = kVarlen ? 0 : b;   // batch coordinate of the q / k / v maps
   const int row_lim = kVarlen ? vl_n : p.Lq;   // rows stored
@@ -143,8 +149,9 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     kv_n = min(kv_p + p.Lq, p.kv_cap);
     kv_lim = min(kv_n, kv_p + q0 + 1);
   }
-  // causal: key tiles 0 .. (q0 + 63) / kBlockN hold a key visible to one of the rows q0 .. q0 + 63
-  const int n_key_walk = kVarlen ? (vl_n + kBlockN - 1) / kBlockN : n_key_tiles;
+  // causal: key tiles 0 .. (q0 + 63) / kBlockN hold a key visible to one of the rows q0 .. q0 + 63.  varlen: a
+  // sequence without keys still walks one wholly masked tile, which loads Q and gives O = 0, LSE = -inf
+  const int n_key_walk = kVarlen ? max(1, (vk_n + kBlockN - 1) / kBlockN) : n_key_tiles;
   const int n_tiles = kCausal ? min(n_key_walk, (q0 + kBlockM - 1) / kBlockN + 1)
                       : kKVCache ? max(1, (min(kv_n, kv_p + q0 + kBlockM) + kBlockN - 1) / kBlockN)
                                  : n_key_walk;
@@ -157,9 +164,9 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
       if (j == 0) tma_load_4d(smem_base + C::kSmemQ + x * C::kQBox, &p.sw_q, 64 * x, h, vl_s + q0, tb, bar);
-      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, vl_s + j * kBlockN, tb,
+      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, vk_s + j * kBlockN, tb,
                   bar);
-      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, vl_s + j * kBlockN, tb,
+      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, vk_s + j * kBlockN, tb,
                   bar);
     }
     if (has_bias) {   // 64 rows x kBlockN keys = kBlockN / 64 boxes of 64 keys
@@ -206,7 +213,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     if (tid < kBlockN) {
       const int key = key0 + tid;
       // KV-cache mode: kpm_cols >= kv_cap >= kv_n, so the key mask is read only below kv_n
-      masked = key >= (kKVCache ? kv_n : kVarlen ? vl_n : p.Lk) || (kpm_row != nullptr && kpm_row[key] != 0);
+      masked = key >= (kKVCache ? kv_n : kVarlen ? vk_n : p.Lk) || (kpm_row != nullptr && kpm_row[key] != 0);
       kadd[st * kBlockN + tid] = masked ? -CUDART_INF_F : 0.f;
     }
     // barrier: every thread is done with tile j-1, so its stage may be refilled with tile j+1
@@ -215,7 +222,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     if (tid == 0 && j + 1 < n_tiles) load_tile(j + 1);
     mbar_wait(bar0 + 8u * st, (uint32_t)((j >> 1) & 1));
     if constexpr (kKVCache || kVarlen) {
-      const int v_lim = kKVCache ? kv_n : vl_n;
+      const int v_lim = kKVCache ? kv_n : vk_n;
       if (key0 + kBlockN > v_lim) {   // zero the V rows at or past n_b: whole 128-byte rows of every column box
         const int r0 = max(v_lim - key0, 0), chunks = (kBlockN - r0) * 8;
         uint8_t* sv = smem + C::kSmemV + st * C::kKVStage;
@@ -282,10 +289,10 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
         }
       }
       if constexpr (kVarlen) {   // the last tile: keys of the next sequence, assigned (their bias is not this one's)
-        if (key0 + kBlockN > vl_n) {
+        if (key0 + kBlockN > vk_n) {
           const int key = key0 + col;
-          if (key >= vl_n) s[4 * i + 0] = s[4 * i + 2] = -CUDART_INF_F;
-          if (key + 1 >= vl_n) s[4 * i + 1] = s[4 * i + 3] = -CUDART_INF_F;
+          if (key >= vk_n) s[4 * i + 0] = s[4 * i + 2] = -CUDART_INF_F;
+          if (key + 1 >= vk_n) s[4 * i + 1] = s[4 * i + 3] = -CUDART_INF_F;
         }
       }
       if constexpr (kLogits) {   // the same swizzled positions as the bias elements above

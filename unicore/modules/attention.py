@@ -38,6 +38,11 @@ with sequence ``b`` on rows ``cu_seqlens[b] .. cu_seqlens[b + 1] - 1`` (int ``[B
 on pad rows, and the attention runs in the varlen mode of the fused kernels (``ops.fused_attention_varlen``; the
 varlen reference elsewhere).  ``attn_bias`` is ``[1|B, H, max_seqlen, max_seqlen]`` (each sequence reads its top-left
 block); rotary positions restart at 0 in every sequence.  No key padding mask, logits, probabilities or cache.
+``CrossMultiheadAttention`` takes a packed query ``[N_q, E]`` (``cu_seqlens`` / ``max_seqlen``) with packed keys and
+values ``[N_k, E]`` (``encoder_cu_seqlens`` / ``encoder_max_seqlen``, the same B sequences) and returns ``[N_q, E]``:
+query ``i`` of sequence ``b`` sees the keys of source sequence ``b`` only, in the varlen mode of the fused kernels with
+separate key sequences.  ``attn_bias`` is then ``[B*H | B | H, max_seqlen, encoder_max_seqlen]``; a sequence without
+source rows gives 0.  No key padding mask or cache.
 
 ``DecoderCache`` holds what incremental decoding keeps between steps: per layer the self-attention keys and values
 ``[B, C, H_kv, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.  A step may
@@ -266,12 +271,18 @@ class CrossMultiheadAttention(nn.Module):
         self.v_proj = nn.Linear(embed_dim, kv_dim, bias=bias)
         self.out_proj = nn.Linear(embed_dim, embed_dim, bias=bias)
 
-    def attend(self, query, key, value, key_padding_mask=None, attn_bias=None, cache=None):
+    def attend(self, query, key, value, key_padding_mask=None, attn_bias=None, cache=None, cu_seqlens=None,
+               max_seqlen=None, encoder_cu_seqlens=None, encoder_max_seqlen=None):
         """Everything up to (not including) ``out_proj``.
 
         ``cache`` (a ``LayerKVCache``): the projected keys and values are computed once, on the prefill, and kept in
         it; a decoding step (``query [B, T, E]``, ``key`` / ``value`` unused) attends to them with
-        ``ops.attention_with_kv_cache``, ``attn_bias`` holding the rows of the T new queries."""
+        ``ops.attention_with_kv_cache``, ``attn_bias`` holding the rows of the T new queries.
+        ``cu_seqlens`` / ``max_seqlen`` and ``encoder_cu_seqlens`` / ``encoder_max_seqlen``: packed sequences, ``query
+        [N_q, E]`` and ``key`` / ``value`` ``[N_k, E]`` -> ``o [N_q, E]`` (see the module docstring)."""
+        if cu_seqlens is not None or encoder_cu_seqlens is not None:
+            return self._attend_packed(query, key, value, key_padding_mask, attn_bias, cache, cu_seqlens, max_seqlen,
+                                       encoder_cu_seqlens, encoder_max_seqlen)
         bsz, tgt_len, embed_dim = query.size()
         if embed_dim != self.embed_dim:
             raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
@@ -302,6 +313,33 @@ class CrossMultiheadAttention(nn.Module):
         o, _, _ = _materialised_attention(qh, kh, vh, key_padding_mask, bias4, self.dropout, self.training, False)
         return o
 
+    def _attend_packed(self, query, key, value, key_padding_mask, attn_bias, cache, cu_seqlens, max_seqlen,
+                       encoder_cu_seqlens, encoder_max_seqlen):
+        if cu_seqlens is None or encoder_cu_seqlens is None:
+            raise ValueError("packed cross-attention takes a packed query (cu_seqlens) and packed keys / values "
+                             "(encoder_cu_seqlens) together")
+        if key_padding_mask is not None or cache is not None:
+            raise ValueError("packed sequences (cu_seqlens) take neither a key padding mask nor a cache")
+        if max_seqlen is None or encoder_max_seqlen is None:
+            raise ValueError("cu_seqlens / encoder_cu_seqlens need max_seqlen / encoder_max_seqlen, host bounds on "
+                             "the lengths")
+        if encoder_cu_seqlens.dim() != 1 or encoder_cu_seqlens.numel() != cu_seqlens.numel():
+            raise ValueError("encoder_cu_seqlens must describe the B = {} sequences of cu_seqlens, not {}".format(
+                cu_seqlens.numel() - 1, tuple(encoder_cu_seqlens.shape)))
+        total, embed_dim = query.size()
+        if embed_dim != self.embed_dim:
+            raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
+        if key.dim() != 2 or value.dim() != 2:
+            raise ValueError("packed cross-attention takes key / value [N_k, E]")
+        H, H_kv, D = self.num_heads, self.num_kv_heads, self.head_dim
+        q = self.q_proj(query).view(total, H, D)
+        k = self.k_proj(key).view(key.size(0), H_kv, D)
+        v = self.v_proj(value).view(value.size(0), H_kv, D)
+        bias4 = _bias_as_4d(attn_bias, cu_seqlens.numel() - 1, H, max_seqlen, encoder_max_seqlen)
+        o = _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias4, self.dropout, self.training, self.scaling,
+                                    False, cu_seqlens_k=encoder_cu_seqlens, max_seqlen_k=encoder_max_seqlen)
+        return o.reshape(total, embed_dim)
+
     def forward(
         self,
         query,
@@ -309,8 +347,14 @@ class CrossMultiheadAttention(nn.Module):
         value,
         key_padding_mask: Optional[Tensor] = None,
         attn_bias: Optional[Tensor] = None,
+        cu_seqlens: Optional[Tensor] = None,
+        max_seqlen: Optional[int] = None,
+        encoder_cu_seqlens: Optional[Tensor] = None,
+        encoder_max_seqlen: Optional[int] = None,
     ) -> Tensor:
-        return self.out_proj(self.attend(query, key, value, key_padding_mask, attn_bias))
+        return self.out_proj(self.attend(query, key, value, key_padding_mask, attn_bias, cu_seqlens=cu_seqlens,
+                                         max_seqlen=max_seqlen, encoder_cu_seqlens=encoder_cu_seqlens,
+                                         encoder_max_seqlen=encoder_max_seqlen))
 
 
 def _same_layout(a: Tensor, b: Tensor) -> bool:

@@ -26,7 +26,10 @@ after every layer, so all layers see the same positions.
 ``TransformerEncoder`` and its layers also take packed sequences: ``emb [N, E]`` with ``cu_seqlens`` (int ``[B + 1]`` on
 the device) and ``max_seqlen`` (a host bound on the lengths) instead of a padded batch and its padding mask.  Every
 token-wise kernel then runs on the N real tokens only, the relative-position bias is built at ``max_seqlen``, and the
-attention runs in the varlen mode of the fused kernels; the output is packed ``[N, E]``.
+attention runs in the varlen mode of the fused kernels; the output is packed ``[N, E]``.  ``TransformerDecoder`` takes
+packed targets the same way, decoder-only or with a packed ``encoder_out [N_k, E]`` described by
+``encoder_cu_seqlens`` / ``encoder_max_seqlen``: its self-attention is causal per sequence and its encoder attention
+sees each target sequence's own source rows (the varlen kernels with separate key sequences).
 """
 import math
 from typing import Optional
@@ -120,6 +123,10 @@ class _BlockMixin:
         packed = {} if kw.get("cu_seqlens") is None else {"cu_seqlens": kw["cu_seqlens"], "max_seqlen": kw["max_seqlen"]}
         kw.pop("cu_seqlens", None)
         kw.pop("max_seqlen", None)
+        if kw.get("encoder_cu_seqlens") is not None:   # packed keys / values of the encoder attention
+            packed.update(encoder_cu_seqlens=kw["encoder_cu_seqlens"], encoder_max_seqlen=kw["encoder_max_seqlen"])
+        kw.pop("encoder_cu_seqlens", None)
+        kw.pop("encoder_max_seqlen", None)
         h = attn_in if self.post_ln else norm(attn_in)
         extra = None
         if isinstance(attn_module, SelfMultiheadAttention):
@@ -129,7 +136,7 @@ class _BlockMixin:
                 extra = (logits, probs)
         else:
             o = attn_module.attend(h, kw["key"], kw["value"], kw.get("key_padding_mask"), kw.get("attn_bias"),
-                                   cache=cache)
+                                   cache=cache, **packed)
         proj = attn_module.out_proj
         if self.post_ln and self._fused_ok(o):
             # out_proj bias + dropout + residual + LayerNorm in one pass over the GEMM output
@@ -267,20 +274,28 @@ class TransformerDecoderLayer(nn.Module, _BlockMixin):
         encoder_padding_mask: Optional[torch.Tensor] = None,
         causal: bool = False,
         cache=None,
+        cu_seqlens: Optional[torch.Tensor] = None,
+        max_seqlen: Optional[int] = None,
+        encoder_cu_seqlens: Optional[torch.Tensor] = None,
+        encoder_max_seqlen: Optional[int] = None,
     ) -> torch.Tensor:
         """``causal`` masks future keys in the self-attention (key j > query i), without a mask tensor on the fused
         path; the encoder attention is unaffected.  ``cache``: this layer's ``LayerKVCache`` of a ``DecoderCache``
         (see ``TransformerDecoder.forward``); on a decoding step the encoder attention uses the encoder keys and values
-        it stored on the prefill, and ``encoder_out`` may be None."""
+        it stored on the prefill, and ``encoder_out`` may be None.  ``cu_seqlens`` / ``max_seqlen``: ``x`` is packed
+        ``[N, E]``; ``encoder_cu_seqlens`` / ``encoder_max_seqlen``: ``encoder_out`` is packed ``[N_k, E]`` (see the
+        module docstring)."""
         x, _ = self._attn_residual(
             self.self_attn, self.self_attn_layer_norm, x, x, key_padding_mask=padding_mask, attn_bias=attn_bias,
-            causal=causal, cache=cache,
+            causal=causal, cache=cache, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
         )
         if encoder_out is not None or (cache is not None and cache.stepping and cache.enc_k is not None):
             x, _ = self._attn_residual(
                 self.encoder_attn, self.encoder_attn_layer_norm, x, x,
                 key=encoder_out, value=encoder_out,
                 key_padding_mask=encoder_padding_mask, attn_bias=encoder_attn_bias, cache=cache,
+                cu_seqlens=cu_seqlens, max_seqlen=max_seqlen, encoder_cu_seqlens=encoder_cu_seqlens,
+                encoder_max_seqlen=encoder_max_seqlen,
             )
         return self._ffn_residual(x)
 
@@ -500,8 +515,14 @@ class TransformerDecoder(nn.Module, _StackMixin):
         attn_mask: Optional[torch.Tensor] = None,
         encoder_attn_mask: Optional[torch.Tensor] = None,
         cache: Optional[DecoderCache] = None,
+        cu_seqlens: Optional[torch.Tensor] = None,
+        max_seqlen: Optional[int] = None,
+        encoder_cu_seqlens: Optional[torch.Tensor] = None,
+        encoder_max_seqlen: Optional[int] = None,
     ) -> torch.Tensor:
-        """Without ``cache`` the whole sequence is decoded at once.  With a ``DecoderCache`` (``new_cache``):
+        """Without ``cache`` the whole sequence is decoded at once: ``emb [B, L, E]`` right-padded as ``padding_mask``
+        says, or packed ``emb [N, E]`` with ``cu_seqlens`` and ``max_seqlen`` (see ``_forward_packed``).  With a
+        ``DecoderCache`` (``new_cache``):
 
         * the first call (the prefill) takes the prompts ``emb [B, L, E]``, right-padded as ``padding_mask`` says, runs
           exactly the path above and stores every layer's keys / values of the L positions and its projected encoder
@@ -514,10 +535,51 @@ class TransformerDecoder(nn.Module, _StackMixin):
           rows of the new queries ``[B*H, T, S]``.  ``padding_mask`` and ``attn_mask`` are not supported on a step.
           ``cache.rewind`` drops tokens again.
         """
+        if cu_seqlens is not None or encoder_cu_seqlens is not None:
+            return self._forward_packed(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
+                                        encoder_attn_mask, cache, cu_seqlens, max_seqlen, encoder_cu_seqlens,
+                                        encoder_max_seqlen)
         if cache is not None:
             return self._forward_cached(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
                                         encoder_attn_mask, cache)
         return self._forward_prefix(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask)
+
+    def _forward_packed(self, emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask,
+                        cache, cu_seqlens, max_seqlen, encoder_cu_seqlens, encoder_max_seqlen):
+        """Packed target sequences ``emb [N, E]`` (``cu_seqlens`` int ``[B + 1]`` on the device, ``max_seqlen`` a host
+        bound on their lengths), and, for encoder-decoder use, a packed ``encoder_out [N_k, E]`` of the same B
+        sequences (``encoder_cu_seqlens``, ``encoder_max_seqlen``).  ``attn_mask`` is ``[B*H | B, max_seqlen,
+        max_seqlen]`` and ``encoder_attn_mask`` ``[B*H | B, max_seqlen, encoder_max_seqlen]``.  Without a mask of that
+        width, ``max_seqlen`` / ``encoder_max_seqlen`` are rounded up to a multiple of 8, which changes no result.
+        The self-attention is causal per sequence when ``auto_regressive``; every token-wise kernel runs on the real
+        rows only.  Returns packed ``[N, E]``.  No padding masks and no cache."""
+        if cu_seqlens is None:
+            raise ValueError("a packed encoder_out (encoder_cu_seqlens) needs a packed target (cu_seqlens)")
+        if max_seqlen is None:
+            raise ValueError("cu_seqlens needs max_seqlen, a host bound on the lengths")
+        if padding_mask is not None or encoder_padding_mask is not None:
+            raise ValueError("packed sequences (cu_seqlens) have no padding_mask or encoder_padding_mask")
+        if cache is not None:
+            raise ValueError("packed sequences (cu_seqlens) do not decode into a cache")
+        if (encoder_out is None) != (encoder_cu_seqlens is None):
+            raise ValueError("a packed target takes a packed encoder_out with encoder_cu_seqlens, or neither")
+        if encoder_cu_seqlens is not None:
+            if encoder_max_seqlen is None:
+                raise ValueError("encoder_cu_seqlens needs encoder_max_seqlen, a host bound on the source lengths")
+            if encoder_cu_seqlens.dim() != 1 or encoder_cu_seqlens.numel() != cu_seqlens.numel():
+                raise ValueError("encoder_cu_seqlens must describe the B = {} sequences of cu_seqlens, not {}".format(
+                    cu_seqlens.numel() - 1, tuple(encoder_cu_seqlens.shape)))
+            if encoder_attn_mask is None:
+                encoder_max_seqlen = int(encoder_max_seqlen) + (-int(encoder_max_seqlen) % 8)
+        x = self._embed_prologue(emb, None)   # no pad rows to zero
+        if attn_mask is None and encoder_attn_mask is None:
+            max_seqlen = int(max_seqlen) + (-int(max_seqlen) % 8)
+        attn_bias, _ = self._compose_bias(x, attn_mask, None, cu_seqlens.numel() - 1, max_seqlen)
+        for layer in self.layers:
+            x = layer(x, encoder_out=encoder_out, attn_bias=attn_bias, encoder_attn_bias=encoder_attn_mask,
+                      causal=self.auto_regressive, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
+                      encoder_cu_seqlens=encoder_cu_seqlens, encoder_max_seqlen=encoder_max_seqlen)
+        return x if self.final_layer_norm is None else self.final_layer_norm(x)
 
     def _forward_prefix(self, emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask,
                         cache=None):

@@ -274,28 +274,58 @@ def _varlen_index(cu_seqlens, max_seqlen, total):
     return rows, valid
 
 
-def attention_varlen_reference(q, k, v, cu_seqlens, max_seqlen, bias=None, dropout_p=0.0, training=True, scale=None,
-                               causal=False):
-    """Plain PyTorch implementation of ``fused_attention_varlen`` (CPU path, fallback and test oracle): the packed
-    rows are scattered to ``[B, max_seqlen]``, ``attention_reference`` runs with the length mask (key ``j`` of
-    sequence ``b`` hidden when ``j >= n_b``), and the real rows are gathered back.  Packed rows that belong to no
-    sequence give 0.  Differentiable in q, k, v and the bias.  Without a bias ``max_seqlen`` is rounded up to a multiple
-    of 8, as on the kernel path, so that both clamp a length to the same bound."""
-    N, H, D = q.shape
+def _varlen_keys(cu_seqlens, max_seqlen, bias, causal, cu_seqlens_k, max_seqlen_k):
+    """``(L, Lk)``: the kernels' query and key widths of a varlen call, after the checks its arguments share.  Without
+    ``cu_seqlens_k`` the keys are the queries' own rows and ``Lk = L``; with it ``max_seqlen_k`` bounds the key
+    lengths, rounded up to a multiple of 8 without a bias as ``max_seqlen`` is."""
     L = _varlen_max_seqlen(max_seqlen, bias)
+    if cu_seqlens_k is None:
+        if max_seqlen_k is not None:
+            raise ValueError("max_seqlen_k goes with cu_seqlens_k")
+        return L, L
+    if causal:
+        raise ValueError("causal attention is not defined with separate key sequences (cu_seqlens_k)")
+    if max_seqlen_k is None:
+        raise ValueError("cu_seqlens_k needs max_seqlen_k, a host bound on the key lengths")
+    if cu_seqlens_k.dim() != 1 or cu_seqlens_k.numel() != cu_seqlens.numel():
+        raise ValueError("cu_seqlens_k must describe the B = {} sequences of cu_seqlens, not {}".format(
+            cu_seqlens.numel() - 1, tuple(cu_seqlens_k.shape)))
+    return L, _varlen_max_seqlen(max_seqlen_k, bias)
+
+
+def attention_varlen_reference(q, k, v, cu_seqlens, max_seqlen, bias=None, dropout_p=0.0, training=True, scale=None,
+                               causal=False, cu_seqlens_k=None, max_seqlen_k=None):
+    """Plain PyTorch implementation of ``fused_attention_varlen`` (CPU path, fallback and test oracle): the packed
+    rows are scattered to ``[B, max_seqlen]`` (k / v to ``[B, max_seqlen_k]`` by ``cu_seqlens_k`` when given),
+    ``attention_reference`` runs with the length mask (key ``j`` of sequence ``b`` hidden when ``j >= n_k``), and the
+    real rows are gathered back.  Packed rows that belong to no sequence give 0, and so do the rows of a sequence
+    without keys, with zero gradients.  Differentiable in q, k, v and the bias.  Without a bias ``max_seqlen`` (and
+    ``max_seqlen_k``) is rounded up to a multiple of 8, as on the kernel path, so that both clamp a length to the same
+    bound."""
+    N, H, D = q.shape
+    L, Lk = _varlen_keys(cu_seqlens, max_seqlen, bias, causal, cu_seqlens_k, max_seqlen_k)
     rows, valid = _varlen_index(cu_seqlens.to(q.device), L, N)
+    if cu_seqlens_k is None:
+        rows_k, valid_k = rows, valid
+    else:
+        rows_k, valid_k = _varlen_index(cu_seqlens_k.to(q.device), Lk, k.shape[0])
     B = rows.shape[0]
 
-    def scatter(x):
+    def scatter(x, rows, valid):
         return torch.where(valid[:, :, None, None], x[rows], torch.zeros((), dtype=x.dtype, device=x.device))
 
-    # the length mask as an additive bias; the rows past n_b see every key, so that they stay finite (they are dropped)
-    hide = (torch.arange(L, device=q.device)[None, None, :] >= valid.sum(1)[:, None, None]) & valid[:, :, None]
-    mask = torch.zeros(B, 1, L, L, dtype=q.dtype, device=q.device).masked_fill(hide[:, None], float("-inf"))
+    # the length mask as an additive bias.  The rows past n_q, and the rows of a sequence without keys, see every
+    # (padded) key, so that they stay finite: the former are dropped, the latter multiplied by 0
+    n_k = valid_k.sum(1)
+    has_keys = n_k > 0
+    hide = (torch.arange(Lk, device=q.device)[None, None, :] >= n_k[:, None, None]) \
+        & (valid & has_keys[:, None])[:, :, None]
+    mask = torch.zeros(B, 1, L, Lk, dtype=q.dtype, device=q.device).masked_fill(hide[:, None], float("-inf"))
     bias = mask if bias is None else bias.to(q.dtype) + mask
-    out = attention_reference(scatter(q), scatter(k), scatter(v), bias, None, dropout_p, training, scale,
-                              causal=causal)
-    # gather back: the rows of no sequence (and the positions past n_b) write into a dropped row N
+    out = attention_reference(scatter(q, rows, valid), scatter(k, rows_k, valid_k), scatter(v, rows_k, valid_k), bias,
+                              None, dropout_p, training, scale, causal=causal)
+    out = out * has_keys[:, None, None, None].to(out.dtype)
+    # gather back: the rows of no sequence (and the positions past n_q) write into a dropped row N
     dest = torch.where(valid, rows, torch.full_like(rows, N)).reshape(-1)
     packed = torch.zeros(N + 1, H, D, dtype=out.dtype, device=out.device).index_put((dest,), out.reshape(-1, H, D))
     return packed[:N]
@@ -304,29 +334,33 @@ def attention_varlen_reference(q, k, v, cu_seqlens, max_seqlen, bias=None, dropo
 class _FusedVarlenAttentionFn(torch.autograd.Function):
     """The varlen kernels' forward and backward (``_C.varlen``), shaped as ``_FusedAttentionFn``: ``qkv`` None or
     the contiguous ``[N, H + 2 * H_kv, D]`` projection that q, k and v are (detached) views of, which then gets one
-    packed gradient."""
+    packed gradient.  ``cu_seqlens_k`` None (self-attention, ``max_seqlen_k`` 0) or the key sequences'
+    description."""
 
     @staticmethod
-    def forward(ctx, qkv, q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal):
+    def forward(ctx, qkv, q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal, cu_seqlens_k,
+                max_seqlen_k):
         p = float(dropout_p) if training else 0.0
         out, lse, bits = native().varlen.fmha_varlen_fwd(q, k, v, cu_seqlens, max_seqlen, bias, p, float(scale),
-                                                         causal=causal)
+                                                         causal=causal, cu_seqlens_k=cu_seqlens_k,
+                                                         max_seqlen_k=max_seqlen_k)
         ctx.p = p
         ctx.causal = causal
         ctx.scale = float(scale)
         ctx.max_seqlen = max_seqlen
+        ctx.max_seqlen_k = max_seqlen_k
         ctx.need_dbias = bias is not None and bias.requires_grad
         ctx.packed_shape = None if qkv is None else qkv.shape
-        ctx.save_for_backward(q, k, v, out, lse, cu_seqlens, bias, bits)
+        ctx.save_for_backward(q, k, v, out, lse, cu_seqlens, bias, bits, cu_seqlens_k)
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        q, k, v, out, lse, cu_seqlens, bias, bits = ctx.saved_tensors
+        q, k, v, out, lse, cu_seqlens, bias, bits, cu_seqlens_k = ctx.saved_tensors
         packed = ctx.packed_shape is not None
         dq, dk, dv, dbias = native().varlen.fmha_varlen_bwd(
             dout.contiguous(), q, k, v, out, lse, cu_seqlens, ctx.max_seqlen, bias, ctx.p, ctx.scale, bits,
-            ctx.need_dbias, packed, causal=ctx.causal
+            ctx.need_dbias, packed, causal=ctx.causal, cu_seqlens_k=cu_seqlens_k, max_seqlen_k=ctx.max_seqlen_k
         )
         if dbias is not None and dbias.dtype != bias.dtype:
             dbias = dbias.to(bias.dtype)
@@ -334,7 +368,7 @@ class _FusedVarlenAttentionFn(torch.autograd.Function):
             dqkv, dq, dk, dv = dq._base.view(ctx.packed_shape), None, None, None
         else:
             dqkv = None
-        return dqkv, dq, dk, dv, None, None, dbias, None, None, None, None
+        return dqkv, dq, dk, dv, None, None, dbias, None, None, None, None, None, None
 
 
 def _varlen_max_seqlen(max_seqlen, bias):
@@ -344,13 +378,18 @@ def _varlen_max_seqlen(max_seqlen, bias):
     return L if bias is not None else L + (-L % 8)
 
 
-def fused_attention_varlen_supported(q, k, v, cu_seqlens, max_seqlen, bias=None) -> bool:
-    if not use_native(q, k, v, cu_seqlens, bias) or not hasattr(native(), "varlen"):
+def fused_attention_varlen_supported(q, k, v, cu_seqlens, max_seqlen, bias=None, cu_seqlens_k=None,
+                                     max_seqlen_k=None) -> bool:
+    if not use_native(q, k, v, cu_seqlens, bias, cu_seqlens_k) or not hasattr(native(), "varlen"):
         return False
     if q.dim() != 3 or k.dim() != 3 or v.dim() != 3 or q.shape[0] < 1 or cu_seqlens.dim() != 1 \
             or cu_seqlens.numel() < 2:
         return False
-    if k.shape[0] != q.shape[0] or v.shape[0] != q.shape[0]:
+    if cu_seqlens_k is None:
+        if k.shape[0] != q.shape[0] or v.shape[0] != q.shape[0] or max_seqlen_k is not None:
+            return False
+    elif k.shape[0] < 1 or v.shape[0] != k.shape[0] or cu_seqlens_k.dim() != 1 \
+            or cu_seqlens_k.numel() != cu_seqlens.numel() or max_seqlen_k is None:
         return False
     if not _kernel_tensors(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0)):
         return False
@@ -359,36 +398,42 @@ def fused_attention_varlen_supported(q, k, v, cu_seqlens, max_seqlen, bias=None)
     if k.shape[1] != v.shape[1] or k.shape[1] < 1 or q.shape[1] % k.shape[1] != 0:
         return False
     L = _varlen_max_seqlen(max_seqlen, bias)
-    if L < 1 or L % 8 != 0:
+    Lk = L if cu_seqlens_k is None else _varlen_max_seqlen(max_seqlen_k, bias)
+    if L < 1 or L % 8 != 0 or Lk < 1 or Lk % 8 != 0:
         return False
     if bias is not None:
         if bias.dim() != 4 or bias.shape[0] not in (1, cu_seqlens.numel() - 1) or bias.shape[1] != q.shape[1]:
             return False
-        if bias.shape[2] != L or bias.shape[3] != L or bias.dtype not in (q.dtype, torch.float32):
+        if bias.shape[2] != L or bias.shape[3] != Lk or bias.dtype not in (q.dtype, torch.float32):
             return False
     return True
 
 
-def _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal, qkv=None):
+def _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal, qkv=None,
+                            cu_seqlens_k=None, max_seqlen_k=None):
     """``fused_attention_varlen`` on q / k / v, which are the views of ``qkv`` when it is given: a contiguous ``qkv``
     then gets one packed gradient."""
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
-    if not fused_attention_varlen_supported(q, k, v, cu_seqlens, max_seqlen, bias):
-        return attention_varlen_reference(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal)
-    L = _varlen_max_seqlen(max_seqlen, bias)
+    L, Lk = _varlen_keys(cu_seqlens, max_seqlen, bias, causal, cu_seqlens_k, max_seqlen_k)
+    if not fused_attention_varlen_supported(q, k, v, cu_seqlens, max_seqlen, bias, cu_seqlens_k, max_seqlen_k):
+        return attention_varlen_reference(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal,
+                                          cu_seqlens_k, max_seqlen_k)
     cu_seqlens = cu_seqlens.to(torch.int32).contiguous()
+    if cu_seqlens_k is not None:
+        cu_seqlens_k = cu_seqlens_k.to(torch.int32).contiguous()
     if bias is not None:
         bias = bias.to(q.dtype).contiguous()
     if qkv is not None and qkv.is_contiguous():
         q, k, v = q.detach(), k.detach(), v.detach()   # autograd sees qkv alone
     else:
         qkv = None
-    return _FusedVarlenAttentionFn.apply(qkv, q, k, v, cu_seqlens, L, bias, dropout_p, training, scale, causal)
+    return _FusedVarlenAttentionFn.apply(qkv, q, k, v, cu_seqlens, L, bias, dropout_p, training, scale, causal,
+                                         cu_seqlens_k, 0 if cu_seqlens_k is None else Lk)
 
 
 def fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias=None, dropout_p=0.0, training=True, scale=None,
-                           causal=False):
+                           causal=False, cu_seqlens_k=None, max_seqlen_k=None):
     """Attention over packed variable-length sequences (no padding): q ``[N, H, D]``, k / v ``[N, H_kv, D]`` with
     ``H_kv`` dividing ``H``, the B sequences back to back; sequence ``b`` holds rows ``cu_seqlens[b] ..
     cu_seqlens[b + 1] - 1`` (int ``[B + 1]`` on the device, never read on the host).  ``max_seqlen``: a host bound
@@ -397,9 +442,16 @@ def fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias=None, dropout_p
     (the rule of the padded call), other widths run ``attention_varlen_reference``.
     ``causal`` masks key j > query i within each sequence.  Returns ``[N, H, D]``: at every real row the result of
     the padded call with ``key_padding_mask = (j >= len_b)``.  Lengths are clamped to ``[0, max_seqlen]`` and the
-    starts to ``[0, N]``."""
+    starts to ``[0, N]``.
+
+    Cross-attention: ``cu_seqlens_k`` (int ``[B + 1]`` on the device, the same B) and ``max_seqlen_k`` describe
+    separate key sequences, k / v ``[N_k, H_kv, D]`` (flash-attention's ``cu_seqlens_q`` / ``cu_seqlens_k``); the bias
+    is then ``[1|B, H, max_seqlen, max_seqlen_k]`` and ``max_seqlen_k`` is rounded up like ``max_seqlen``.  Query i of
+    sequence b sees its keys j < n_k; a sequence without keys gives 0 at its rows, with zero gradients.  Not with
+    ``causal`` (``ValueError``)."""
     kv_group(q.shape[1], k.unsqueeze(0), v.unsqueeze(0))
-    return _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal)
+    return _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias, dropout_p, training, scale, causal,
+                                   cu_seqlens_k=cu_seqlens_k, max_seqlen_k=max_seqlen_k)
 
 
 def fused_attention_varlen_qkvpacked(qkv, cu_seqlens, max_seqlen, bias=None, dropout_p=0.0, training=True,
