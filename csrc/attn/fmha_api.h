@@ -75,6 +75,11 @@ struct FmhaFwdParams {
   // Causal is defined only for cu_seqlens_k == cu_seqlens (the bindings refuse it otherwise).
   const int* cu_seqlens_k;   // [B + 1] int32 on the device
   int packed_rows_k;         // N_k
+  // Packed chunks into a cache (fmha_kvcache_varlen_fwd): varlen and kvcache both set.  q / O are packed [N, H, D] as
+  // in varlen mode, with {s_b, T_b} = fmha_varlen_seq(cu_seqlens, b, Lq, N) and Lq = max_seqlen; k / v are the
+  // [B, C, H_kv, D] caches of the KV-cache mode (Lk = C).  Query i < T_b of sequence b sees key j iff j < n_b and
+  // j <= p_b + i, with p_b as above and n_b = min(p_b + T_b, kv_cap); the bias is [bias_batch * H, Lq, Lb] (row i for
+  // query i) and the key mask [B, kpm_cols].  cu_seqlens_k is not read.  No dropout, lse null.
 };
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
 
@@ -93,7 +98,9 @@ __device__ __forceinline__ int2 fmha_varlen_seq(const int* cu_seqlens, int b, in
 // Copies the T new rows of k_new / v_new [B, T, H, D] into rows p_b + i of the [B, C, H, D] caches, p_b =
 // clamp(seqlens[b], 0, C), bitwise, with 16-byte vectors; rows at or past C are skipped.  H is the caches' head count
 // (H_kv under grouped-query attention).  It runs as a launch of its own before the KV-cache forward, which reads those
-// rows from every query tile of a (b, h).
+// rows from every query tile of a (b, h).  Packed chunks (cu_seqlens set): k_new / v_new are [N, H, D] (batch strides
+// 0), T is max_seqlen, and sequence b copies its T_b rows s_b + i, {s_b, T_b} = fmha_varlen_seq(cu_seqlens, b, T, N),
+// into rows p_b + i.
 struct KvCacheAppendParams {
   const void* k_new;       // [B, T, H, D] via strides (elements)
   const void* v_new;
@@ -103,6 +110,8 @@ struct KvCacheAppendParams {
   long long kn_sb, kn_sl, kn_sh, vn_sb, vn_sl, vn_sh;
   long long kc_sb, kc_sl, kc_sh, vc_sb, vc_sl, vc_sh;
   int B, T, H, D, C;
+  const int* cu_seqlens;   // [B + 1] int32 on the device, or null (padded [B, T, H, D] rows); appended so that no
+  int packed_rows;         // earlier field moves.  packed_rows = N
 };
 void launch_kv_cache_append(const KvCacheAppendParams& p, cudaStream_t stream);
 

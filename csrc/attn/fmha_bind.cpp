@@ -63,8 +63,10 @@ void fill_common(ub::FmhaFwdParams& p, const Tensor& q, const Tensor& k, const T
   const int q_box_rows = forward ? ub::kFwdQBoxRows : ub::kBwdBoxRows;
   const int kv_box_rows = forward ? ub::fmha_fwd_kv_box_rows(p.D) : ub::kBwdBoxRows;
   bool ok = ub::make_head_tile_map_sw128(&p.sw_q, p.q, bf16, p.B, p.Lq, p.H, p.D, p.q_sb, p.q_sl, p.q_sh, q_box_rows);
-  ok = ok && ub::make_head_tile_map_sw128(&p.sw_k, p.k, bf16, p.B, p.Lk, H_kv, p.D, p.k_sb, p.k_sl, p.k_sh, kv_box_rows);
-  ok = ok && ub::make_head_tile_map_sw128(&p.sw_v, p.v, bf16, p.B, p.Lk, H_kv, p.D, p.v_sb, p.v_sl, p.v_sh, kv_box_rows);
+  // k / v have the batch of q, except the caches of packed chunks (fmha_kvcache_varlen_fwd), whose q is one batch
+  const int B_kv = (int)k.size(0);
+  ok = ok && ub::make_head_tile_map_sw128(&p.sw_k, p.k, bf16, B_kv, p.Lk, H_kv, p.D, p.k_sb, p.k_sl, p.k_sh, kv_box_rows);
+  ok = ok && ub::make_head_tile_map_sw128(&p.sw_v, p.v, bf16, B_kv, p.Lk, H_kv, p.D, p.v_sb, p.v_sl, p.v_sh, kv_box_rows);
   if (p.bias != nullptr) ok = ok && ub::make_bias_tile_map_sw128(&p.sw_bias, p.bias, bf16, p.bias_batch * p.H, p.Lq, p.Lk);
   TORCH_CHECK(ok, "cuTensorMapEncodeTiled failed for the attention operands");
 }
@@ -206,18 +208,25 @@ std::tuple<Tensor, Tensor, Tensor, OptTensor> fmha_bwd(const Tensor& dout, const
   return {dq, dk, dv, dbias};
 }
 
-// q / k_cache / v_cache / k_new / v_new: [B, L, heads, D] with the B, D and dtype of q, read as 16-byte vectors
-void check_decode_operand(const Tensor& t, const char* name, const Tensor& q, int64_t L, int64_t heads) {
-  check_operand(t, name, q.device(), {q.scalar_type()}, {q.size(0), L, heads, q.size(3)}, kAligned);
-  TORCH_CHECK(t.stride(3) == 1 && t.stride(0) % 8 == 0 && t.stride(1) % 8 == 0 && t.stride(2) % 8 == 0, name,
-              " needs a contiguous last dim and strides that are multiples of 8 elements");
+// An operand of `sizes` (the last one D) with the dtype of q, read as 16-byte vectors: a contiguous last dim and
+// every other stride a multiple of 8 elements
+void check_row_operand(const Tensor& t, const char* name, const Tensor& q, at::IntArrayRef sizes) {
+  check_operand(t, name, q.device(), {q.scalar_type()}, sizes, kAligned);
+  bool ok = t.stride(-1) == 1;
+  for (int64_t d = 0; d + 1 < t.dim(); ++d) ok = ok && t.stride(d) % 8 == 0;
+  TORCH_CHECK(ok, name, " needs a contiguous last dim and strides that are multiples of 8 elements");
 }
 
-// The value cache [B, C, H_kv, D] fixes the key / value head count H_kv, which must divide the H query heads of q
-// (grouped-query attention); k_cache, k_new and v_new are then checked against it.  Returns H_kv.
-int64_t check_cache_heads(const Tensor& q, const Tensor& v_cache) {
-  check_decode_operand(v_cache, "v_cache", q, kAnySize, kAnySize);
-  kv_group(q.size(2), v_cache.size(2), "v_cache");
+// q / k_cache / v_cache / k_new / v_new: [B, L, heads, D] with the B, D and dtype of q, read as 16-byte vectors
+void check_decode_operand(const Tensor& t, const char* name, const Tensor& q, int64_t L, int64_t heads) {
+  check_row_operand(t, name, q, {q.size(0), L, heads, q.size(3)});
+}
+
+// The value cache [B, C, H_kv, D] (D that of q, [..., H, D]) fixes the key / value head count H_kv, which must divide
+// the H query heads of q (grouped-query attention); k_cache, k_new and v_new are then checked against it.  Returns H_kv.
+int64_t check_cache_heads(const Tensor& q, int64_t B, const Tensor& v_cache) {
+  check_row_operand(v_cache, "v_cache", q, {B, kAnySize, kAnySize, q.size(-1)});
+  kv_group(q.size(-2), v_cache.size(2), "v_cache");
   return v_cache.size(2);
 }
 
@@ -234,7 +243,7 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   const int64_t B = q.size(0), H = q.size(2), D = q.size(3);
   TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
   check_decode_operand(q, "q", q, kAnySize, H);
-  const int64_t H_kv = check_cache_heads(q, v_cache);
+  const int64_t H_kv = check_cache_heads(q, B, v_cache);
   check_decode_operand(k_cache, "k_cache", q, kAnySize, H_kv);
   const int64_t C = k_cache.size(1);
   TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
@@ -314,29 +323,26 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   return out;
 }
 
-// A chunk of T >= 2 queries per sequence against a [B, C, H, D] key / value cache, in the KV-cache mode of the wgmma
-// forward (fmha_api.h).  With seqlens the T rows of k_new / v_new are first appended at rows seqlens[b] + i (a launch
-// of its own), and query i sees the keys j <= seqlens[b] + i; without seqlens every query sees all C rows.  max_len
-// is a host bound on seqlens, as in fmha_decode.  The bias is [1|B, H, T, Lb] with Lb % 8 == 0 (its TMA row stride).
-Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& seqlens,
-                        int64_t max_len, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
-                        const OptTensor& kpm, double scale) {
-  check_operand(q, "q", q.device(), k16Bit, any_shape(4), kAligned);
-  const int64_t B = q.size(0), T = q.size(1), H = q.size(2), D = q.size(3);
-  TORCH_CHECK(T >= 2, "fmha_kvcache_fwd takes chunks of T >= 2 queries (fmha_decode takes T = 1)");
-  TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
-  check_decode_operand(q, "q", q, kAnySize, H);
-  const int64_t H_kv = check_cache_heads(q, v_cache);
-  check_decode_operand(k_cache, "k_cache", q, kAnySize, H_kv);
+// The checks a chunk into a key / value cache shares in its padded (fmha_kvcache_fwd) and packed
+// (fmha_kvcache_varlen_fwd) forms, for B sequences of up to T new queries with the H heads and head dim D of q
+// ([..., H, D]): the [B, C, H_kv, D] caches (H_kv dividing H, one capacity C >= 1), k_new / v_new given together and
+// exactly when seqlens is, the host bound max_len + T <= C, a bias [1|B, H, T, Lb] with Lb % 8 == 0 (its TMA row
+// stride) and a bool key mask [B, Lk], each with a column for every key that can be visible.  k_new / v_new are the
+// caller's to check (their layout is the form's).  Returns {H_kv, kv_cap}.
+std::pair<int64_t, int64_t> check_cache_chunk(const Tensor& q, int64_t B, int64_t T, const Tensor& k_cache,
+                                              const Tensor& v_cache, const OptTensor& seqlens, int64_t max_len,
+                                              const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
+                                              const OptTensor& kpm) {
+  const int64_t H = q.size(-2);
+  TORCH_CHECK(ub::fmha_head_dim_supported(q.size(-1)),
+              "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
+  const int64_t H_kv = check_cache_heads(q, B, v_cache);
+  check_row_operand(k_cache, "k_cache", q, {B, kAnySize, H_kv, q.size(-1)});
   const int64_t C = k_cache.size(1);
   TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
   const bool append = has(k_new);
   TORCH_CHECK(append == has(v_new), "k_new and v_new go together");
   TORCH_CHECK(append == has(seqlens), "a chunk with seqlens appends k_new / v_new, and one without does not");
-  if (append) {
-    check_decode_operand(*k_new, "k_new", q, T, H_kv);
-    check_decode_operand(*v_new, "v_new", q, T, H_kv);
-  }
   check_operand(seqlens, "seqlens", q.device(), {at::kInt}, {B});
   TORCH_CHECK(max_len >= 0, "max_len must not be negative");
   const int64_t bound = append ? max_len + T : C;   // visible keys of any batch
@@ -349,11 +355,24 @@ Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   }
   check_operand(kpm, "key_padding_mask", q.device(), {at::kBool}, {B, kAnySize});
   TORCH_CHECK(!has(kpm) || kpm->size(1) >= bound, "key_padding_mask must have a column for every key that can be visible");
-  const c10::cuda::CUDAGuard guard(q.device());
+  int64_t cap = C;
+  if (has(bias)) cap = std::min<int64_t>(cap, bias->size(3));
+  if (has(kpm)) cap = std::min<int64_t>(cap, kpm->size(1));
+  return {H_kv, cap};
+}
+
+// Runs a chunk that check_cache_chunk accepted: q4 is [B', T, H, D] as the q map reads it (the padded chunk, or the
+// packed rows as the one batch of a [1, N, H, D] view) and out its result; k_new / v_new are appended first (a launch
+// of its own), from [B, T, H_kv, D] or, with cu_seqlens, from packed [N, H_kv, D] rows.
+void run_cache_chunk(const Tensor& q4, int64_t B, int64_t T, const Tensor& k_cache, const Tensor& v_cache,
+                     const OptTensor& seqlens, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
+                     const OptTensor& kpm, int64_t cap, double scale, const Tensor* cu_seqlens, Tensor& out) {
   ub::FmhaFwdParams p{};
-  // q / k / v as the forward takes them (K / V maps over the C cache rows); the bias has Lb columns, not C, so its
-  // map is made below
-  fill_common(p, q, k_cache, v_cache, std::nullopt, kpm, 0.0, scale, /*forward=*/true);
+  // q / k / v as the forward takes them (K / V maps over the C cache rows of the B caches); the bias has Lb columns,
+  // not C, so its map is made below
+  fill_common(p, q4, k_cache, v_cache, std::nullopt, kpm, 0.0, scale, /*forward=*/true);
+  p.B = (int)B;
+  p.Lq = (int)T;
   if (has(bias)) {
     p.bias = bias->data_ptr();
     p.bias_batch = (int)bias->size(0);
@@ -364,30 +383,88 @@ Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_
   p.kvcache = 1;
   p.seqlens = has(seqlens) ? seqlens->data_ptr<int>() : nullptr;
   p.kpm_cols = has(kpm) ? (int)kpm->size(1) : 0;
-  int64_t cap = C;
-  if (has(bias)) cap = std::min<int64_t>(cap, bias->size(3));
-  if (has(kpm)) cap = std::min<int64_t>(cap, kpm->size(1));
   p.kv_cap = (int)cap;
-  Tensor out = torch::empty({B, T, H, D}, q.options());
+  if (cu_seqlens != nullptr) {
+    p.varlen = 1;
+    p.cu_seqlens = cu_seqlens->data_ptr<int>();
+    p.packed_rows = (int)q4.size(1);
+  }
   p.out = out.data_ptr();
   p.lse = nullptr;
-  if (append) {
+  if (has(k_new)) {
+    const bool packed = cu_seqlens != nullptr;   // [N, H_kv, D] rows: no batch stride
     ub::KvCacheAppendParams a{};
     a.k_new = k_new->data_ptr();
     a.v_new = v_new->data_ptr();
     a.k_cache = k_cache.data_ptr();
     a.v_cache = v_cache.data_ptr();
     a.seqlens = p.seqlens;
-    a.kn_sb = k_new->stride(0); a.kn_sl = k_new->stride(1); a.kn_sh = k_new->stride(2);
-    a.vn_sb = v_new->stride(0); a.vn_sl = v_new->stride(1); a.vn_sh = v_new->stride(2);
+    a.kn_sb = packed ? 0 : k_new->stride(0); a.kn_sl = k_new->stride(packed ? 0 : 1); a.kn_sh = k_new->stride(-2);
+    a.vn_sb = packed ? 0 : v_new->stride(0); a.vn_sl = v_new->stride(packed ? 0 : 1); a.vn_sh = v_new->stride(-2);
     a.kc_sb = p.k_sb; a.kc_sl = p.k_sl; a.kc_sh = p.k_sh;
     a.vc_sb = p.v_sb; a.vc_sl = p.v_sl; a.vc_sh = p.v_sh;
-    a.B = p.B; a.T = p.Lq; a.H = (int)H_kv; a.D = p.D; a.C = p.Lk;
+    a.B = p.B; a.T = p.Lq; a.H = (int)k_cache.size(2); a.D = p.D; a.C = p.Lk;
+    a.cu_seqlens = p.cu_seqlens;
+    a.packed_rows = p.packed_rows;
     ub::launch_kv_cache_append(a, cur_stream());
     check_launch("kv_cache_append");
   }
   ub::launch_fmha_fwd(p, cur_stream());
+}
+
+// A chunk of T >= 2 queries per sequence against a [B, C, H, D] key / value cache, in the KV-cache mode of the wgmma
+// forward (fmha_api.h).  With seqlens the T rows of k_new / v_new are first appended at rows seqlens[b] + i (a launch
+// of its own), and query i sees the keys j <= seqlens[b] + i; without seqlens every query sees all C rows.  max_len
+// is a host bound on seqlens, as in fmha_decode.  The bias is [1|B, H, T, Lb] with Lb % 8 == 0 (its TMA row stride).
+Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& seqlens,
+                        int64_t max_len, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
+                        const OptTensor& kpm, double scale) {
+  check_operand(q, "q", q.device(), k16Bit, any_shape(4), kAligned);
+  const int64_t B = q.size(0), T = q.size(1), H = q.size(2), D = q.size(3);
+  TORCH_CHECK(T >= 2, "fmha_kvcache_fwd takes chunks of T >= 2 queries (fmha_decode takes T = 1)");
+  check_decode_operand(q, "q", q, kAnySize, H);
+  const auto [H_kv, cap] = check_cache_chunk(q, B, T, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias, kpm);
+  if (has(k_new)) {
+    check_decode_operand(*k_new, "k_new", q, T, H_kv);
+    check_decode_operand(*v_new, "v_new", q, T, H_kv);
+  }
+  const c10::cuda::CUDAGuard guard(q.device());
+  Tensor out = torch::empty({B, T, H, D}, q.options());
+  run_cache_chunk(q, B, T, k_cache, v_cache, seqlens, k_new, v_new, bias, kpm, cap, scale, nullptr, out);
   check_launch("fmha_kvcache_fwd");
+  return out;
+}
+
+// Packed chunks into a [B, C, H_kv, D] key / value cache: q [N, H, D] holds B sequences back to back, sequence b's
+// T_b new queries on rows s_b .. s_b + T_b - 1 with {s_b, T_b} clamped from cu_seqlens (int32 [B + 1] on the device)
+// as in the varlen mode (fmha_api.h), and max_seqlen a host bound on T_b (any value >= 1: the KV-cache mode takes
+// any T).  With seqlens the rows of k_new / v_new [N, H_kv, D] are first appended at rows seqlens[b] + i, i < T_b
+// (rows at or past C are skipped), and query i sees the keys j <= seqlens[b] + i; without seqlens every query sees
+// all C rows.  max_len is a host bound on seqlens.  The bias is [1|B, H, max_seqlen, Lb] (row i for query i of every
+// sequence) with Lb % 8 == 0, the key mask [B, Lk].  Returns [N, H, D]; rows of no sequence are not written.
+Tensor fmha_kvcache_varlen_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cu_seqlens,
+                               int64_t max_seqlen, const OptTensor& seqlens, int64_t max_len, const OptTensor& k_new,
+                               const OptTensor& v_new, const OptTensor& bias, const OptTensor& kpm, double scale) {
+  check_operand(q, "q", q.device(), k16Bit, any_shape(3), kAligned);
+  const int64_t N = q.size(0), H = q.size(1), D = q.size(2);
+  check_row_operand(q, "q", q, {kAnySize, H, D});
+  TORCH_CHECK(N >= 1, "q must have N >= 1 packed rows");
+  TORCH_CHECK(q.stride(1) == D, "q head stride must be head_dim");   // (head, 16-byte chunk) is one TMA dimension
+  check_operand(cu_seqlens, "cu_seqlens", q.device(), {at::kInt}, {kAnySize});
+  const int64_t B = cu_seqlens.size(0) - 1;
+  TORCH_CHECK(B >= 1, "cu_seqlens must have B + 1 >= 2 entries");
+  TORCH_CHECK(max_seqlen >= 1, "max_seqlen must be positive");
+  const auto [H_kv, cap] = check_cache_chunk(q, B, max_seqlen, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
+                                             kpm);
+  if (has(k_new)) {
+    check_row_operand(*k_new, "k_new", q, {N, H_kv, D});
+    check_row_operand(*v_new, "v_new", q, {N, H_kv, D});
+  }
+  const c10::cuda::CUDAGuard guard(q.device());
+  Tensor out = torch::empty({N, H, D}, q.options());
+  run_cache_chunk(q.unsqueeze(0), B, max_seqlen, k_cache, v_cache, seqlens, k_new, v_new, bias, kpm, cap, scale,
+                  &cu_seqlens, out);
+  check_launch("fmha_kvcache_varlen_fwd");
   return out;
 }
 // ---- varlen: packed sequences described by cu_seqlens (fmha_api.h) ------------------------------------------------
@@ -570,6 +647,9 @@ void register_fmha(pybind11::module_& m) {
   kv.def("fmha_kvcache_fwd", &fmha_kvcache_fwd, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"),
          py::arg("seqlens"), py::arg("max_len"), py::arg("k_new"), py::arg("v_new"), py::arg("bias"),
          py::arg("key_padding_mask"), py::arg("scale"));
+  kv.def("fmha_kvcache_varlen_fwd", &fmha_kvcache_varlen_fwd, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"),
+         py::arg("cu_seqlens"), py::arg("max_seqlen"), py::arg("seqlens"), py::arg("max_len"), py::arg("k_new"),
+         py::arg("v_new"), py::arg("bias"), py::arg("key_padding_mask"), py::arg("scale"));
   // packed variable-length sequences: its own submodule, _C.varlen
   auto vl = m.def_submodule("varlen", "packed variable-length sequences described by cu_seqlens");
   vl.def("fmha_varlen_fwd", &fmha_varlen_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("cu_seqlens"),

@@ -279,9 +279,17 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_combine_kernel(const Fmh
 }
 
 // Row i of k_new / v_new -> row p_b + i of the caches (fmha_api.h).  CTA (i, b) copies all H cache heads of K and V,
-// one 16-byte vector per thread and step; a row at or past C is skipped.
+// one 16-byte vector per thread and step; a row at or past C is skipped.  kPacked: k_new / v_new are packed [N, H, D]
+// and sequence b's rows are s_b + i, i < T_b ({s_b, T_b} = fmha_varlen_seq(cu_seqlens, b, T, N)).
+template <bool kPacked>
 __global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCacheAppendParams p) {
   const int i = blockIdx.x, b = blockIdx.y;
+  int s_b = 0;   // packed: the first row of sequence b in k_new / v_new, whose batch stride is 0
+  if constexpr (kPacked) {
+    const int2 sn = fmha_varlen_seq(p.cu_seqlens, b, p.T, p.packed_rows);
+    if (i >= sn.y) return;
+    s_b = sn.x;
+  }
   const int pos = min(max(p.seqlens[b], 0), p.C) + i;
   if (pos >= p.C) return;
   const int nch = p.D / 8, per = p.H * nch;   // 16-byte chunks of one row of one tensor
@@ -289,7 +297,7 @@ __global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCache
     const bool is_v = x >= per;
     const int h = (x % per) / nch, c = x % nch;
     const uint16_t* src = reinterpret_cast<const uint16_t*>(is_v ? p.v_new : p.k_new) +
-                          (long long)b * (is_v ? p.vn_sb : p.kn_sb) + (long long)i * (is_v ? p.vn_sl : p.kn_sl) +
+                          (long long)b * (is_v ? p.vn_sb : p.kn_sb) + (long long)(s_b + i) * (is_v ? p.vn_sl : p.kn_sl) +
                           (long long)h * (is_v ? p.vn_sh : p.kn_sh) + 8 * c;
     uint16_t* dst = reinterpret_cast<uint16_t*>(is_v ? p.v_cache : p.k_cache) +
                     (long long)b * (is_v ? p.vc_sb : p.kc_sb) + (long long)pos * (is_v ? p.vc_sl : p.kc_sl) +
@@ -301,7 +309,8 @@ __global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCache
 }  // namespace
 
 void launch_kv_cache_append(const KvCacheAppendParams& p, cudaStream_t stream) {
-  kv_cache_append_kernel<<<dim3(p.T, p.B), kThreads, 0, stream>>>(p);
+  if (p.cu_seqlens != nullptr) kv_cache_append_kernel<true><<<dim3(p.T, p.B), kThreads, 0, stream>>>(p);
+  else kv_cache_append_kernel<false><<<dim3(p.T, p.B), kThreads, 0, stream>>>(p);
 }
 
 int fmha_decode_num_splits(int B, int H, int len_bound, int num_sms) {

@@ -106,11 +106,15 @@ UB_DEVICE void quad_transpose4(uint32_t (&w)[4], int c) {
 // assignment and their V rows are zeroed, as in the KV-cache mode.  A sequence with n_k = 0 walks tile 0 wholly masked
 // (Q arrives with the first tile), so its rows get O = 0 and LSE = -inf.  Only rows below n_q are stored.  Causal
 // composes (its diagonal is per sequence, with the keys the queries' own rows); logits mode does not.
+// kKVCache && kVarlen: packed chunks into a cache (fmha_api.h).  Queries and O are packed as in varlen mode (rows s_b +
+// i, CTAs past n_q exit, only rows below n_q are stored); keys and values come from the caches at batch coordinate b,
+// and the visibility, tile count, stale-row handling and tile order are the KV-cache mode's with T_b = n_q in place of
+// Lq.  The varlen key description (cu_seqlens_k) is not read.
 template <typename T, int DP, bool kLogits, bool kCausal, bool kKVCache, bool kVarlen = false>
 __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
   static_assert(!(kKVCache && (kLogits || kCausal)), "the KV-cache mode is neither causal nor logits mode");
-  static_assert(!(kVarlen && (kLogits || kKVCache)), "the varlen mode is neither logits nor KV-cache mode");
+  static_assert(!(kVarlen && kLogits), "the varlen mode is not logits mode");
   using C = FwdCfg<DP>;
   constexpr int kBlockN = C::kBlockN;
   constexpr int kWords = kBlockN / 32;   // keep-bit words per row of a key tile
@@ -131,11 +135,14 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
     vl_s = sn.x;
     vl_n = sn.y;
     if (q0 >= vl_n) return;
-    const int2 sk = fmha_varlen_seq(p.cu_seqlens_k, b, p.Lk, p.packed_rows_k);
-    vk_s = sk.x;
-    vk_n = sk.y;
+    if constexpr (!kKVCache) {
+      const int2 sk = fmha_varlen_seq(p.cu_seqlens_k, b, p.Lk, p.packed_rows_k);
+      vk_s = sk.x;
+      vk_n = sk.y;
+    }
   }
-  const int tb = kVarlen ? 0 : b;   // batch coordinate of the q / k / v maps
+  const int tb = kVarlen ? 0 : b;   // batch coordinate of the q map
+  const int tbk = (kVarlen && !kKVCache) ? 0 : b;   // and of the k / v maps (a cache keeps the padded layout)
   const int row_lim = kVarlen ? vl_n : p.Lq;   // rows stored
   const uint32_t bar0 = smem_base + C::kSmemBar;   // bar0 + 8 * stage: K / V / bias of a key tile (+ Q on the first)
   float* kadd = reinterpret_cast<float*>(smem + C::kSmemKAdd);
@@ -146,7 +153,7 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   int kv_p = 0, kv_n = 0, kv_lim = 0;
   if constexpr (kKVCache) {
     kv_p = p.seqlens != nullptr ? min(max(p.seqlens[b], 0), p.Lk) : p.Lk;
-    kv_n = min(kv_p + p.Lq, p.kv_cap);
+    kv_n = min(kv_p + (kVarlen ? vl_n : p.Lq), p.kv_cap);
     kv_lim = min(kv_n, kv_p + q0 + 1);
   }
   // causal: key tiles 0 .. (q0 + 63) / kBlockN hold a key visible to one of the rows q0 .. q0 + 63.  varlen: a
@@ -164,9 +171,9 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
       if (j == 0) tma_load_4d(smem_base + C::kSmemQ + x * C::kQBox, &p.sw_q, 64 * x, h, vl_s + q0, tb, bar);
-      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, vk_s + j * kBlockN, tb,
+      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, vk_s + j * kBlockN, tbk,
                   bar);
-      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, vk_s + j * kBlockN, tb,
+      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, vk_s + j * kBlockN, tbk,
                   bar);
     }
     if (has_bias) {   // 64 rows x kBlockN keys = kBlockN / 64 boxes of 64 keys
@@ -288,7 +295,9 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
           if (key + 1 >= lim1) s[4 * i + 3] = -CUDART_INF_F;
         }
       }
-      if constexpr (kVarlen) {   // the last tile: keys of the next sequence, assigned (their bias is not this one's)
+      // the last tile: keys of the next sequence, assigned (their bias is not this one's).  Not with a cache, whose
+      // stale rows the KV-cache branch above has hidden (vk_n is 0 there)
+      if constexpr (kVarlen && !kKVCache) {
         if (key0 + kBlockN > vk_n) {
           const int key = key0 + col;
           if (key >= vk_n) s[4 * i + 0] = s[4 * i + 2] = -CUDART_INF_F;
@@ -460,7 +469,8 @@ void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream) {
   const std::false_type no;
   const std::true_type yes;
   if (p.varlen) {
-    if (p.causal) dispatch(no, yes, no, yes);
+    if (p.kvcache) dispatch(no, no, yes, yes);
+    else if (p.causal) dispatch(no, yes, no, yes);
     else dispatch(no, no, no, yes);
   } else if (p.kvcache) dispatch(no, no, yes, no);
   else if (p.logits != nullptr) dispatch(yes, no, no, no);

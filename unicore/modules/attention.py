@@ -37,12 +37,18 @@ with sequence ``b`` on rows ``cu_seqlens[b] .. cu_seqlens[b + 1] - 1`` (int ``[B
 ``max_seqlen`` a host bound on the lengths; the output is packed too.  No row is padding, so the projections do no work
 on pad rows, and the attention runs in the varlen mode of the fused kernels (``ops.fused_attention_varlen``; the
 varlen reference elsewhere).  ``attn_bias`` is ``[1|B, H, max_seqlen, max_seqlen]`` (each sequence reads its top-left
-block); rotary positions restart at 0 in every sequence.  No key padding mask, logits, probabilities or cache.
+block); rotary positions restart at 0 in every sequence.  No key padding mask, logits or probabilities.  With a
+``cache`` the packed rows are each sequence's new tokens (a different count per sequence, 0 included): they are
+appended at ``seqlens[b] + i``, rotated at those positions, and attend to the cache up to their own position
+(``ops.attention_with_kv_cache_varlen``), ``attn_bias`` then holding ``[1|B, H, max_seqlen, Lb]`` rows of the new
+queries.  On an empty cache this is the prefill; there is one packed path for both.
 ``CrossMultiheadAttention`` takes a packed query ``[N_q, E]`` (``cu_seqlens`` / ``max_seqlen``) with packed keys and
 values ``[N_k, E]`` (``encoder_cu_seqlens`` / ``encoder_max_seqlen``, the same B sequences) and returns ``[N_q, E]``:
 query ``i`` of sequence ``b`` sees the keys of source sequence ``b`` only, in the varlen mode of the fused kernels with
 separate key sequences.  ``attn_bias`` is then ``[B*H | B | H, max_seqlen, encoder_max_seqlen]``; a sequence without
-source rows gives 0.  No key padding mask or cache.
+source rows gives 0.  No key padding mask.  A packed query with a ``cache`` and padded ``key`` / ``value [B, S, E]``
+(no ``encoder_cu_seqlens``) is a decoding call: the prefill stores the projected keys / values as the padded path does,
+and every packed call attends to them with ``key_padding_mask [B, S]`` (``ops.attention_with_kv_cache_varlen``).
 
 ``DecoderCache`` holds what incremental decoding keeps between steps: per layer the self-attention keys and values
 ``[B, C, H_kv, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.  A step may
@@ -217,8 +223,8 @@ class SelfMultiheadAttention(nn.Module):
     def _attend_packed(self, query, key_padding_mask, attn_bias, return_attn, causal, cache, cu_seqlens, max_seqlen):
         if return_attn:
             raise ValueError("packed sequences (cu_seqlens) do not return attention weights")
-        if key_padding_mask is not None or cache is not None:
-            raise ValueError("packed sequences (cu_seqlens) take neither a key padding mask nor a cache")
+        if key_padding_mask is not None:
+            raise ValueError("packed sequences (cu_seqlens) take no key padding mask")
         if max_seqlen is None:
             raise ValueError("cu_seqlens needs max_seqlen, a host bound on the lengths")
         total, embed_dim = query.size()
@@ -227,11 +233,15 @@ class SelfMultiheadAttention(nn.Module):
         H, H_kv, D = self.num_heads, self.num_kv_heads, self.head_dim
         qkv = ops.linear(query, self.in_proj.weight, self.in_proj.bias).view(total, H + 2 * H_kv, D)
         if self.rotary_dim is not None:
-            # one token per row of the rotary op, at its position inside its sequence
-            pos = ops.varlen_positions(cu_seqlens, total)
+            # one token per row of the rotary op, at its position inside its sequence (after the cached tokens)
+            pos = ops.varlen_positions(cu_seqlens, total, None if cache is None else cache.seqlens)
             qkv = ops.rotary_embedding(qkv.view(total, 1, H + 2 * H_kv, D), self.inv_freq, H + H_kv, pos)
             qkv = qkv.view(total, H + 2 * H_kv, D)
         q, k, v = (t[:, 0] for t in _split_packed(qkv[:, None], H_kv))
+        if cache is not None:   # the prefill (from seqlens = 0) and every step alike: append, then attend
+            o = ops.attention_with_kv_cache_varlen(q, cache.k, cache.v, cu_seqlens, max_seqlen, cache.seqlens,
+                                                   cache.max_len, k_new=k, v_new=v, bias=attn_bias, scale=self.scaling)
+            return o.reshape(total, embed_dim), None, None
         bias4 = _bias_as_4d(attn_bias, cu_seqlens.numel() - 1, H, max_seqlen, max_seqlen)
         o = _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias4, self.dropout, self.training, self.scaling,
                                     causal, qkv)
@@ -315,6 +325,9 @@ class CrossMultiheadAttention(nn.Module):
 
     def _attend_packed(self, query, key, value, key_padding_mask, attn_bias, cache, cu_seqlens, max_seqlen,
                        encoder_cu_seqlens, encoder_max_seqlen):
+        if cache is not None and cu_seqlens is not None and encoder_cu_seqlens is None:
+            return self._attend_packed_cached(query, key, value, key_padding_mask, attn_bias, cache, cu_seqlens,
+                                              max_seqlen)
         if cu_seqlens is None or encoder_cu_seqlens is None:
             raise ValueError("packed cross-attention takes a packed query (cu_seqlens) and packed keys / values "
                              "(encoder_cu_seqlens) together")
@@ -338,6 +351,30 @@ class CrossMultiheadAttention(nn.Module):
         bias4 = _bias_as_4d(attn_bias, cu_seqlens.numel() - 1, H, max_seqlen, encoder_max_seqlen)
         o = _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias4, self.dropout, self.training, self.scaling,
                                     False, cu_seqlens_k=encoder_cu_seqlens, max_seqlen_k=encoder_max_seqlen)
+        return o.reshape(total, embed_dim)
+
+    def _attend_packed_cached(self, query, key, value, key_padding_mask, attn_bias, cache, cu_seqlens, max_seqlen):
+        """A packed query ``[N, E]`` against the encoder keys / values of ``cache``: the prefill projects and stores the
+        padded ``key`` / ``value [B, S, E]`` first.  ``key_padding_mask [B, S]``; ``attn_bias [B*H | B | H, max_seqlen,
+        S]`` or ``[1|B, H, max_seqlen, S]``, row i for query i of every sequence."""
+        if max_seqlen is None:
+            raise ValueError("cu_seqlens needs max_seqlen, a host bound on the lengths")
+        total, embed_dim = query.size()
+        if embed_dim != self.embed_dim:
+            raise ValueError("query dim {} != embed_dim {}".format(embed_dim, self.embed_dim))
+        B, H, H_kv, D = cu_seqlens.numel() - 1, self.num_heads, self.num_kv_heads, self.head_dim
+        if not cache.stepping:
+            if key is None or key.dim() != 3 or key.size(0) != B:
+                raise ValueError("the prefill of a packed query stores a padded encoder_out [B = {}, S, E]".format(B))
+            src_len = key.size(1)
+            cache.store_encoder(self.k_proj(key).view(B, src_len, H_kv, D), self.v_proj(value).view(B, src_len, H_kv, D))
+        src_len = cache.enc_k.size(1)
+        if attn_bias is not None and attn_bias.dim() == 3 and attn_bias.shape[0] not in (B * H, H):
+            attn_bias = attn_bias.view(B, 1, max_seqlen, src_len)   # [B, ...]: the same rows for every head
+        bias4 = _bias_as_4d(attn_bias, B, H, max_seqlen, src_len)
+        q = self.q_proj(query).view(total, H, D)
+        o = ops.attention_with_kv_cache_varlen(q, cache.enc_k, cache.enc_v, cu_seqlens, max_seqlen, bias=bias4,
+                                               key_padding_mask=key_padding_mask, scale=self.scaling)
         return o.reshape(total, embed_dim)
 
     def forward(

@@ -29,7 +29,9 @@ token-wise kernel then runs on the N real tokens only, the relative-position bia
 attention runs in the varlen mode of the fused kernels; the output is packed ``[N, E]``.  ``TransformerDecoder`` takes
 packed targets the same way, decoder-only or with a packed ``encoder_out [N_k, E]`` described by
 ``encoder_cu_seqlens`` / ``encoder_max_seqlen``: its self-attention is causal per sequence and its encoder attention
-sees each target sequence's own source rows (the varlen kernels with separate key sequences).
+sees each target sequence's own source rows (the varlen kernels with separate key sequences).  With a ``DecoderCache``
+the packed decoder takes each sequence's new tokens, a different count per sequence, into the cache (the prefill on
+an empty one), through ``ops.attention_with_kv_cache_varlen``.
 """
 import math
 from typing import Optional
@@ -39,6 +41,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from unicore import ops, utils
+from unicore_b200.ops.attention_ops import _varlen_lengths
 
 from .attention import CrossMultiheadAttention, DecoderCache, SelfMultiheadAttention
 from .norm import LayerNorm
@@ -552,15 +555,17 @@ class TransformerDecoder(nn.Module, _StackMixin):
         max_seqlen]`` and ``encoder_attn_mask`` ``[B*H | B, max_seqlen, encoder_max_seqlen]``.  Without a mask of that
         width, ``max_seqlen`` / ``encoder_max_seqlen`` are rounded up to a multiple of 8, which changes no result.
         The self-attention is causal per sequence when ``auto_regressive``; every token-wise kernel runs on the real
-        rows only.  Returns packed ``[N, E]``.  No padding masks and no cache."""
+        rows only.  Returns packed ``[N, E]``.  No padding masks.  With a ``cache``: ``_forward_packed_cached``."""
         if cu_seqlens is None:
             raise ValueError("a packed encoder_out (encoder_cu_seqlens) needs a packed target (cu_seqlens)")
         if max_seqlen is None:
             raise ValueError("cu_seqlens needs max_seqlen, a host bound on the lengths")
+        if cache is not None:
+            return self._forward_packed_cached(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
+                                               encoder_attn_mask, cache, cu_seqlens, int(max_seqlen),
+                                               encoder_cu_seqlens)
         if padding_mask is not None or encoder_padding_mask is not None:
             raise ValueError("packed sequences (cu_seqlens) have no padding_mask or encoder_padding_mask")
-        if cache is not None:
-            raise ValueError("packed sequences (cu_seqlens) do not decode into a cache")
         if (encoder_out is None) != (encoder_cu_seqlens is None):
             raise ValueError("a packed target takes a packed encoder_out with encoder_cu_seqlens, or neither")
         if encoder_cu_seqlens is not None:
@@ -579,6 +584,35 @@ class TransformerDecoder(nn.Module, _StackMixin):
             x = layer(x, encoder_out=encoder_out, attn_bias=attn_bias, encoder_attn_bias=encoder_attn_mask,
                       causal=self.auto_regressive, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen,
                       encoder_cu_seqlens=encoder_cu_seqlens, encoder_max_seqlen=encoder_max_seqlen)
+        return x if self.final_layer_norm is None else self.final_layer_norm(x)
+
+    def _forward_packed_cached(self, emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
+                               encoder_attn_mask, cache, cu_seqlens, max_seqlen, encoder_cu_seqlens):
+        """Packed new tokens into a ``DecoderCache``: ``emb [N, E]``, sequence b's ``T_b`` tokens on rows
+        ``cu_seqlens[b] ..`` (clamped as the varlen kernels clamp them, ``T_b <= max_seqlen``) at positions
+        ``seqlens[b] .. seqlens[b] + T_b - 1``; ``T_b`` may differ per sequence and be 0.  On an empty cache the call is
+        the prefill, which also stores the projected padded ``encoder_out [B, S, E]``; every call appends each layer's
+        keys / values of its tokens, attends with ``encoder_padding_mask [B, S]`` and ``encoder_attn_mask [B*H | B,
+        max_seqlen, S]``, then advances ``cache.seqlens`` by ``T_b`` on the device (clamped to the capacity) and
+        ``cache.max_len`` by ``max_seqlen``.  Returns ``[N, E]``.  Nothing is read on the host."""
+        self._check_no_dropout()
+        if encoder_cu_seqlens is not None:
+            raise ValueError("a packed encoder_out (encoder_cu_seqlens) does not go into a cache: give it padded, "
+                             "[B, S, E] with encoder_padding_mask")
+        if padding_mask is not None or attn_mask is not None:
+            raise ValueError("packed sequences (cu_seqlens) into a cache take no padding_mask or attn_mask")
+        if cu_seqlens.dim() != 1 or cu_seqlens.numel() != cache.seqlens.numel() + 1:
+            raise ValueError("cu_seqlens must have B + 1 = {} entries for the cache's sequences, not {}".format(
+                cache.seqlens.numel() + 1, tuple(cu_seqlens.shape)))
+        _check_room(cache, max_seqlen)
+        x = self._embed_prologue(emb, None)
+        attn_bias = self._step_rel_pos_bias(cache, x, max_seqlen) if self.rel_pos else None
+        for layer, lc in zip(self.layers, cache.layers):
+            x = layer(x, encoder_out=encoder_out, attn_bias=attn_bias, encoder_padding_mask=encoder_padding_mask,
+                      encoder_attn_bias=encoder_attn_mask, cache=lc, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen)
+        _, lengths = _varlen_lengths(cu_seqlens.to(cache.seqlens.device), max_seqlen, emb.size(0))
+        cache.seqlens.copy_((cache.seqlens.clamp(0, cache.capacity) + lengths).clamp(max=cache.capacity))
+        cache.max_len += max_seqlen
         return x if self.final_layer_norm is None else self.final_layer_norm(x)
 
     def _forward_prefix(self, emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask, encoder_attn_mask,

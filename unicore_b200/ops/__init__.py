@@ -5,6 +5,8 @@ from .attention_ops import (  # noqa: F401
     attention_varlen_reference,
     attention_with_kv_cache,
     attention_with_kv_cache_reference,
+    attention_with_kv_cache_varlen,
+    attention_with_kv_cache_varlen_reference,
     fused_attention,
     fused_attention_qkvpacked,
     fused_attention_supported,

@@ -253,22 +253,32 @@ def fused_attention_qkvpacked(qkv, bias=None, key_padding_mask=None, dropout_p=0
     return _fused_attention(q, k, v, bias, key_padding_mask, dropout_p, training, scale, return_logits, causal, qkv)
 
 
-def varlen_positions(cu_seqlens, total):
+def varlen_positions(cu_seqlens, total, offsets=None):
     """int32 ``[total]``: the position of each packed row inside its sequence (``cu_seqlens [B + 1]``), computed on
-    the device, so that no length is read on the host."""
+    the device, so that no length is read on the host.  ``offsets`` (int ``[B]`` on the device): added to the
+    positions of sequence b's rows, as a packed step into a cache places them after the ``seqlens[b]`` cached ones."""
     cu = cu_seqlens.to(torch.long)
     rows = torch.arange(total, device=cu.device)
     seq = torch.searchsorted(cu[1:], rows, right=True).clamp(max=cu.numel() - 1)
-    return (rows - cu[seq]).to(torch.int32)
+    pos = rows - cu[seq]
+    if offsets is not None:   # rows past the last sequence take its offset
+        pos = pos + offsets.to(device=cu.device, dtype=torch.long)[seq.clamp(max=offsets.numel() - 1)]
+    return pos.to(torch.int32)
+
+
+def _varlen_lengths(cu_seqlens, max_seqlen, total):
+    """``(s [B], n [B])``, int64 on the device: each sequence's first packed row and length with the kernels' clamps,
+    ``s_b = clamp(cu[b], 0, N)`` and ``n_b = clamp(cu[b + 1] - cu[b], 0, min(L, N - s_b))``."""
+    cu = cu_seqlens.to(torch.long)
+    start = cu[:-1].clamp(0, total)
+    return start, torch.minimum((cu[1:] - cu[:-1]).clamp(min=0), (total - start).clamp(max=max_seqlen))
 
 
 def _varlen_index(cu_seqlens, max_seqlen, total):
     """``(rows [B, L], valid [B, L])``: the packed row of position ``i`` of sequence ``b`` and whether it exists, with
-    the kernels' clamps: ``s_b = clamp(cu[b], 0, N)``, ``n_b = clamp(cu[b + 1] - cu[b], 0, min(L, N - s_b))``."""
-    cu = cu_seqlens.to(torch.long)
-    start = cu[:-1].clamp(0, total)
-    n = torch.minimum((cu[1:] - cu[:-1]).clamp(min=0), (total - start).clamp(max=max_seqlen))
-    pos = torch.arange(max_seqlen, device=cu.device)
+    the kernels' clamps (``_varlen_lengths``)."""
+    start, n = _varlen_lengths(cu_seqlens, max_seqlen, total)
+    pos = torch.arange(max_seqlen, device=start.device)
     valid = pos[None, :] < n[:, None]
     rows = torch.where(valid, start[:, None] + pos[None, :], torch.zeros_like(valid, dtype=torch.long))
     return rows, valid
@@ -468,19 +478,21 @@ def _check_no_grad(*tensors):
                            "torch.inference_mode(), or detach the inputs")
 
 
-def _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new):
+def _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, T=None):
     """The arguments of ``attention_with_kv_cache`` checked, as ``(T, append, max_len, bound)``: ``max_len`` the host
     bound on ``seqlens`` (by default the most the capacity allows; None without ``seqlens`` unless given) and
-    ``bound`` the keys any query can see, ``max_len`` plus the appended rows, else the capacity C."""
-    kv_group(q.shape[2], k_cache, v_cache)
+    ``bound`` the keys any query can see, ``max_len`` plus the appended rows, else the capacity C.  ``T``: the new
+    queries per sequence (default ``q.shape[1]``; the host bound ``max_seqlen`` of packed chunks, whose q / k_new /
+    v_new are ``[N, heads, D]``)."""
+    kv_group(q.shape[-2], k_cache, v_cache)
     append = k_new is not None
     if append != (v_new is not None):
         raise ValueError("k_new and v_new go together")
     if append and seqlens is None:
         raise ValueError("appending needs seqlens (the row to write)")
-    if append and (k_new.shape[2] != k_cache.shape[2] or v_new.shape[2] != k_cache.shape[2]):
+    if append and (k_new.shape[-2] != k_cache.shape[2] or v_new.shape[-2] != k_cache.shape[2]):
         raise ValueError("k_new / v_new must have the {} heads of the caches".format(k_cache.shape[2]))
-    T = q.shape[1]
+    T = q.shape[1] if T is None else int(T)
     if T > 1 and seqlens is not None and not append:
         raise ValueError("a chunk of T > 1 queries with seqlens appends k_new / v_new")
     C = k_cache.shape[1]
@@ -527,7 +539,14 @@ def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len
         n = seqlens.long().clamp(0, C)
     else:
         n = torch.full((B,), C, dtype=torch.long, device=q.device)
-    # the keys past the columns of the bias or of the key mask are hidden
+    return _kv_cache_attend_reference(q, k_cache, v_cache, n, future, K, bias, key_padding_mask, scale)
+
+
+def _kv_cache_attend_reference(q, k_cache, v_cache, n, future, K, bias, key_padding_mask, scale):
+    """The attention of the cache references after their appends: q ``[B, T, H, D]`` against cache rows ``j < n_b``
+    (``n [B]``) and ``j < K`` (the keys any query can see), and ``j <= future[b, i]`` when ``future [B, T]`` is given;
+    the keys past the columns of the bias or of the key mask are hidden too."""
+    H = q.shape[2]
     if bias is not None:
         K = min(K, bias.shape[-1])
     if key_padding_mask is not None:
@@ -564,32 +583,32 @@ def _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padd
     return True
 
 
-def _native_cache_operands(q, seqlens, bias, key_padding_mask, bound):
-    """``seqlens``, the bias and the key mask as ``fmha_decode`` (T = 1) and ``fmha_kvcache_fwd`` (T > 1) take them:
+def _native_cache_operands(q, seqlens, bias, key_padding_mask, bound, B, T, chunk):
+    """``seqlens``, the bias and the key mask as ``fmha_decode`` (one query per sequence) and the chunk kernel
+    (``chunk``: ``fmha_kvcache_fwd`` or ``fmha_kvcache_varlen_fwd``, up to T queries) take them for B sequences:
     int32 lengths, a bool key mask and a bias in the dtype of q, each with a contiguous last dim.  A bias or key mask
     narrower than the ``bound`` visible keys is widened with -inf / True, which hides the keys past it as the
     reference's clamp to its columns does.  Operands that are already so are passed on as they are."""
-    T = q.shape[1]
     if seqlens is not None and (seqlens.dtype != torch.int32 or not seqlens.is_contiguous()):
         seqlens = seqlens.to(torch.int32).contiguous()
     if bias is not None:
         Lb = bias.shape[-1]
         width = max(Lb, bound)
         bias = bias.to(q.dtype)
-        if T > 1:   # read by TMA: a row for every query head, of a multiple of 8 columns
-            bias = bias.expand(bias.shape[0], q.shape[2], T, Lb)
+        if chunk:   # read by TMA: a row for every query head, of a multiple of 8 columns
+            bias = bias.expand(bias.shape[0], q.shape[-2], T, Lb)
             width += -width % 8
         if width != Lb:
             bias = F.pad(bias, (0, width - Lb), value=float("-inf"))
-        if T > 1 or bias.stride(-1) != 1:
+        if chunk or bias.stride(-1) != 1:
             bias = bias.contiguous()
     if key_padding_mask is not None:
         if key_padding_mask.dtype != torch.bool or key_padding_mask.stride(-1) != 1:
             key_padding_mask = key_padding_mask.to(torch.bool).contiguous()
         cols = key_padding_mask.shape[1]
         if cols < bound:
-            key_padding_mask = torch.cat([key_padding_mask, key_padding_mask.new_ones(q.shape[0], bound - cols)], 1)
-        if T > 1:
+            key_padding_mask = torch.cat([key_padding_mask, key_padding_mask.new_ones(B, bound - cols)], 1)
+        if chunk:
             key_padding_mask = key_padding_mask.contiguous()
     return seqlens, bias, key_padding_mask
 
@@ -617,7 +636,8 @@ def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_n
     if not _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask):
         return attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
                                                  key_padding_mask, scale)
-    seqlens, bias, key_padding_mask = _native_cache_operands(q, seqlens, bias, key_padding_mask, bound)
+    seqlens, bias, key_padding_mask = _native_cache_operands(q, seqlens, bias, key_padding_mask, bound, q.shape[0], T,
+                                                             T > 1)
     max_len = 0 if max_len is None else int(max_len)
     if T == 1:
         # A step captured in a CUDA graph runs with the capacity as its host bound, far above most true lengths: each
@@ -626,3 +646,107 @@ def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_n
                                     float(scale), split_by_length=torch.cuda.is_current_stream_capturing())
     return native().kvcache.fmha_kvcache_fwd(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
                                              key_padding_mask, float(scale))
+
+
+def _kv_cache_varlen_plan(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens, max_len, k_new, v_new):
+    """``attention_with_kv_cache_varlen``'s arguments checked, as ``_kv_cache_plan``'s result for chunks of up to
+    ``max_seqlen`` queries."""
+    if q.dim() != 3 or (k_new is not None and k_new.dim() != 3) or (v_new is not None and v_new.dim() != 3):
+        raise ValueError("packed chunks take q [N, H, D] and k_new / v_new [N, H_kv, D]")
+    if cu_seqlens.dim() != 1 or cu_seqlens.numel() != k_cache.shape[0] + 1:
+        raise ValueError("cu_seqlens must have B + 1 = {} entries for the caches' B = {} sequences, not {}".format(
+            k_cache.shape[0] + 1, k_cache.shape[0], tuple(cu_seqlens.shape)))
+    if int(max_seqlen) < 1:
+        raise ValueError("max_seqlen must be positive, not {}".format(max_seqlen))
+    if seqlens is not None and k_new is None:
+        raise ValueError("packed chunks with seqlens append k_new / v_new")
+    return _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, T=max_seqlen)
+
+
+def attention_with_kv_cache_varlen_reference(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens=None, max_len=None,
+                                             k_new=None, v_new=None, bias=None, key_padding_mask=None, scale=None):
+    """Plain PyTorch implementation of ``attention_with_kv_cache_varlen`` (CPU path, fallback and test oracle).
+
+    Performs the append in place like the kernels, ``T_b`` rows per sequence: rows ``p_b + i`` of the caches,
+    ``p_b = seqlens[b]`` clamped to ``[0, C]``, become packed rows ``s_b + i`` of ``k_new / v_new``, and rows at or past
+    ``C`` are skipped.  At every real row the result is what ``attention_with_kv_cache_reference`` gives for that
+    sequence alone with ``T = T_b``; packed rows of no sequence give 0."""
+    T, _, _, K = _kv_cache_varlen_plan(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens, max_len, k_new, v_new)
+    N, H, D = q.shape
+    B, C = k_cache.shape[:2]
+    scale = scale if scale is not None else 1.0 / math.sqrt(D)
+    rows, valid = _varlen_index(cu_seqlens.to(q.device), T, N)   # [B, T]: packed row of query i of sequence b
+    future = None
+    if seqlens is not None:
+        dev = k_cache.device
+        p = seqlens.long().to(dev).clamp(0, C)
+        pos = p[:, None] + torch.arange(T, device=dev)[None, :]   # [B, T]
+        write = valid.to(dev) & (pos < C)
+        src, seq = rows.to(dev), torch.arange(B, device=dev)
+        for i in range(T):   # one row per sequence at a time; a row not written keeps what it holds
+            at, keep = pos[:, i].clamp(max=C - 1), ~write[:, i, None, None]
+            k_cache[seq, at] = torch.where(keep, k_cache[seq, at], k_new[src[:, i]].to(k_cache.dtype))
+            v_cache[seq, at] = torch.where(keep, v_cache[seq, at], v_new[src[:, i]].to(v_cache.dtype))
+        n = (p + valid.sum(1).to(dev)).clamp(max=C)
+        future = pos.to(q.device)   # query i of sequence b sees keys j <= p_b + i
+    else:
+        n = torch.full((B,), C, dtype=torch.long, device=q.device)
+    qp = torch.where(valid[:, :, None, None], q[rows], torch.zeros((), dtype=q.dtype, device=q.device))
+    out = _kv_cache_attend_reference(qp, k_cache, v_cache, n, future, K, bias, key_padding_mask, scale)
+    # gather back: the positions past T_b write into a dropped row N
+    dest = torch.where(valid, rows, torch.full_like(rows, N)).reshape(-1)
+    packed = torch.zeros(N + 1, H, D, dtype=out.dtype, device=out.device).index_put((dest,), out.reshape(-1, H, D))
+    return packed[:N]
+
+
+def _kvcache_varlen_supported(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask) -> bool:
+    """True when ``kvcache.fmha_kvcache_varlen_fwd`` takes the operands."""
+    if not use_native(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask) \
+            or not hasattr(getattr(native(), "kvcache", None), "fmha_kvcache_varlen_fwd"):
+        return False
+    if q.shape[0] < 1 or q.stride(1) != q.shape[-1]:   # the q map takes (head, 16-byte chunk) as one dimension
+        return False
+    if not _kernel_tensors(q[None], k_cache, v_cache, None if k_new is None else k_new[None],
+                           None if v_new is None else v_new[None]):
+        return False
+    if bias is not None and bias.stride(-1) != 1 and bias.shape[-1] > 1:
+        return False
+    return True
+
+
+def attention_with_kv_cache_varlen(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens=None, max_len=None,
+                                   k_new=None, v_new=None, bias=None, key_padding_mask=None, scale=None):
+    """``attention_with_kv_cache`` for packed chunks: each sequence brings its own number of new queries.
+
+    q: ``[N, H, D]``, the B sequences' new queries back to back; sequence b's ``T_b`` queries are rows ``s_b .. s_b +
+    T_b - 1`` with ``s_b = clamp(cu_seqlens[b], 0, N)`` and ``T_b = clamp(cu_seqlens[b + 1] - cu_seqlens[b], 0,
+    min(max_seqlen, N - s_b))`` (``cu_seqlens`` int ``[B + 1]`` on the device; ``max_seqlen`` a host bound on ``T_b``,
+    any value >= 1).  ``T_b = 0`` is allowed: that sequence adds nothing.  k_cache / v_cache: ``[B, C, H_kv, D]``.
+    ``k_new`` / ``v_new`` ``[N, H_kv, D]`` (needed with ``seqlens``): rows ``s_b + i`` are written bitwise into cache
+    rows ``p_b + i``, ``p_b = clamp(seqlens[b], 0, C)``, before the attention; rows at or past ``C`` are skipped.  Query
+    ``i`` of sequence b then sees cache rows ``0 .. p_b + i``.  With ``seqlens=None`` every query sees all C rows
+    (cross-attention against stored encoder keys).  ``max_len``: a host bound on ``seqlens`` (default: the most the
+    capacity allows); ``max_len + max_seqlen > C`` raises.  bias: ``[1|B, H, max_seqlen, Lb]``, row i for query i of
+    every sequence; key_padding_mask: bool ``[B, Lk]``; a narrower bias or key mask hides the keys past its columns.  A
+    query with no visible unmasked key gives 0.  Returns ``[N, H, D]``; at every real row the result of
+    ``attention_with_kv_cache`` on that sequence alone with ``T = T_b``.  Rows of q that belong to no sequence are not
+    written by the kernel (0 on the reference path), as in ``fused_attention_varlen``.  No dropout and no backward, and
+    no device value is read on the host, so a step does not synchronise.
+
+    It runs in the KV-cache mode of the wgmma forward for every ``T_b``, one-token sequences included: the host cannot
+    tell that every ``T_b`` is 1 without reading ``cu_seqlens``.  For pure one-token decoding a padded ``[B, 1, H, D]``
+    step (``attention_with_kv_cache``, split-KV) or a captured step stays the fast path."""
+    _check_no_grad(q, k_cache, v_cache, k_new, v_new, bias)
+    T, _, max_len, bound = _kv_cache_varlen_plan(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens, max_len,
+                                                 k_new, v_new)
+    if scale is None:
+        scale = 1.0 / math.sqrt(q.shape[-1])
+    if not _kvcache_varlen_supported(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask):
+        return attention_with_kv_cache_varlen_reference(q, k_cache, v_cache, cu_seqlens, T, seqlens, max_len, k_new,
+                                                        v_new, bias, key_padding_mask, scale)
+    B = k_cache.shape[0]
+    seqlens, bias, key_padding_mask = _native_cache_operands(q, seqlens, bias, key_padding_mask, bound, B, T, True)
+    cu_seqlens = cu_seqlens.to(torch.int32).contiguous()
+    return native().kvcache.fmha_kvcache_varlen_fwd(q, k_cache, v_cache, cu_seqlens, T, seqlens,
+                                                    0 if max_len is None else int(max_len), k_new, v_new, bias,
+                                                    key_padding_mask, float(scale))
