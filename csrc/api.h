@@ -148,7 +148,7 @@ void launch_bias_dropout_add_ln_fwd(const void* x, const void* bias, const void*
                                     const void* beta, void* y, void* summed, float* mean, float* rstd, int rows,
                                     int cols, float p, float eps, unsigned long long seed, unsigned long long offset,
                                     int dtype, cudaStream_t stream);
-// dsum = dLN(dy); dx = dropout_mask * dsum / (1-p); dbias (nullable) = column sums of dx at every width: v3 / v2 sum
+// dsum = dLN(dy); dx = dropout_mask * dsum / P(keep); dbias (nullable) = column sums of dx at every width: v3 / v2 sum
 // the fp32 values in the same pass, v1 sums the rounded dx with launch_column_sum afterwards (two more launches)
 void launch_bias_dropout_add_ln_bwd(const void* dy, const void* summed, const float* mean, const float* rstd,
                                     const void* gamma, void* dsum, void* dx, void* dgamma, void* dbeta,

@@ -18,6 +18,7 @@
 namespace ub {
 
 #define UB_DEVICE __device__ __forceinline__
+#define UB_HOST_DEVICE __host__ __device__ __forceinline__
 
 // ------------------------------------------------------------------------------------------------
 // 16-byte vector access
@@ -167,6 +168,9 @@ UB_DEVICE uint32_t dropout_thresh14(float p) {
   return t <= 0.f ? 0u : (t >= 16383.f ? 16383u : (uint32_t)t);
 }
 UB_DEVICE float dropout_keep_scale14(uint32_t t14) { return 16384.f / (16384.f - (float)t14); }
+// The same rule for the 16-bit threshold of dropout_keep8 (keep <=> u16 >= t16, P(keep) = (65536 - t16) / 65536), so
+// that E[dropout(x)] = x exactly for the rate the kernels draw, not for the requested p.
+UB_HOST_DEVICE float dropout_keep_scale16(uint32_t t16) { return 65536.f / (65536.f - (float)t16); }
 UB_DEVICE uint32_t keep_mask2(uint32_t rnd, uint32_t t14x2) {
   const uint32_t u = rnd & 0x3fff3fffu;
   return __hge2_mask(*reinterpret_cast<const __half2*>(&u), *reinterpret_cast<const __half2*>(&t14x2));
@@ -322,7 +326,7 @@ UB_DEVICE void dropout_lane_masks8(uint64_t seed, uint64_t offset, uint64_t idx8
   m[3] = keep_mask2(r.w, t14x2);
 }
 
-UB_DEVICE uint32_t dropout_thresh16(float p) {
+UB_HOST_DEVICE uint32_t dropout_thresh16(float p) {
   float t = p * 65536.f + 0.5f;
   return t >= 65535.f ? 65535u : (uint32_t)t;
 }

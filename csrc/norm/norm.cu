@@ -1147,7 +1147,7 @@ template <typename T, bool kRMS, bool kFused>
 static void run_fwd(const void* x, const void* gamma, const void* beta, void* y, float* mean, float* rstd, int rows,
                     int cols, float eps, const void* bias, const void* residual, void* summed, float p,
                     unsigned long long seed, unsigned long long offset, cudaStream_t stream) {
-  const float keep_scale = p > 0.f ? 1.f / (1.f - p) : 1.f;
+  const float keep_scale = p > 0.f ? dropout_keep_scale16(dropout_thresh16(p)) : 1.f;
   const NormPlan pl = norm_plan(rows, cols, dtype_of<T>(), kFused ? kNormFusedFwd : kNormFwd);
   if (pl.gen == 3) {
     run_fwd_v3<T, kRMS, kFused>(pl, x, gamma, beta, y, mean, rstd, rows, cols, eps, bias, residual, summed, p,
@@ -1175,7 +1175,7 @@ template <typename T, bool kRMS, bool kFused>
 static void run_bwd(const void* dy, const void* x, const float* mean, const float* rstd, const void* gamma, void* dx,
                     void* dgamma, void* dbeta, void* dbias, float* part, int rows, int cols, void* dx_drop, float p,
                     unsigned long long seed, unsigned long long offset, int acc_mask, cudaStream_t stream) {
-  const float keep_scale = p > 0.f ? 1.f / (1.f - p) : 1.f;
+  const float keep_scale = p > 0.f ? dropout_keep_scale16(dropout_thresh16(p)) : 1.f;
   const NormPlan pl = norm_plan(rows, cols, dtype_of<T>(), kNormBwd);
   if (pl.gen == 0) return;  // no kernel for this width (the bindings refuse it)
   if (pl.gen == 3) {

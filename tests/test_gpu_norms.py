@@ -268,21 +268,27 @@ def _fused_case(nat, x, bias, res, w, b, dy, p, sinks=()):
     return y, mean, rstd, summed, dsum, dx, dg, db, dbias
 
 
+# p = 0.5 puts the 16-bit threshold at the top bit of each random lane
+FUSED_PS = [0.1, 0.0, 0.5]
+
+
+@pytest.mark.parametrize("p", FUSED_PS)
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("nvec", [n for n in NVECS if n not in V1_NVECS])
-def test_bias_dropout_add_ln_all_paths(nvec, dtype):
-    check_fused_all_paths(nvec, dtype)
+def test_bias_dropout_add_ln_all_paths(nvec, dtype, p):
+    check_fused_all_paths(nvec, dtype, p)
 
 
+@pytest.mark.parametrize("p", FUSED_PS)
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("nvec", V1_NVECS)
-def test_bias_dropout_add_ln_dbias_at_gen1_widths(nvec, dtype):
+def test_bias_dropout_add_ln_dbias_at_gen1_widths(nvec, dtype, p):
     """The v1 widths return dbias too: a column sum of the rounded dx that runs after the norm kernel, into a sink as
     well.  Every other check is the one of the v3 / v2 widths."""
-    check_fused_all_paths(nvec, dtype)
+    check_fused_all_paths(nvec, dtype, p)
 
 
-def check_fused_all_paths(nvec, dtype):
+def check_fused_all_paths(nvec, dtype, p):
     nat = _native()
     cols = nvec * 8
     rows = plan_rows(cols, dtype, ("fused", "bwd"))
@@ -296,71 +302,72 @@ def check_fused_all_paths(nvec, dtype):
     b = torch.randn(cols, device="cuda", generator=g).to(dtype)
     dy = torch.randn(rows, cols, device="cuda", generator=g).to(dtype)
     u, tiny = UNIT[dtype], _tiny(dtype)
-    for p in (0.1, 0.0):
-        torch.cuda.manual_seed(11)  # the same Philox state for every run compared below
-        y, mean, rstd, summed, dsum, dx, dg, db, dbias = _fused_case(nat, x, bias, res, w, b, dy, p)
-        assert dbias is not None  # at every width
-        # the keep mask, read from dx (zero where the element was dropped, or where dsum underflowed to zero: there
-        # the forward's sum tells, it differs from the residual where x + bias was added); forward and backward agree
-        keep = (dx != 0) | ((dsum == 0) & (summed != res)) if p > 0 else torch.ones_like(dx, dtype=torch.bool)
-        if p > 0:
-            rate = keep.double().mean().item()
-            assert abs(rate - (1 - p)) < 6 * math.sqrt(p * (1 - p) / keep.numel()) + 2.0 ** -16, rate
-        scale = 1.0 / (1.0 - p)
-        # summed = residual + keep * (x + bias) / (1 - p): a few fp32 roundings, one rounding to the output type
-        for s in _chunks(rows, cols):
-            h = keep[s].double() * (x[s].double() + bias.double()) * scale
-            ref = res[s].double() + h
-            comp = 4 * E32 * (res[s].double().abs() + h.abs())
-            _assert_within(summed[s], ref, u * (ref.abs() + comp) + comp + tiny, "summed")
-        # LayerNorm of the stored (rounded) sum, and its backward from the saved statistics
-        check_forward(summed, w, b, y, mean, rstd, False)
-        dg_r = torch.zeros(cols, dtype=torch.float64, device="cuda")
-        db_r, dg_a, db_a, dbi_r, dbi_a = (torch.zeros_like(dg_r) for _ in range(5))
-        for s, dsr, comp, dyd, xh in backward_ref(dy, summed, mean, rstd, w, False):
-            _assert_within(dsum[s], dsr, u * (dsr.abs() + comp) + comp + tiny, "dsum")
-            k = keep[s].double() * scale
-            dxr, dxc = dsr * k, (comp + 2 * E32 * dsr.abs()) * k
-            _assert_within(dx[s], dxr, u * (dxr.abs() + dxc) + dxc + tiny, "dx")
-            dg_r += (dyd * xh).sum(0)
-            dg_a += (dyd * xh).abs().sum(0)
-            db_r += dyd.sum(0)
-            db_a += dyd.abs().sum(0)
-            dbi_r += dxr.sum(0)
-            # the per-element error of the dx terms enters the column sum: fp32 ones at v3 / v2 widths, the rounded dx
-            # (the bound checked above) at v1 widths
-            dxe = u * (dxr.abs() + dxc) + dxc + tiny if plan["gen"] == 1 else dxc
-            dbi_a += (dxr.abs() + dxe / E32 / bias_chain).sum(0)
-        check_param_grad(dg, dg_r, dg_a, dtype, chain, "dgamma")
-        check_param_grad(db, db_r, db_a, dtype, chain, "dbeta")
-        check_param_grad(dbias, dbi_r, dbi_a, dtype, bias_chain, "dbias")
-        # deterministic backward
-        torch.cuda.manual_seed(11)
-        again = _fused_case(nat, x, bias, res, w, b, dy, p)
-        assert torch.equal(summed, again[3])
-        for got, rep in zip((dsum, dx, dg, db, dbias), again[4:]):
-            assert torch.equal(got, rep)
-        if nvec not in (96, 192, 520) or p == 0:
-            continue
-        # gradient sinks (one width per generation): sink = base + gradient with one rounding, nothing else written
-        arena = torch.randn(3 * cols + 64, device="cuda").to(dtype)
-        before = arena.clone()
-        views = (arena[16:16 + cols], arena[32 + cols:32 + 2 * cols], arena[48 + 2 * cols:48 + 3 * cols])
-        bases = [v.clone() for v in views]
-        torch.cuda.manual_seed(11)
-        fw = nat.bias_dropout_add_ln_fwd(x, bias, res, w, b, p, EPS)
-        assert torch.equal(fw[3], summed)
-        out = nat.bias_dropout_add_ln_bwd(dy, fw[3], fw[1], fw[2], w, p, fw[4], fw[5], True, *views)
-        assert torch.equal(out[0], dsum) and torch.equal(out[1], dx)  # same mask as the run above
-        for got, view, base, ref, absum, ch, what in zip(out[2:], views, bases, (dg_r, db_r, dbi_r),
-                                                         (dg_a, db_a, dbi_a), (chain, chain, bias_chain),
-                                                         ("dgamma", "dbeta", "dbias")):
-            assert got.data_ptr() == view.data_ptr()
-            check_param_grad(got, ref, absum, dtype, ch, what + " sink", base)
-        outside = torch.ones_like(arena, dtype=torch.bool)
-        for v in views:
-            outside[(v.data_ptr() - arena.data_ptr()) // arena.element_size():][:cols] = False
-        assert torch.equal(arena[outside], before[outside])
+    torch.cuda.manual_seed(11)  # the same Philox state for every run compared below
+    y, mean, rstd, summed, dsum, dx, dg, db, dbias = _fused_case(nat, x, bias, res, w, b, dy, p)
+    assert dbias is not None  # at every width
+    # the keep mask, read from dx (zero where the element was dropped, or where dsum underflowed to zero: there
+    # the forward's sum tells, it differs from the residual where x + bias was added); forward and backward agree
+    keep = (dx != 0) | ((dsum == 0) & (summed != res)) if p > 0 else torch.ones_like(dx, dtype=torch.bool)
+    if p > 0:
+        rate = keep.double().mean().item()
+        assert abs(rate - (1 - p)) < 6 * math.sqrt(p * (1 - p) / keep.numel()) + 2.0 ** -16, rate
+    # kept elements are scaled by 1 / P(keep) of the 16-bit threshold the kernels compare against
+    t16 = min(int(p * 65536 + 0.5), 65535)
+    scale = 65536 / (65536 - t16)
+    # summed = residual + keep * (x + bias) * scale: a few fp32 roundings, one rounding to the output type
+    for s in _chunks(rows, cols):
+        h = keep[s].double() * (x[s].double() + bias.double()) * scale
+        ref = res[s].double() + h
+        comp = 4 * E32 * (res[s].double().abs() + h.abs())
+        _assert_within(summed[s], ref, u * (ref.abs() + comp) + comp + tiny, "summed")
+    # LayerNorm of the stored (rounded) sum, and its backward from the saved statistics
+    check_forward(summed, w, b, y, mean, rstd, False)
+    dg_r = torch.zeros(cols, dtype=torch.float64, device="cuda")
+    db_r, dg_a, db_a, dbi_r, dbi_a = (torch.zeros_like(dg_r) for _ in range(5))
+    for s, dsr, comp, dyd, xh in backward_ref(dy, summed, mean, rstd, w, False):
+        _assert_within(dsum[s], dsr, u * (dsr.abs() + comp) + comp + tiny, "dsum")
+        k = keep[s].double() * scale
+        dxr, dxc = dsr * k, (comp + 2 * E32 * dsr.abs()) * k
+        _assert_within(dx[s], dxr, u * (dxr.abs() + dxc) + dxc + tiny, "dx")
+        dg_r += (dyd * xh).sum(0)
+        dg_a += (dyd * xh).abs().sum(0)
+        db_r += dyd.sum(0)
+        db_a += dyd.abs().sum(0)
+        dbi_r += dxr.sum(0)
+        # the per-element error of the dx terms enters the column sum: fp32 ones at v3 / v2 widths, the rounded dx
+        # (the bound checked above) at v1 widths
+        dxe = u * (dxr.abs() + dxc) + dxc + tiny if plan["gen"] == 1 else dxc
+        dbi_a += (dxr.abs() + dxe / E32 / bias_chain).sum(0)
+    check_param_grad(dg, dg_r, dg_a, dtype, chain, "dgamma")
+    check_param_grad(db, db_r, db_a, dtype, chain, "dbeta")
+    check_param_grad(dbias, dbi_r, dbi_a, dtype, bias_chain, "dbias")
+    # deterministic backward
+    torch.cuda.manual_seed(11)
+    again = _fused_case(nat, x, bias, res, w, b, dy, p)
+    assert torch.equal(summed, again[3])
+    for got, rep in zip((dsum, dx, dg, db, dbias), again[4:]):
+        assert torch.equal(got, rep)
+    if nvec not in (96, 192, 520) or p == 0:
+        return
+    # gradient sinks (one width per generation): sink = base + gradient with one rounding, nothing else written
+    arena = torch.randn(3 * cols + 64, device="cuda").to(dtype)
+    before = arena.clone()
+    views = (arena[16:16 + cols], arena[32 + cols:32 + 2 * cols], arena[48 + 2 * cols:48 + 3 * cols])
+    bases = [v.clone() for v in views]
+    torch.cuda.manual_seed(11)
+    fw = nat.bias_dropout_add_ln_fwd(x, bias, res, w, b, p, EPS)
+    assert torch.equal(fw[3], summed)
+    out = nat.bias_dropout_add_ln_bwd(dy, fw[3], fw[1], fw[2], w, p, fw[4], fw[5], True, *views)
+    assert torch.equal(out[0], dsum) and torch.equal(out[1], dx)  # same mask as the run above
+    for got, view, base, ref, absum, ch, what in zip(out[2:], views, bases, (dg_r, db_r, dbi_r),
+                                                     (dg_a, db_a, dbi_a), (chain, chain, bias_chain),
+                                                     ("dgamma", "dbeta", "dbias")):
+        assert got.data_ptr() == view.data_ptr()
+        check_param_grad(got, ref, absum, dtype, ch, what + " sink", base)
+    outside = torch.ones_like(arena, dtype=torch.bool)
+    for v in views:
+        outside[(v.data_ptr() - arena.data_ptr()) // arena.element_size():][:cols] = False
+    assert torch.equal(arena[outside], before[outside])
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
