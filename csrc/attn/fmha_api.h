@@ -80,10 +80,33 @@ struct FmhaFwdParams {
   // [B, C, H_kv, D] caches of the KV-cache mode (Lk = C).  Query i < T_b of sequence b sees key j iff j < n_b and
   // j <= p_b + i, with p_b as above and n_b = min(p_b + T_b, kv_cap); the bias is [bias_batch * H, Lq, Lb] (row i for
   // query i) and the key mask [B, kpm_cols].  cu_seqlens_k is not read.  No dropout, lse null.
+  // Paged caches (KV-cache mode, padded or packed; appended so that no earlier field moves): k / v are pools
+  // [num_blocks, block_size, H_kv, D] named by block_table [B, blocks_per_seq] (see fmha_paged_block below), and
+  // Lk = C = blocks_per_seq * block_size.  Every rule above holds with cache row j of sequence b read from row
+  // j % block_size of its block j / block_size.  block_size is a multiple of 128, so each key tile of the forward lies
+  // inside one block.  Null: the [B, C, H, D] caches above.
+  const int* block_table;
+  int block_size, blocks_per_seq, num_blocks;
 };
 void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream);
 
+// Paged key / value caches (fmha_kvcache_fwd, fmha_kvcache_varlen_fwd, fmha_decode and the cache append with a
+// block_table): a pool [num_blocks, block_size, H_kv, D] holds the rows of every sequence in blocks of block_size
+// rows (a multiple of 128), and block_table [B, M] (int32 on the device) names them: entry (b, i) is the block that
+// holds rows i * block_size .. (i + 1) * block_size - 1 of sequence b, -1 none.  The per-sequence capacity is
+// C = M * block_size, and with the rows so mapped every kernel computes what it computes on a [B, C, H_kv, D] cache:
+// bitwise the result of the contiguous call on the cache gathered through the table.  An entry outside
+// [0, num_blocks) never causes a write (the append skips that row); a read through it is clamped into the pool, so
+// its value is unspecified but no table value reaches outside a tensor.  The block allocator (kv_blocks.cu) never
+// hands out such entries.
 #ifdef __CUDACC__
+// the pool block of row `row` of sequence b, clamped into the pool (for reads)
+__device__ __forceinline__ int fmha_paged_block(const int* block_table, int b, int row, int block_size, int m,
+                                                int num_blocks) {
+  const int blk = block_table[(long long)b * m + row / block_size];
+  return blk < 0 ? 0 : (blk >= num_blocks ? num_blocks - 1 : blk);
+}
+
 // Varlen mode: {s_b, n_b} of sequence b (L = max_seqlen, N = packed rows), clamped as documented above, so that no
 // value of cu_seqlens makes a kernel reach outside a tensor
 __device__ __forceinline__ int2 fmha_varlen_seq(const int* cu_seqlens, int b, int L, int N) {
@@ -112,8 +135,34 @@ struct KvCacheAppendParams {
   int B, T, H, D, C;
   const int* cu_seqlens;   // [B + 1] int32 on the device, or null (padded [B, T, H, D] rows); appended so that no
   int packed_rows;         // earlier field moves.  packed_rows = N
+  // Paged caches (appended so that no earlier field moves): k_cache / v_cache are pools [num_blocks, block_size, H,
+  // D] (kc_sb / vc_sb the block strides) and row pos of sequence b goes to block block_table[b, pos / block_size],
+  // row pos % block_size; C = blocks_per_seq * block_size.  A row whose entry is outside [0, num_blocks) is skipped.
+  const int* block_table;  // [B, blocks_per_seq] int32 on the device, or null
+  int block_size, blocks_per_seq, num_blocks;
 };
 void launch_kv_cache_append(const KvCacheAppendParams& p, cudaStream_t stream);
+
+// Block allocator of paged caches (kv_blocks.cu).  One CTA each, no atomics: the sequences are walked in order with a
+// block-wide scan, so the block ids handed out depend only on the inputs, and nothing is read on the host (both can be
+// captured in a CUDA graph).  free_list [num_blocks] is a stack whose top is free_list[*free_count - 1]; *free_count
+// is clamped to [0, num_blocks] on entry, lengths[b] to [0, C] with C = blocks_per_seq * block_size.
+//  * reserve: every entry (b, i) with i < ceil(lengths[b] / block_size) and block_table[b, i] < 0 takes the next block
+//    off the top of the stack, in the order (b, i) ascending.  When the stack runs out the entry stays -1 and
+//    *overflow is set to 1 (it is never cleared here).
+//  * release: every entry (b, i) with i >= ceil(lengths[b] / block_size) becomes -1; the ones in [0, num_blocks) are
+//    pushed onto the stack in the order (b, i) ascending (a push past num_blocks, only possible for a table that names
+//    a block twice, is dropped).
+struct KvBlocksParams {
+  int* block_table;        // [B, blocks_per_seq]
+  int* free_list;          // [num_blocks]
+  int* free_count;         // [1]
+  int* overflow;           // [1] (reserve only)
+  const int* lengths;      // [B]
+  int B, blocks_per_seq, block_size, num_blocks;
+};
+void launch_kv_blocks_reserve(const KvBlocksParams& p, cudaStream_t stream);
+void launch_kv_blocks_release(const KvBlocksParams& p, cudaStream_t stream);
 
 struct FmhaBwdParams {
   FmhaFwdParams f;   // same inputs as forward (out/lse hold the forward results)
@@ -179,6 +228,12 @@ struct FmhaDecodeParams {
   // query head h reads cache head h / kv_group (grouped-query attention; the caches and k_new / v_new hold
   // H / kv_group heads); 1 = one cache head per query head
   int kv_group;
+  // Paged caches (appended so that no earlier field moves): k_cache / v_cache are pools [num_blocks, block_size,
+  // H_kv, D] (kc_sb / vc_sb the block strides), C = blocks_per_seq * block_size, and key j of sequence b is row
+  // j % block_size of block block_table[b, j / block_size] (fmha_paged_block).  The new row is stored only when its
+  // entry is in [0, num_blocks).  Null: [B, C, H, D] caches.
+  const int* block_table;
+  int block_size, blocks_per_seq, num_blocks;
 };
 constexpr int kDecodeCtasPerSm = 3;        // 72 KB of shared memory each
 constexpr int kDecodeMinSplitKeys = 256;   // the split heuristic makes no shorter split

@@ -230,6 +230,38 @@ int64_t check_cache_heads(const Tensor& q, int64_t B, const Tensor& v_cache) {
   return v_cache.size(2);
 }
 
+// Paged caches (fmha_api.h): with a block table (int32 [B, M >= 1] on the device of q), k_cache / v_cache are pools
+// [num_blocks, block_size, H_kv, D] with one block size, a multiple of 128.  Returns the leading extent the caches are
+// checked with afterwards: num_blocks, or B without a table.
+int64_t check_paged(const OptTensor& block_table, const Tensor& q, int64_t B, const Tensor& k_cache,
+                    const Tensor& v_cache) {
+  if (!has(block_table)) return B;
+  check_operand(*block_table, "block_table", q.device(), {at::kInt}, {B, kAnySize});
+  TORCH_CHECK(block_table->size(1) >= 1, "block_table must have M >= 1 columns");
+  check_operand(k_cache, "k_cache", q.device(), {q.scalar_type()}, any_shape(4), kAligned);
+  check_operand(v_cache, "v_cache", q.device(), {q.scalar_type()}, any_shape(4), kAligned);
+  const int64_t nb = v_cache.size(0), bs = v_cache.size(1);
+  TORCH_CHECK(nb >= 1 && k_cache.size(0) == nb && k_cache.size(1) == bs,
+              "paged k_cache / v_cache must be pools [num_blocks >= 1, block_size, H_kv, D] of the same shape");
+  TORCH_CHECK(bs >= 128 && bs % 128 == 0, "the block size of paged caches must be a multiple of 128, not ", bs);
+  TORCH_CHECK(block_table->size(1) * bs <= INT32_MAX, "block_table covers more rows than int32 indexes");
+  return nb;
+}
+
+// The per-sequence capacity: M * block_size with a block table, else the rows of the caches
+int64_t cache_capacity(const OptTensor& block_table, const Tensor& k_cache) {
+  return has(block_table) ? block_table->size(1) * k_cache.size(1) : k_cache.size(1);
+}
+
+// The paged fields of FmhaFwdParams, FmhaDecodeParams or KvCacheAppendParams (all null / 0 without a table)
+template <typename P>
+void set_paged(P& p, const OptTensor& block_table, const Tensor& k_cache) {
+  p.block_table = has(block_table) ? block_table->data_ptr<int>() : nullptr;
+  p.block_size = has(block_table) ? (int)k_cache.size(1) : 0;
+  p.blocks_per_seq = has(block_table) ? (int)block_table->size(1) : 0;
+  p.num_blocks = has(block_table) ? (int)k_cache.size(0) : 0;
+}
+
 // One query row per (b, h) against a [B, C, H_kv, D] key / value cache (fmha_api.h).  max_len is a host bound on
 // seqlens (the device values are never read here, so a decode step does not synchronise); with k_new / v_new the row
 // seqlens[b] is appended first and counts as visible, so up to max_len + 1 keys are.  num_splits = 0 picks the split
@@ -238,15 +270,18 @@ int64_t check_cache_heads(const Tensor& q, int64_t B, const Tensor& v_cache) {
 // true lengths are far below it); the split count still comes from the bound.
 Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& seqlens,
                    int64_t max_len, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
-                   const OptTensor& kpm, double scale, int64_t num_splits, bool split_by_length) {
+                   const OptTensor& kpm, double scale, int64_t num_splits, bool split_by_length,
+                   const OptTensor& block_table) {
   check_operand(q, "q", q.device(), k16Bit, {kAnySize, 1, kAnySize, kAnySize}, kAligned);
   const int64_t B = q.size(0), H = q.size(2), D = q.size(3);
   TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
   check_decode_operand(q, "q", q, kAnySize, H);
-  const int64_t H_kv = check_cache_heads(q, B, v_cache);
-  check_decode_operand(k_cache, "k_cache", q, kAnySize, H_kv);
-  const int64_t C = k_cache.size(1);
-  TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
+  const int64_t Bc = check_paged(block_table, q, B, k_cache, v_cache);
+  const int64_t H_kv = check_cache_heads(q, Bc, v_cache);
+  check_row_operand(k_cache, "k_cache", q, {Bc, kAnySize, H_kv, D});
+  TORCH_CHECK(v_cache.size(1) == k_cache.size(1) && k_cache.size(1) >= 1,
+              "k_cache / v_cache must have the same capacity C >= 1");
+  const int64_t C = cache_capacity(block_table, k_cache);
   const bool append = has(k_new);
   TORCH_CHECK(append == has(v_new), "k_new and v_new go together");
   TORCH_CHECK(!append || has(seqlens), "appending needs seqlens (the row to write)");
@@ -283,6 +318,7 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
   p.kc_sb = k_cache.stride(0); p.kc_sl = k_cache.stride(1); p.kc_sh = k_cache.stride(2);
   p.v_cache = v_cache.data_ptr();
   p.vc_sb = v_cache.stride(0); p.vc_sl = v_cache.stride(1); p.vc_sh = v_cache.stride(2);
+  set_paged(p, block_table, k_cache);
   if (append) {
     p.k_new = k_new->data_ptr();
     p.kn_sb = k_new->stride(0); p.kn_sh = k_new->stride(2);
@@ -328,18 +364,21 @@ Tensor fmha_decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache
 // ([..., H, D]): the [B, C, H_kv, D] caches (H_kv dividing H, one capacity C >= 1), k_new / v_new given together and
 // exactly when seqlens is, the host bound max_len + T <= C, a bias [1|B, H, T, Lb] with Lb % 8 == 0 (its TMA row
 // stride) and a bool key mask [B, Lk], each with a column for every key that can be visible.  k_new / v_new are the
-// caller's to check (their layout is the form's).  Returns {H_kv, kv_cap}.
+// caller's to check (their layout is the form's).  With a block table the caches are pools (check_paged) and C =
+// M * block_size.  Returns {H_kv, kv_cap}.
 std::pair<int64_t, int64_t> check_cache_chunk(const Tensor& q, int64_t B, int64_t T, const Tensor& k_cache,
                                               const Tensor& v_cache, const OptTensor& seqlens, int64_t max_len,
                                               const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
-                                              const OptTensor& kpm) {
+                                              const OptTensor& kpm, const OptTensor& block_table) {
   const int64_t H = q.size(-2);
   TORCH_CHECK(ub::fmha_head_dim_supported(q.size(-1)),
               "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
-  const int64_t H_kv = check_cache_heads(q, B, v_cache);
-  check_row_operand(k_cache, "k_cache", q, {B, kAnySize, H_kv, q.size(-1)});
-  const int64_t C = k_cache.size(1);
-  TORCH_CHECK(v_cache.size(1) == C && C >= 1, "k_cache / v_cache must have the same capacity C >= 1");
+  const int64_t Bc = check_paged(block_table, q, B, k_cache, v_cache);
+  const int64_t H_kv = check_cache_heads(q, Bc, v_cache);
+  check_row_operand(k_cache, "k_cache", q, {Bc, kAnySize, H_kv, q.size(-1)});
+  TORCH_CHECK(v_cache.size(1) == k_cache.size(1) && k_cache.size(1) >= 1,
+              "k_cache / v_cache must have the same capacity C >= 1");
+  const int64_t C = cache_capacity(block_table, k_cache);
   const bool append = has(k_new);
   TORCH_CHECK(append == has(v_new), "k_new and v_new go together");
   TORCH_CHECK(append == has(seqlens), "a chunk with seqlens appends k_new / v_new, and one without does not");
@@ -366,13 +405,16 @@ std::pair<int64_t, int64_t> check_cache_chunk(const Tensor& q, int64_t B, int64_
 // of its own), from [B, T, H_kv, D] or, with cu_seqlens, from packed [N, H_kv, D] rows.
 void run_cache_chunk(const Tensor& q4, int64_t B, int64_t T, const Tensor& k_cache, const Tensor& v_cache,
                      const OptTensor& seqlens, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
-                     const OptTensor& kpm, int64_t cap, double scale, const Tensor* cu_seqlens, Tensor& out) {
+                     const OptTensor& kpm, int64_t cap, double scale, const Tensor* cu_seqlens,
+                     const OptTensor& block_table, Tensor& out) {
   ub::FmhaFwdParams p{};
-  // q / k / v as the forward takes them (K / V maps over the C cache rows of the B caches); the bias has Lb columns,
-  // not C, so its map is made below
+  // q / k / v as the forward takes them (K / V maps over the C cache rows of the B caches, or over the block_size
+  // rows of the num_blocks pool blocks); the bias has Lb columns, not C, so its map is made below
   fill_common(p, q4, k_cache, v_cache, std::nullopt, kpm, 0.0, scale, /*forward=*/true);
   p.B = (int)B;
   p.Lq = (int)T;
+  p.Lk = (int)cache_capacity(block_table, k_cache);
+  set_paged(p, block_table, k_cache);
   if (has(bias)) {
     p.bias = bias->data_ptr();
     p.bias_batch = (int)bias->size(0);
@@ -406,6 +448,7 @@ void run_cache_chunk(const Tensor& q4, int64_t B, int64_t T, const Tensor& k_cac
     a.B = p.B; a.T = p.Lq; a.H = (int)k_cache.size(2); a.D = p.D; a.C = p.Lk;
     a.cu_seqlens = p.cu_seqlens;
     a.packed_rows = p.packed_rows;
+    set_paged(a, block_table, k_cache);
     ub::launch_kv_cache_append(a, cur_stream());
     check_launch("kv_cache_append");
   }
@@ -418,19 +461,20 @@ void run_cache_chunk(const Tensor& q4, int64_t B, int64_t T, const Tensor& k_cac
 // is a host bound on seqlens, as in fmha_decode.  The bias is [1|B, H, T, Lb] with Lb % 8 == 0 (its TMA row stride).
 Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const OptTensor& seqlens,
                         int64_t max_len, const OptTensor& k_new, const OptTensor& v_new, const OptTensor& bias,
-                        const OptTensor& kpm, double scale) {
+                        const OptTensor& kpm, double scale, const OptTensor& block_table) {
   check_operand(q, "q", q.device(), k16Bit, any_shape(4), kAligned);
   const int64_t B = q.size(0), T = q.size(1), H = q.size(2), D = q.size(3);
   TORCH_CHECK(T >= 2, "fmha_kvcache_fwd takes chunks of T >= 2 queries (fmha_decode takes T = 1)");
   check_decode_operand(q, "q", q, kAnySize, H);
-  const auto [H_kv, cap] = check_cache_chunk(q, B, T, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias, kpm);
+  const auto [H_kv, cap] = check_cache_chunk(q, B, T, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias, kpm,
+                                             block_table);
   if (has(k_new)) {
     check_decode_operand(*k_new, "k_new", q, T, H_kv);
     check_decode_operand(*v_new, "v_new", q, T, H_kv);
   }
   const c10::cuda::CUDAGuard guard(q.device());
   Tensor out = torch::empty({B, T, H, D}, q.options());
-  run_cache_chunk(q, B, T, k_cache, v_cache, seqlens, k_new, v_new, bias, kpm, cap, scale, nullptr, out);
+  run_cache_chunk(q, B, T, k_cache, v_cache, seqlens, k_new, v_new, bias, kpm, cap, scale, nullptr, block_table, out);
   check_launch("fmha_kvcache_fwd");
   return out;
 }
@@ -444,7 +488,8 @@ Tensor fmha_kvcache_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_
 // sequence) with Lb % 8 == 0, the key mask [B, Lk].  Returns [N, H, D]; rows of no sequence are not written.
 Tensor fmha_kvcache_varlen_fwd(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cu_seqlens,
                                int64_t max_seqlen, const OptTensor& seqlens, int64_t max_len, const OptTensor& k_new,
-                               const OptTensor& v_new, const OptTensor& bias, const OptTensor& kpm, double scale) {
+                               const OptTensor& v_new, const OptTensor& bias, const OptTensor& kpm, double scale,
+                               const OptTensor& block_table) {
   check_operand(q, "q", q.device(), k16Bit, any_shape(3), kAligned);
   const int64_t N = q.size(0), H = q.size(1), D = q.size(2);
   check_row_operand(q, "q", q, {kAnySize, H, D});
@@ -455,7 +500,7 @@ Tensor fmha_kvcache_varlen_fwd(const Tensor& q, const Tensor& k_cache, const Ten
   TORCH_CHECK(B >= 1, "cu_seqlens must have B + 1 >= 2 entries");
   TORCH_CHECK(max_seqlen >= 1, "max_seqlen must be positive");
   const auto [H_kv, cap] = check_cache_chunk(q, B, max_seqlen, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
-                                             kpm);
+                                             kpm, block_table);
   if (has(k_new)) {
     check_row_operand(*k_new, "k_new", q, {N, H_kv, D});
     check_row_operand(*v_new, "v_new", q, {N, H_kv, D});
@@ -463,9 +508,86 @@ Tensor fmha_kvcache_varlen_fwd(const Tensor& q, const Tensor& k_cache, const Ten
   const c10::cuda::CUDAGuard guard(q.device());
   Tensor out = torch::empty({N, H, D}, q.options());
   run_cache_chunk(q.unsqueeze(0), B, max_seqlen, k_cache, v_cache, seqlens, k_new, v_new, bias, kpm, cap, scale,
-                  &cu_seqlens, out);
+                  &cu_seqlens, block_table, out);
   check_launch("fmha_kvcache_varlen_fwd");
   return out;
+}
+
+// The append of fmha_kvcache_fwd alone: rows i of k_new / v_new [B, T, H_kv, D] go to rows seqlens[b] + i of the
+// [B, C, H_kv, D] caches, or with a block table through it into the pools (fmha_api.h); rows at or past C, and rows
+// whose table entry is outside the pool, are skipped.  Bitwise.
+void kv_cache_append(const Tensor& k_new, const Tensor& v_new, const Tensor& k_cache, const Tensor& v_cache,
+                     const Tensor& seqlens, const OptTensor& block_table) {
+  check_operand(k_new, "k_new", k_new.device(), k16Bit, any_shape(4), kAligned);
+  const int64_t B = k_new.size(0), T = k_new.size(1), H_kv = k_new.size(2), D = k_new.size(3);
+  TORCH_CHECK(ub::fmha_head_dim_supported(D), "head_dim must be a multiple of 8 from 8 to 128 (8, 16, ..., 128)");
+  TORCH_CHECK(B >= 1 && T >= 1, "k_new must have B >= 1 sequences of T >= 1 rows");
+  check_row_operand(k_new, "k_new", k_new, {B, T, H_kv, D});
+  check_row_operand(v_new, "v_new", k_new, {B, T, H_kv, D});
+  const int64_t Bc = check_paged(block_table, k_new, B, k_cache, v_cache);
+  check_row_operand(k_cache, "k_cache", k_new, {Bc, kAnySize, H_kv, D});
+  check_row_operand(v_cache, "v_cache", k_new, {Bc, k_cache.size(1), H_kv, D});
+  TORCH_CHECK(k_cache.size(1) >= 1, "k_cache / v_cache must have C >= 1 rows");
+  check_operand(seqlens, "seqlens", k_new.device(), {at::kInt}, {B});
+  const c10::cuda::CUDAGuard guard(k_new.device());
+  ub::KvCacheAppendParams a{};
+  a.k_new = k_new.data_ptr();
+  a.v_new = v_new.data_ptr();
+  a.k_cache = k_cache.data_ptr();
+  a.v_cache = v_cache.data_ptr();
+  a.seqlens = seqlens.data_ptr<int>();
+  a.kn_sb = k_new.stride(0); a.kn_sl = k_new.stride(1); a.kn_sh = k_new.stride(2);
+  a.vn_sb = v_new.stride(0); a.vn_sl = v_new.stride(1); a.vn_sh = v_new.stride(2);
+  a.kc_sb = k_cache.stride(0); a.kc_sl = k_cache.stride(1); a.kc_sh = k_cache.stride(2);
+  a.vc_sb = v_cache.stride(0); a.vc_sl = v_cache.stride(1); a.vc_sh = v_cache.stride(2);
+  a.B = (int)B; a.T = (int)T; a.H = (int)H_kv; a.D = (int)D; a.C = (int)cache_capacity(block_table, k_cache);
+  set_paged(a, block_table, k_cache);
+  ub::launch_kv_cache_append(a, cur_stream());
+  check_launch("kv_cache_append");
+}
+
+// The block allocator of paged caches (fmha_api.h): block_table int32 [B, M], free_list int32 [num_blocks >= 1],
+// free_count and overflow int32 [1], lengths int32 [B], all contiguous on one device.
+ub::KvBlocksParams check_kv_blocks(const Tensor& block_table, const Tensor& free_list, const Tensor& free_count,
+                                   const Tensor& lengths, int64_t block_size, const Tensor* overflow) {
+  const c10::Device dev = block_table.device();
+  check_operand(block_table, "block_table", dev, {at::kInt}, any_shape(2));
+  const int64_t B = block_table.size(0), M = block_table.size(1);
+  TORCH_CHECK(B >= 1 && M >= 1, "block_table must be [B >= 1, M >= 1]");
+  check_operand(free_list, "free_list", dev, {at::kInt}, {kAnySize});
+  TORCH_CHECK(free_list.size(0) >= 1 && free_list.size(0) <= INT32_MAX, "free_list must have num_blocks >= 1 entries");
+  check_operand(free_count, "free_count", dev, {at::kInt}, {1}, kContig | kNumel);
+  check_operand(lengths, "lengths", dev, {at::kInt}, {B});
+  if (overflow != nullptr) check_operand(*overflow, "overflow", dev, {at::kInt}, {1}, kContig | kNumel);
+  TORCH_CHECK(block_size >= 1 && M * block_size <= INT32_MAX,
+              "block_size must be positive, and M * block_size fit int32");
+  ub::KvBlocksParams p{};
+  p.block_table = block_table.data_ptr<int>();
+  p.free_list = free_list.data_ptr<int>();
+  p.free_count = free_count.data_ptr<int>();
+  p.overflow = overflow != nullptr ? overflow->data_ptr<int>() : nullptr;
+  p.lengths = lengths.data_ptr<int>();
+  p.B = (int)B;
+  p.blocks_per_seq = (int)M;
+  p.block_size = (int)block_size;
+  p.num_blocks = (int)free_list.size(0);
+  return p;
+}
+
+void kv_blocks_reserve(const Tensor& block_table, const Tensor& free_list, const Tensor& free_count,
+                       const Tensor& lengths, int64_t block_size, const Tensor& overflow) {
+  const ub::KvBlocksParams p = check_kv_blocks(block_table, free_list, free_count, lengths, block_size, &overflow);
+  const c10::cuda::CUDAGuard guard(block_table.device());
+  ub::launch_kv_blocks_reserve(p, cur_stream());
+  check_launch("kv_blocks_reserve");
+}
+
+void kv_blocks_release(const Tensor& block_table, const Tensor& free_list, const Tensor& free_count,
+                       const Tensor& lengths, int64_t block_size) {
+  const ub::KvBlocksParams p = check_kv_blocks(block_table, free_list, free_count, lengths, block_size, nullptr);
+  const c10::cuda::CUDAGuard guard(block_table.device());
+  ub::launch_kv_blocks_release(p, cur_stream());
+  check_launch("kv_blocks_release");
 }
 // ---- varlen: packed sequences described by cu_seqlens (fmha_api.h) ------------------------------------------------
 // q [N_q, H, D], k / v [N_k, H_kv, D] (head slices of one projection are fine), cu_seqlens int32 [B + 1] on the
@@ -640,16 +762,25 @@ void register_fmha(pybind11::module_& m) {
         py::arg("need_dbias"), py::arg("packed_grad"), py::arg("dlogits") = py::none(), py::arg("causal") = false);
   m.def("fmha_decode", &fmha_decode, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("seqlens"),
         py::arg("max_len"), py::arg("k_new"), py::arg("v_new"), py::arg("bias"), py::arg("key_padding_mask"),
-        py::arg("scale"), py::arg("num_splits") = 0, py::arg("split_by_length") = false);
+        py::arg("scale"), py::arg("num_splits") = 0, py::arg("split_by_length") = false,
+        py::arg("block_table") = py::none());
   // its own submodule, _C.kvcache; tests/test_gpu_attention_kvcache_chunk.py runs the operand-rejection table of
   // tests/test_gpu_bindings.py over it
   auto kv = m.def_submodule("kvcache", "multi-token steps into a key / value cache");
   kv.def("fmha_kvcache_fwd", &fmha_kvcache_fwd, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"),
          py::arg("seqlens"), py::arg("max_len"), py::arg("k_new"), py::arg("v_new"), py::arg("bias"),
-         py::arg("key_padding_mask"), py::arg("scale"));
+         py::arg("key_padding_mask"), py::arg("scale"), py::arg("block_table") = py::none());
   kv.def("fmha_kvcache_varlen_fwd", &fmha_kvcache_varlen_fwd, py::arg("q"), py::arg("k_cache"), py::arg("v_cache"),
          py::arg("cu_seqlens"), py::arg("max_seqlen"), py::arg("seqlens"), py::arg("max_len"), py::arg("k_new"),
-         py::arg("v_new"), py::arg("bias"), py::arg("key_padding_mask"), py::arg("scale"));
+         py::arg("v_new"), py::arg("bias"), py::arg("key_padding_mask"), py::arg("scale"),
+         py::arg("block_table") = py::none());
+  // paged caches: the append on its own (a prefill's rows, a reorder's rows written back) and the block allocator
+  kv.def("kv_cache_append", &kv_cache_append, py::arg("k_new"), py::arg("v_new"), py::arg("k_cache"),
+         py::arg("v_cache"), py::arg("seqlens"), py::arg("block_table") = py::none());
+  kv.def("kv_blocks_reserve", &kv_blocks_reserve, py::arg("block_table"), py::arg("free_list"), py::arg("free_count"),
+         py::arg("lengths"), py::arg("block_size"), py::arg("overflow"));
+  kv.def("kv_blocks_release", &kv_blocks_release, py::arg("block_table"), py::arg("free_list"), py::arg("free_count"),
+         py::arg("lengths"), py::arg("block_size"));
   // packed variable-length sequences: its own submodule, _C.varlen
   auto vl = m.def_submodule("varlen", "packed variable-length sequences described by cu_seqlens");
   vl.def("fmha_varlen_fwd", &fmha_varlen_fwd, py::arg("q"), py::arg("k"), py::arg("v"), py::arg("cu_seqlens"),

@@ -23,6 +23,11 @@
 //     stage straight from k_new / v_new (not from the cache), and the one of the first query head of the group stores
 //     it bitwise into the caches.  No CTA reads row pos of (b, h / G) from the caches - every other key range ends
 //     before it - so the write needs no ordering against any read, and one launch both appends and attends.
+//   * Paged caches (kPaged, fmha_api.h): the row of key j is row j % block_size of pool block
+//     block_table[b, j / block_size].  Warp 0 loads the blocks of tile t + kStages before the math of tile t and
+//     issues its copies after it, so the table load's latency is hidden; the owner stores the new row through the
+//     table too, and skips the store when its entry is outside the pool.  Ranges, splits and the combine are
+//     unchanged.
 //   * Bounds: n_b is clamped to the cache capacity C (and to the columns of the bias / key mask), pos to n_b - 1, for
 //     any device value of seqlens: no read or write outside the tensors.  A row whose visible keys are all masked
 //     gives O = 0.
@@ -31,6 +36,7 @@
 #include <math_constants.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "../common.cuh"
 #include "fmha_api.h"
@@ -59,7 +65,7 @@ struct DecCfg {
 
 UB_DEVICE int clampi(int x, int lo, int hi) { return x < lo ? lo : (x > hi ? hi : x); }
 
-template <typename T, int NC>
+template <typename T, int NC, bool kPaged>
 __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeParams p) {
   using C = DecCfg<NC>;
   extern __shared__ __align__(16) unsigned char smem[];
@@ -82,18 +88,41 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeP
   const int start = s * chunk;
   const int end = s == p.num_splits - 1 ? n : min(start + chunk, n);
 
-  const T* kc = reinterpret_cast<const T*>(p.k_cache) + (long long)b * p.kc_sb + (long long)hk * p.kc_sh;
-  const T* vc = reinterpret_cast<const T*>(p.v_cache) + (long long)b * p.vc_sb + (long long)hk * p.vc_sh;
+  // contiguous: batch b of the caches; paged: the pools, whose block is chosen per row
+  const long long kc_b = kPaged ? 0LL : (long long)b * p.kc_sb, vc_b = kPaged ? 0LL : (long long)b * p.vc_sb;
+  const T* kc = reinterpret_cast<const T*>(p.k_cache) + kc_b + (long long)hk * p.kc_sh;
+  const T* vc = reinterpret_cast<const T*>(p.v_cache) + vc_b + (long long)hk * p.vc_sh;
+  // offsets (elements) of row `key` from kc / vc
+  auto k_row = [&](int key) -> long long {
+    if constexpr (kPaged)
+      return (long long)fmha_paged_block(p.block_table, b, key, p.block_size, p.blocks_per_seq, p.num_blocks) *
+                 p.kc_sb + (long long)(key % p.block_size) * p.kc_sl;
+    else
+      return (long long)key * p.kc_sl;
+  };
+  auto v_row = [&](int key) -> long long {
+    if constexpr (kPaged)
+      return (long long)fmha_paged_block(p.block_table, b, key, p.block_size, p.blocks_per_seq, p.num_blocks) *
+                 p.vc_sb + (long long)(key % p.block_size) * p.vc_sl;
+    else
+      return (long long)key * p.vc_sl;
+  };
   const T* kn = append ? reinterpret_cast<const T*>(p.k_new) + (long long)b * p.kn_sb + (long long)hk * p.kn_sh : nullptr;
   const T* vn = append ? reinterpret_cast<const T*>(p.v_new) + (long long)b * p.vn_sb + (long long)hk * p.vn_sh : nullptr;
   // one CTA of the group stores the new row; the other G - 1 take it from k_new / v_new into their stage only
-  const bool owner = append && gq == 0 && start <= pos && pos < end;
+  bool owner = append && gq == 0 && start <= pos && pos < end;
+  if constexpr (kPaged) {   // no write through an entry outside the pool
+    if (owner) {
+      const int blk = p.block_table[(long long)b * p.blocks_per_seq + pos / p.block_size];
+      owner = blk >= 0 && blk < p.num_blocks;
+    }
+  }
   if (owner && tid < 2 * nch) {
     // bitwise copy of the new row into the caches (see the append invariant above)
     const int c = tid % nch;
     const bool is_v = tid >= nch;
     const Vec16 w = ld_global_v4((is_v ? vn : kn) + 8 * c);
-    T* dst = const_cast<T*>(is_v ? vc + (long long)pos * p.vc_sl : kc + (long long)pos * p.kc_sl);
+    T* dst = const_cast<T*>(is_v ? vc + v_row(pos) : kc + k_row(pos));
     st_global_v4(dst + 8 * c, w);
   }
 
@@ -108,8 +137,45 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeP
     for (int r = lane; r < nrows; r += 32) {
       const int key = r0 + r;
       const bool is_new = key == pos;
-      bulk_g2s(dk + r * row_bytes, is_new ? kn : kc + (long long)key * p.kc_sl, row_bytes, bar);
-      bulk_g2s(dv + r * row_bytes, is_new ? vn : vc + (long long)key * p.vc_sl, row_bytes, bar);
+      bulk_g2s(dk + r * row_bytes, is_new ? kn : kc + k_row(key), row_bytes, bar);
+      bulk_g2s(dv + r * row_bytes, is_new ? vn : vc + v_row(key), row_bytes, bar);
+    }
+  };
+  // paged: lane l of warp 0 copies rows l and l + 32 of a tile; their pool blocks are loaded a tile ahead (before the
+  // math of tile t for the copies of tile t + kStages), so the table load's latency does not hold up warp 0
+  // A tile (kTile <= 64 rows) spans at most two blocks (block_size >= 128), so one division per tile places its rows.
+  constexpr int kRowsPerLane = C::kTile / 32;
+  auto row_blocks = [&](int t, int (&blk)[kRowsPerLane], int (&row)[kRowsPerLane]) {
+    const int r0 = start + t * C::kTile, nrows = min(C::kTile, end - r0);
+    const int e0 = r0 / p.block_size, off0 = r0 - e0 * p.block_size;
+#pragma unroll
+    for (int i = 0; i < kRowsPerLane; ++i) {
+      const int r = lane + 32 * i, o = off0 + r;
+      const bool next = o >= p.block_size;
+      row[i] = next ? o - p.block_size : o;
+      blk[i] = 0;
+      if (r < nrows) {
+        const int x = p.block_table[(long long)b * p.blocks_per_seq + e0 + (next ? 1 : 0)];
+        blk[i] = x < 0 ? 0 : (x >= p.num_blocks ? p.num_blocks - 1 : x);   // fmha_paged_block's clamp
+      }
+    }
+  };
+  auto issue_paged = [&](int t, const int (&blk)[kRowsPerLane], const int (&row)[kRowsPerLane]) {
+    const int st = t % kStages, r0 = start + t * C::kTile, nrows = min(C::kTile, end - r0);
+    const uint32_t bar = bar0 + 8 * st, dk = smem0 + st * C::kStageBytes, dv = dk + C::kTile * row_bytes;
+    if (lane == 0) bulk_expect_tx(bar, 2u * nrows * row_bytes);
+    __syncwarp();
+#pragma unroll
+    for (int i = 0; i < kRowsPerLane; ++i) {
+      const int r = lane + 32 * i;
+      if (r < nrows) {
+        const int key = r0 + r;
+        const bool is_new = key == pos;
+        const T* ks = is_new ? kn : kc + blk[i] * p.kc_sb + (long long)row[i] * p.kc_sl;
+        const T* vs = is_new ? vn : vc + blk[i] * p.vc_sb + (long long)row[i] * p.vc_sl;
+        bulk_g2s(dk + r * row_bytes, ks, row_bytes, bar);
+        bulk_g2s(dv + r * row_bytes, vs, row_bytes, bar);
+      }
     }
   };
   if (tid == 0) {
@@ -117,8 +183,19 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeP
     bulk_bar_init_fence();
   }
   __syncthreads();
-  if (tid < 32)
-    for (int t = 0; t < min(kStages, ntiles); ++t) issue(t);
+  if (tid < 32) {
+    if constexpr (kPaged) {   // every table load of the first stages first, so that their latencies overlap
+      int blk[kStages][kRowsPerLane], row[kStages][kRowsPerLane];
+#pragma unroll
+      for (int t = 0; t < kStages; ++t)
+        if (t < ntiles) row_blocks(t, blk[t], row[t]);
+#pragma unroll
+      for (int t = 0; t < kStages; ++t)
+        if (t < ntiles) issue_paged(t, blk[t], row[t]);
+    } else {
+      for (int t = 0; t < min(kStages, ntiles); ++t) issue(t);
+    }
+  }
 
   // ---- query chunks of this lane, pre-scaled by scale * log2e ------------------------------------------------------
   const float qs = p.scale * kLog2e;
@@ -147,6 +224,10 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeP
 
   float m = -CUDART_INF_F, l = 0.f;
   for (int t = 0; t < ntiles; ++t) {
+    int next_blk[kRowsPerLane], next_row[kRowsPerLane];   // paged: tile t + kStages's rows, placed before the math
+    if constexpr (kPaged) {
+      if (tid < 32 && t + kStages < ntiles) row_blocks(t + kStages, next_blk, next_row);
+    }
     const int st = t % kStages, r0 = start + t * C::kTile, nrows = min(C::kTile, end - r0);
     bulk_wait(bar0 + 8 * st, (t / kStages) & 1);
     const unsigned char* sk = smem + st * C::kStageBytes;
@@ -209,7 +290,10 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_kernel(const FmhaDecodeP
       m = m_new;
     }
     __syncthreads();   // every thread is done with stage st
-    if (tid < 32 && t + kStages < ntiles) issue(t + kStages);
+    if (tid < 32 && t + kStages < ntiles) {
+      if constexpr (kPaged) issue_paged(t + kStages, next_blk, next_row);
+      else issue(t + kStages);
+    }
   }
 
   // ---- merge the 16 group states in group order --------------------------------------------------------------------
@@ -280,8 +364,9 @@ __global__ void __launch_bounds__(kThreads) fmha_decode_combine_kernel(const Fmh
 
 // Row i of k_new / v_new -> row p_b + i of the caches (fmha_api.h).  CTA (i, b) copies all H cache heads of K and V,
 // one 16-byte vector per thread and step; a row at or past C is skipped.  kPacked: k_new / v_new are packed [N, H, D]
-// and sequence b's rows are s_b + i, i < T_b ({s_b, T_b} = fmha_varlen_seq(cu_seqlens, b, T, N)).
-template <bool kPacked>
+// and sequence b's rows are s_b + i, i < T_b ({s_b, T_b} = fmha_varlen_seq(cu_seqlens, b, T, N)).  kPaged: the row
+// goes through the block table into the pools, and a row whose entry is outside the pool is skipped.
+template <bool kPacked, bool kPaged>
 __global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCacheAppendParams p) {
   const int i = blockIdx.x, b = blockIdx.y;
   int s_b = 0;   // packed: the first row of sequence b in k_new / v_new, whose batch stride is 0
@@ -292,6 +377,13 @@ __global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCache
   }
   const int pos = min(max(p.seqlens[b], 0), p.C) + i;
   if (pos >= p.C) return;
+  long long cb = b, cl = pos;   // cache batch (pool block) and row
+  if constexpr (kPaged) {   // a row whose entry is outside the pool is skipped
+    const int blk = p.block_table[(long long)b * p.blocks_per_seq + pos / p.block_size];
+    if (blk < 0 || blk >= p.num_blocks) return;
+    cb = blk;
+    cl = pos % p.block_size;
+  }
   const int nch = p.D / 8, per = p.H * nch;   // 16-byte chunks of one row of one tensor
   for (int x = threadIdx.x; x < 2 * per; x += kThreads) {
     const bool is_v = x >= per;
@@ -300,7 +392,7 @@ __global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCache
                           (long long)b * (is_v ? p.vn_sb : p.kn_sb) + (long long)(s_b + i) * (is_v ? p.vn_sl : p.kn_sl) +
                           (long long)h * (is_v ? p.vn_sh : p.kn_sh) + 8 * c;
     uint16_t* dst = reinterpret_cast<uint16_t*>(is_v ? p.v_cache : p.k_cache) +
-                    (long long)b * (is_v ? p.vc_sb : p.kc_sb) + (long long)pos * (is_v ? p.vc_sl : p.kc_sl) +
+                    cb * (is_v ? p.vc_sb : p.kc_sb) + cl * (is_v ? p.vc_sl : p.kc_sl) +
                     (long long)h * (is_v ? p.vc_sh : p.kc_sh) + 8 * c;
     st_global_v4(dst, ld_global_v4(src));
   }
@@ -309,8 +401,14 @@ __global__ void __launch_bounds__(kThreads) kv_cache_append_kernel(const KvCache
 }  // namespace
 
 void launch_kv_cache_append(const KvCacheAppendParams& p, cudaStream_t stream) {
-  if (p.cu_seqlens != nullptr) kv_cache_append_kernel<true><<<dim3(p.T, p.B), kThreads, 0, stream>>>(p);
-  else kv_cache_append_kernel<false><<<dim3(p.T, p.B), kThreads, 0, stream>>>(p);
+  const dim3 grid(p.T, p.B);
+  if (p.block_table != nullptr) {
+    if (p.cu_seqlens != nullptr) kv_cache_append_kernel<true, true><<<grid, kThreads, 0, stream>>>(p);
+    else kv_cache_append_kernel<false, true><<<grid, kThreads, 0, stream>>>(p);
+  } else {
+    if (p.cu_seqlens != nullptr) kv_cache_append_kernel<true, false><<<grid, kThreads, 0, stream>>>(p);
+    else kv_cache_append_kernel<false, false><<<grid, kThreads, 0, stream>>>(p);
+  }
 }
 
 int fmha_decode_num_splits(int B, int H, int len_bound, int num_sms) {
@@ -330,13 +428,18 @@ void launch_fmha_decode(const FmhaDecodeParams& p, cudaStream_t stream) {
     kern<<<grid, kThreads, smem_bytes, stream>>>(p);
     if (p.num_splits > 1) combine<<<dim3(p.H, p.B), kThreads, 0, stream>>>(p);
   };
-  if (p.D <= 64) {
-    if (p.is_bf16) run(fmha_decode_kernel<__nv_bfloat16, 1>, fmha_decode_combine_kernel<__nv_bfloat16>, DecCfg<1>::kSmemBytes);
-    else run(fmha_decode_kernel<__half, 1>, fmha_decode_combine_kernel<__half>, DecCfg<1>::kSmemBytes);
-  } else {
-    if (p.is_bf16) run(fmha_decode_kernel<__nv_bfloat16, 2>, fmha_decode_combine_kernel<__nv_bfloat16>, DecCfg<2>::kSmemBytes);
-    else run(fmha_decode_kernel<__half, 2>, fmha_decode_combine_kernel<__half>, DecCfg<2>::kSmemBytes);
-  }
+  auto by_type = [&](auto paged) {
+    constexpr bool kPg = decltype(paged)::value;
+    if (p.D <= 64) {
+      if (p.is_bf16) run(fmha_decode_kernel<__nv_bfloat16, 1, kPg>, fmha_decode_combine_kernel<__nv_bfloat16>, DecCfg<1>::kSmemBytes);
+      else run(fmha_decode_kernel<__half, 1, kPg>, fmha_decode_combine_kernel<__half>, DecCfg<1>::kSmemBytes);
+    } else {
+      if (p.is_bf16) run(fmha_decode_kernel<__nv_bfloat16, 2, kPg>, fmha_decode_combine_kernel<__nv_bfloat16>, DecCfg<2>::kSmemBytes);
+      else run(fmha_decode_kernel<__half, 2, kPg>, fmha_decode_combine_kernel<__half>, DecCfg<2>::kSmemBytes);
+    }
+  };
+  if (p.block_table != nullptr) by_type(std::true_type{});
+  else by_type(std::false_type{});
 }
 
 }  // namespace ub

@@ -110,11 +110,16 @@ UB_DEVICE void quad_transpose4(uint32_t (&w)[4], int c) {
 // i, CTAs past n_q exit, only rows below n_q are stored); keys and values come from the caches at batch coordinate b,
 // and the visibility, tile count, stale-row handling and tile order are the KV-cache mode's with T_b = n_q in place of
 // Lq.  The varlen key description (cu_seqlens_k) is not read.
-template <typename T, int DP, bool kLogits, bool kCausal, bool kKVCache, bool kVarlen = false>
+// kPaged (with kKVCache, padded or packed): k / v are pools [num_blocks, block_size, H_kv, D] (fmha_api.h).  Key tile
+// j lies inside one block (block_size is a multiple of kBlockN), so load_tile takes the batch coordinate of its K / V
+// boxes from the block table and the row from j * kBlockN % block_size; the tiles, their order and the arithmetic are
+// the contiguous call's.
+template <typename T, int DP, bool kLogits, bool kCausal, bool kKVCache, bool kVarlen = false, bool kPaged = false>
 __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_constant__ FmhaFwdParams p) {
   static_assert(!(kLogits && kCausal), "causal attention is not instantiated in logits mode");
   static_assert(!(kKVCache && (kLogits || kCausal)), "the KV-cache mode is neither causal nor logits mode");
   static_assert(!(kVarlen && kLogits), "the varlen mode is not logits mode");
+  static_assert(!kPaged || kKVCache, "paged caches are a KV-cache mode");
   using C = FwdCfg<DP>;
   constexpr int kBlockN = C::kBlockN;
   constexpr int kWords = kBlockN / 32;   // keep-bit words per row of a key tile
@@ -165,16 +170,26 @@ __global__ void __launch_bounds__(kFwdThreads, 2) fmha_fwd_kernel(const __grid_c
   const int bias_nb = (p.bias_batch > 1 ? b : 0) * p.H + h;
   // the TMA unit counts the zero-filled columns D..DP-1 of a box as transferred bytes
   constexpr uint32_t kKVBytes = C::kKVStage, kBiasBytes = C::kBiasStage, kQBytes = C::kBoxes * C::kQBox;
+  // paged: the pool block of key tile j.  Thread 0 loads the block of tile j + 2 right after requesting tile j + 1, so
+  // the table load's latency passes during tile j's math instead of delaying the next request (and the warpgroup)
+  auto tile_block = [&](int j) {
+    return fmha_paged_block(p.block_table, b, j * kBlockN, p.block_size, p.blocks_per_seq, p.num_blocks);
+  };
+  int next_block = 0;
   auto load_tile = [&](int j) {   // one thread; the first tile's phase also covers Q (one arrival per phase)
     const uint32_t st = (uint32_t)(j & 1), bar = bar0 + 8u * st;
     mbar_expect_tx(bar, 2 * kKVBytes + (has_bias ? kBiasBytes : 0u) + (j == 0 ? kQBytes : 0u));
+    int kv_row = vk_s + j * kBlockN, kv_b = tbk;   // paged: the tile's block and its row inside it
+    if constexpr (kPaged) {
+      kv_b = j == 0 ? tile_block(0) : next_block;
+      kv_row = j * kBlockN % p.block_size;
+      if (j + 1 < n_tiles) next_block = tile_block(j + 1);
+    }
 #pragma unroll
     for (int x = 0; x < C::kBoxes; ++x) {   // column boxes 0..63 and 64..127
       if (j == 0) tma_load_4d(smem_base + C::kSmemQ + x * C::kQBox, &p.sw_q, 64 * x, h, vl_s + q0, tb, bar);
-      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, vk_s + j * kBlockN, tbk,
-                  bar);
-      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, vk_s + j * kBlockN, tbk,
-                  bar);
+      tma_load_4d(smem_base + C::kSmemK + st * C::kKVStage + x * C::kKVBox, &p.sw_k, 64 * x, hk, kv_row, kv_b, bar);
+      tma_load_4d(smem_base + C::kSmemV + st * C::kKVStage + x * C::kKVBox, &p.sw_v, 64 * x, hk, kv_row, kv_b, bar);
     }
     if (has_bias) {   // 64 rows x kBlockN keys = kBlockN / 64 boxes of 64 keys
 #pragma unroll
@@ -453,29 +468,32 @@ void launch_fmha_fwd(const FmhaFwdParams& p, cudaStream_t stream) {
     cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes);
     kern<<<grid, kFwdThreads, smem_bytes, stream>>>(p);
   };
-  auto dispatch = [&](auto logits, auto causal, auto kvcache, auto varlen) {
+  auto dispatch = [&](auto logits, auto causal, auto kvcache, auto varlen, auto paged) {
     constexpr bool kLogits = decltype(logits)::value, kCausal = decltype(causal)::value;
-    constexpr bool kKV = decltype(kvcache)::value, kVL = decltype(varlen)::value;
+    constexpr bool kKV = decltype(kvcache)::value, kVL = decltype(varlen)::value, kPg = decltype(paged)::value;
     if (p.D <= 64) {
-      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits, kCausal, kKV, kVL>, FwdCfg<64>::kSmemBytes);
-      else run(fmha_fwd_kernel<__half, 64, kLogits, kCausal, kKV, kVL>, FwdCfg<64>::kSmemBytes);
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 64, kLogits, kCausal, kKV, kVL, kPg>, FwdCfg<64>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 64, kLogits, kCausal, kKV, kVL, kPg>, FwdCfg<64>::kSmemBytes);
     } else {
-      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits, kCausal, kKV, kVL>, FwdCfg<128>::kSmemBytes);
-      else run(fmha_fwd_kernel<__half, 128, kLogits, kCausal, kKV, kVL>, FwdCfg<128>::kSmemBytes);
+      if (p.is_bf16) run(fmha_fwd_kernel<__nv_bfloat16, 128, kLogits, kCausal, kKV, kVL, kPg>, FwdCfg<128>::kSmemBytes);
+      else run(fmha_fwd_kernel<__half, 128, kLogits, kCausal, kKV, kVL, kPg>, FwdCfg<128>::kSmemBytes);
     }
   };
   // causal + logits is refused by the binding (fmha_bind.cpp); the KV-cache mode sets neither, and the varlen
   // bindings never set logits
   const std::false_type no;
   const std::true_type yes;
+  const bool paged = p.kvcache && p.block_table != nullptr;   // the bindings set a block table in KV-cache mode only
   if (p.varlen) {
-    if (p.kvcache) dispatch(no, no, yes, yes);
-    else if (p.causal) dispatch(no, yes, no, yes);
-    else dispatch(no, no, no, yes);
-  } else if (p.kvcache) dispatch(no, no, yes, no);
-  else if (p.logits != nullptr) dispatch(yes, no, no, no);
-  else if (p.causal) dispatch(no, yes, no, no);
-  else dispatch(no, no, no, no);
+    if (paged) dispatch(no, no, yes, yes, yes);
+    else if (p.kvcache) dispatch(no, no, yes, yes, no);
+    else if (p.causal) dispatch(no, yes, no, yes, no);
+    else dispatch(no, no, no, yes, no);
+  } else if (paged) dispatch(no, no, yes, no, yes);
+  else if (p.kvcache) dispatch(no, no, yes, no, no);
+  else if (p.logits != nullptr) dispatch(yes, no, no, no, no);
+  else if (p.causal) dispatch(no, yes, no, no, no);
+  else dispatch(no, no, no, no, no);
 }
 
 }  // namespace ub

@@ -52,7 +52,10 @@ and every packed call attends to them with ``key_padding_mask [B, S]`` (``ops.at
 
 ``DecoderCache`` holds what incremental decoding keeps between steps: per layer the self-attention keys and values
 ``[B, C, H_kv, D]`` and the projected encoder keys and values, the device lengths and a host bound on them.  A step may
-add one token or a chunk of several per sequence, and ``rewind`` drops tokens again.
+add one token or a chunk of several per sequence, and ``rewind`` drops tokens again.  A paged ``DecoderCache``
+(``block_size`` set) keeps the self-attention keys and values in pools ``[num_blocks, block_size, H_kv, D]`` per layer
+instead, with one block table, free stack and overflow flag shared by the layers: a sequence holds blocks only for the
+rows it has, and gives them back when it is rewound.
 """
 from typing import Optional
 
@@ -60,7 +63,7 @@ import torch
 from torch import Tensor, nn
 
 from unicore import ops
-from unicore_b200.ops.attention_ops import _fused_attention, _fused_attention_varlen, _split_packed
+from unicore_b200.ops.attention_ops import _fused_attention, _fused_attention_varlen, _paged_gather, _split_packed
 
 
 def _bias_as_4d(attn_bias: Optional[Tensor], bsz: int, heads: int, tgt: int, src: int) -> Optional[Tensor]:
@@ -196,7 +199,7 @@ class SelfMultiheadAttention(nn.Module):
             if return_attn:
                 raise ValueError("a decoding step does not return attention weights")
             o = ops.attention_with_kv_cache(q, cache.k, cache.v, cache.seqlens, cache.max_len, k_new=k, v_new=v,
-                                            bias=attn_bias, scale=self.scaling)
+                                            bias=attn_bias, scale=self.scaling, block_table=cache.block_table)
             return o.reshape(bsz, tgt_len, embed_dim), None, None
         if cache is not None:
             cache.store_prefix(k, v)
@@ -240,7 +243,8 @@ class SelfMultiheadAttention(nn.Module):
         q, k, v = (t[:, 0] for t in _split_packed(qkv[:, None], H_kv))
         if cache is not None:   # the prefill (from seqlens = 0) and every step alike: append, then attend
             o = ops.attention_with_kv_cache_varlen(q, cache.k, cache.v, cu_seqlens, max_seqlen, cache.seqlens,
-                                                   cache.max_len, k_new=k, v_new=v, bias=attn_bias, scale=self.scaling)
+                                                   cache.max_len, k_new=k, v_new=v, bias=attn_bias, scale=self.scaling,
+                                                   block_table=cache.block_table)
             return o.reshape(total, embed_dim), None, None
         bias4 = _bias_as_4d(attn_bias, cu_seqlens.numel() - 1, H, max_seqlen, max_seqlen)
         o = _fused_attention_varlen(q, k, v, cu_seqlens, max_seqlen, bias4, self.dropout, self.training, self.scaling,
@@ -400,8 +404,8 @@ def _same_layout(a: Tensor, b: Tensor) -> bool:
 
 class LayerKVCache:
     """One decoder layer's share of a ``DecoderCache``: self-attention keys / values ``k``, ``v`` ``[B, C, H_kv, D]``
-    and the projected encoder keys / values ``enc_k``, ``enc_v`` ``[B, S, H_kv, D]`` (None until the prefill stores
-    them)."""
+    (pools ``[num_blocks, block_size, H_kv, D]`` of a paged cache) and the projected encoder keys / values ``enc_k``,
+    ``enc_v`` ``[B, S, H_kv, D]`` (None until the prefill stores them)."""
 
     def __init__(self, owner, k, v):
         self.owner = owner
@@ -421,9 +425,18 @@ class LayerKVCache:
     def max_len(self):
         return self.owner.max_len
 
+    @property
+    def block_table(self):
+        """The paged cache's ``[B, M]`` block table, None for a contiguous cache."""
+        return self.owner.block_table
+
     def store_prefix(self, k, v):
-        """Rows ``0 .. L-1`` of the self-attention cache from the prefill's ``[B, L, H, D]`` keys and values."""
+        """Rows ``0 .. L-1`` of the self-attention cache from the prefill's ``[B, L, H, D]`` keys and values (through
+        the block table of a paged cache, whose rows without a block are skipped)."""
         with torch.no_grad():
+            if self.block_table is not None:
+                ops.kv_cache_append(k, v, self.k, self.v, torch.zeros_like(self.seqlens), self.block_table)
+                return
             self.k[:, :k.size(1)].copy_(k)
             self.v[:, :v.size(1)].copy_(v)
 
@@ -437,19 +450,27 @@ class LayerKVCache:
         else:
             self.enc_k, self.enc_v = k.detach(), v.detach()
 
+    def _reorder_encoder(self, index):
+        if self.enc_k is None:
+            return
+        if index.numel() != self.enc_k.size(0):
+            self.enc_k, self.enc_v = self.enc_k.index_select(0, index), self.enc_v.index_select(0, index)
+            return
+        with torch.no_grad():
+            for buf in (self.enc_k, self.enc_v):
+                buf.copy_(buf.index_select(0, index))
+
     def reorder(self, index):
         """In place when ``index`` keeps the batch size: only the rows below the host bound ``max_len`` can be read,
         so only they are gathered (into a temporary) and written back.  A new batch size rebinds the buffers."""
         n = self.owner.max_len
         if index.numel() != self.k.size(0):
             self.k, self.v = self.k.index_select(0, index), self.v.index_select(0, index)
-            if self.enc_k is not None:
-                self.enc_k, self.enc_v = self.enc_k.index_select(0, index), self.enc_v.index_select(0, index)
-            return
-        bufs = [self.k[:, :n], self.v[:, :n]] + ([self.enc_k, self.enc_v] if self.enc_k is not None else [])
-        with torch.no_grad():
-            for buf in bufs:
-                buf.copy_(buf.index_select(0, index))
+        else:
+            with torch.no_grad():
+                for buf in (self.k[:, :n], self.v[:, :n]):
+                    buf.copy_(buf.index_select(0, index))
+        self._reorder_encoder(index)
 
 
 class DecoderCache:
@@ -457,23 +478,70 @@ class DecoderCache:
 
     ``layers``: one ``LayerKVCache`` per layer.  ``seqlens``: int32 ``[B]`` on the device, the tokens decoded so far per
     sequence (the position of the next one).  ``max_len``: a host-side upper bound on ``seqlens`` (0 = empty cache), so
-    that no step has to read the device lengths.  ``capacity``: rows of the self-attention buffers.  ``heads``: the
-    key / value heads of the layers (``H_kv`` under grouped-query attention)."""
+    that no step has to read the device lengths.  ``capacity``: rows of the self-attention buffers per sequence.
+    ``heads``: the key / value heads of the layers (``H_kv`` under grouped-query attention).
 
-    def __init__(self, num_layers, batch_size, capacity, heads, head_dim, dtype, device):
+    Paged (``block_size`` set): every layer's ``k`` / ``v`` is a pool ``[num_blocks, block_size, H_kv, D]``, and the
+    layers share ``block_table`` (int32 ``[B, capacity / block_size]``, -1 = no block), the free stack ``free_list``
+    (int32 ``[num_blocks]``, top at ``free_count - 1``), ``free_count`` and ``overflow`` (int32 ``[1]`` each, on the
+    device).  Every call that adds tokens reserves blocks for them first (``reserve``), ``rewind`` releases the blocks
+    past the new lengths, and a pool that runs out sets ``overflow`` (the rows without a block are then not stored).
+    The first blocks handed out are 0, 1, 2, ...  Otherwise the cache behaves as the contiguous one."""
+
+    def __init__(self, num_layers, batch_size, capacity, heads, head_dim, dtype, device, block_size=None,
+                 num_blocks=None):
         self.capacity = capacity
         self.seqlens = torch.zeros(batch_size, dtype=torch.int32, device=device)
         self.max_len = 0
-        shape = (batch_size, capacity, heads, head_dim)
+        self.block_size = block_size
+        self.block_table = self.free_list = self.free_count = self.overflow = None
+        if block_size is None:
+            shape = (batch_size, capacity, heads, head_dim)
+        else:
+            shape = (num_blocks, block_size, heads, head_dim)
+            self.block_table = torch.full((batch_size, capacity // block_size), -1, dtype=torch.int32, device=device)
+            self.free_list = torch.arange(num_blocks - 1, -1, -1, dtype=torch.int32, device=device)
+            self.free_count = torch.full((1,), num_blocks, dtype=torch.int32, device=device)
+            self.overflow = torch.zeros(1, dtype=torch.int32, device=device)
         self.layers = [
             LayerKVCache(self, torch.zeros(shape, dtype=dtype, device=device),
                          torch.zeros(shape, dtype=dtype, device=device))
             for _ in range(num_layers)
         ]
 
+    @property
+    def paged(self):
+        return self.block_size is not None
+
+    def reserve(self, lengths):
+        """Paged: blocks for every row below ``lengths[b]`` (int ``[B]`` on the device) that has none, before a call
+        stores those rows.  Nothing is read on the host.  A no-op for a contiguous cache."""
+        if self.paged:
+            ops.kv_blocks_reserve(self.block_table, self.free_list, self.free_count, lengths, self.block_size,
+                                  self.overflow)
+
+    def _release(self):
+        """Paged: the blocks past ``seqlens`` back onto the free stack."""
+        if self.paged:
+            ops.kv_blocks_release(self.block_table, self.free_list, self.free_count, self.seqlens, self.block_size)
+
+    def free_blocks(self):
+        """Paged: the blocks on the free stack (reads the device, so it synchronises)."""
+        return int(self.free_count.item())
+
+    def overflowed(self):
+        """Paged: whether a reservation has found the pool empty since the cache was made (reads the device)."""
+        return bool(self.overflow.item())
+
     def reorder(self, index):
         """Select (and repeat) sequences of the batch along ``index`` in every buffer, as beam search does.  With as
-        many entries as sequences it writes into the existing buffers (a captured decoding step keeps reading them)."""
+        many entries as sequences it writes into the existing buffers (a captured decoding step keeps reading them).
+        Paged: the rows below ``max_len`` are gathered through the table, every block is released, the sequences
+        reserve blocks again in their new order and the rows are written back through the new table, so the contents
+        are those of a contiguous cache's ``reorder``."""
+        if self.paged:
+            self._reorder_paged(index)
+            return
         for layer in self.layers:
             layer.reorder(index)
         if index.numel() == self.seqlens.numel():
@@ -481,17 +549,45 @@ class DecoderCache:
         else:
             self.seqlens = self.seqlens.index_select(0, index)
 
+    def _reorder_paged(self, index):
+        n, same = self.max_len, index.numel() == self.seqlens.numel()
+        rows = []
+        if n > 0:
+            table = self.block_table[:, :-(-n // self.block_size)]   # the entries of the rows below max_len
+            with torch.no_grad():
+                for layer in self.layers:
+                    k = _paged_gather(layer.k, table)[:, :n].index_select(0, index)
+                    v = _paged_gather(layer.v, table)[:, :n].index_select(0, index)
+                    rows.append((k, v))
+        seqlens = self.seqlens.index_select(0, index)
+        self.seqlens.zero_()
+        self._release()
+        if same:
+            self.seqlens.copy_(seqlens)
+        else:
+            self.seqlens = seqlens
+            self.block_table = torch.full((index.numel(), self.block_table.size(1)), -1, dtype=torch.int32,
+                                          device=self.block_table.device)
+        self.reserve(self.seqlens)
+        for layer, (k, v) in zip(self.layers, rows):
+            layer.store_prefix(k, v)
+        for layer in self.layers:
+            layer._reorder_encoder(index)
+
     def rewind(self, n):
         """Drop the last ``n`` tokens of every sequence (an int), or ``n[b]`` of sequence b (an integer ``[B]`` tensor
         on the device), as speculative decoding does after verifying a chunk of draft tokens: ``seqlens -= n``, clamped
         at 0, without a host synchronisation.  An int also lowers ``max_len``; a tensor leaves it, a valid bound.  The
         rows past ``seqlens`` are never read, so nothing else is reset; rewinding every token empties the cache, and
-        the next call is a prefill again."""
+        the next call is a prefill again.  Paged: the blocks wholly past the new lengths go back to the free stack, so
+        a sequence rewound to 0 holds no memory."""
         if isinstance(n, torch.Tensor):
             self.seqlens.sub_(n.to(device=self.seqlens.device, dtype=self.seqlens.dtype)).clamp_(min=0)
+            self._release()
             return
         n = int(n)
         if n < 0:
             raise ValueError("rewind takes a count of tokens >= 0, not {}".format(n))
         self.seqlens.sub_(n).clamp_(min=0)
         self.max_len = max(self.max_len - n, 0)
+        self._release()

@@ -605,13 +605,15 @@ class TransformerDecoder(nn.Module, _StackMixin):
             raise ValueError("cu_seqlens must have B + 1 = {} entries for the cache's sequences, not {}".format(
                 cache.seqlens.numel() + 1, tuple(cu_seqlens.shape)))
         _check_room(cache, max_seqlen)
+        _, lengths = _varlen_lengths(cu_seqlens.to(cache.seqlens.device), max_seqlen, emb.size(0))
+        new_lengths = (cache.seqlens.clamp(0, cache.capacity) + lengths).clamp(max=cache.capacity)
+        cache.reserve(new_lengths)
         x = self._embed_prologue(emb, None)
         attn_bias = self._step_rel_pos_bias(cache, x, max_seqlen) if self.rel_pos else None
         for layer, lc in zip(self.layers, cache.layers):
             x = layer(x, encoder_out=encoder_out, attn_bias=attn_bias, encoder_padding_mask=encoder_padding_mask,
                       encoder_attn_bias=encoder_attn_mask, cache=lc, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen)
-        _, lengths = _varlen_lengths(cu_seqlens.to(cache.seqlens.device), max_seqlen, emb.size(0))
-        cache.seqlens.copy_((cache.seqlens.clamp(0, cache.capacity) + lengths).clamp(max=cache.capacity))
+        cache.seqlens.copy_(new_lengths)
         cache.max_len += max_seqlen
         return x if self.final_layer_norm is None else self.final_layer_norm(x)
 
@@ -631,18 +633,40 @@ class TransformerDecoder(nn.Module, _StackMixin):
         return x
 
     # ---- incremental decoding ------------------------------------------------------------------------------------
-    def new_cache(self, batch_size, capacity, dtype=None, device=None) -> DecoderCache:
+    def new_cache(self, batch_size, capacity, dtype=None, device=None, block_size=None,
+                  num_blocks=None) -> DecoderCache:
         """An empty ``DecoderCache`` for ``batch_size`` sequences of up to ``capacity`` tokens (prompt included).
-        ``capacity <= max_seq_len``: the relative-position table ends there."""
+        ``capacity <= max_seq_len``: the relative-position table ends there.
+
+        ``block_size`` (a multiple of 128 that divides ``capacity``): a paged cache, whose layers keep their keys and
+        values in pools of ``num_blocks`` blocks of ``block_size`` rows, handed to the sequences as they grow.
+        ``num_blocks`` defaults to ``batch_size * capacity / block_size``, which never runs out; a smaller pool serves
+        a batch whose lengths are mostly below the capacity.  ``None`` (the default) is the contiguous
+        ``[batch_size, capacity, H_kv, D]`` cache."""
         if not self.auto_regressive:
             raise ValueError("incremental decoding needs an auto-regressive decoder")
         if capacity > self.max_seq_len:
             raise ValueError("capacity {} exceeds max_seq_len {}".format(capacity, self.max_seq_len))
+        if block_size is None:
+            if num_blocks is not None:
+                raise ValueError("num_blocks goes with block_size (a paged cache)")
+        else:
+            if int(block_size) != block_size or block_size < 1 or block_size % ops.PAGED_BLOCK_MULTIPLE != 0:
+                raise ValueError("block_size must be a positive multiple of {}, not {}".format(
+                    ops.PAGED_BLOCK_MULTIPLE, block_size))
+            if capacity < 1 or capacity % block_size != 0:
+                raise ValueError("capacity {} must be a positive multiple of block_size {}".format(capacity,
+                                                                                                  block_size))
+            if num_blocks is None:
+                num_blocks = batch_size * capacity // block_size
+            if int(num_blocks) != num_blocks or num_blocks < 1:
+                raise ValueError("num_blocks must be a positive integer, not {}".format(num_blocks))
+            block_size, num_blocks = int(block_size), int(num_blocks)
         weight = self.emb_layer_norm.weight
         heads = self.attention_heads
         kv_heads = self.attention_kv_heads or heads   # grouped-query attention caches H_kv heads
         return DecoderCache(len(self.layers), batch_size, capacity, kv_heads, self.embed_dim // heads,
-                            dtype or weight.dtype, device or weight.device)
+                            dtype or weight.dtype, device or weight.device, block_size, num_blocks)
 
     def _check_no_dropout(self):
         rates = [self.emb_dropout]
@@ -680,12 +704,14 @@ class TransformerDecoder(nn.Module, _StackMixin):
             L = emb.size(1)
             if L > cache.capacity:
                 raise ValueError("the prompt ({} tokens) exceeds the cache capacity {}".format(L, cache.capacity))
+            if padding_mask is None:
+                lengths = torch.full_like(cache.seqlens, L)
+            else:
+                lengths = L - padding_mask.to(device=cache.seqlens.device, dtype=torch.int32).sum(1)
+            cache.reserve(lengths)   # paged: blocks for the unpadded rows, before the layers store them
             x = self._forward_prefix(emb, encoder_out, padding_mask, encoder_padding_mask, attn_mask,
                                      encoder_attn_mask, cache)
-            if padding_mask is None:
-                cache.seqlens.fill_(L)
-            else:
-                cache.seqlens.copy_(L - padding_mask.to(torch.int32).sum(1))
+            cache.seqlens.copy_(lengths)
             cache.max_len = L
             return x
         T = emb.size(1)
@@ -703,6 +729,7 @@ class TransformerDecoder(nn.Module, _StackMixin):
         attends and advances ``cache.seqlens`` by T on the device.  Every host-side shape follows ``cache.max_len``
         (and ``bias_cols``), which the caller advances."""
         T = emb.size(1)
+        cache.reserve(cache.seqlens + T)
         x = self._embed_prologue(emb, None)
         attn_bias = self._step_rel_pos_bias(cache, x, T, bias_cols) if self.rel_pos else None
         for layer, lc in zip(self.layers, cache.layers):
@@ -776,7 +803,8 @@ class CapturedDecoderStep:
 
     def _buffers(self):
         """Every tensor the graph reads or writes besides its own intermediates."""
-        bufs = [self.cache.seqlens, self._emb, self._enc_pad, self._enc_bias]
+        bufs = [self.cache.seqlens, self._emb, self._enc_pad, self._enc_bias, self.cache.block_table,
+                self.cache.free_list, self.cache.free_count, self.cache.overflow]
         for lc in self.cache.layers:
             bufs += [lc.k, lc.v, lc.enc_k, lc.enc_v]
         return bufs
@@ -787,7 +815,7 @@ class CapturedDecoderStep:
     def _capture(self):
         model, cache, T = self.model, self.cache, self.T
         k = cache.layers[0].k
-        B, cap = k.size(0), cache.capacity
+        B, cap = cache.seqlens.numel(), cache.capacity   # a paged cache's k is a pool: its size(0) is not B
         self._graph = self._out = None   # the old graph's memory pool goes back to the allocator
         if self._emb is None or self._emb.size(0) != B:
             self._emb = torch.zeros(B, T, model.embed_dim, dtype=k.dtype, device=k.device)

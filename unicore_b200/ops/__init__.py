@@ -1,12 +1,14 @@
 """Python surface of the hand-written sm_90a kernels (+ PyTorch fallbacks for CPU runs)."""
 from ._native import HAS_CUDA_EXT, USE_NATIVE, native, use_native  # noqa: F401
 from .attention_ops import (  # noqa: F401
+    PAGED_BLOCK_MULTIPLE,
     attention_reference,
     attention_varlen_reference,
     attention_with_kv_cache,
     attention_with_kv_cache_reference,
     attention_with_kv_cache_varlen,
     attention_with_kv_cache_varlen_reference,
+    cache_capacity,
     fused_attention,
     fused_attention_qkvpacked,
     fused_attention_supported,
@@ -14,6 +16,9 @@ from .attention_ops import (  # noqa: F401
     fused_attention_varlen_qkvpacked,
     fused_attention_varlen_supported,
     fused_head_dim_supported,
+    kv_blocks_release,
+    kv_blocks_reserve,
+    kv_cache_append,
     kv_group,
     varlen_positions,
 )

@@ -32,6 +32,14 @@ decoding, a chunked prefill, the candidates of speculative decoding) runs in the
 cache rows up to ``seqlens[b] + i``, so K and V are streamed once per 64-query tile instead of once per token.  Both
 take every head dim the fused kernels take and have no backward.
 
+Paged caches: with ``block_table`` (int ``[B, M]`` on the device) the caches of ``attention_with_kv_cache`` and
+``attention_with_kv_cache_varlen`` are pools ``[num_blocks, block_size, H_kv, D]`` shared by all sequences:
+``block_table[b, i]`` is the block holding rows ``i * block_size .. (i + 1) * block_size - 1`` of sequence ``b`` (-1:
+none), ``block_size`` is a multiple of 128 and the per-sequence capacity is ``C = M * block_size``.  The kernels read
+and append through the table and compute bitwise what the contiguous call computes on the cache gathered through it.
+An append into a row whose entry is outside ``[0, num_blocks)`` is skipped, and reading such a row gives an unspecified
+value.  ``kv_blocks_reserve`` / ``kv_blocks_release`` hand blocks out of a free stack and back, on the device.
+
 Grouped-query attention: every op takes k / v (and the caches) with ``H_kv`` heads where ``H_kv`` divides the ``H``
 query heads.  Query head ``h`` reads key / value head ``h // G``, ``G = H // H_kv`` - the order of
 ``k.repeat_interleave(G, dim=2)`` - and everything else (bias, key mask, dropout, logits, causal) stays per query head,
@@ -478,13 +486,63 @@ def _check_no_grad(*tensors):
                            "torch.inference_mode(), or detach the inputs")
 
 
-def _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, T=None):
+PAGED_BLOCK_MULTIPLE = 128
+
+
+def _check_block_table(block_table, k_cache, v_cache, B):
+    """A paged cache's arguments checked: ``block_table`` an integer ``[B, M >= 1]`` and ``k_cache`` / ``v_cache``
+    pools ``[num_blocks, block_size, H_kv, D]`` of one shape, ``block_size`` a multiple of 128."""
+    if block_table.dim() != 2 or block_table.shape[0] != B or block_table.shape[1] < 1:
+        raise ValueError("block_table must be [B = {}, M >= 1], not {}".format(B, tuple(block_table.shape)))
+    if block_table.dtype not in (torch.int32, torch.int64):
+        raise ValueError("block_table must be int32 or int64, not {}".format(block_table.dtype))
+    if k_cache.dim() != 4 or k_cache.shape[:2] != v_cache.shape[:2] or k_cache.shape[0] < 1:
+        raise ValueError("paged caches must be pools [num_blocks, block_size, H_kv, D] of one shape, not {} and {}"
+                         .format(tuple(k_cache.shape), tuple(v_cache.shape)))
+    if k_cache.shape[1] % PAGED_BLOCK_MULTIPLE != 0:
+        raise ValueError("the block size of paged caches must be a multiple of {}, not {}".format(
+            PAGED_BLOCK_MULTIPLE, k_cache.shape[1]))
+
+
+def cache_capacity(k_cache, block_table=None):
+    """Rows per sequence of a key / value cache: ``C`` of ``[B, C, H_kv, D]``, or ``M * block_size`` of a pool
+    ``[num_blocks, block_size, H_kv, D]`` named by ``block_table [B, M]``."""
+    return k_cache.shape[1] if block_table is None else block_table.shape[1] * k_cache.shape[1]
+
+
+def _paged_gather(cache, block_table):
+    """``[B, C, ...]``: the rows of every sequence gathered through the table from the pool (entries outside the pool
+    clamped into it, as the kernels clamp their reads)."""
+    idx = block_table.long().to(cache.device).clamp(0, cache.shape[0] - 1)
+    return cache[idx].reshape(idx.shape[0], idx.shape[1] * cache.shape[1], *cache.shape[2:])
+
+
+def _cache_store(cache, block_table, rows, write, values):
+    """``cache`` row ``rows[b, i]`` of sequence b becomes ``values[b, i]`` where ``write [B, T]``: batch b of a
+    contiguous cache, or through ``block_table`` into the pool, skipping the rows whose entry is outside it."""
+    B = rows.shape[0]
+    seq = torch.arange(B, device=cache.device)[:, None].expand_as(rows)
+    rows = rows.clamp(0, cache_capacity(cache, block_table) - 1)
+    if block_table is None:
+        dst_b, dst_r = seq, rows
+    else:
+        bs = cache.shape[1]
+        dst_b = block_table.long().to(cache.device)[seq, rows // bs]
+        dst_r = rows % bs
+        write = write & (dst_b >= 0) & (dst_b < cache.shape[0])
+    cache[dst_b[write], dst_r[write]] = values[write].to(cache.dtype)
+
+
+def _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, T=None, block_table=None, B=None):
     """The arguments of ``attention_with_kv_cache`` checked, as ``(T, append, max_len, bound)``: ``max_len`` the host
     bound on ``seqlens`` (by default the most the capacity allows; None without ``seqlens`` unless given) and
     ``bound`` the keys any query can see, ``max_len`` plus the appended rows, else the capacity C.  ``T``: the new
     queries per sequence (default ``q.shape[1]``; the host bound ``max_seqlen`` of packed chunks, whose q / k_new /
-    v_new are ``[N, heads, D]``)."""
+    v_new are ``[N, heads, D]``).  ``block_table``: the caches are pools (``_check_block_table``) of ``B`` sequences
+    (default ``q.shape[0]``) and C is ``M * block_size``."""
     kv_group(q.shape[-2], k_cache, v_cache)
+    if block_table is not None:
+        _check_block_table(block_table, k_cache, v_cache, q.shape[0] if B is None else B)
     append = k_new is not None
     if append != (v_new is not None):
         raise ValueError("k_new and v_new go together")
@@ -495,7 +553,7 @@ def _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, T=None):
     T = q.shape[1] if T is None else int(T)
     if T > 1 and seqlens is not None and not append:
         raise ValueError("a chunk of T > 1 queries with seqlens appends k_new / v_new")
-    C = k_cache.shape[1]
+    C = cache_capacity(k_cache, block_table)
     new_rows = T if append else 0
     if seqlens is not None and max_len is None:
         max_len = C - new_rows
@@ -506,14 +564,30 @@ def _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, T=None):
 
 
 def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len=None, k_new=None, v_new=None,
-                                      bias=None, key_padding_mask=None, scale=None):
+                                      bias=None, key_padding_mask=None, scale=None, block_table=None):
     """Plain PyTorch implementation of ``attention_with_kv_cache`` (CPU path, fallback and test oracle).
 
     Performs the append in place like the kernels.  One query (T = 1): row ``seqlens[b]`` (clamped to ``C - 1``) of the
     caches becomes ``k_new[b] / v_new[b]``.  A chunk (T > 1): rows ``p_b + i``, ``p_b = seqlens[b]`` clamped to
     ``[0, C]``, become ``k_new[b, i] / v_new[b, i]``, rows at or past ``C`` are skipped, and query ``i`` sees key ``j``
     only when ``j <= p_b + i``.  Keys past the visible length are masked; a row with no visible unmasked key gives 0.
+    ``block_table``: the caches are pools; the call runs on the caches gathered through the table, and the appended
+    rows are written back through it (rows whose entry is outside the pool are skipped).
     """
+    if block_table is not None:
+        T, append, _, _ = _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, block_table=block_table)
+        kc, vc = _paged_gather(k_cache, block_table), _paged_gather(v_cache, block_table)
+        out = attention_with_kv_cache_reference(q, kc, vc, seqlens, max_len, k_new, v_new, bias, key_padding_mask,
+                                                scale)
+        if append:
+            C = kc.shape[1]
+            if T == 1:
+                start = seqlens.long().to(kc.device).clamp(0, C - 1)
+            else:
+                start = seqlens.long().to(kc.device).clamp(0, C)
+            rows = start[:, None] + torch.arange(T, device=kc.device)[None, :]
+            _write_back(k_cache, v_cache, kc, vc, block_table, rows, rows < C)
+        return out
     T, append, _, K = _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new)
     B, _, H, D = q.shape
     C = k_cache.shape[1]
@@ -540,6 +614,14 @@ def attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens=None, max_len
     else:
         n = torch.full((B,), C, dtype=torch.long, device=q.device)
     return _kv_cache_attend_reference(q, k_cache, v_cache, n, future, K, bias, key_padding_mask, scale)
+
+
+def _write_back(k_cache, v_cache, kc, vc, block_table, rows, write):
+    """The rows ``rows [B, T]`` (where ``write``) of the gathered caches ``kc`` / ``vc`` stored back into the pools."""
+    at = rows.clamp(0, kc.shape[1] - 1)
+    seq = torch.arange(rows.shape[0], device=kc.device)[:, None]
+    _cache_store(k_cache, block_table, rows, write, kc[seq, at])
+    _cache_store(v_cache, block_table, rows, write, vc[seq, at])
 
 
 def _kv_cache_attend_reference(q, k_cache, v_cache, n, future, K, bias, key_padding_mask, scale):
@@ -569,9 +651,9 @@ def _kv_cache_attend_reference(q, k_cache, v_cache, n, future, K, bias, key_padd
     return torch.einsum("bhqk,bkhd->bqhd", probs, v)
 
 
-def _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask) -> bool:
+def _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask, block_table=None) -> bool:
     """True when ``fmha_decode`` (T = 1) or ``kvcache.fmha_kvcache_fwd`` (T > 1) takes the operands."""
-    if not use_native(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask) \
+    if not use_native(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask, block_table) \
             or not hasattr(native(), "fmha_decode"):
         return False
     if q.dim() != 4 or q.shape[1] < 1 or (q.shape[1] > 1 and not hasattr(native(), "kvcache")):
@@ -614,7 +696,7 @@ def _native_cache_operands(q, seqlens, bias, key_padding_mask, bound, B, T, chun
 
 
 def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_new=None, v_new=None, bias=None,
-                            key_padding_mask=None, scale=None):
+                            key_padding_mask=None, scale=None, block_table=None):
     """Attention of T new queries per sequence against a key / value cache: one decoding step (T = 1) or a chunk.
 
     q: ``[B, T, H, D]``; k_cache / v_cache: ``[B, C, H_kv, D]`` with ``H_kv`` dividing ``H`` (strided views are fine,
@@ -628,49 +710,78 @@ def attention_with_kv_cache(q, k_cache, v_cache, seqlens=None, max_len=None, k_n
     are ignored); key_padding_mask: bool ``[B, Lk]``, True = masked; a narrower bias or key mask hides the keys past
     its columns.  A query whose visible keys are all masked gives 0.  Returns ``[B, T, H, D]``.  No dropout and no
     backward.  Under CUDA-graph capture (``max_len`` then a fixed bound such as the capacity) a one-token step divides
-    each sequence's device length over the split-KV splits."""
+    each sequence's device length over the split-KV splits.  ``block_table`` (int ``[B, M]`` on the device): the
+    caches are pools ``[num_blocks, block_size, H_kv, D]`` and ``C = M * block_size`` (see the module docstring)."""
     _check_no_grad(q, k_cache, v_cache, k_new, v_new, bias)
-    T, _, max_len, bound = _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new)
+    T, _, max_len, bound = _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new,
+                                          block_table=block_table)
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
-    if not _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask):
+    if not _decode_supported(q, k_cache, v_cache, seqlens, k_new, v_new, bias, key_padding_mask, block_table):
         return attention_with_kv_cache_reference(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
-                                                 key_padding_mask, scale)
+                                                 key_padding_mask, scale, block_table)
     seqlens, bias, key_padding_mask = _native_cache_operands(q, seqlens, bias, key_padding_mask, bound, q.shape[0], T,
                                                              T > 1)
+    block_table = _native_table(block_table)
     max_len = 0 if max_len is None else int(max_len)
     if T == 1:
         # A step captured in a CUDA graph runs with the capacity as its host bound, far above most true lengths: each
         # (b, h) then spreads its own device length over the splits, not the bound (or most splits would be empty).
         return native().fmha_decode(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias, key_padding_mask,
-                                    float(scale), split_by_length=torch.cuda.is_current_stream_capturing())
+                                    float(scale), split_by_length=torch.cuda.is_current_stream_capturing(),
+                                    block_table=block_table)
     return native().kvcache.fmha_kvcache_fwd(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, bias,
-                                             key_padding_mask, float(scale))
+                                             key_padding_mask, float(scale), block_table=block_table)
 
 
-def _kv_cache_varlen_plan(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens, max_len, k_new, v_new):
+def _native_table(block_table):
+    """The block table as the kernels take it: int32 and contiguous (passed on as it is when it already is)."""
+    if block_table is not None and (block_table.dtype != torch.int32 or not block_table.is_contiguous()):
+        block_table = block_table.to(torch.int32).contiguous()
+    return block_table
+
+
+def _kv_cache_varlen_plan(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens, max_len, k_new, v_new,
+                          block_table=None):
     """``attention_with_kv_cache_varlen``'s arguments checked, as ``_kv_cache_plan``'s result for chunks of up to
     ``max_seqlen`` queries."""
     if q.dim() != 3 or (k_new is not None and k_new.dim() != 3) or (v_new is not None and v_new.dim() != 3):
         raise ValueError("packed chunks take q [N, H, D] and k_new / v_new [N, H_kv, D]")
-    if cu_seqlens.dim() != 1 or cu_seqlens.numel() != k_cache.shape[0] + 1:
+    B = k_cache.shape[0] if block_table is None else block_table.shape[0]
+    if cu_seqlens.dim() != 1 or cu_seqlens.numel() != B + 1:
         raise ValueError("cu_seqlens must have B + 1 = {} entries for the caches' B = {} sequences, not {}".format(
-            k_cache.shape[0] + 1, k_cache.shape[0], tuple(cu_seqlens.shape)))
+            B + 1, B, tuple(cu_seqlens.shape)))
     if int(max_seqlen) < 1:
         raise ValueError("max_seqlen must be positive, not {}".format(max_seqlen))
     if seqlens is not None and k_new is None:
         raise ValueError("packed chunks with seqlens append k_new / v_new")
-    return _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, T=max_seqlen)
+    return _kv_cache_plan(q, k_cache, v_cache, seqlens, max_len, k_new, v_new, T=max_seqlen, block_table=block_table,
+                          B=B)
 
 
 def attention_with_kv_cache_varlen_reference(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens=None, max_len=None,
-                                             k_new=None, v_new=None, bias=None, key_padding_mask=None, scale=None):
+                                             k_new=None, v_new=None, bias=None, key_padding_mask=None, scale=None,
+                                             block_table=None):
     """Plain PyTorch implementation of ``attention_with_kv_cache_varlen`` (CPU path, fallback and test oracle).
 
     Performs the append in place like the kernels, ``T_b`` rows per sequence: rows ``p_b + i`` of the caches,
     ``p_b = seqlens[b]`` clamped to ``[0, C]``, become packed rows ``s_b + i`` of ``k_new / v_new``, and rows at or past
     ``C`` are skipped.  At every real row the result is what ``attention_with_kv_cache_reference`` gives for that
-    sequence alone with ``T = T_b``; packed rows of no sequence give 0."""
+    sequence alone with ``T = T_b``; packed rows of no sequence give 0.  ``block_table``: pools, as in
+    ``attention_with_kv_cache_reference``."""
+    if block_table is not None:
+        T, _, _, _ = _kv_cache_varlen_plan(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens, max_len, k_new, v_new,
+                                           block_table)
+        kc, vc = _paged_gather(k_cache, block_table), _paged_gather(v_cache, block_table)
+        out = attention_with_kv_cache_varlen_reference(q, kc, vc, cu_seqlens, max_seqlen, seqlens, max_len, k_new,
+                                                       v_new, bias, key_padding_mask, scale)
+        if seqlens is not None:
+            C = kc.shape[1]
+            _, n = _varlen_lengths(cu_seqlens.to(kc.device), T, q.shape[0])
+            i = torch.arange(T, device=kc.device)[None, :]
+            rows = seqlens.long().to(kc.device).clamp(0, C)[:, None] + i
+            _write_back(k_cache, v_cache, kc, vc, block_table, rows, (i < n[:, None]) & (rows < C))
+        return out
     T, _, _, K = _kv_cache_varlen_plan(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens, max_len, k_new, v_new)
     N, H, D = q.shape
     B, C = k_cache.shape[:2]
@@ -699,9 +810,10 @@ def attention_with_kv_cache_varlen_reference(q, k_cache, v_cache, cu_seqlens, ma
     return packed[:N]
 
 
-def _kvcache_varlen_supported(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask) -> bool:
+def _kvcache_varlen_supported(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask,
+                              block_table=None) -> bool:
     """True when ``kvcache.fmha_kvcache_varlen_fwd`` takes the operands."""
-    if not use_native(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask) \
+    if not use_native(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask, block_table) \
             or not hasattr(getattr(native(), "kvcache", None), "fmha_kvcache_varlen_fwd"):
         return False
     if q.shape[0] < 1 or q.stride(1) != q.shape[-1]:   # the q map takes (head, 16-byte chunk) as one dimension
@@ -715,7 +827,8 @@ def _kvcache_varlen_supported(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v
 
 
 def attention_with_kv_cache_varlen(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens=None, max_len=None,
-                                   k_new=None, v_new=None, bias=None, key_padding_mask=None, scale=None):
+                                   k_new=None, v_new=None, bias=None, key_padding_mask=None, scale=None,
+                                   block_table=None):
     """``attention_with_kv_cache`` for packed chunks: each sequence brings its own number of new queries.
 
     q: ``[N, H, D]``, the B sequences' new queries back to back; sequence b's ``T_b`` queries are rows ``s_b .. s_b +
@@ -735,18 +848,109 @@ def attention_with_kv_cache_varlen(q, k_cache, v_cache, cu_seqlens, max_seqlen, 
 
     It runs in the KV-cache mode of the wgmma forward for every ``T_b``, one-token sequences included: the host cannot
     tell that every ``T_b`` is 1 without reading ``cu_seqlens``.  For pure one-token decoding a padded ``[B, 1, H, D]``
-    step (``attention_with_kv_cache``, split-KV) or a captured step stays the fast path."""
+    step (``attention_with_kv_cache``, split-KV) or a captured step stays the fast path.  ``block_table``: paged
+    caches, as in ``attention_with_kv_cache``."""
     _check_no_grad(q, k_cache, v_cache, k_new, v_new, bias)
     T, _, max_len, bound = _kv_cache_varlen_plan(q, k_cache, v_cache, cu_seqlens, max_seqlen, seqlens, max_len,
-                                                 k_new, v_new)
+                                                 k_new, v_new, block_table)
     if scale is None:
         scale = 1.0 / math.sqrt(q.shape[-1])
-    if not _kvcache_varlen_supported(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask):
+    if not _kvcache_varlen_supported(q, k_cache, v_cache, cu_seqlens, seqlens, k_new, v_new, bias, key_padding_mask,
+                                     block_table):
         return attention_with_kv_cache_varlen_reference(q, k_cache, v_cache, cu_seqlens, T, seqlens, max_len, k_new,
-                                                        v_new, bias, key_padding_mask, scale)
-    B = k_cache.shape[0]
+                                                        v_new, bias, key_padding_mask, scale, block_table)
+    B = cu_seqlens.numel() - 1
     seqlens, bias, key_padding_mask = _native_cache_operands(q, seqlens, bias, key_padding_mask, bound, B, T, True)
     cu_seqlens = cu_seqlens.to(torch.int32).contiguous()
     return native().kvcache.fmha_kvcache_varlen_fwd(q, k_cache, v_cache, cu_seqlens, T, seqlens,
                                                     0 if max_len is None else int(max_len), k_new, v_new, bias,
-                                                    key_padding_mask, float(scale))
+                                                    key_padding_mask, float(scale),
+                                                    block_table=_native_table(block_table))
+
+
+# ---- paged caches: the append on its own and the block allocator ----------------------------------------------------
+def kv_cache_append(k_new, v_new, k_cache, v_cache, seqlens, block_table=None):
+    """Rows ``i`` of ``k_new`` / ``v_new [B, T, H_kv, D]`` written bitwise into rows ``p_b + i`` of the caches, ``p_b =
+    clamp(seqlens[b], 0, C)``: ``[B, C, H_kv, D]``, or pools through ``block_table`` (``attention_with_kv_cache``).
+    Rows at or past ``C``, and rows whose table entry is outside the pool, are skipped.  This is the append of a chunk
+    step without its attention: a paged prefill stores its keys and values with it (``seqlens`` = 0)."""
+    B, T = k_new.shape[:2]
+    if block_table is not None:
+        _check_block_table(block_table, k_cache, v_cache, B)
+    if use_native(k_new, v_new, k_cache, v_cache, seqlens, block_table) and _kernel_tensors(k_new, v_new, k_cache,
+                                                                                            v_cache):
+        native().kvcache.kv_cache_append(k_new, v_new, k_cache, v_cache, seqlens.to(torch.int32).contiguous(),
+                                         _native_table(block_table))
+        return
+    C = cache_capacity(k_cache, block_table)
+    rows = seqlens.long().to(k_cache.device).clamp(0, C)[:, None] + torch.arange(T, device=k_cache.device)[None, :]
+    _cache_store(k_cache, block_table, rows, rows < C, k_new)
+    _cache_store(v_cache, block_table, rows, rows < C, v_new)
+
+
+def _check_kv_blocks(block_table, free_list, free_count, lengths, block_size, overflow=None):
+    for name, t in (("block_table", block_table), ("free_list", free_list), ("free_count", free_count),
+                    ("overflow", overflow)):
+        if t is not None and (t.dtype != torch.int32 or not t.is_contiguous()):
+            raise ValueError("{} must be a contiguous int32 tensor (it is updated in place)".format(name))
+    if block_table.dim() != 2 or free_list.dim() != 1 or free_list.numel() < 1 or free_count.numel() != 1 \
+            or (overflow is not None and overflow.numel() != 1):
+        raise ValueError("the allocator takes block_table [B, M], free_list [num_blocks >= 1], free_count [1] and "
+                         "overflow [1]")
+    if lengths.shape != (block_table.shape[0],):
+        raise ValueError("lengths must be [B = {}], not {}".format(block_table.shape[0], tuple(lengths.shape)))
+    if int(block_size) < 1:
+        raise ValueError("block_size must be positive, not {}".format(block_size))
+    return lengths.to(device=block_table.device, dtype=torch.int32).contiguous()
+
+
+def _kv_blocks_flags(block_table, lengths, block_size):
+    """``(kept [B, M], table [B * M] int64)``: the entries below ``ceil(clamp(lengths[b], 0, C) / block_size)``."""
+    B, M = block_table.shape
+    n = lengths.long().clamp(0, M * block_size)
+    kept = torch.arange(M, device=block_table.device)[None, :] < ((n + block_size - 1) // block_size)[:, None]
+    return kept, block_table.reshape(-1).long()
+
+
+def kv_blocks_reserve(block_table, free_list, free_count, lengths, block_size, overflow):
+    """Give every sequence b a block for each table entry below ``ceil(clamp(lengths[b], 0, C) / block_size)`` that
+    has none (< 0), off the top of the free stack (``free_list[free_count - 1]`` first), in the order (b, i)
+    ascending.  When the stack runs out the entry stays -1 and ``overflow`` (int32 ``[1]``) is set to 1.  All int32
+    tensors on one device, updated in place; nothing is read on the host, so a CUDA graph can hold the call.  The
+    block ids depend only on the inputs (``kv_blocks`` kernels, or the same result in PyTorch)."""
+    lengths = _check_kv_blocks(block_table, free_list, free_count, lengths, block_size, overflow)
+    if use_native(block_table, free_list, free_count, lengths, overflow):
+        native().kvcache.kv_blocks_reserve(block_table, free_list, free_count, lengths, int(block_size), overflow)
+        return
+    kept, table = _kv_blocks_flags(block_table, lengths, block_size)
+    NB = free_list.numel()
+    need = kept.reshape(-1) & (table < 0)
+    k = need.long().cumsum(0) - need.long()   # the stack slot each needing entry takes, counted from the top
+    count = free_count.long().clamp(0, NB)
+    give = need & (k < count)
+    src = (count - 1 - k).clamp(0, NB - 1)
+    block_table.copy_(torch.where(give, free_list.long()[src], table).view_as(block_table))
+    overflow.copy_(torch.where((need & ~give).any(), torch.ones_like(overflow), overflow))
+    free_count.copy_(count - torch.minimum(need.long().sum(), count))
+
+
+def kv_blocks_release(block_table, free_list, free_count, lengths, block_size):
+    """Push every block at or past entry ``ceil(clamp(lengths[b], 0, C) / block_size)`` of sequence b back onto the
+    free stack, in the order (b, i) ascending, and set those entries to -1.  Entries outside ``[0, num_blocks)`` are
+    dropped, not pushed.  In place and on the device, as ``kv_blocks_reserve``."""
+    lengths = _check_kv_blocks(block_table, free_list, free_count, lengths, block_size)
+    if use_native(block_table, free_list, free_count, lengths):
+        native().kvcache.kv_blocks_release(block_table, free_list, free_count, lengths, int(block_size))
+        return
+    kept, table = _kv_blocks_flags(block_table, lengths, block_size)
+    NB = free_list.numel()
+    drop = ~kept.reshape(-1)
+    push = drop & (table >= 0) & (table < NB)
+    count = free_count.long().clamp(0, NB)
+    slot = count + push.long().cumsum(0) - push.long()
+    ok = push & (slot < NB)
+    stack = torch.cat([free_list.long(), free_list.new_zeros(1, dtype=torch.long)])   # slot NB: dropped writes
+    stack.scatter_(0, torch.where(ok, slot, torch.full_like(slot, NB)), table)
+    free_list.copy_(stack[:NB])
+    block_table.copy_(torch.where(drop, torch.full_like(table, -1), table).view_as(block_table))
+    free_count.copy_(torch.minimum(count + push.long().sum(), torch.full_like(count, NB)))
